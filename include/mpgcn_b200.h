@@ -31,8 +31,10 @@
 extern "C" {
 #endif
 
-#define MPGCN_B200_ABI_VERSION 3   /* 2: extras struct, prepared supports, LSTM training pair, dg_absmax, dyn graphs;
-                                      3: layer parts (origin-row / support shards), bias_act, relu_backward, region tags */
+#define MPGCN_B200_ABI_VERSION 4   /* 2: extras struct, prepared supports, LSTM training pair, dg_absmax, dyn graphs;
+                                      3: layer parts (origin-row / support shards), bias_act, relu_backward, region tags;
+                                      4: peer push removed: mpgcn_bdgcn_part loses peer_g / peer_rank / peer_out,
+                                         mpgcn_rows_reduce_bias_act loses part_rows */
 
 #if defined(__GNUC__)
 #define MPGCN_API __attribute__((visibility("default")))
@@ -124,19 +126,12 @@ MPGCN_API int mpgcn_bdgcn_backward_ex(const float* d_out, const float* out, cons
  * mpgcn_bias_act.  backward_part takes dPre [B,N,N,H] for every origin row m (the caller masks its own rows with
  * mpgcn_relu_backward and all-gathers them / has them replicated) and returns dX for its rows ([B,rows,N,C]; K shard: the
  * partial sum over its d, to be all-reduced) and dW for its slice (row shard: partial over its rows, to be all-reduced).
- *   X [B,rows,N,C]   pre_partial [B,N,N,H]   saved: mpgcn_bdgcn_part_saved_bytes   d_pre [B,N,N,H]   dX [B,rows,N,C] or NULL
+ *   X [B,rows,N,C]   pre_partial [B,N,N,H] (required)   saved: mpgcn_bdgcn_part_saved_bytes   d_pre [B,N,N,H]   dX [B,rows,N,C] or NULL
  *   extras (nullable): go_prepared / gd_prepared (supports converted once by mpgcn_bdgcn_prepare_supports), d_out_absmax (= max|d_pre|
  *   already known), d_pre_f16 + d_pre_scale2 (backward: the fp16 dPre produced by mpgcn_relu_backward_scatter_f16). */
 typedef struct mpgcn_bdgcn_part {
   int row0, rows;
   int Ko, Kd;
-  /* forward_part, optional (precision 1): PUSH the partial into peer memory from the contraction's own epilogue instead of writing
-   * pre_partial (which may then be NULL).  peer_out[r] = rank r's staging buffer [peer_g slots][B][N/peer_g][N][H] fp32 (this rank's
-   * own buffer, or a peer's mapped into this process); output row m is stored into buffer m / (N/peer_g), slot peer_rank -- so after
-   * a barrier every rank holds, in its slot j, rank j's partial for ITS rows and sums them locally (mpgcn_rows_reduce_bias_act with
-   * part_rows = rows).  The NVLink transfer overlaps the MMAs tile by tile.  peer_g = 0: off. */
-  int peer_g, peer_rank;
-  void* peer_out[8];
 } mpgcn_bdgcn_part;
 MPGCN_API size_t mpgcn_bdgcn_part_saved_bytes(int B, int N, int C, int H, int precision, const mpgcn_bdgcn_part* part);
 MPGCN_API size_t mpgcn_bdgcn_part_fwd_workspace_bytes(int B, int N, int C, int H, int dynamic, int precision, const mpgcn_bdgcn_part* part);
@@ -156,13 +151,11 @@ MPGCN_API int mpgcn_relu_backward(const float* d_out, const float* out, int act,
  * collective.  `partials` / `dsts` are HOST arrays of g <= 8 DEVICE pointers to [B,N,N,H] fp32 buffers -- the rank's own and its peers'
  * buffers mapped into this process (symmetric memory / CUDA IPC); the caller places a barrier between the producers and these calls.
  *   rows_reduce_bias_act:  out[b,r,e,h] = act( sum_j partials[j][b, row0 + r, e, h] + bias[h] )   out [B,rows,N,H]
- *        (part_rows = N: the parts are whole [B,N,N,H] partials; part_rows = rows: they are staging slots [B,rows,N,H] that already
- *        hold only this rank's rows -- what the peer push of mpgcn_bdgcn_forward_part leaves -- and row0 is not used)
  *        = reduce-scatter of the partial pre-activations (each rank reads ITS rows from every rank) + MPGCN.py:47-49;
  *   relu_backward_scatter: d_pre = d_out * [out > 0] (d_out, out [B,rows,N,H]) stored to rows [row0, row0 + rows) of EVERY dsts[j];
  *        db[h] = sum d_pre (nullable)   = ReLU mask + all-gather of dPre. */
 MPGCN_API int mpgcn_rows_reduce_bias_act(float* out, const float* const* partials, int g, const float* bias, int act, int B, int N, int row0,
-                               int rows, int part_rows, int H, void* stream);
+                               int rows, int H, void* stream);
 MPGCN_API int mpgcn_relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N,
                                 int row0, int rows, int H, void* stream);
 /* The same for the tensor-core path with its fp16 cast folded in: absmax = device scalar holding the GLOBAL max|d_out| (every rank's

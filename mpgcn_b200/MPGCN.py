@@ -22,7 +22,6 @@ never materialises the `[B*N*N, T, C]` output sequence.
 from __future__ import annotations
 
 import contextlib
-import os
 
 import torch
 from torch import nn
@@ -85,8 +84,7 @@ class MPGCN(nn.Module):
         self.gcn_num_layers = gcn_num_layers
         self.lstm_precision = None      # None -> ops.default_precision(); or "auto" / "fp16" / "fp32"
         # True: evaluate the M branches on M CUDA streams (they are independent until the head, reference MPGCN.py:101-110), so that
-        # the HBM-bound elementwise kernels of one branch run beside the tensor-bound contractions of the other; None -> env
-        # MPGCN_B200_BRANCH_STREAMS (default off)
+        # the HBM-bound elementwise kernels of one branch run beside the tensor-bound contractions of the other; None -> off
         self.branch_streams = None
         self._streams = None
         self.branch_models = nn.ModuleList()
@@ -119,8 +117,7 @@ class MPGCN(nn.Module):
         assert (len(x_seq.shape) == 5) & (self.num_nodes == x_seq.shape[2] == x_seq.shape[3])
         assert len(G_list) == self.M
         B, N = x_seq.shape[0], self.num_nodes
-        use_streams = self.branch_streams if self.branch_streams is not None else os.environ.get("MPGCN_B200_BRANCH_STREAMS", "0") == "1"
-        use_streams = bool(use_streams) and x_seq.is_cuda and self.M > 1
+        use_streams = bool(self.branch_streams) and x_seq.is_cuda and self.M > 1
         capturing = use_streams and torch.cuda.is_current_stream_capturing()
         cur = torch.cuda.current_stream() if use_streams else None
         if use_streams and (self._streams is None or self._streams[0].device != x_seq.device):

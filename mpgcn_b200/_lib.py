@@ -73,7 +73,7 @@ _SIGS = {
     "mpgcn_relu_backward_scatter_f16": (ctypes.c_int, [_c_f, _c_f, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, _c_f, _c_f, _c_f] +
                                         [ctypes.c_int] * 5 + [ctypes.c_void_p]),
     "mpgcn_absmax": (ctypes.c_int, [_c_f, ctypes.c_longlong, _c_f, ctypes.c_void_p]),
-    "mpgcn_rows_reduce_bias_act": (ctypes.c_int, [_c_f, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, _c_f, ctypes.c_int] + [ctypes.c_int] * 6 + [ctypes.c_void_p]),
+    "mpgcn_rows_reduce_bias_act": (ctypes.c_int, [_c_f, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, _c_f, ctypes.c_int] + [ctypes.c_int] * 5 + [ctypes.c_void_p]),
     "mpgcn_relu_backward_scatter": (ctypes.c_int, [_c_f, _c_f, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, _c_f] + [ctypes.c_int] * 5 +
                                     [ctypes.c_void_p]),
     "mpgcn_bias_act": (ctypes.c_int, [_c_f, _c_f, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
@@ -81,7 +81,7 @@ _SIGS = {
     "mpgcn_lstm_last_backward": (ctypes.c_int, [_c_f] * 12 + [ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int,
                                                 ctypes.c_int, ctypes.c_void_p]),
 }
-ABI_VERSION = 3          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
+ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
 
@@ -94,8 +94,7 @@ class BdgcnExtras(ctypes.Structure):
 
 class BdgcnPart(ctypes.Structure):
     """mpgcn_bdgcn_part (include/mpgcn_b200.h): origin rows [row0, row0 + rows), Ko origin / Kd destination supports."""
-    _fields_ = [("row0", ctypes.c_int), ("rows", ctypes.c_int), ("Ko", ctypes.c_int), ("Kd", ctypes.c_int),
-                ("peer_g", ctypes.c_int), ("peer_rank", ctypes.c_int), ("peer_out", ctypes.c_void_p * 8)]
+    _fields_ = [("row0", ctypes.c_int), ("rows", ctypes.c_int), ("Ko", ctypes.c_int), ("Kd", ctypes.c_int)]
 
 
 def build(verbose: bool = False) -> str:

@@ -19,19 +19,13 @@ static BdgcnShape mk(int B, int N, int K, int C, int H, int dynamic, int act) {
   BdgcnShape s;
   s.B = B; s.N = N; s.K = K; s.C = C; s.H = H; s.dynamic = dynamic; s.act = act;
   s.R = N; s.row0 = 0; s.Ko = K; s.Kd = K; s.partial = 0;      // the whole layer
-  s.peer_g = 0; s.peer_rank = 0;
-  for (int j = 0; j < 8; ++j) s.peer_out[j] = nullptr;
   return s;
 }
 
 // a PART of the layer (include/mpgcn_b200.h: mpgcn_bdgcn_part)
 static BdgcnShape mk_part(int B, int N, int C, int H, int dynamic, const mpgcn_bdgcn_part* part) {
   BdgcnShape s = mk(B, N, part ? (part->Ko > part->Kd ? part->Ko : part->Kd) : 1, C, H, dynamic, 0);
-  if (part) {
-    s.R = part->rows; s.row0 = part->row0; s.Ko = part->Ko; s.Kd = part->Kd;
-    s.peer_g = part->peer_g; s.peer_rank = part->peer_rank;
-    for (int j = 0; j < 8; ++j) s.peer_out[j] = static_cast<float*>(part->peer_out[j]);
-  }
+  if (part) { s.R = part->rows; s.row0 = part->row0; s.Ko = part->Ko; s.Kd = part->Kd; }
   s.partial = 1;
   return s;
 }
@@ -173,16 +167,7 @@ int mpgcn_bdgcn_forward_part(const float* X, const float* G_o, const float* G_d,
   MPGCN_CHECK(part != nullptr, "mpgcn_bdgcn_forward_part: part descriptor is NULL");
   const BdgcnShape s = mk_part(B, N, C, H, dynamic ? 1 : 0, part);
   if (int e = check_part(s, precision)) return e;
-  MPGCN_CHECK(X && G_o && G_d && W && workspace, "mpgcn_bdgcn_forward_part: null pointer argument");
-  if (s.peer_g > 0) {
-    MPGCN_CHECK(precision == PREC_FP16_TC, "mpgcn_bdgcn_forward_part: the peer-memory push is implemented in the tensor-core epilogue only");
-    MPGCN_CHECK(s.peer_g <= 8 && s.N % s.peer_g == 0 && s.peer_rank >= 0 && s.peer_rank < s.peer_g, "mpgcn_bdgcn_forward_part: bad peer layout g=%d rank=%d N=%d",
-                s.peer_g, s.peer_rank, s.N);
-    for (int j = 0; j < s.peer_g; ++j)
-      MPGCN_CHECK(s.peer_out[j] != nullptr && (reinterpret_cast<uintptr_t>(s.peer_out[j]) & 31) == 0, "mpgcn_bdgcn_forward_part: peer buffer %d null or misaligned", j);
-  } else {
-    MPGCN_CHECK(pre_partial != nullptr, "mpgcn_bdgcn_forward_part: pre_partial is NULL");
-  }
+  MPGCN_CHECK(X && G_o && G_d && W && pre_partial && workspace, "mpgcn_bdgcn_forward_part: null pointer argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ProfRegion region(PROF_LAYER_FWD, layer_flops(s, false) * s.R / s.N * (s.Ko + s.Kd) / (2.0 * s.K), st);
   if (precision == PREC_FP16_TC)
@@ -218,9 +203,9 @@ int mpgcn_bias_act(float* x, const float* bias, int act, long long n, int H, voi
 }
 
 int mpgcn_rows_reduce_bias_act(float* out, const float* const* partials, int g, const float* bias, int act, int B, int N, int row0, int rows,
-                               int part_rows, int H, void* stream) {
+                               int H, void* stream) {
   MPGCN_CHECK(out && partials && B >= 1 && (act == 0 || act == 1), "mpgcn_rows_reduce_bias_act: bad argument");
-  return rows_reduce_bias_act(out, partials, g, bias, act, B, N, row0, rows, part_rows, H, static_cast<cudaStream_t>(stream));
+  return rows_reduce_bias_act(out, partials, g, bias, act, B, N, row0, rows, H, static_cast<cudaStream_t>(stream));
 }
 
 int mpgcn_relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N, int row0,

@@ -17,7 +17,6 @@
 #include "kernels.h"
 #include "tc_engine.cuh"
 
-#include <stdlib.h>
 #include <string.h>
 
 namespace mpgcn {
@@ -65,13 +64,6 @@ int map_chunks(CUtensorMap* m, const __half* t, long long k_rows, long long k_st
   const uint32_t box[4] = {32, (uint32_t)box_k, (uint32_t)box_r, 1};
   return make_tmap_f16(m, t, 4, dims, str, box, TMAP_SW64);
 }
-// flat tensor T[z][k][cols]: dims (col, k, z, 1), box (32, box_k)
-int map_flat(CUtensorMap* m, const __half* t, long long cols, long long k_rows, long long z_count, int box_k, int box_cols = 32) {
-  const uint64_t dims[4] = {(uint64_t)cols, (uint64_t)k_rows, (uint64_t)z_count, 1};
-  const uint64_t str[3] = {(uint64_t)cols * 2, (uint64_t)cols * k_rows * 2, (uint64_t)cols * k_rows * 2 * (uint64_t)z_count};
-  const uint32_t box[4] = {(uint32_t)box_cols, (uint32_t)box_k, 1, 1};
-  return make_tmap_f16(m, t, 4, dims, str, box, box_cols == 64 ? TMAP_SW128 : TMAP_SW64);
-}
 // K-major plane tensor T[plane][rows][32]: dims (k=32, row, plane, 1), box (32, 128)
 int map_planes(CUtensorMap* m, const __half* t, long long rows, long long planes, int box_planes = 1) {
   const uint64_t dims[4] = {32, (uint64_t)rows, (uint64_t)planes, 1};
@@ -80,17 +72,6 @@ int map_planes(CUtensorMap* m, const __half* t, long long rows, long long planes
   return make_tmap_f16(m, t, 4, dims, str, box, TMAP_SW64);
 }
 }  // namespace
-
-// How the flat B operands (U16 of FWD_B, dP16 of BWD_V: k rows 64 KB apart, the chunks of a row contiguous) are fetched.
-// MPGCN_B200_FLAT_B = 0 (default): one permuted SWIZZLE_64B box per tile; 1 = one 32-column box per chunk.
-static bool flat_b_boxes() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MPGCN_B200_FLAT_B");
-    v = (e && atoi(e) == 1) ? 1 : 0;
-  }
-  return v == 1;
-}
 
 bool tc_supported(const BdgcnShape& s) {
   return s.C == 32 && s.H == 32 && s.Ko >= 1 && s.Ko <= 8 && s.Kd >= 1 && s.Kd <= 8 && s.N >= 1 && s.B >= 1 && s.R >= 1 && s.row0 >= 0 &&
@@ -218,11 +199,9 @@ static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, in
   const long long NN = (long long)rn(s);
   GemmParams p;
   init_params(p);
-  static int mode = -1;     // A/B knob: 0 default, 1 = W streams with A (one plane per k-block), 2 = W resident, one plane per k-block
-  if (mode < 0) { const char* e = getenv("MPGCN_B200_MIX_MODE"); mode = e ? atoi(e) : 0; }
   const size_t w_bytes = (size_t)Kout * w_halves * Kin * 32 * 64;      // Kin * w_halves tiles of Kout chunks x [32 k][64 B]
   int bk = 32;
-  if (mode == 0 && (Kin == 2 || Kin == 3)) {
+  if (Kin == 2 || Kin == 3) {
     // One k-block per tile: a single TMA box brings the Kin planes of a 128-cell tile (the single-thread producer / MMA loops
     // cost ~0.3 us per k-block, which bounded the per-plane version at a third of the HBM rate), W resident in shared memory
     bk = 32 * Kin;
@@ -237,8 +216,8 @@ static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, in
     // segment s: plane = b*Kin + (s % Kin); weight rows (s % Kin)*32 of half s / Kin  (half 0 = fp16(W), half 1 = fp16(W - half 0))
     p.am = omap(1, kBig, Kin, 1, 0, Kin, 0);
     p.bm = omap(1, 1, 0, 0, 32, Kin, 1);
-    if (mode == 1 || w_bytes > 160 * 1024) { p.kb_total = Kin * w_halves; p.kb_per_seg = 1; }      // large K: W streams with A
-    else { p.kb_total = Kin; p.kb_per_seg = 1; p.b_res_reps = w_halves; }                           // W resident, A plane by plane
+    if (w_bytes > 160 * 1024) { p.kb_total = Kin * w_halves; p.kb_per_seg = 1; }          // large K: W streams with A
+    else { p.kb_total = Kin; p.kb_per_seg = 1; p.b_res_reps = w_halves; }              // W resident, A plane by plane
   }
   p.MT = ceil_div(NN, 128); p.NT = 1; p.Z = s.B; p.R = Kout;
   p.ep.out = d16; p.ep.out_f16 = 1;
@@ -260,12 +239,7 @@ static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16,
     if (int e = map_support_mn(&p.a_map, go16, N, Np, (long long)K * N, s.dynamic ? s.B : 1)) return e;
     // U16 [b][(o,n)][e][h] read as (h, k = (o,n) rows, r = e, b): dims listed with non-monotonic strides (the r stride,
     // 64 B, is smaller than the k stride) so that ONE box (32 ch, 64 k, 4|8 r) lands in the canonical [r][k][64 B] layout
-    if (flat_b_boxes()) {
-      if (int e = map_flat(&p.b_map, u16, (long long)N * 32, (long long)K * N, s.B, 64)) return e;
-      p.b_flat = 1;
-    } else {
-      if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, s.B, (long long)K * N * N * 32, 64, 8)) return e;
-    }
+    if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, s.B, (long long)K * N * N * 32, 64, 8)) return e;
     p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, 0);
     p.bm = omap(1, kBig, 1, 0, 0);
     p.kb_total = p.kb_per_seg = ceil_div((long long)K * N, 64);
@@ -280,12 +254,7 @@ static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16,
       const uint32_t box[4] = {64, 64, 1, 1};
       if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
     }
-    if (flat_b_boxes()) {
-      if (int e = map_flat(&p.b_map, u16, (long long)N * 32, R, (long long)s.B * K, 64)) return e;
-      p.b_flat = 1;
-    } else {
-      if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * K, (long long)R * N * 32, 64, 8)) return e;
-    }
+    if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * K, (long long)R * N * 32, 64, 8)) return e;
     p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, N);          // k coordinate += o * N
     p.bm = omap(1, kBig, K, 1, 0);                          // plane = b*K + o
     p.kb_per_seg = ceil_div(R, 64);
@@ -296,13 +265,6 @@ static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16,
   p.ep.sZ = (long long)N * N * 32; p.ep.sI = (long long)N * 32; p.ep.sR = 32;
   p.ep.m_valid = N; p.ep.r_valid = N;
   p.ep.bias = s.partial ? nullptr : bias; p.ep.relu = s.partial ? 0 : s.act;
-  if (s.partial && s.peer_g > 0) {        // push every row of the partial into its owner's staging slot for this rank (NVLink P2P stores)
-    p.ep.peer_g = s.peer_g; p.ep.peer_rows = N / s.peer_g;
-    p.ep.peer_sZ = (long long)p.ep.peer_rows * N * 32;
-    p.ep.peer_slot = (long long)s.peer_rank * s.B * p.ep.peer_sZ;
-    for (int j = 0; j < s.peer_g; ++j) p.ep.peer_out[j] = s.peer_out[j];
-    p.ep.out16 = nullptr;
-  }
   // pre[b,m,e,:] += sum_o (G_o[m,m] - fp16(G_o[m,m])) * U16[b,o,m,e,:]   (delta_o is zero outside the slab: the row n = m of U
   // exists only for row0 <= m < row0 + R; corr_src is moved so that row index m addresses slab row m - row0)
   p.ep.corr_src = u16 - (long long)s.row0 * N * 32; p.ep.corr_delta = delta_o; p.ep.corr_nseg = K;
@@ -325,12 +287,8 @@ static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16
     const uint32_t box[4] = {64, 128, 1, 1};
     if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
   }
-  if (flat_b_boxes()) {
-    if (int e = map_flat(&p.b_map, dp16, (long long)N * 32, N, s.B, 64)) return e;
-    p.b_flat = 1;
-  } else {   // dP16 [b][m][e][h] read as (h, k = m, r = e, b), see run_fwd_b
-    if (int e = map_chunks(&p.b_map, dp16, N, (long long)N * 32, N, 32, s.B, (long long)N * N * 32, 64, 8)) return e;
-  }
+  // dP16 [b][m][e][h] read as (h, k = m, r = e, b), see run_fwd_b
+  if (int e = map_chunks(&p.b_map, dp16, N, (long long)N * 32, N, 32, s.B, (long long)N * N * 32, 64, 8)) return e;
   p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + o
   p.bm = omap(K, kBig, 1, 0, 0);
   p.MT = ceil_div(R, 128); p.NT = ceil_div(N, 8); p.Z = s.B * K; p.R = 8;

@@ -63,10 +63,8 @@ int mask_delta_rows(const float* delta, float* out, size_t planes, int N, int ro
 int bias_act_inplace(float* x, const float* bias, int act, size_t n, int H, cudaStream_t s);
 // exchange steps of the origin-row shard fused into elementwise kernels over peer memory (parts / dsts: HOST arrays of g <= 8 DEVICE
 // pointers to [B][N][N][H] buffers, the rank's own and its peers' NVLink-mapped ones)
-// part_rows: origin rows held by each part buffer -- N (whole [B][N][N][H] partials, the rank's rows start at row0) or `rows`
-// (staging slots [B][rows][N][H] that already hold only the rank's rows)
-int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int part_rows,
-                         int H, cudaStream_t s);
+int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int H,
+                         cudaStream_t s);
 // the same with the fp16 cast of the tensor-core path folded in: scale2 = [S, 1/S] from the GLOBAL max|d_out| (device scalar), values
 // stored as fp16(S * d_pre) -- half the bytes on the wire and no cast / absmax pass over the gathered tensor on any rank
 int relu_backward_scatter_f16(const float* d_out, const float* out, int act, __half* const* dsts, int g, float* db, const float* absmax,
@@ -120,10 +118,6 @@ struct BdgcnShape {
   int Ko, Kd;       // supports in G_o / in G_d; W is the [Ko*Kd*C, H] slice in (o, d, l) row order
   int partial;      // forward writes the raw partial pre-activation sum_{o, n in slab} ... (no bias, no activation);
                     // backward receives dPre (already masked) instead of dOut
-  // forward of a part, optional: PUSH the partial into peer memory instead of writing it locally -- row m goes to
-  // peer_out[m / (N / peer_g)] (that owner's staging buffer [peer_g slots][B][N / peer_g][N][H]), slot peer_rank
-  int peer_g, peer_rank;
-  float* peer_out[8];
   bool whole() const { return R == N && row0 == 0 && Ko == K && Kd == K && !partial; }
 };
 enum Precision { PREC_FP32_SIMT = 0, PREC_FP16_TC = 1 };

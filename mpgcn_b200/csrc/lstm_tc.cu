@@ -19,8 +19,6 @@
 // Per thread: cell rows g, g + 8 of the warp's 16 (index h), units u = 8 jn + 2 q + e (slot s = 2 jn + e, jn < 4).
 #include "kernels.h"
 
-#include <stdlib.h>
-
 namespace mpgcn {
 namespace lstm_tc {
 
@@ -35,26 +33,6 @@ constexpr int HX_LD = 56;       // hx tile [128 cells][48 columns] row stride
 // SFU primitives (2 ulp each); ex2 saturates to 0 / +inf and rcp(inf) = 0, which are the limits the activations need.
 __device__ __forceinline__ float ex2_(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-
-// 2^x WITHOUT the SFU, for x <= 40: round-to-nearest split x = n + f through the 1.5 * 2^23 trick, degree-6 polynomial of 2^f on
-// [-0.5, 0.5] (Cephes exp2f coefficients; measured max relative error 1.0e-7, the SFU's ex2.approx is 2 ulp = 2.4e-7), 2^n added into
-// the exponent field.  11 FMA / ALU-pipe instructions instead of one of the 7 SFU operations per unit and step, for kernels
-// whose SFU queue is the bottleneck while issue slots are free.
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.f);
-  const float t = x + 12582912.f;
-  const float f = x - (t - 12582912.f);
-  float p = 1.535336188319500e-4f;
-  p = fmaf(p, f, 1.339887440266574e-3f);
-  p = fmaf(p, f, 9.618437357674640e-3f);
-  p = fmaf(p, f, 5.550332471162809e-2f);
-  p = fmaf(p, f, 2.402264791363012e-1f);
-  p = fmaf(p, f, 6.931472028550421e-1f);
-  p = fmaf(p, f, 1.f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// POLY = how many of the five exponentials per unit and step take the polynomial (0: none; 1: tanh(c); 2: tanh(c) and the o gate)
-template <int POLY, int WHICH> __device__ __forceinline__ float ex2_sel(float x) { return (WHICH < POLY) ? ex2_poly(x) : ex2_(x); }
 
 // x enters the gate MMA as fp16 hi + lo (exact to ~22 bits for |x| < 65504); both parts saturate instead of overflowing to inf,
 // so larger inputs give finite (saturated-gate) results rather than NaN
@@ -143,7 +121,7 @@ __device__ __forceinline__ size_t save_off(long long tile, int T, int t, int war
 // ---------------------------------------------------------------------------------------
 constexpr int FWD_THREADS = 256;
 
-template <bool SAVE, int POLY>
+template <bool SAVE>
 __global__ void __launch_bounds__(FWD_THREADS, 2)
 lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                    const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
@@ -195,14 +173,14 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
           const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
           const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
           const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float p = 1.f + ex2_sel<POLY, 1>(fminf(acc[12 + jn][k], 40.f));
+          const float p = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
           const float pig = ai * ag;
           const float r = rcp_(pig * af);
           const float gi = r * (ag * af);                    // sigmoid(i)
           const float gg = fmaf(r + r, ai * af, -1.f);       // tanh(g)
           const float gf = r * pig;                          // sigmoid(f)
           c[h][s] = fmaf(gf, c[h][s], gi * gg);
-          const float ac = 1.f + ex2_sel<POLY, 0>(fminf(-2.8853900817779268f * c[h][s], 40.f));
+          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * c[h][s], 40.f));
           const float r2 = rcp_(p * ac);
           hv[h][s] = (r2 * ac) * fmaf(r2 + r2, p, -1.f);     // sigmoid(o) * tanh(c)
         }
@@ -240,7 +218,6 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
 constexpr int BWD_THREADS = 256;
 constexpr size_t kBwdSmem = (size_t)(G4 * WX_LD + C * WT_LD + 2 * CELLS * DA_LD + 2 * CELLS * HX_LD) * sizeof(__half) + G4 * sizeof(float);
 
-template <int POLY>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
@@ -329,8 +306,8 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
           const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
           const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
           const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float ao = 1.f + ex2_sel<POLY, 1>(fminf(acc[12 + jn][k], 40.f));
-          const float ac = 1.f + ex2_sel<POLY, 0>(fminf(-2.8853900817779268f * fc[s], 40.f));
+          const float ao = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
+          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * fc[s], 40.f));
           const float pig = ai * ag;
           const float r1 = rcp_(pig * af), r2 = rcp_(ao * ac);      // 7 SFU ops per unit: see the forward kernel
           const float gi = r1 * (ag * af), gg = fmaf(r1 + r1, ai * af, -1.f), gf = r1 * pig;
@@ -437,18 +414,6 @@ __global__ void copy_vec_kernel(const float* src, float* dst, int n) {
 // ---------------------------------------------------------------------------------------
 bool lstm_tc_supported(int T, int C) { return C == 32 && T >= 1 && T <= 256; }
 
-// MPGCN_B200_LSTM_POLY = 0 | 1 | 2: how many of the five exponentials per unit and step are evaluated by ex2_poly (FMA pipe)
-// instead of the SFU (1: tanh(c); 2: tanh(c) and the o gate).  Default 0: all on the SFU.
-static int lstm_poly_knob() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MPGCN_B200_LSTM_POLY");
-    v = e ? atoi(e) : 0;
-    if (v < 0 || v > 2) v = 0;
-  }
-  return v;
-}
-
 static int lstm_grid(long long cells, int per_sm) {
   const long long tiles = (cells + lstm_tc::CELLS - 1) / lstm_tc::CELLS;
   long long g = (long long)per_sm * device_sm_count();
@@ -468,12 +433,9 @@ int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_h
   using namespace lstm_tc;
   const long long cells = (long long)B * NN;
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm forward: saved buffer must be 16-byte aligned");
-  using Kern = void (*)(const float*, const float*, const float*, const float*, const float*, float*, __half*, long long, int, long long);
-  static const Kern kerns[2][3] = {{lstm_fwd_tc_kernel<false, 0>, lstm_fwd_tc_kernel<false, 1>, lstm_fwd_tc_kernel<false, 2>},
-                                   {lstm_fwd_tc_kernel<true, 0>, lstm_fwd_tc_kernel<true, 1>, lstm_fwd_tc_kernel<true, 2>}};
-  const int sv = saved ? 1 : 0;
+  auto kern = saved ? lstm_fwd_tc_kernel<true> : lstm_fwd_tc_kernel<false>;
   prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)cells * T, st);
-  kerns[sv][lstm_poly_knob()]<<<lstm_grid(cells, 2), FWD_THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells, T, NN);
+  kern<<<lstm_grid(cells, 2), FWD_THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -499,15 +461,11 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4 * C, st));
   MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4, st));
   if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  using KernB = void (*)(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, float*, float*,
-                         const __half*, const float*, long long, int, long long);
-  static const KernB kernb[3] = {lstm_bwd_saved_tc_kernel<0>, lstm_bwd_saved_tc_kernel<1>, lstm_bwd_saved_tc_kernel<2>};
-  static DynSmemAttr attr_b[3] = {};
-  const int var = lstm_poly_knob();
-  if (int e = ensure_dyn_smem(kernb[var], (int)kBwdSmem, attr_b[var])) return e;
+  static DynSmemAttr attr_b = {};
+  if (int e = ensure_dyn_smem(lstm_bwd_saved_tc_kernel, (int)kBwdSmem, attr_b)) return e;
   prof_begin(PROF_LSTM_BWD, 12.0 * C * (C + 1) * (double)cells * T, st);
-  kernb[var]<<<lstm_grid(cells, 1), BWD_THREADS, kBwdSmem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x,
-                                                                 static_cast<const __half*>(saved), scale2, cells, T, NN);
+  lstm_bwd_saved_tc_kernel<<<lstm_grid(cells, 1), BWD_THREADS, kBwdSmem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x,
+                                                                               static_cast<const __half*>(saved), scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   prof_count(PROF_ELEMENTWISE);

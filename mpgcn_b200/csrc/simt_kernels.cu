@@ -7,8 +7,6 @@
 // the fp16 tensor path).  It is NOT a CPU fallback: everything here runs on the GPU.
 #include "kernels.h"
 
-#include <stdlib.h>
-
 namespace mpgcn {
 
 // ---------------------------------------------------------------------------------------
@@ -182,12 +180,13 @@ int cvt_f32_to_f16_hilo(const float* src, __half* hi, __half* lo, size_t n, cuda
   return 0;
 }
 
-// delta[p][i] = G_p[i,i] - fp16(G_p[i,i]) where the diagonal entry DOMINATES its column (G_ii^2 > tau * sum_{c != i} G_ci^2),
+// delta[p][i] = G_p[i,i] - fp16(G_p[i,i]) where the diagonal entry DOMINATES its column (G_ii^2 > kDiagTau * sum_{c != i} G_ci^2),
 // else 0.  The contraction epilogues add delta * (the diagonal operand row) back, which removes the one rounding error that
 // matters when a support is close to the identity (Chebyshev / random-walk T_k of a sparse graph); for a dense support the
 // diagonal is one of N comparable terms, the remainder is noise-level, and a zero delta lets the epilogue skip the re-read
 // of the operand tensor altogether.
-__global__ void diag_delta_kernel(const float* __restrict__ G, float* __restrict__ delta, size_t planes, int N, float tau) {
+constexpr float kDiagTau = 0.0625f;
+__global__ void diag_delta_kernel(const float* __restrict__ G, float* __restrict__ delta, size_t planes, int N) {
   // block = 32 columns x 32 row groups of one plane; blockIdx.x enumerates (plane, column block)
   __shared__ float s_sq[32][33];
   const int cblocks = (N + 31) / 32;
@@ -196,7 +195,7 @@ __global__ void diag_delta_kernel(const float* __restrict__ G, float* __restrict
   const int rg = threadIdx.x >> 5;
   const float* plane = G + p * (size_t)N * N;
   float sq = 0.f;
-  if (i < N && tau >= 0.f)
+  if (i < N)
     for (int c = rg; c < N; c += 32) { const float v = plane[(size_t)c * N + i]; sq = fmaf(v, v, sq); }   // 128-byte rows per warp
   s_sq[rg][threadIdx.x & 31] = sq;
   __syncthreads();
@@ -206,17 +205,15 @@ __global__ void diag_delta_kernel(const float* __restrict__ G, float* __restrict
     for (int r = 0; r < 32; ++r) col += s_sq[r][threadIdx.x];
     const float g = plane[(size_t)i * N + i];
     float d = g - __half2float(f2h_sat(g));
-    if (tau >= 0.f && !(g * g > tau * (col - g * g))) d = 0.f;
+    if (!(g * g > kDiagTau * (col - g * g))) d = 0.f;
     delta[p * N + i] = d;
   }
 }
 int support_diag_delta(const float* G, float* delta, size_t planes, int N, cudaStream_t s) {
-  static float tau = -2.f;
-  if (tau == -2.f) { const char* e = getenv("MPGCN_B200_DIAG_TAU"); tau = e ? (float)atof(e) : 0.0625f; }   // < 0: always correct
   prof_count(PROF_ELEMENTWISE);
   const size_t blocks = planes * (size_t)((N + 31) / 32);
   MPGCN_CHECK(blocks < (1ull << 31), "support_diag_delta: too many planes");
-  diag_delta_kernel<<<(unsigned)blocks, 1024, 0, s>>>(G, delta, planes, N, tau);
+  diag_delta_kernel<<<(unsigned)blocks, 1024, 0, s>>>(G, delta, planes, N);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }
@@ -516,17 +513,16 @@ __global__ void rows_reduce_bias_act_kernel(float4* __restrict__ out, PeerPtrs p
     out[b * slab4 + i] = acc;
   }
 }
-int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int part_rows,
-                         int H, cudaStream_t s) {
+int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int H,
+                         cudaStream_t s) {
   MPGCN_CHECK(g >= 1 && g <= 8, "rows_reduce: %d ranks unsupported (1..8)", g);
-  MPGCN_CHECK(part_rows == N || part_rows == rows, "rows_reduce: part buffers must hold N or `rows` origin rows (got %d)", part_rows);
   MPGCN_CHECK(H % 4 == 0 && row0 >= 0 && rows >= 1 && row0 + rows <= N, "rows_reduce: bad slab rows [%d, %d) of %d, H=%d", row0, row0 + rows, N, H);
   PeerPtrs pp{};
   for (int j = 0; j < g; ++j) {
     MPGCN_CHECK(parts[j] != nullptr && (reinterpret_cast<uintptr_t>(parts[j]) & 15) == 0, "rows_reduce: partial buffer %d null or misaligned", j);
     pp.p[j] = const_cast<float*>(parts[j]);
   }
-  const size_t slab4 = (size_t)rows * N * H / 4, full4 = (size_t)part_rows * N * H / 4, off4 = part_rows == N ? (size_t)row0 * N * H / 4 : 0;
+  const size_t slab4 = (size_t)rows * N * H / 4, full4 = (size_t)N * N * H / 4, off4 = (size_t)row0 * N * H / 4;
   dim3 grid(grid_for(slab4, 256), (unsigned)B);
   prof_begin(PROF_EXCHANGE, 0.0, s);
   rows_reduce_bias_act_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<float4*>(out), pp, g, bias, act, slab4, full4, off4, H / 4);

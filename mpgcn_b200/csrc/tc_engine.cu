@@ -210,7 +210,7 @@ static int launch_impl(GemmParams& p, cudaStream_t stream) {
   const int nres = p.b_res_reps * p.kb_total;
   int stages;
   if (nres) {
-    MPGCN_CHECK(p.NT == 1 && p.kb_per_seg == 1 && !p.split_k && !p.b_flat && p.bm.z_mul == 0, "resident B needs a tile-independent B operand");
+    MPGCN_CHECK(p.NT == 1 && p.kb_per_seg == 1 && !p.split_k && p.bm.z_mul == 0, "resident B needs a tile-independent B operand");
     MPGCN_CHECK((size_t)nres * b_stage + 2 * (size_t)C::A_STAGE + kEpiBytes + 1536 <= (size_t)kMaxSmem, "resident B operand does not fit in shared memory");
     stages = (int)((kMaxSmem - 1024 - 512 - kEpiBytes - (size_t)nres * b_stage) / (size_t)C::A_STAGE);
   } else {

@@ -54,20 +54,12 @@ struct Epilogue {
   const float* corr_delta;
   long long cZ, cI, cR, cSeg;
   int corr_nseg;             // <= 8
-  // optional PUSH of a partial result into peer memory (origin-row shard, FWD_B): row i belongs to owner i / peer_rows and is
-  // stored at peer_out[owner] + peer_slot + z * peer_sZ + (i % peer_rows) * sI (+ r * sR + channel) -- the owner's staging slot
-  // for THIS rank, over NVLink when the owner is another GPU.  The transfer rides in the epilogue, tile by tile, under the MMAs
-  // of the next tile; peer_g == 0: plain store to `out`.
-  float* peer_out[8];
-  int peer_g, peer_rows;
-  long long peer_slot, peer_sZ;
 };
 
 struct alignas(64) GemmParams {
   CUtensorMap a_map;
   CUtensorMap b_map;
   OperandMap am, bm;
-  int b_flat;                // 1: B tile = R separate (32 x BK) boxes of a flat [rows][cols] tensor
   int MT, NT, Z;             // tile grid: tile id = (z * NT + nt) * MT + mt
   int R;                     // 32-column chunks per tile
   int kb_total, kb_per_seg;  // k-blocks over all segments / per segment
@@ -148,7 +140,7 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-__device__ __forceinline__ void store_chunk(const Epilogue& ep, void* out_ptr, float alpha, const float* sbias, long long off,
+__device__ __forceinline__ void store_chunk(const Epilogue& ep, float alpha, const float* sbias, long long off,
                                             uint32_t (&acc)[32], float& amax) {
   float v[32];
 #pragma unroll
@@ -163,14 +155,14 @@ __device__ __forceinline__ void store_chunk(const Epilogue& ep, void* out_ptr, f
     for (int c = 0; c < 32; ++c) amax = fmaxf(amax, fabsf(v[c]));
   }
   if (ep.out_f16) {        // 64 bytes per row and chunk: two 32-byte stores
-    __half* dst = reinterpret_cast<__half*>(out_ptr) + off;
+    __half* dst = reinterpret_cast<__half*>(ep.out) + off;
 #pragma unroll
     for (int q = 0; q < 2; ++q)
       st_global_256(dst + 16 * q, pack_h2(v[16 * q + 0], v[16 * q + 1]), pack_h2(v[16 * q + 2], v[16 * q + 3]),
                     pack_h2(v[16 * q + 4], v[16 * q + 5]), pack_h2(v[16 * q + 6], v[16 * q + 7]), pack_h2(v[16 * q + 8], v[16 * q + 9]),
                     pack_h2(v[16 * q + 10], v[16 * q + 11]), pack_h2(v[16 * q + 12], v[16 * q + 13]), pack_h2(v[16 * q + 14], v[16 * q + 15]));
   } else {                 // 128 bytes per row and chunk: four 32-byte stores
-    float* dst = reinterpret_cast<float*>(out_ptr) + off;
+    float* dst = reinterpret_cast<float*>(ep.out) + off;
 #pragma unroll
     for (int q = 0; q < 4; ++q)
       st_global_256(dst + 8 * q, __float_as_uint(v[8 * q + 0]), __float_as_uint(v[8 * q + 1]), __float_as_uint(v[8 * q + 2]),
@@ -261,14 +253,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
     } else {                      // A_MN64: dims (ch, k, chunk, z), 4 chunks per tile
       tma_load_4d(a_dst, &p.a_map, &full[p_stage], 0, kA, p_mt * 4, zA);
     }
-    if (NRES) {
-      // B is resident
-    } else if (!p.b_flat) {       // dims (ch, k, r, z)
+    if (!NRES)                    // dims (ch, k, r, z); a resident B was loaded once up front
       tma_load_4d(b_dst, &p.b_map, &full[p_stage], 0, kB, p_nt * R, zB);
-    } else {                      // dims (col, k, z, 1): one 32-column box per chunk
-      for (int j = 0; j < R; ++j)
-        tma_load_4d(b_dst + (size_t)j * BK * 64, &p.b_map, &full[p_stage], (p_nt * R + j) * 32, kB, zB, 0);
-    }
     if (++p_stage == S) { p_stage = 0; p_phase ^= 1u; }
     if (++p_kk == p.kb_per_seg) {
       p_kk = 0;
@@ -365,13 +351,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
       // ---- epilogue: two chunks at a time through the staging buffer, then one thread per (row, chunk) as a 32-channel row ----
       const int half = tw >> 6, rr = tw & 63;
       const int i = mt * 128 + wg * 64 + rr;
-      long long base = (long long)z * p.ep.sZ + (long long)i * p.ep.sI;
-      void* out_ptr = p.ep.out;
-      if (p.ep.peer_g > 0 && i < p.ep.m_valid) {      // push this row of the partial result into its owner's staging slot
-        const int owner = i / p.ep.peer_rows;
-        out_ptr = p.ep.peer_out[owner];
-        base = p.ep.peer_slot + (long long)z * p.ep.peer_sZ + (long long)(i - owner * p.ep.peer_rows) * p.ep.sI;
-      }
+      const long long base = (long long)z * p.ep.sZ + (long long)i * p.ep.sI;
       float dl[8];
       long long cbase = 0;
       bool any_corr = false;
@@ -431,7 +411,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
                 }
               }
             }
-            store_chunk(p.ep, out_ptr, alpha, sbias, base + (long long)r * p.ep.sR, regs, amax);
+            store_chunk(p.ep, alpha, sbias, base + (long long)r * p.ep.sR, regs, amax);
           }
           named_bar_sync(1 + wg, 128);
         }

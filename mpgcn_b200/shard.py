@@ -65,14 +65,8 @@ class ShardPlan:
 # compute back end (the C ABI); tests replace it by a CPU stand-in to exercise the exchange logic under gloo
 # ------------------------------------------------------------------------------------------------
 class CudaEngine:
-    def _part(self, row0, rows, Ko, Kd, push=None):
-        part = _lib.BdgcnPart(row0, rows, Ko, Kd)
-        if push is not None:            # (rank, [g staging-buffer pointers]): FWD_B pushes its partial into peer memory
-            part.peer_rank, ptrs = push
-            part.peer_g = len(ptrs)
-            for j, ptr in enumerate(ptrs):
-                part.peer_out[j] = ptr
-        return part
+    def _part(self, row0, rows, Ko, Kd):
+        return _lib.BdgcnPart(row0, rows, Ko, Kd)
 
     def prepared(self, G, Gc, planes, N, prec):
         """fp16 staging of a support stack, converted once per tensor (mpgcn_b200.ops cache) and reused by every layer, forward and
@@ -82,16 +76,15 @@ class CudaEngine:
         with torch.cuda.device(Gc.device):
             return ops._prepared_supports(_lib.load(), G, Gc, planes, N)
 
-    def forward_part(self, X, Go, Gd, dynamic, W, N, row0, Ko, Kd, prec, keep, out=None, preps=(None, None), push=None):
-        """X [B,rows,N,C] -> (raw partial pre-activation [B,N,N,H] (written into `out` if given; None with `push`, which sends every
-        output row straight into its owner's staging buffer from the contraction's epilogue), Z stash or None)"""
+    def forward_part(self, X, Go, Gd, dynamic, W, N, row0, Ko, Kd, prec, keep, out=None, preps=(None, None)):
+        """X [B,rows,N,C] -> (raw partial pre-activation [B,N,N,H] (written into `out` if given), Z stash or None)"""
         lib = _lib.load()
         ops._require_cuda(X, "X")
         B, rows, _, C = X.shape
         H = W.shape[1]
-        part = self._part(row0, rows, Ko, Kd, push)
+        part = self._part(row0, rows, Ko, Kd)
         pp = ctypes.addressof(part)
-        pre = None if push is not None else (out if out is not None else torch.empty((B, N, N, H), dtype=torch.float32, device=X.device))
+        pre = out if out is not None else torch.empty((B, N, N, H), dtype=torch.float32, device=X.device)
         saved = ops._scratch(lib.mpgcn_bdgcn_part_saved_bytes(B, N, C, H, prec, pp), X.device) if keep else None
         ws = ops._scratch(lib.mpgcn_bdgcn_part_fwd_workspace_bytes(B, N, C, H, int(dynamic), prec, pp), X.device)
         ex = _lib.BdgcnExtras()
@@ -140,15 +133,15 @@ class CudaEngine:
                                                d_out.shape[-1], ops._stream()), "relu_backward")
         return d_pre, db
 
-    def rows_reduce_bias_act(self, ptrs, B, N, row0, rows, H, bias, act, device, slots=False):
+    def rows_reduce_bias_act(self, ptrs, B, N, row0, rows, H, bias, act, device):
         """out [B,rows,N,H] = act(sum over the g buffers at `ptrs` of the rank's rows + bias); the buffers are whole [B,N,N,H]
-        partials (own + peers') or, with slots=True, the local staging slots [B,rows,N,H] the peer push filled"""
+        partials (own + peers')"""
         lib = _lib.load()
         out = torch.empty((B, rows, N, H), dtype=torch.float32, device=device)
         arr = (ctypes.c_void_p * len(ptrs))(*ptrs)
         with torch.cuda.device(device):
-            _lib.check(lib.mpgcn_rows_reduce_bias_act(out.data_ptr(), arr, len(ptrs), ops._ptr(bias), int(act), B, N, row0, rows,
-                                                      rows if slots else N, H, ops._stream()), "rows_reduce_bias_act")
+            _lib.check(lib.mpgcn_rows_reduce_bias_act(out.data_ptr(), arr, len(ptrs), ops._ptr(bias), int(act), B, N, row0, rows, H,
+                                                      ops._stream()), "rows_reduce_bias_act")
         return out
 
     def relu_backward_scatter(self, d_out, out, act, ptrs, N, row0, want_db):
@@ -230,20 +223,11 @@ class PeerExchange:
         return t.view(shape), hdl
 
 
-def _push_enabled() -> bool:
-    """MPGCN_B200_SHARD_PUSH=1: push every output row of the partial from the FWD_B epilogue into its owner's staging slot (the
-    fused compute + exchange kernel) instead of pulling the rows in mpgcn_rows_reduce_bias_act.  Default off: bit-identical, but the
-    epilogue's 32-byte stores land 128 KB apart, which NVLink carries worse than the pull kernel's contiguous streams."""
-    import os
-    return os.environ.get("MPGCN_B200_SHARD_PUSH", "0") == "1"
-
-
 def enable_peer_exchange(plan, device) -> bool:
     """Try to switch the row shard of `plan` to the peer-memory exchange (NCCL backend, CUDA symmetric memory available on every
     rank).  Collective.  Returns whether it is on; on failure anywhere every rank stays on the NCCL collectives."""
-    import os
     ok = 0
-    if plan.kind == "row" and _backend(plan.group) == "nccl" and os.environ.get("MPGCN_B200_SHARD_EXCHANGE", "peer") == "peer":
+    if plan.kind == "row" and _backend(plan.group) == "nccl":
         try:
             px = PeerExchange(plan, device)
             ok = 1
@@ -371,19 +355,9 @@ class _RowShardLayerFn(torch.autograd.Function):
             preps = (go_p, go_p if G_d is G_o else _ENGINE.prepared(G_d, Gdc, planes, N, prec))
             ctx.preps = preps
             bias = None if b is None else _f32c(b)
-            if prec == _lib.PREC_FP16_TC and _push_enabled():
-                # fused compute + exchange: the FWD_B epilogue stores every output row into its OWNER's staging slot for this rank
-                # (NVLink P2P stores, tile by tile under the MMAs); after the barrier each rank sums its g local slots
-                _, saved = _ENGINE.forward_part(Xc, Goc, Gdc, dynamic, Wc, N, plan.row_lo, K, K, prec, keep, preps=preps,
-                                                push=(plan.rank, list(hdl.buffer_ptrs)))
-                hdl.barrier()
-                slot = B * rows * N * H * 4
-                out = _ENGINE.rows_reduce_bias_act([buf.data_ptr() + j * slot for j in range(plan.world)], B, N, plan.row_lo, rows, H, bias, act,
-                                                   X.device, slots=True)
-            else:
-                _, saved = _ENGINE.forward_part(Xc, Goc, Gdc, dynamic, Wc, N, plan.row_lo, K, K, prec, keep, out=buf, preps=preps)
-                hdl.barrier()
-                out = _ENGINE.rows_reduce_bias_act(list(hdl.buffer_ptrs), B, N, plan.row_lo, rows, H, bias, act, X.device)
+            _, saved = _ENGINE.forward_part(Xc, Goc, Gdc, dynamic, Wc, N, plan.row_lo, K, K, prec, keep, out=buf, preps=preps)
+            hdl.barrier()
+            out = _ENGINE.rows_reduce_bias_act(list(hdl.buffer_ptrs), B, N, plan.row_lo, rows, H, bias, act, X.device)
             ctx.meta = (dynamic, act, prec, b is not None, N, K, C, keep)
             ctx.plan = plan
             ctx.stash = [saved]

@@ -50,7 +50,7 @@ def _precisions(C, H, K):
 
 def test_library_is_the_cuda_one(cuda_device):
     lib = _lib.load()
-    assert lib.mpgcn_abi_version() == _lib.ABI_VERSION == 3
+    assert lib.mpgcn_abi_version() == _lib.ABI_VERSION == 4
     assert torch.cuda.get_device_capability(cuda_device) == (9, 0), "tests expect a Hopper (sm_90) device"
 
 

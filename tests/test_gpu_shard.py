@@ -176,40 +176,6 @@ def test_peer_exchange_kernels_on_one_gpu(cuda_device):
     assert torch.equal(dX_a, dX_b) and torch.equal(dW_a, dW_b)
 
 
-@pytest.mark.parametrize("N,g,dyn", [(136, 4, False), (512, 2, True), (600, 3, False)])
-def test_fused_push_epilogue_on_one_gpu(N, g, dyn, cuda_device):
-    """FWD_B with the peer push (every output row stored into its owner's staging slot from the contraction's epilogue), the g
-    "ranks" emulated on one GPU: after all ranks ran, owner r's g slots summed with bias + ReLU == the whole layer's rows of r,
-    and the pushed partials are bit-identical to the locally written ones."""
-    dev = cuda_device
-    torch.manual_seed(N)
-    B, K, C = 2, 3, 32
-    rows = N // g
-    X = torch.tanh(torch.randn(B, N, N, C, device=dev))
-    mk = (lambda: torch.randn(B, K, N, N, device=dev) / N ** 0.5) if dyn else (lambda: torch.randn(K, N, N, device=dev) / N ** 0.5)
-    Go = mk()
-    Gd = mk() if dyn else Go
-    W = torch.randn(K * K * C, C, device=dev) * 0.05
-    bias = torch.randn(C, device=dev) * 0.1
-    eng = shard.CudaEngine()
-    staging = [torch.full((g, B, rows, N, C), float("nan"), device=dev) for _ in range(g)]      # one staging buffer per owner
-    ptrs = [t.data_ptr() for t in staging]
-    local = []
-    for r in range(g):
-        Xp = X[:, r * rows:(r + 1) * rows].contiguous()
-        eng.forward_part(Xp, Go, Gd, dyn, W, N, r * rows, K, K, 1, False, push=(r, ptrs))
-        pre, _ = eng.forward_part(Xp, Go, Gd, dyn, W, N, r * rows, K, K, 1, False)
-        local.append(pre)
-    torch.cuda.synchronize()
-    whole, _ = abi.forward(X, Go, Gd if dyn else Go, W, bias, True, "fp32")
-    slot = B * rows * N * C * 4
-    for owner in range(g):
-        for r in range(g):
-            assert torch.equal(staging[owner][r], local[r][:, owner * rows:(owner + 1) * rows]), f"slot {r} of owner {owner}"
-        out = eng.rows_reduce_bias_act([staging[owner].data_ptr() + j * slot for j in range(g)], B, N, owner * rows, rows, C, bias, 1, dev, slots=True)
-        _check(out, whole[:, owner * rows:(owner + 1) * rows], 1e-3, f"push N={N} g={g} owner {owner}: summed slots == whole layer rows")
-
-
 def test_hybrid_row_x_batch_shard_nccl_world4(tmp_path):
     """world 4 = 2 batch groups x 2 row ranks (bench.py --shard row --row-ranks 2) on 4 GPUs: the row exchange (peer memory) stays
     inside a group, the gradients are summed over all ranks and averaged over the groups; vs the whole model on one GPU.

@@ -166,7 +166,7 @@ def test_gradient_hint_routing_is_graph_based():
 
 def test_c_abi_rejects_bad_arguments_without_a_gpu():
     """Argument validation happens before any CUDA call: empty / malformed shapes, unknown precisions, bad layer parts and bad
-    peer layouts come back as error codes with a message (`mpgcn_last_error`), never as a crash -- also on a box without a GPU."""
+    exchange slabs come back as error codes with a message (`mpgcn_last_error`), never as a crash -- also on a box without a GPU."""
     import ctypes
     from mpgcn_b200 import _lib
     lib = _lib.load()
@@ -186,16 +186,13 @@ def test_c_abi_rejects_bad_arguments_without_a_gpu():
     assert "bad layer part" in err()
     assert lib.mpgcn_bdgcn_forward_part(one, one, one, 0, one, one, None, one, 1 << 20, 2, 8, 32, 32, 0, None, None, None) != 0 and "part descriptor" in err()
     part = _lib.BdgcnPart(0, 4, 3, 3)
-    part.peer_g, part.peer_rank = 3, 0                     # N = 8 is not a multiple of 3 ranks; and the push needs precision 1
-    assert lib.mpgcn_bdgcn_forward_part(one, one, one, 0, one, None, None, one, 1 << 20, 2, 8, 32, 32, 1, ctypes.addressof(part), None, None) != 0
-    assert "peer layout" in err()
-    assert lib.mpgcn_bdgcn_forward_part(one, one, one, 0, one, None, None, one, 1 << 20, 2, 8, 32, 32, 0, ctypes.addressof(part), None, None) != 0
-    assert "tensor-core epilogue only" in err()
+    for prec in (0, 1):                                    # a valid part with no pre_partial buffer
+        assert lib.mpgcn_bdgcn_forward_part(one, one, one, 0, one, None, None, one, 1 << 20, 2, 8, 32, 32, prec, ctypes.addressof(part), None, None) != 0
+        assert "null pointer" in err()
     # exchange kernels
     arr = (ctypes.c_void_p * 9)(*[256] * 9)
-    assert lib.mpgcn_rows_reduce_bias_act(one, arr, 9, None, 1, 1, 8, 0, 4, 8, 32, None) != 0 and "ranks unsupported" in err()
-    assert lib.mpgcn_rows_reduce_bias_act(one, arr, 2, None, 1, 1, 8, 6, 4, 8, 32, None) != 0 and "bad slab" in err()
-    assert lib.mpgcn_rows_reduce_bias_act(one, arr, 2, None, 1, 1, 8, 0, 4, 5, 32, None) != 0 and "part buffers" in err()
+    assert lib.mpgcn_rows_reduce_bias_act(one, arr, 9, None, 1, 1, 8, 0, 4, 32, None) != 0 and "ranks unsupported" in err()
+    assert lib.mpgcn_rows_reduce_bias_act(one, arr, 2, None, 1, 1, 8, 6, 4, 32, None) != 0 and "bad slab" in err()
     assert lib.mpgcn_relu_backward_scatter(one, one, 1, arr, 2, None, 1, 8, 6, 4, 32, None) != 0 and "bad slab" in err()
     # LSTM
     assert lib.mpgcn_lstm_last_forward(one, one, one, one, one, one, 0, 4, 16, 32, 0, None) != 0 and "empty input" in err()
