@@ -148,6 +148,16 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
+
+// fp32 -> fp16 round-to-nearest-even, saturating at +-65504 instead of producing inf; NaN stays NaN (a clamp with
+// fminf / fmaxf would turn it into a finite number).  Every in-range value converts exactly as __float2half_rn does.
+__device__ __forceinline__ __half f2h_sat(float x) { return __float2half_rn(fabsf(x) > 65504.f ? copysignf(65504.f, x) : x); }
+// the same for a pair, in one instruction (F2FP.SATFINITE): low half = a, high half = b, as __floats2half2_rn(a, b)
+__device__ __forceinline__ uint32_t f2h2_sat_bits(float a, float b) {
+  uint32_t r;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+  return r;
+}
 #endif  // __CUDACC__
 
 // ----------------------------------------------------------------------------------------

@@ -126,11 +126,6 @@ int simt_sgemm(const SgemmParams& p, cudaStream_t stream) {
 // ---------------------------------------------------------------------------------------
 // elementwise / layout kernels
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ __half f2h_sat(float x) {
-  // round-to-nearest-even, saturating to +-65504 instead of producing inf
-  return __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
-}
-
 __global__ void cvt_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t n4 = n / 4;

@@ -135,10 +135,7 @@ __device__ __forceinline__ void st_global_256(void* ptr, uint32_t a0, uint32_t a
   d[0] = make_uint4(a0, a1, a2, a3);
   d[1] = make_uint4(a4, a5, a6, a7);
 }
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) { return f2h2_sat_bits(a, b); }   // an fp16 operand never holds inf
 
 __device__ __forceinline__ void store_chunk(const Epilogue& ep, float alpha, const float* sbias, long long off,
                                             uint32_t (&acc)[32], float& amax) {

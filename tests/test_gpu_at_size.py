@@ -21,6 +21,7 @@ from torch import nn
 import abi
 from conftest import golden_names, record_parity
 from oracle import mpgcn_oracle as orc
+from test_gpu_engine_stages import diag_rule, diag_supports
 from test_oracle_golden import load_big
 
 import MPGCN as shim
@@ -80,9 +81,14 @@ def test_layer_matches_reference_fixture_at_size(name, cuda_device):
 
 def _supports(rng, kind, K, N, batch):
     """'dense': N(0,1)/sqrt(N) (no identity shortcut).  'rw': the trainer's random-walk diffusion supports (T_0 = I) of a
-    U[0,1) flow, built by the oracle's Adj_Processor restatement -- the kind with a dominant diagonal."""
+    U[0,1) flow, built by the oracle's Adj_Processor restatement.  'diag': alpha I + sparse off-diagonals with alpha not
+    representable in fp16 -- the diagonal dominates its column, so the engine's remainder correction (DESIGN.md section 3) acts."""
     if kind == "dense":
         g = (rng.standard_normal((max(batch, 1), K, N, N)) / np.sqrt(N)).astype(np.float32)
+    elif kind == "diag":
+        g = diag_supports(rng, max(batch, 1) * K, N).reshape(max(batch, 1), K, N, N)
+        delta, _ = diag_rule(g.reshape(-1, N, N))
+        assert np.count_nonzero(delta) >= 0.5 * delta.size, "the 'diag' supports must make the remainder correction fire"
     else:
         g = orc.adj_process(rng.random((max(batch, 1), N, N)).astype(np.float32), "random_walk_diffusion", K - 1).astype(np.float32)
     return g if batch else g[0]
@@ -99,6 +105,9 @@ AT_SIZE = [
     (1000, 3, 1, False, "dense"), (1000, 3, 1, True, "rw"),
     (1000, 6, 1, False, "dense"),
     (2000, 3, 1, False, "dense"),
+    # K = 4, 5, 7, 8 (channel-mix tile widths 4, 5, 7, 8; W streamed through the ring at K >= 7) and N = 1, 64, 65, 128
+    (1, 4, 2, True, "diag"), (64, 5, 2, False, "diag"), (65, 7, 2, True, "dense"), (128, 8, 2, False, "diag"),
+    (128, 4, 2, True, "dense"), (200, 5, 1, True, "diag"), (257, 7, 1, False, "diag"), (300, 8, 1, True, "dense"),
 ]
 
 

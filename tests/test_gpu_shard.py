@@ -85,6 +85,32 @@ def test_layer_parts_match_standin_and_sum_to_the_whole_layer(kind, N, world, K,
         _check(dW_all.view(K * K * C, C), dWw, tb, f"parts {kind} N={N} x{world} {prec_name}: dW")
 
 
+@pytest.mark.parametrize("N,dyn", [(130, False), (258, True)])
+def test_row_shard_fp16_partials_on_dominant_diagonals_sum_to_the_whole_layer(N, dyn, cuda_device):
+    """Row shard over 2 ranks on supports whose diagonal remainder correction fires: the fp16 partial pre-activations of both
+    ranks, summed, equal the fp16 whole layer (no bias, no activation) to 1e-5.  A slab's Z16 and U16 rows come from the same
+    kernels on the same bits as the whole layer's; only the FWD_B accumulation order differs.  So this pins what the slab adds:
+    the origin remainders masked to the slab's rows and the zero-filled rows past the slab edge."""
+    from test_gpu_engine_stages import diag_supports
+    dev = cuda_device
+    rng = np.random.default_rng(N)
+    B, K, C, world = 2, 3, 32, 2
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    X = t(np.tanh(rng.standard_normal((B, N, N, C))).astype(np.float32))
+    shape = (B, K, N, N) if dyn else (K, N, N)
+    Gd = t(diag_supports(rng, (B if dyn else 1) * K, N).reshape(shape))
+    Go = t(diag_supports(rng, B * K, N).reshape(shape)) if dyn else Gd
+    W = t((rng.standard_normal((K * K * C, C)) * (2.0 / (K * K * C + C)) ** 0.5).astype(np.float32))
+    cuda = shard.CudaEngine()
+    total = torch.zeros(B, N, N, C, dtype=torch.float64, device=dev)
+    for r in range(world):
+        plan = shard.ShardPlan("row", r, world, N, K)
+        pre, _ = cuda.forward_part(X[:, plan.row_lo:plan.row_hi].contiguous(), Go, Gd, dyn, W, N, plan.row_lo, K, K, 1, False)
+        total += pre.double()
+    whole, _ = abi.forward(X, Go, Gd, W, torch.zeros(C, device=dev), False, "fp16", want_saved=False)
+    _check(total, whole, 1e-5, f"row shard N={N} x{world} {'dyn' if dyn else 'static'}/diag fp16: sum of partials == fp16 whole layer")
+
+
 def test_bias_act_and_relu_backward_kernels(cuda_device):
     torch.manual_seed(0)
     x = torch.randn(3, 17, 19, 32, device=cuda_device)
