@@ -73,9 +73,20 @@ int map_planes(CUtensorMap* m, const __half* t, long long rows, long long planes
 }
 }  // namespace
 
+// Any number of supports: the N^3 contractions index supports through z and k-segments, the channel mixes and BWD_DW split
+// more than 8 output supports into column groups, and the FWD_B epilogue walks its remainders 8 segments at a time.
 bool tc_supported(const BdgcnShape& s) {
-  return s.C == 32 && s.H == 32 && s.Ko >= 1 && s.Ko <= 8 && s.Kd >= 1 && s.Kd <= 8 && s.N >= 1 && s.B >= 1 && s.R >= 1 && s.row0 >= 0 &&
-         s.row0 + s.R <= s.N;
+  return s.C == 32 && s.H == 32 && s.Ko >= 1 && s.Kd >= 1 && s.N >= 1 && s.B >= 1 && s.R >= 1 && s.row0 >= 0 && s.row0 + s.R <= s.N;
+}
+
+// The int indices that grow with the number of supports: the plane index z = b*K + k (p.Z of FWD_A / BWD_V, TMA plane
+// coordinates of every contraction), the k coordinate o*N + n of FWD_B's support map, and the Ko*Kd*32*32 weight elements
+// of permute_w_bwd / reduce_dw_partials.  (Tile counts are checked at launch; byte sizes are size_t.)
+static int check_index_range(const BdgcnShape& s) {
+  const long long K = s.Ko > s.Kd ? s.Ko : s.Kd;
+  MPGCN_CHECK((long long)s.B * K < (1ll << 31) && K * s.N + 128 < (1ll << 31) && (long long)s.Ko * s.Kd * 32 * 32 < (1ll << 31),
+              "tensor-core path: B=%d N=%d Ko=%d Kd=%d overflows the engine's 32-bit plane and row indices", s.B, s.N, s.Ko, s.Kd);
+  return 0;
 }
 
 // cells of an activation slab: R origin rows x N destinations
@@ -110,11 +121,15 @@ static FwdLayout fwd_layout(const BdgcnShape& s) {
   return L;
 }
 size_t tc_fwd_ws_bytes(const BdgcnShape& s) { return fwd_layout(s).total; }
+// BWD_DW tile columns: all Ko chunks in one tile up to 8, else ceil(Ko / 8) column tiles of dw_chunks(Ko) chunks each (the
+// last one partly past Ko: TMA zero-fills those chunks and the epilogue skips them)
+static int dw_col_tiles(int Ko) { return ceil_div(Ko, 8); }
+static int dw_chunks(int Ko) { return ceil_div(Ko, dw_col_tiles(Ko)); }
 static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total) {
   const int kbps = ceil_div((long long)rn(s), 64);
   const int total = s.B * kbps;
-  const int MT = ceil_div(s.Kd, 4);
-  int want = device_sm_count() / MT;
+  const int tiles = ceil_div(s.Kd, 4) * dw_col_tiles(s.Ko);     // tiles per slice
+  int want = device_sm_count() / tiles;
   if (want < 1) want = 1;
   int per = ceil_div(total, want);
   if (per < 1) per = 1;
@@ -194,37 +209,52 @@ static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16,
 }
 
 // MIX: D16[b][r][row][32] = sum_{seg < Kin} A16[b][seg][row][32] * Wm16[r][(seg,32)][32], r < Kout   (both channel mixes)
-static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, int w_halves, __half* d16, int tag, int Kin, int Kout,
-                   cudaStream_t st) {
+// One tile emits all the output planes of its rows as Kout chunks of 32 columns, so one launch covers Kout <= 8 (the widest
+// wgmma, N = 256).  More output planes go in ceil(Kout / 8) groups of balanced size, one launch each: group [r0, r0 + Rg) sees
+// W from its first output plane on and writes from output plane r0 on, with the same plane stride.  Each group re-reads A.
+static int run_mix_group(const BdgcnShape& s, const __half* a16, const __half* w16, int w_halves, __half* d16, int tag, int Kin,
+                         int Kout, int r0, int Rg, cudaStream_t st) {
   const long long NN = (long long)rn(s);
   GemmParams p;
   init_params(p);
-  const size_t w_bytes = (size_t)Kout * w_halves * Kin * 32 * 64;      // Kin * w_halves tiles of Kout chunks x [32 k][64 B]
+  w16 += (size_t)r0 * Kin * 32 * 32;                                  // W rows of output plane r0, every half
+  d16 += (size_t)r0 * NN * 32;
+  const size_t w_bytes = (size_t)Rg * w_halves * Kin * 32 * 64;        // Kin * w_halves tiles of Rg chunks x [32 k][64 B]
   int bk = 32;
   if (Kin == 2 || Kin == 3) {
     // One k-block per tile: a single TMA box brings the Kin planes of a 128-cell tile (the single-thread producer / MMA loops
     // cost ~0.3 us per k-block, which bounded the per-plane version at a third of the HBM rate), W resident in shared memory
     bk = 32 * Kin;
     if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin, Kin)) return e;
-    if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Kout, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, bk, Kout)) return e;
+    if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Rg, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, bk, Rg)) return e;
     p.am = omap(1, kBig, Kin, 0, 0);               // z = b -> first plane b*Kin
     p.bm = omap(1, 1, 0, 1, 0);                    // resident tile index = weight half
     p.kb_total = 1; p.kb_per_seg = 1; p.b_res_reps = w_halves;
   } else {
     if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin)) return e;
-    if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Kout, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, 32, Kout)) return e;
+    if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Rg, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, 32, Rg)) return e;
     // segment s: plane = b*Kin + (s % Kin); weight rows (s % Kin)*32 of half s / Kin  (half 0 = fp16(W), half 1 = fp16(W - half 0))
     p.am = omap(1, kBig, Kin, 1, 0, Kin, 0);
     p.bm = omap(1, 1, 0, 0, 32, Kin, 1);
     if (w_bytes > 160 * 1024) { p.kb_total = Kin * w_halves; p.kb_per_seg = 1; }          // large K: W streams with A
     else { p.kb_total = Kin; p.kb_per_seg = 1; p.b_res_reps = w_halves; }              // W resident, A plane by plane
   }
-  p.MT = ceil_div(NN, 128); p.NT = 1; p.Z = s.B; p.R = Kout;
+  p.MT = ceil_div(NN, 128); p.NT = 1; p.Z = s.B; p.R = Rg;
   p.ep.out = d16; p.ep.out_f16 = 1;
   p.ep.sZ = (long long)Kout * NN * 32; p.ep.sI = 32; p.ep.sR = NN * 32;
-  p.ep.m_valid = (int)NN; p.ep.r_valid = Kout;
-  prof_set_next(tag, 2.0 * s.B * (double)Kin * Kout * NN * 32 * 32);   // algorithmic flops (the fp16 hi/lo weight split doubles the executed MMAs)
+  p.ep.m_valid = (int)NN; p.ep.r_valid = Rg;
+  prof_set_next(tag, 2.0 * s.B * (double)Kin * Rg * NN * 32 * 32);   // algorithmic flops (the fp16 hi/lo weight split doubles the executed MMAs)
   return tc::launch_contract(tc::A_K64, bk, p, st);
+}
+static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, int w_halves, __half* d16, int tag, int Kin, int Kout,
+                   cudaStream_t st) {
+  const int groups = ceil_div(Kout, 8);
+  for (int g = 0, r0 = 0; g < groups; ++g) {
+    const int Rg = Kout / groups + (g < Kout % groups ? 1 : 0);     // 9 -> 5 + 4, 17 -> 6 + 6 + 5
+    if (int e = run_mix_group(s, a16, w16, w_halves, d16, tag, Kin, Kout, r0, Rg, st)) return e;
+    r0 += Rg;
+  }
+  return 0;
 }
 
 // FWD_B: out[b][m][e][h] = act( sum_{(o,n)} G_o[row0 + n][m] U16[b][o][n][e][h] + bias[h] )      n < R, every m < N
@@ -309,12 +339,12 @@ static int run_bwd_dw(const BdgcnShape& s, const __half* z16, const __half* v16,
   GemmParams p;
   init_params(p);
   if (int e = map_chunks(&p.a_map, z16, NN, 32, Kd, NN * 32, s.B, (long long)Kd * NN * 32, 64, 4)) return e;
-  if (int e = map_chunks(&p.b_map, v16, NN, 32, Ko, NN * 32, s.B, (long long)Ko * NN * 32, 64, Ko)) return e;
+  if (int e = map_chunks(&p.b_map, v16, NN, 32, Ko, NN * 32, s.B, (long long)Ko * NN * 32, 64, dw_chunks(Ko))) return e;
   p.am = omap(1, 1, 0, 1, 0);           // z (slice) ignored; batch element = segment
   p.bm = omap(1, 1, 0, 1, 0);
   int per = 1, total = 1;
   const int slices = dw_slices(s, &per, &total);
-  p.MT = ceil_div(Kd, 4); p.NT = 1; p.Z = slices; p.R = Ko;
+  p.MT = ceil_div(Kd, 4); p.NT = dw_col_tiles(Ko); p.Z = slices; p.R = dw_chunks(Ko);   // output chunk r = nt * R + j
   p.kb_total = total; p.kb_per_seg = ceil_div(NN, 64);
   p.split_k = 1; p.kb_per_slice = per;
   p.ep.out = partials; p.ep.out_f16 = 0;
@@ -381,7 +411,8 @@ static int resolve_side(const BdgcnShape& s, int K, const float* G, const void* 
 // ---------------------------------------------------------------------------------------
 int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
                      float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st) {
-  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and K <= 8 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  if (int e = check_index_range(s)) return e;
   const size_t NN = rn(s);
   const FwdLayout L = fwd_layout(s);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_forward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
@@ -422,7 +453,8 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
                       cudaStream_t st) {
-  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and K <= 8 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  if (int e = check_index_range(s)) return e;
   MPGCN_CHECK(saved != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
   const int act = s.partial ? 0 : s.act;       // a partial call receives dPre: the mask was applied by the caller, after the exchange
   MPGCN_CHECK(out != nullptr || ex.out_f16 != nullptr || !act, "bdgcn_backward: the ReLU mask needs `out` or its fp16 copy");

@@ -53,7 +53,7 @@ struct Epilogue {
   const __half* corr_src;
   const float* corr_delta;
   long long cZ, cI, cR, cSeg;
-  int corr_nseg;             // <= 8
+  int corr_nseg;             // any count: the epilogue walks the segments 8 at a time
 };
 
 struct alignas(64) GemmParams {
@@ -349,19 +349,23 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
       const int half = tw >> 6, rr = tw & 63;
       const int i = mt * 128 + wg * 64 + rr;
       const long long base = (long long)z * p.ep.sZ + (long long)i * p.ep.sI;
+      // the remainders of the first 8 segments stay in registers for the whole tile; those of segments 8.. (more than 8
+      // supports) are re-read per chunk, 8 at a time
       float dl[8];
       long long cbase = 0;
+      const float* dsrc = nullptr;    // delta of segment 0 of this row: segment sg at dsrc[sg * m_valid]
       bool any_corr = false;
       if (p.ep.corr_src != nullptr) {
         const int zA = ((z / p.am.z_div) % p.am.z_mod) * p.am.z_mul;
         const int zB = ((z / p.bm.z_div) % p.bm.z_mod) * p.bm.z_mul;
         cbase = (long long)zB * p.ep.cZ + (long long)i * p.ep.cI;
+        dsrc = p.ep.corr_delta + (long long)zA * p.ep.corr_nseg * p.ep.m_valid + i;
 #pragma unroll
         for (int sgi = 0; sgi < 8; ++sgi) {
-          dl[sgi] = (sgi < p.ep.corr_nseg && i < p.ep.m_valid)
-                        ? __ldg(p.ep.corr_delta + ((long long)zA * p.ep.corr_nseg + sgi) * p.ep.m_valid + i) : 0.f;
+          dl[sgi] = (sgi < p.ep.corr_nseg && i < p.ep.m_valid) ? __ldg(dsrc + (long long)sgi * p.ep.m_valid) : 0.f;
           any_corr |= (dl[sgi] != 0.f);
         }
+        for (int sg = 8; sg < p.ep.corr_nseg && !any_corr && i < p.ep.m_valid; ++sg) any_corr = __ldg(dsrc + (long long)sg * p.ep.m_valid) != 0.f;
       }
 #pragma unroll
       for (int j0 = 0; j0 < 8; j0 += 2) {
@@ -389,11 +393,16 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
               regs[c] = __float_as_uint(v.x); regs[c + 1] = __float_as_uint(v.y);
               regs[c + 2] = __float_as_uint(v.z); regs[c + 3] = __float_as_uint(v.w);
             }
-            if (any_corr) {
+            // segments in groups of 8 (one group for <= 8 supports), in segment order
+            for (int sg0 = 0; any_corr && sg0 < p.ep.corr_nseg; sg0 += 8) {
+              float dg[8];
+#pragma unroll
+              for (int sgi = 0; sgi < 8; ++sgi)
+                dg[sgi] = sg0 == 0 ? dl[sgi] : (sg0 + sgi < p.ep.corr_nseg ? __ldg(dsrc + (long long)(sg0 + sgi) * p.ep.m_valid) : 0.f);
 #pragma unroll
               for (int sgi = 0; sgi < 8; ++sgi) {
-                if (sgi < p.ep.corr_nseg && dl[sgi] != 0.f) {
-                  const uint4* src = reinterpret_cast<const uint4*>(p.ep.corr_src + cbase + (long long)sgi * p.ep.cSeg + (long long)r * p.ep.cR);
+                if (sg0 + sgi < p.ep.corr_nseg && dg[sgi] != 0.f) {
+                  const uint4* src = reinterpret_cast<const uint4*>(p.ep.corr_src + cbase + (long long)(sg0 + sgi) * p.ep.cSeg + (long long)r * p.ep.cR);
 #pragma unroll
                   for (int qq = 0; qq < 4; ++qq) {
                     const uint4 v = __ldg(src + qq);
@@ -401,8 +410,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                       const float2 f = __half22float2(h2[e]);
-                      regs[8 * qq + 2 * e] = __float_as_uint(fmaf(dl[sgi], f.x, __uint_as_float(regs[8 * qq + 2 * e])));
-                      regs[8 * qq + 2 * e + 1] = __float_as_uint(fmaf(dl[sgi], f.y, __uint_as_float(regs[8 * qq + 2 * e + 1])));
+                      regs[8 * qq + 2 * e] = __float_as_uint(fmaf(dg[sgi], f.x, __uint_as_float(regs[8 * qq + 2 * e])));
+                      regs[8 * qq + 2 * e + 1] = __float_as_uint(fmaf(dg[sgi], f.y, __uint_as_float(regs[8 * qq + 2 * e + 1])));
                     }
                   }
                 }
