@@ -15,7 +15,8 @@
  *   - return value 0 = success; non-zero = failure, message from mpgcn_last_error()
  *     (thread-local).  Nothing ever aborts the process;
  *   - `precision`: 0 = exact fp32 CUDA-core kernels; 1 = fp16-operand / fp32-accumulate
- *     wgmma tensor-core engine (requires C == H == 32; any number of supports K);
+ *     wgmma tensor-core engine (requires C and H to be multiples of 32, H <= 1024, C != H allowed;
+ *     any number of supports K);
  *   - tensors must be 16-byte aligned; the outputs of the precision-1 layer (`out`, `dX`, `out_f16`) 32-byte aligned
  *     (256-bit stores).  Allocator-returned buffers always are;
  *   - `workspace` is caller-owned scratch of at least the size the matching *_workspace_bytes

@@ -35,7 +35,7 @@ static int check_part(const BdgcnShape& s, int precision) {
               "bad layer part: rows [%d, %d) of N=%d, Ko=%d, Kd=%d", s.row0, s.row0 + s.R, s.N, s.Ko, s.Kd);
   MPGCN_CHECK(precision == PREC_FP32_SIMT || precision == PREC_FP16_TC, "unknown precision %d", precision);
   if (precision == PREC_FP16_TC)
-    MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C == H == 32 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+    MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
   return 0;
 }
 
@@ -50,7 +50,7 @@ static int check_shape(const BdgcnShape& s, int precision) {
   MPGCN_CHECK(precision == PREC_FP32_SIMT || precision == PREC_FP16_TC, "unknown precision %d", precision);
   MPGCN_CHECK(s.act == 0 || s.act == 1, "unknown activation code %d", s.act);
   if (precision == PREC_FP16_TC)
-    MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C == H == 32 (got C=%d H=%d K=%d)", s.C, s.H, s.K);
+    MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024 (got C=%d H=%d K=%d)", s.C, s.H, s.K);
   return 0;
 }
 

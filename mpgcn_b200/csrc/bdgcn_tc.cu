@@ -2,18 +2,25 @@
 //
 // Same factored algebra as bdgcn_simt.cu (reference: BDGCN.forward of MPGCN.py; factoring:
 // SURVEY.md section 7.1); each contraction is one launch of tc::contract_kernel with operands
-// described by TMA tensor maps over fp16 copies living in the caller's workspace:
+// described by TMA tensor maps over fp16 copies living in the caller's workspace.
 //
-//   forward   X16 [B][n][c][l]      G16 [zg][K][N][Np]  (Np = N rounded up to 8, rows padded)
-//             Z16 [B][d][n][e][l]   (saved for backward)   U16 [B][o][n][e][h]
-//     FWD_A   Z = X x2 G_d          A_MN128 (G_d [c][e])     B = X16  (ch, c, n, b)
-//     FWD_MIX U = sum_d Z_d W[o,d]  A_K64   (Z plane)        B = W16  (h, (d,l), o)
-//     FWD_B   out = act(sum_o G_o^T x1 U_o + b)   A_MN128 (G flat [(o,n)][m])  B = U16 flat
-//   backward  dP16 [B][m][e][h]   V16 [B][o][n][e][h]   Y16 [B][d][n][e][l]   Wq16 [d][o][h][l]
-//     BWD_V   V = G_o x1 dPre       A_K128  (G_o [n][m])     B = dP16 flat
-//     BWD_DW  dW = Z^T V            A_MN64  (Z)              B = V16  (h, row, o, b)   split-K
-//     BWD_MIX Y = sum_o V_o W[o,d]^T  A_K64 (V plane)        B = Wq16 (l, (o,h), d)
-//     BWD_DX  dX = sum_d Y_d x2 G_d^T A_K128 (G_d [c][e])    B = Y16  (l, e, n, (b,d))
+// Channel widths C = 32 cC and H = 32 cH.  The copies of the caller's tensors (X16, dP16) keep their channel-last layout; the
+// engine's intermediates hold 32-channel "chunk planes" [..][rows][e][32] (lc < cC indexes an input chunk, hc < cH an output
+// chunk; at C = H = 32 every chunk index is 0 and the layouts are the single-chunk ones):
+//
+//   forward   X16 [B][n][c][C]      G16 [zg][K][N][Np]  (Np = N rounded up to 8, rows padded)
+//             Z16 [B][d][lc][n][e][32]  (saved for backward)   U16 [B][hc][o][n][e][32]
+//     FWD_A   Z = X x2 G_d          A_MN128 (G_d [c][e])     B = X16 chunk lc (ch, c, n, b)        one launch per lc
+//     FWD_MIX U = sum_d Z_d W[o,d]  A_K64   (Z plane)        B = W16  [(hc,o)][(d,lc,l)][32]       Kd cC -> Ko cH planes
+//     FWD_B   out = act(sum_o G_o^T x1 U_o + b)   A_MN128 (G flat [(o,n)][m])  B = U16 chunk hc flat  one launch per hc
+//   backward  dP16 [B][m][e][H]   V16 [B][o][hc][n][e][32]   Y16 [B][d][lc][n][e][32]   Wq16 [(d,lc)][(o,hc,h)][32]
+//     BWD_V   V = G_o x1 dPre       A_K128  (G_o [n][m])     B = dP16 chunk hc flat                one launch per hc
+//     BWD_DW  dW = Z^T V            A_MN64  (Z, Kd cC chunks)  B = V16 (Ko cH chunks)   split-K
+//     BWD_MIX Y = sum_o V_o W[o,d]^T  A_K64 (V plane)        B = Wq16                              Ko cH -> Kd cC planes
+//     BWD_DX  dX = sum_d Y_d x2 G_d^T A_K128 (G_d [c][e])    B = Y16 chunk lc (l, e, n, (b,d))     one launch per lc
+// The N^3 contractions act on each channel on its own, so a chunk is a 32-channel layer to them; the chunk planes are laid out
+// so that the per-chunk launch addresses them through a base offset and strides (plane index (b*K + d)*cC + lc of Z16 / Y16
+// and (b*Ko + o)*cH + hc of V16 are affine in the launch's z = b*K + d; U16 keeps FWD_B's flat (o, n) contraction per chunk).
 #include "kernels.h"
 #include "tc_engine.cuh"
 
@@ -74,18 +81,25 @@ int map_planes(CUtensorMap* m, const __half* t, long long rows, long long planes
 }  // namespace
 
 // Any number of supports: the N^3 contractions index supports through z and k-segments, the channel mixes and BWD_DW split
-// more than 8 output supports into column groups, and the FWD_B epilogue walks its remainders 8 segments at a time.
+// more than 8 output planes into column groups, and the FWD_B epilogue walks its remainders 8 segments at a time.  Any
+// channel widths that are multiples of 32 up to 1024: a layer of width 32 c is c chunk planes to the mixes and BWD_DW and c
+// launches of the N^3 contractions (the ReLU / bias-gradient pass keeps one channel per thread of a block: H <= 1024).
 bool tc_supported(const BdgcnShape& s) {
-  return s.C == 32 && s.H == 32 && s.Ko >= 1 && s.Kd >= 1 && s.N >= 1 && s.B >= 1 && s.R >= 1 && s.row0 >= 0 && s.row0 + s.R <= s.N;
+  return s.C >= 32 && s.C % 32 == 0 && s.H >= 32 && s.H % 32 == 0 && s.H <= 1024 && s.Ko >= 1 && s.Kd >= 1 && s.N >= 1 && s.B >= 1 &&
+         s.R >= 1 && s.row0 >= 0 && s.row0 + s.R <= s.N;
 }
 
-// The int indices that grow with the number of supports: the plane index z = b*K + k (p.Z of FWD_A / BWD_V, TMA plane
-// coordinates of every contraction), the k coordinate o*N + n of FWD_B's support map, and the Ko*Kd*32*32 weight elements
-// of permute_w_bwd / reduce_dw_partials.  (Tile counts are checked at launch; byte sizes are size_t.)
+// The int indices that grow with the number of supports and chunks: the plane index b*Kd*cC + .. / b*Ko*cH + .. (TMA plane
+// coordinates of every contraction, p.Z of FWD_A / BWD_V), the k coordinate o*N + n of FWD_B's support map, and the
+// Ko*Kd*C*H weight elements of the weight permutations / reduce_dw_partials.  (Tile counts are checked at launch; byte sizes
+// are size_t.)
 static int check_index_range(const BdgcnShape& s) {
   const long long K = s.Ko > s.Kd ? s.Ko : s.Kd;
-  MPGCN_CHECK((long long)s.B * K < (1ll << 31) && K * s.N + 128 < (1ll << 31) && (long long)s.Ko * s.Kd * 32 * 32 < (1ll << 31),
-              "tensor-core path: B=%d N=%d Ko=%d Kd=%d overflows the engine's 32-bit plane and row indices", s.B, s.N, s.Ko, s.Kd);
+  const long long in_planes = (long long)s.Kd * (s.C / 32), out_planes = (long long)s.Ko * (s.H / 32);
+  const long long planes = in_planes > out_planes ? in_planes : out_planes;
+  MPGCN_CHECK((long long)s.B * planes < (1ll << 31) && K * s.N + 128 < (1ll << 31) && (long long)s.Ko * s.Kd * s.C * s.H < (1ll << 31),
+              "tensor-core path: B=%d N=%d Ko=%d Kd=%d C=%d H=%d overflows the engine's 32-bit plane and row indices", s.B, s.N, s.Ko,
+              s.Kd, s.C, s.H);
   return 0;
 }
 
@@ -108,11 +122,11 @@ static size_t take(size_t& off, size_t bytes) {
 static FwdLayout fwd_layout(const BdgcnShape& s) {
   FwdLayout L;
   size_t off = 0;
-  L.x16 = take(off, (size_t)s.B * rn(s) * 32 * 2);
+  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2);
   L.gd16 = take(off, g16_elems(s, s.Kd) * 2);
   L.go16 = take(off, g16_elems(s, s.Ko) * 2);
-  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * 32 * 32 * 2);      // [hi | lo]
-  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * 32 * 2);
+  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2);    // [hi | lo]
+  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
   L.dd = take(off, g_planes(s, s.Kd) * s.N * 4);   // support-diagonal fp16 remainders (destination / origin)
   L.dgo = take(off, g_planes(s, s.Ko) * s.N * 4);
   L.dgo_masked = take(off, g_planes(s, s.Ko) * s.N * 4);   // origin remainders restricted to the row slab
@@ -121,14 +135,17 @@ static FwdLayout fwd_layout(const BdgcnShape& s) {
   return L;
 }
 size_t tc_fwd_ws_bytes(const BdgcnShape& s) { return fwd_layout(s).total; }
-// BWD_DW tile columns: all Ko chunks in one tile up to 8, else ceil(Ko / 8) column tiles of dw_chunks(Ko) chunks each (the
-// last one partly past Ko: TMA zero-fills those chunks and the epilogue skips them)
-static int dw_col_tiles(int Ko) { return ceil_div(Ko, 8); }
-static int dw_chunks(int Ko) { return ceil_div(Ko, dw_col_tiles(Ko)); }
+// BWD_DW: rows are the Kd*cC chunks of Z16, 4 per m-tile; columns are the Ko*cH chunks of V16, all in one tile up to 8,
+// else ceil(n / 8) column tiles of dw_chunks(n) chunks each (the last one partly past n: TMA zero-fills those chunks and the
+// epilogue skips them)
+static int dw_row_chunks(const BdgcnShape& s) { return s.Kd * (s.C / 32); }
+static int dw_col_chunks(const BdgcnShape& s) { return s.Ko * (s.H / 32); }
+static int dw_col_tiles(int n) { return ceil_div(n, 8); }
+static int dw_chunks(int n) { return ceil_div(n, dw_col_tiles(n)); }
 static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total) {
   const int kbps = ceil_div((long long)rn(s), 64);
   const int total = s.B * kbps;
-  const int tiles = ceil_div(s.Kd, 4) * dw_col_tiles(s.Ko);     // tiles per slice
+  const int tiles = ceil_div(dw_row_chunks(s), 4) * dw_col_tiles(dw_col_chunks(s));     // tiles per slice
   int want = device_sm_count() / tiles;
   if (want < 1) want = 1;
   int per = ceil_div(total, want);
@@ -140,15 +157,15 @@ static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total) {
 static BwdLayout bwd_layout(const BdgcnShape& s) {
   BwdLayout L;
   size_t off = 0;
-  L.dp16 = take(off, (size_t)s.B * s.N * s.N * 32 * 2);        // dPre: every origin row m, always
+  L.dp16 = take(off, (size_t)s.B * s.N * s.N * s.H * 2);       // dPre: every origin row m, always
   L.gd16 = take(off, g16_elems(s, s.Kd) * 2);
   L.go16 = take(off, g16_elems(s, s.Ko) * 2);
-  L.v16 = take(off, (size_t)s.B * s.Ko * rn(s) * 32 * 2);
-  L.y16 = take(off, (size_t)s.B * s.Kd * rn(s) * 32 * 2);
-  L.wq16 = take(off, (size_t)s.Ko * s.Kd * 32 * 32 * 2);
+  L.v16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
+  L.y16 = take(off, (size_t)s.B * s.Kd * rn(s) * s.C * 2);
+  L.wq16 = take(off, (size_t)s.Ko * s.Kd * s.C * s.H * 2);
   int per = 1, total = 1;
   const int slices = dw_slices(s, &per, &total);
-  L.partials = take(off, (size_t)slices * ceil_div(s.Kd, 4) * 128 * s.Ko * 32 * 4);
+  L.partials = take(off, (size_t)slices * ceil_div(dw_row_chunks(s), 4) * 128 * s.Ko * s.H * 4);
   L.scale = take(off, 64);
   L.total = align_up(off, 1024);
   return L;
@@ -186,26 +203,31 @@ long long tc_debug_offset(const BdgcnShape& s, int which) {
 // individual contractions.  Activations are [B][*][R rows n][N][32] slabs (R = N for a whole layer); supports G_d has Kd
 // planes per sample, G_o has Ko.
 // ---------------------------------------------------------------------------------------
-// FWD_A:  Z16[b][d][n][e][l] = sum_c G_d[c][e] X16[b][n][c][l]
+// FWD_A:  Z16[b][d][lc][n][e][l] = sum_c G_d[c][e] X16[b][n][c][32 lc + l]      one launch per input chunk lc
 static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16, __half* z16, const float* delta_d, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N);
-  GemmParams p;
-  init_params(p);
-  if (int e = map_support_mn(&p.a_map, gd16, N, Np, N, (long long)g_planes(s, K))) return e;
-  if (int e = map_chunks(&p.b_map, x16, N, 32, R, (long long)N * 32, s.B, (long long)R * N * 32, 64, 8)) return e;
-  p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + d -> support index
-  p.bm = omap(K, kBig, 1, 0, 0);                        // -> b
-  p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B * K; p.R = 8;
-  p.z_inner = K;                                        // the K supports of one (sample, row block) run back to back: X16 block from L2
-  p.kb_total = p.kb_per_seg = ceil_div(N, 64);
-  p.ep.out = z16; p.ep.out_f16 = 1;
-  p.ep.sZ = (long long)R * N * 32; p.ep.sI = 32; p.ep.sR = (long long)N * 32;
-  p.ep.m_valid = N; p.ep.r_valid = R;
-  // Z[b,d,n,e,:] += (G_d[e,e] - fp16(G_d[e,e])) * X16[b,n,e,:]
-  p.ep.corr_src = x16; p.ep.corr_delta = delta_d; p.ep.corr_nseg = 1;
-  p.ep.cZ = (long long)R * N * 32; p.ep.cI = 32; p.ep.cR = (long long)N * 32; p.ep.cSeg = 0;
-  prof_set_next(PROF_FWD_A, 2.0 * s.B * K * (double)R * N * N * 32);
-  return tc::launch_contract(tc::A_MN128, 64, p, st);
+  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32;
+  const long long NN = (long long)rn(s);
+  for (int lc = 0; lc < cC; ++lc) {
+    const __half* xc = x16 + lc * 32;
+    GemmParams p;
+    init_params(p);
+    if (int e = map_support_mn(&p.a_map, gd16, N, Np, N, (long long)g_planes(s, K))) return e;
+    if (int e = map_chunks(&p.b_map, xc, N, C, R, (long long)N * C, s.B, (long long)R * N * C, 64, 8)) return e;
+    p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + d -> support index
+    p.bm = omap(K, kBig, 1, 0, 0);                        // -> b
+    p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B * K; p.R = 8;
+    p.z_inner = K;                                        // the K supports of one (sample, row block) run back to back: X16 block from L2
+    p.kb_total = p.kb_per_seg = ceil_div(N, 64);
+    p.ep.out = z16 + lc * NN * 32; p.ep.out_f16 = 1;      // plane (b*K + d)*cC + lc
+    p.ep.sZ = cC * NN * 32; p.ep.sI = 32; p.ep.sR = (long long)N * 32;
+    p.ep.m_valid = N; p.ep.r_valid = R;
+    // Z[b,d,n,e,:] += (G_d[e,e] - fp16(G_d[e,e])) * X16[b,n,e,:]
+    p.ep.corr_src = xc; p.ep.corr_delta = delta_d; p.ep.corr_nseg = 1;
+    p.ep.cZ = (long long)R * N * C; p.ep.cI = C; p.ep.cR = (long long)N * C; p.ep.cSeg = 0;
+    prof_set_next(PROF_FWD_A, 2.0 * s.B * K * (double)R * N * N * 32);
+    if (int e = tc::launch_contract(tc::A_MN128, 64, p, st)) return e;
+  }
+  return 0;
 }
 
 // MIX: D16[b][r][row][32] = sum_{seg < Kin} A16[b][seg][row][32] * Wm16[r][(seg,32)][32], r < Kout   (both channel mixes)
@@ -257,122 +279,136 @@ static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, in
   return 0;
 }
 
-// FWD_B: out[b][m][e][h] = act( sum_{(o,n)} G_o[row0 + n][m] U16[b][o][n][e][h] + bias[h] )      n < R, every m < N
-static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16, const float* bias, float* out, __half* out16,
+// FWD_B: out[b][m][e][32 hc + h] = act( sum_{(o,n)} G_o[row0 + n][m] U16[b][hc][o][n][e][h] + bias[32 hc + h] )
+//        n < R, every m < N; one launch per output chunk hc
+static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16_all, const float* bias, float* out, __half* out16,
                      const float* delta_o, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N);
+  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32;
   const bool slab = !(R == N && s.row0 == 0);
-  GemmParams p;
-  init_params(p);
-  if (!slab) {
-    // whole layer: the contraction index (o, n) is a plain row index of the flat [K*N][N] support stack and of U16
-    if (int e = map_support_mn(&p.a_map, go16, N, Np, (long long)K * N, s.dynamic ? s.B : 1)) return e;
-    // U16 [b][(o,n)][e][h] read as (h, k = (o,n) rows, r = e, b): dims listed with non-monotonic strides (the r stride,
-    // 64 B, is smaller than the k stride) so that ONE box (32 ch, 64 k, 4|8 r) lands in the canonical [r][k][64 B] layout
-    if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, s.B, (long long)K * N * N * 32, 64, 8)) return e;
-    p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, 0);
-    p.bm = omap(1, kBig, 1, 0, 0);
-    p.kb_total = p.kb_per_seg = ceil_div((long long)K * N, 64);
-  } else {
-    // origin-row slab: one k-segment per support o.  A = rows [row0, row0 + R) of G_o (k coordinate o*N + kk inside the flat
-    // stack, base pointer moved to row0); B = U16 [b][o][n < R]: TMA zero-fills rows >= R, which also cancels the rows of the
-    // NEXT slab that the last k-block of a segment reads from G.
-    const long long gplanes = s.dynamic ? s.B : 1;
-    {
-      const uint64_t dims[4] = {(uint64_t)N, (uint64_t)((long long)K * N - s.row0), (uint64_t)gplanes, 1};
-      const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)K * N * Np * 2, (uint64_t)K * N * Np * 2 * (uint64_t)gplanes};
-      const uint32_t box[4] = {64, 64, 1, 1};
+  for (int hc = 0; hc < cH; ++hc) {
+    const __half* u16 = u16_all + (size_t)hc * K * rn(s) * 32;
+    GemmParams p;
+    init_params(p);
+    if (!slab) {
+      // whole layer: the contraction index (o, n) is a plain row index of the flat [K*N][N] support stack and of U16
+      if (int e = map_support_mn(&p.a_map, go16, N, Np, (long long)K * N, s.dynamic ? s.B : 1)) return e;
+      // U16 [b][hc][(o,n)][e][h] read as (h, k = (o,n) rows, r = e, b): dims listed with non-monotonic strides (the r stride,
+      // 64 B, is smaller than the k stride) so that ONE box (32 ch, 64 k, 4|8 r) lands in the canonical [r][k][64 B] layout
+      if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, s.B, (long long)cH * K * N * N * 32, 64, 8)) return e;
+      p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, 0);
+      p.bm = omap(1, kBig, 1, 0, 0);
+      p.kb_total = p.kb_per_seg = ceil_div((long long)K * N, 64);
+    } else {
+      // origin-row slab: one k-segment per support o.  A = rows [row0, row0 + R) of G_o (k coordinate o*N + kk inside the flat
+      // stack, base pointer moved to row0); B = U16 [b][hc][o][n < R]: TMA zero-fills rows >= R, which also cancels the rows of
+      // the NEXT slab that the last k-block of a segment reads from G.
+      const long long gplanes = s.dynamic ? s.B : 1;
+      {
+        const uint64_t dims[4] = {(uint64_t)N, (uint64_t)((long long)K * N - s.row0), (uint64_t)gplanes, 1};
+        const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)K * N * Np * 2, (uint64_t)K * N * Np * 2 * (uint64_t)gplanes};
+        const uint32_t box[4] = {64, 64, 1, 1};
+        if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
+      }
+      if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * cH * K - (long long)hc * K, (long long)R * N * 32, 64, 8)) return e;
+      p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, N);          // k coordinate += o * N
+      p.bm = omap(1, kBig, cH * K, 1, 0);                     // plane = (b*cH + hc)*K + o, from this chunk's base
+      p.kb_per_seg = ceil_div(R, 64);
+      p.kb_total = K * p.kb_per_seg;
+    }
+    p.MT = ceil_div(N, 128); p.NT = ceil_div(N, 8); p.Z = s.B; p.R = 8;
+    p.ep.out = out + hc * 32; p.ep.out_f16 = 0; p.ep.out16 = out16 ? out16 + hc * 32 : nullptr;
+    p.ep.sZ = (long long)N * N * H; p.ep.sI = (long long)N * H; p.ep.sR = H;
+    p.ep.m_valid = N; p.ep.r_valid = N;
+    p.ep.bias = (s.partial || !bias) ? nullptr : bias + hc * 32; p.ep.relu = s.partial ? 0 : s.act;
+    // pre[b,m,e,:] += sum_o (G_o[m,m] - fp16(G_o[m,m])) * U16[b,hc,o,m,e,:]   (delta_o is zero outside the slab: the row n = m of
+    // U exists only for row0 <= m < row0 + R; corr_src is moved so that row index m addresses slab row m - row0)
+    p.ep.corr_src = u16 - (long long)s.row0 * N * 32; p.ep.corr_delta = delta_o; p.ep.corr_nseg = K;
+    // (the epilogue forms the sample offset as zB * cZ with zB = b in the flat mode and b*cH*K in the slab mode)
+    p.ep.cZ = slab ? (long long)R * N * 32 : (long long)cH * K * R * N * 32;
+    p.ep.cSeg = (long long)R * N * 32; p.ep.cI = (long long)N * 32; p.ep.cR = 32;
+    prof_set_next(PROF_FWD_B, 2.0 * s.B * K * (double)R * N * N * 32);
+    if (int e = tc::launch_contract(tc::A_MN128, 64, p, st)) return e;
+  }
+  return 0;
+}
+
+// BWD_V: V16[b][o][hc][n][e][h] = sum_m G_o[row0 + n][m] dP16[b][m][e][32 hc + h]       n < R; one launch per output chunk hc
+static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16, __half* v16, cudaStream_t st) {
+  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32;
+  const long long NN = (long long)rn(s);
+  for (int hc = 0; hc < cH; ++hc) {
+    GemmParams p;
+    init_params(p);
+    {   // rows [row0, row0 + R) of every support plane, K-major
+      const long long nz = (long long)g_planes(s, K);
+      const uint64_t dims[4] = {(uint64_t)N, (uint64_t)R, (uint64_t)nz, 1};
+      const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)N * Np * 2, (uint64_t)N * Np * 2 * (uint64_t)nz};
+      const uint32_t box[4] = {64, 128, 1, 1};
       if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
     }
-    if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * K, (long long)R * N * 32, 64, 8)) return e;
-    p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, N);          // k coordinate += o * N
-    p.bm = omap(1, kBig, K, 1, 0);                          // plane = b*K + o
-    p.kb_per_seg = ceil_div(R, 64);
-    p.kb_total = K * p.kb_per_seg;
+    // dP16 [b][m][e][H] chunk hc read as (h, k = m, r = e, b), see run_fwd_b
+    if (int e = map_chunks(&p.b_map, dp16 + hc * 32, N, (long long)N * H, N, H, s.B, (long long)N * N * H, 64, 8)) return e;
+    p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + o
+    p.bm = omap(K, kBig, 1, 0, 0);
+    p.MT = ceil_div(R, 128); p.NT = ceil_div(N, 8); p.Z = s.B * K; p.R = 8;
+    p.z_inner = K;                                        // dP16 block of one (sample, e block) serves the K supports back to back
+    p.kb_total = p.kb_per_seg = ceil_div(N, 64);
+    p.ep.out = v16 + hc * NN * 32; p.ep.out_f16 = 1;      // plane (b*K + o)*cH + hc
+    p.ep.sZ = cH * NN * 32; p.ep.sI = (long long)N * 32; p.ep.sR = 32;
+    p.ep.m_valid = R; p.ep.r_valid = N;
+    prof_set_next(PROF_BWD_V, 2.0 * s.B * K * (double)R * N * N * 32);
+    if (int e = tc::launch_contract(tc::A_K128, 64, p, st)) return e;
   }
-  p.MT = ceil_div(N, 128); p.NT = ceil_div(N, 8); p.Z = s.B; p.R = 8;
-  p.ep.out = out; p.ep.out_f16 = 0; p.ep.out16 = out16;
-  p.ep.sZ = (long long)N * N * 32; p.ep.sI = (long long)N * 32; p.ep.sR = 32;
-  p.ep.m_valid = N; p.ep.r_valid = N;
-  p.ep.bias = s.partial ? nullptr : bias; p.ep.relu = s.partial ? 0 : s.act;
-  // pre[b,m,e,:] += sum_o (G_o[m,m] - fp16(G_o[m,m])) * U16[b,o,m,e,:]   (delta_o is zero outside the slab: the row n = m of U
-  // exists only for row0 <= m < row0 + R; corr_src is moved so that row index m addresses slab row m - row0)
-  p.ep.corr_src = u16 - (long long)s.row0 * N * 32; p.ep.corr_delta = delta_o; p.ep.corr_nseg = K;
-  // (the epilogue forms the sample offset as zB * cZ with zB = b in the flat mode and b*K in the slab mode)
-  p.ep.cZ = slab ? (long long)R * N * 32 : (long long)K * R * N * 32;
-  p.ep.cSeg = (long long)R * N * 32; p.ep.cI = (long long)N * 32; p.ep.cR = 32;
-  prof_set_next(PROF_FWD_B, 2.0 * s.B * K * (double)R * N * N * 32);
-  return tc::launch_contract(tc::A_MN128, 64, p, st);
+  return 0;
 }
 
-// BWD_V: V16[b][o][n][e][h] = sum_m G_o[row0 + n][m] dP16[b][m][e][h]       n < R
-static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16, __half* v16, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N);
-  GemmParams p;
-  init_params(p);
-  {   // rows [row0, row0 + R) of every support plane, K-major
-    const long long nz = (long long)g_planes(s, K);
-    const uint64_t dims[4] = {(uint64_t)N, (uint64_t)R, (uint64_t)nz, 1};
-    const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)N * Np * 2, (uint64_t)N * Np * 2 * (uint64_t)nz};
-    const uint32_t box[4] = {64, 128, 1, 1};
-    if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
-  }
-  // dP16 [b][m][e][h] read as (h, k = m, r = e, b), see run_fwd_b
-  if (int e = map_chunks(&p.b_map, dp16, N, (long long)N * 32, N, 32, s.B, (long long)N * N * 32, 64, 8)) return e;
-  p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + o
-  p.bm = omap(K, kBig, 1, 0, 0);
-  p.MT = ceil_div(R, 128); p.NT = ceil_div(N, 8); p.Z = s.B * K; p.R = 8;
-  p.z_inner = K;                                        // dP16 block of one (sample, e block) serves the K supports back to back
-  p.kb_total = p.kb_per_seg = ceil_div(N, 64);
-  p.ep.out = v16; p.ep.out_f16 = 1;
-  p.ep.sZ = (long long)R * N * 32; p.ep.sI = (long long)N * 32; p.ep.sR = 32;
-  p.ep.m_valid = R; p.ep.r_valid = N;
-  prof_set_next(PROF_BWD_V, 2.0 * s.B * K * (double)R * N * N * 32);
-  return tc::launch_contract(tc::A_K128, 64, p, st);
-}
-
-// BWD_DW: P[slice][mt][(d%4)*32+l][o][h] = sum over the slice's (b,row) range of Z16[b][d][row][l] V16[b][o][row][h]
+// BWD_DW: P[slice][a*32 + l][(o*cH + hc)*32 + h] = sum over the slice's (b,row) range of Z16 chunk a = d*cC + lc [b][row][l] times
+// V16 chunk (o, hc) [b][row][h]; that is P[slice][d*C + c][o*H + h'] in W's channel numbering
 static int run_bwd_dw(const BdgcnShape& s, const __half* z16, const __half* v16, float* partials, int* slices_out, int* mt_out,
                       cudaStream_t st) {
-  const int Ko = s.Ko, Kd = s.Kd;
+  const int rows = dw_row_chunks(s), cols = dw_col_chunks(s);
   const long long NN = (long long)rn(s);
   GemmParams p;
   init_params(p);
-  if (int e = map_chunks(&p.a_map, z16, NN, 32, Kd, NN * 32, s.B, (long long)Kd * NN * 32, 64, 4)) return e;
-  if (int e = map_chunks(&p.b_map, v16, NN, 32, Ko, NN * 32, s.B, (long long)Ko * NN * 32, 64, dw_chunks(Ko))) return e;
+  if (int e = map_chunks(&p.a_map, z16, NN, 32, rows, NN * 32, s.B, (long long)rows * NN * 32, 64, 4)) return e;
+  if (int e = map_chunks(&p.b_map, v16, NN, 32, cols, NN * 32, s.B, (long long)cols * NN * 32, 64, dw_chunks(cols))) return e;
   p.am = omap(1, 1, 0, 1, 0);           // z (slice) ignored; batch element = segment
   p.bm = omap(1, 1, 0, 1, 0);
   int per = 1, total = 1;
   const int slices = dw_slices(s, &per, &total);
-  p.MT = ceil_div(Kd, 4); p.NT = dw_col_tiles(Ko); p.Z = slices; p.R = dw_chunks(Ko);   // output chunk r = nt * R + j
+  p.MT = ceil_div(rows, 4); p.NT = dw_col_tiles(cols); p.Z = slices; p.R = dw_chunks(cols);   // output chunk r = nt * R + j
   p.kb_total = total; p.kb_per_seg = ceil_div(NN, 64);
   p.split_k = 1; p.kb_per_slice = per;
   p.ep.out = partials; p.ep.out_f16 = 0;
-  p.ep.sZ = (long long)p.MT * 128 * Ko * 32; p.ep.sI = (long long)Ko * 32; p.ep.sR = 32;
-  p.ep.m_valid = p.MT * 128; p.ep.r_valid = Ko;
+  p.ep.sZ = (long long)p.MT * 128 * cols * 32; p.ep.sI = (long long)cols * 32; p.ep.sR = 32;
+  p.ep.m_valid = p.MT * 128; p.ep.r_valid = cols;
   *slices_out = slices;
   *mt_out = p.MT;
-  prof_set_next(PROF_BWD_DW, 2.0 * s.B * (double)Ko * Kd * NN * 32 * 32);
+  prof_set_next(PROF_BWD_DW, 2.0 * s.B * (double)s.Ko * s.Kd * NN * s.C * s.H);
   return tc::launch_contract(tc::A_MN64, 64, p, st);
 }
 
-// BWD_DX: dX[b][n][c][l] = sum_{d,e} G_d[c][e] Y16[b][d][n][e][l]       n < R
+// BWD_DX: dX[b][n][c][32 lc + l] = sum_{d,e} G_d[c][e] Y16[b][d][lc][n][e][l]       n < R; one launch per input chunk lc
 static int run_bwd_dx(const BdgcnShape& s, const __half* gd16, const __half* y16, float* dX, const float* inv_scale, float* dx_absmax,
                       cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N);
-  GemmParams p;
-  init_params(p);
-  if (int e = map_support_k(&p.a_map, gd16, N, Np, (long long)g_planes(s, K))) return e;
-  if (int e = map_chunks(&p.b_map, y16, N, 32, R, (long long)N * 32, (long long)s.B * K, (long long)R * N * 32, 64, 8)) return e;
-  p.am = omap(1, s.dynamic ? kBig : 1, s.dynamic ? K : 0, 1, 0);   // support index = (b*K) + d
-  p.bm = omap(1, kBig, K, 1, 0);                                    // plane = b*K + d
-  p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B; p.R = 8;
-  p.kb_per_seg = ceil_div(N, 64); p.kb_total = K * p.kb_per_seg;
-  p.ep.out = dX; p.ep.out_f16 = 0; p.ep.alpha_dev = inv_scale; p.ep.absmax_out = dx_absmax;
-  p.ep.sZ = (long long)R * N * 32; p.ep.sI = 32; p.ep.sR = (long long)N * 32;
-  p.ep.m_valid = N; p.ep.r_valid = R;
-  prof_set_next(PROF_BWD_DX, 2.0 * s.B * K * (double)R * N * N * 32);
-  return tc::launch_contract(tc::A_K128, 64, p, st);
+  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32;
+  const long long NN = (long long)rn(s);
+  for (int lc = 0; lc < cC; ++lc) {
+    GemmParams p;
+    init_params(p);
+    if (int e = map_support_k(&p.a_map, gd16, N, Np, (long long)g_planes(s, K))) return e;
+    if (int e = map_chunks(&p.b_map, y16 + lc * NN * 32, N, 32, R, (long long)N * 32, (long long)s.B * K * cC - lc, NN * 32, 64, 8)) return e;
+    p.am = omap(1, s.dynamic ? kBig : 1, s.dynamic ? K : 0, 1, 0);   // support index = (b*K) + d
+    p.bm = omap(1, kBig, K * cC, cC, 0);                              // plane = (b*K + d)*cC, from this chunk's base
+    p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B; p.R = 8;
+    p.kb_per_seg = ceil_div(N, 64); p.kb_total = K * p.kb_per_seg;
+    p.ep.out = dX + lc * 32; p.ep.out_f16 = 0; p.ep.alpha_dev = inv_scale; p.ep.absmax_out = dx_absmax;   // max over every chunk
+    p.ep.sZ = (long long)R * N * C; p.ep.sI = C; p.ep.sR = (long long)N * C;
+    p.ep.m_valid = N; p.ep.r_valid = R;
+    prof_set_next(PROF_BWD_DX, 2.0 * s.B * K * (double)R * N * N * 32);
+    if (int e = tc::launch_contract(tc::A_K128, 64, p, st)) return e;
+  }
+  return 0;
 }
 
 // Prepared supports: [planes][N][Np] fp16 (padding zeroed) followed, 256-byte aligned, by the [planes][N] diagonal remainders.
@@ -411,7 +447,8 @@ static int resolve_side(const BdgcnShape& s, int K, const float* G, const void* 
 // ---------------------------------------------------------------------------------------
 int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
                      float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st) {
-  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
+              s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
   const size_t NN = rn(s);
   const FwdLayout L = fwd_layout(s);
@@ -429,7 +466,7 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
 
   const __half* x16 = static_cast<const __half*>(ex.x_f16);
   if (x16 == nullptr) {
-    if (int e = cvt_f32_to_f16(X, x16_ws, (size_t)s.B * NN * 32, st)) return e;
+    if (int e = cvt_f32_to_f16(X, x16_ws, (size_t)s.B * NN * s.C, st)) return e;
     x16 = x16_ws;
   }
   SideG gd{}, go{};
@@ -442,10 +479,12 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
     if (int e = mask_delta_rows(go.delta, masked, g_planes(s, s.Ko), s.N, s.row0, s.R, st)) return e;
     delta_o = masked;
   }
-  const size_t wn = (size_t)s.Ko * s.Kd * 32 * 32;
-  if (int e = cvt_f32_to_f16_hilo(W, w16, w16 + wn, wn, st)) return e;
+  const size_t wn = (size_t)s.Ko * s.Kd * s.C * s.H;
+  if (s.H == 32) {      // the mix's W order [(hc,o)][(d,lc,l)][h] is then W's own [o][d][c][h]
+    if (int e = cvt_f32_to_f16_hilo(W, w16, w16 + wn, wn, st)) return e;
+  } else if (int e = permute_w_mix(W, w16, w16 + wn, s.Ko, s.Kd, s.C, s.H, st)) return e;
   if (int e = run_fwd_a(s, gd.g16, x16, z16, gd.delta, st)) return e;
-  if (int e = run_mix(s, z16, w16, 2, u16, PROF_FWD_MIX, s.Kd, s.Ko, st)) return e;
+  if (int e = run_mix(s, z16, w16, 2, u16, PROF_FWD_MIX, s.Kd * (s.C / 32), s.Ko * (s.H / 32), st)) return e;
   if (int e = run_fwd_b(s, go.g16, u16, bias, out, static_cast<__half*>(ex.out_f16), delta_o, st)) return e;
   return 0;
 }
@@ -453,7 +492,8 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
                       cudaStream_t st) {
-  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C = H = 32 and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
+  MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
+              s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
   MPGCN_CHECK(saved != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
   const int act = s.partial ? 0 : s.act;       // a partial call receives dPre: the mask was applied by the caller, after the exchange
@@ -482,12 +522,12 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
   } else {
     __half* dp16_ws = reinterpret_cast<__half*>(wb + L.dp16);
     float* scale2_ws = reinterpret_cast<float*>(wb + L.scale);
-    if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * 32, st));
-    if (int e = grad_scale_prepare(d_out, (size_t)s.B * NNfull * 32, scale2_ws, ex.d_out_absmax, st)) return e;
+    if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * s.H, st));
+    if (int e = grad_scale_prepare(d_out, (size_t)s.B * NNfull * s.H, scale2_ws, ex.d_out_absmax, st)) return e;
     if (ex.out_f16 != nullptr && act) {
-      if (int e = relu_bwd_prep_f16mask(d_out, static_cast<const __half*>(ex.out_f16), act, dp16_ws, db, (size_t)s.B * NNfull * 32, 32, scale2_ws, st)) return e;
+      if (int e = relu_bwd_prep_f16mask(d_out, static_cast<const __half*>(ex.out_f16), act, dp16_ws, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st)) return e;
     } else {
-      if (int e = relu_bwd_prep(d_out, out, act, dp16_ws, nullptr, db, (size_t)s.B * NNfull * 32, 32, scale2_ws, st)) return e;
+      if (int e = relu_bwd_prep(d_out, out, act, dp16_ws, nullptr, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st)) return e;
     }
   }
   SideG gd{}, go{};
@@ -500,11 +540,13 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
   if (int e = run_bwd_v(s, go.g16, dp16, v16, st)) return e;
   int slices = 0, mt = 0;
   if (int e = run_bwd_dw(s, z16, v16, partials, &slices, &mt, st)) return e;
-  if (int e = reduce_dw_partials(partials, dW, slices, mt, s.Ko, s.Kd, scale2 + 1, st)) return e;
+  if (int e = reduce_dw_partials(partials, dW, slices, mt, s.Ko, s.Kd, s.C, s.H, scale2 + 1, st)) return e;
   if (dX) {
     if (ex.dx_absmax) MPGCN_CUDA(cudaMemsetAsync(ex.dx_absmax, 0, sizeof(float), st));
-    if (int e = permute_w_bwd(W, wq16, nullptr, s.Ko, s.Kd, 32, 32, st)) return e;
-    if (int e = run_mix(s, v16, wq16, 1, y16, PROF_BWD_MIX, s.Ko, s.Kd, st)) return e;
+    if (s.C == 32) {    // the mix's W order [(d,lc)][(o,hc,h)][l] is then permute_w_bwd's [d][o][h][l]
+      if (int e = permute_w_bwd(W, wq16, nullptr, s.Ko, s.Kd, 32, s.H, st)) return e;
+    } else if (int e = permute_w_mix(W, wq16, nullptr, s.Ko, s.Kd, s.C, s.H, st)) return e;
+    if (int e = run_mix(s, v16, wq16, 1, y16, PROF_BWD_MIX, s.Ko * (s.H / 32), s.Kd * (s.C / 32), st)) return e;
     if (int e = run_bwd_dx(s, gd.g16, y16, dX, scale2 + 1, ex.dx_absmax, st)) return e;
   }
   return 0;

@@ -55,8 +55,11 @@ int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __h
 int grad_scale_prepare(const float* d_out, size_t n, float* scale2, const float* absmax_hint, cudaStream_t s);
 // W[o][d][l][h] fp32 (o < Ko, d < Kd) -> Wq[d][o][h][l] (fp16 and/or fp32)
 int permute_w_bwd(const float* W, __half* wq16, float* wq32, int Ko, int Kd, int C, int H, cudaStream_t s);
-// dW[o][d][l][h] = sum_slices P[slice][mt][(d%4)*32 + l][o][h]   (C = H = 32; o < Ko, d < Kd)
-int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, const float* inv_scale, cudaStream_t s);
+// W[o][d][c][h] fp32 -> the fp16 W operand of a tensor-core channel mix (bdgcn_tc.cu), C and H multiples of 32, c = 32 lc + l,
+// h = 32 hc + h':  lo != null: forward, hi / lo = fp16 split as [(hc,o)][(d,lc)][l][h'];  lo == null: backward, [(d,lc)][(o,hc)][h'][l]
+int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s);
+// dW[o][d][c][h] = sum_slices P[slice][d*C + c][o*H + h]   (P: [slice][MT*128 rows][Ko*H]; o < Ko, d < Kd)
+int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, int C, int H, const float* inv_scale, cudaStream_t s);
 // out[p][i] = (row0 <= i < row0 + rows) ? delta[p][i] : 0   (diagonal remainders restricted to an origin-row slab)
 int mask_delta_rows(const float* delta, float* out, size_t planes, int N, int row0, int rows, cudaStream_t s);
 // x[i] = act(x[i] + bias[i % H]) in place (bias nullable; act 0 none / 1 ReLU): the epilogue a partial layer call leaves out

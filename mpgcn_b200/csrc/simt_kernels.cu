@@ -331,13 +331,20 @@ __global__ void relu_bwd_prep_f16mask_kernel(const float4* __restrict__ d_out, c
   }
 }
 
+// block size of the four-channel kernels: a multiple of H / 4 (a thread keeps its channel quad across the grid-stride loop) with
+// at least one thread per channel for the bias-gradient reduction; 256 for every H <= 256 whose quad count divides 256
+static int quad_block(int H) {
+  const int H4 = H / 4;
+  return H4 * (256 / H4 > 4 ? 256 / H4 : 4);
+}
+
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d16, float* db, size_t n, int H, const float* scale,
                           cudaStream_t s) {
   if (n == 0) return 0;
-  MPGCN_CHECK(H % 4 == 0 && 256 % (H / 4) == 0 && n % 4 == 0, "relu_bwd_prep_f16mask: H=%d / n=%zu unsupported", H, n);
+  MPGCN_CHECK(H % 4 == 0 && H >= 4 && H <= 1024 && n % 4 == 0, "relu_bwd_prep_f16mask: H=%d / n=%zu unsupported", H, n);
   MPGCN_CHECK(((reinterpret_cast<uintptr_t>(d_out) & 15) | (reinterpret_cast<uintptr_t>(out16) & 7) | (reinterpret_cast<uintptr_t>(d16) & 7)) == 0,
               "relu_bwd_prep_f16mask: misaligned pointer");
-  const int threads = 256;
+  const int threads = quad_block(H);
   prof_count(PROF_ELEMENTWISE);
   relu_bwd_prep_f16mask_kernel<<<grid_for(n / 4, threads), threads, 4 * threads * sizeof(float), s>>>(
       reinterpret_cast<const float4*>(d_out), reinterpret_cast<const uint2*>(out16), relu, reinterpret_cast<uint2*>(d16), db, n / 4, H / 4, scale);
@@ -352,7 +359,7 @@ int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d16, f
   const bool aligned = ((reinterpret_cast<uintptr_t>(d_out) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(d32)) & 15) == 0 &&
                        (reinterpret_cast<uintptr_t>(d16) & 7) == 0;
   if (H % 4 == 0 && 256 % (H / 4) == 0 && n % 4 == 0 && aligned) {
-    const int threads = 256;
+    const int threads = quad_block(H);
     unsigned blocks = grid_for(n / 4, threads);
     prof_count(PROF_ELEMENTWISE);
     relu_bwd_prep_vec4_kernel<<<blocks, threads, 4 * threads * sizeof(float), s>>>(
@@ -426,27 +433,58 @@ int permute_w_bwd(const float* W, __half* wq16, float* wq32, int Ko, int Kd, int
   return 0;
 }
 
-__global__ void reduce_dw_kernel(const float* __restrict__ P, float* __restrict__ dW, int slices, int MT, int Ko, int Kd,
+// W[o][d][32 lc + l][32 hc + h] -> one [32][32] block per (output plane, input plane) of a channel mix, see kernels.h
+__global__ void permute_w_mix_kernel(const float* __restrict__ W, __half* __restrict__ hi, __half* __restrict__ lo, int Ko, int Kd, int C,
+                                     int H) {
+  const int cC = C / 32, cH = H / 32;
+  const int total = Ko * Kd * C * H;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int e0 = i % 32, e1 = (i / 32) % 32, blk = i / 1024;
+    int o, d, lc, hc, l, h;
+    if (lo) {      // forward: i = ((hc*Ko + o)*Kd*cC + d*cC + lc)*1024 + l*32 + h
+      h = e0; l = e1;
+      const int sp = blk % (Kd * cC), r = blk / (Kd * cC);
+      d = sp / cC; lc = sp % cC; o = r % Ko; hc = r / Ko;
+    } else {       // backward: i = ((d*cC + lc)*Ko*cH + o*cH + hc)*1024 + h*32 + l
+      l = e0; h = e1;
+      const int sp = blk % (Ko * cH), r = blk / (Ko * cH);
+      o = sp / cH; hc = sp % cH; d = r / cC; lc = r % cC;
+    }
+    const float v = W[((size_t)(o * Kd + d) * C + lc * 32 + l) * H + hc * 32 + h];
+    const __half x = f2h_sat(v);
+    hi[i] = x;
+    if (lo) lo[i] = f2h_sat(v - __half2float(x));
+  }
+}
+
+int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s) {
+  MPGCN_CHECK(C % 32 == 0 && H % 32 == 0, "permute_w_mix: C=%d H=%d are not multiples of 32", C, H);
+  prof_count(PROF_ELEMENTWISE);
+  permute_w_mix_kernel<<<grid_for((size_t)Ko * Kd * C * H, 256), 256, 0, s>>>(W, hi, lo, Ko, Kd, C, H);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+__global__ void reduce_dw_kernel(const float* __restrict__ P, float* __restrict__ dW, int slices, int MT, int Ko, int Kd, int C, int H,
                                  const float* __restrict__ inv_scale) {
   const float a = inv_scale ? __ldg(inv_scale) : 1.f;
-  // dW index i = ((o*Kd + d)*32 + l)*32 + h ; partial row = (d%4)*32 + l of m-tile d/4
-  const int total = Ko * Kd * 32 * 32;
+  // dW index i = ((o*Kd + d)*C + c)*H + h ; partial row d*C + c (= m-tile (d*C + c) / 128), column o*H + h
+  const int total = Ko * Kd * C * H;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int h = i % 32;
-    const int l = (i / 32) % 32;
-    const int d = (i / 1024) % Kd;
-    const int o = i / (1024 * Kd);
-    const int mt = d / 4;
-    const size_t row = (size_t)mt * 128 + (d % 4) * 32 + l;
+    const int h = i % H;
+    const int c = (i / H) % C;
+    const int d = (i / (H * C)) % Kd;
+    const int o = i / (H * C * Kd);
+    const size_t row = (size_t)d * C + c;
     float sum = 0.f;
-    for (int s = 0; s < slices; ++s) sum += P[(((size_t)s * MT * 128 + row) * Ko + o) * 32 + h];
+    for (int s = 0; s < slices; ++s) sum += P[((size_t)s * MT * 128 + row) * Ko * H + (size_t)o * H + h];
     dW[i] = sum * a;
   }
 }
 
-int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, const float* inv_scale, cudaStream_t s) {
+int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, int C, int H, const float* inv_scale, cudaStream_t s) {
   prof_count(PROF_ELEMENTWISE);
-  reduce_dw_kernel<<<grid_for((size_t)Ko * Kd * 1024, 256), 256, 0, s>>>(P, dW, slices, MT, Ko, Kd, inv_scale);
+  reduce_dw_kernel<<<grid_for((size_t)Ko * Kd * C * H, 256), 256, 0, s>>>(P, dW, slices, MT, Ko, Kd, C, H, inv_scale);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }

@@ -36,7 +36,7 @@ def resolve_precision(name, B, N, K, C, H) -> int:
         return _lib.PREC_FP16_TC if lib.mpgcn_bdgcn_precision_supported(B, N, K, C, H, _lib.PREC_FP16_TC) else _lib.PREC_FP32
     code = _PREC_NAMES[name]
     if not lib.mpgcn_bdgcn_precision_supported(B, N, K, C, H, code):
-        raise RuntimeError(f"precision {name!r} does not support B={B} N={N} K={K} C={C} H={H} (tensor path needs C == H == 32)")
+        raise RuntimeError(f"precision {name!r} does not support B={B} N={N} K={K} C={C} H={H} (tensor path needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024)")
     return code
 
 

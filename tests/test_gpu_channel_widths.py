@@ -1,0 +1,547 @@
+"""The tensor-core BDGCN layer (precision 1) at channel widths other than 32.
+
+Any C and H that are multiples of 32 run on the tensor cores, C != H included (the first layer of a branch has C =
+lstm_hidden_dim).  A "chunk" is 32 consecutive channels, cC = C / 32 and cH = H / 32: the N^3 contractions run once per chunk
+(they act on each channel on its own), the channel mixes see Kd*cC input and Ko*cH output planes, and BWD_DW tiles Kd*cC by
+Ko*cH chunks (DESIGN.md section 5).
+
+  * CPU: the oracle against fixtures of the unmodified reference (`tests/golden/wide_*`, tools/gen_golden_wide.py); which
+    shapes the tensor path accepts.
+  * GPU: every stage against float64 with the helpers and bounds of test_gpu_engine_stages.py, reading the chunk layouts back
+    from the workspaces; the layer against the fixtures and the factored oracle at size; the whole model at hidden 64; a row
+    shard.
+"""
+import math
+
+import numpy as np
+import pytest
+import torch
+from torch import nn
+
+import abi
+import test_gpu_at_size as at_size
+from conftest import golden_names, load_golden, record_parity
+from oracle import mpgcn_oracle as orc
+from oracle.gen_golden import layer_fixture
+from test_gpu_engine_stages import (Bound, Slope, _assert_and_record, _chunks, _garbage, bits, contract, dense_supports, diag_rule,
+                                    diag_supports, expected_scale, f16_sat, fwd_a_ref, fwd_b_ref, hilo, mix_ref)
+
+import MPGCN as shim
+from mpgcn_b200 import _lib, ops, shard
+from tools.gen_golden_wide import params_checksum, wide_model_params
+
+FIXTURE_TOL = 2e-5
+FWD_TOL = {"fp32": 5e-5, "fp16": 1e-3}
+BWD_TOL = {"fp32": 2e-4, "fp16": 2e-3}
+LOOSE_FP16_GRAD = 8e-2
+
+
+def _rel_check(a, ref, tol, what, l2_only=False):
+    a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a
+    ref = ref.detach().cpu().numpy() if isinstance(ref, torch.Tensor) else ref
+    linf, l2 = orc.rel_errors(a, ref)
+    record_parity(what, linf, l2, tol)
+    assert np.isfinite(linf) and l2 <= tol and (l2_only or linf <= tol), f"{what}: rel_Linf={linf:.3e} rel_L2={l2:.3e} > {tol}"
+    return linf, l2
+
+
+def _graph(g):
+    return (g["G_o"], g["G_d"]) if int(g["dynamic"]) else g["G"]
+
+
+def _model_params(g):
+    """The parameters of a wide model fixture, regenerated from its seed (tools/gen_golden_wide.py) and checked against the
+    stored checksum -> {state_dict key: float32 array}."""
+    hid, K, N = int(g["hidden"]), int(g["K"]), g["x_seq"].shape[2]
+    shapes = {k: v.shape for k, v in _model(N, K, hid, 0, "cpu").state_dict().items()}
+    params = wide_model_params(int(g["seed"]), shapes)
+    assert abs(float(params_checksum(params)) - float(g["params_checksum"])) < 1e-6, "numpy RNG stream changed: regenerate the fixture"
+    return params
+
+
+def _check_model_grads(grads, g, tol, what):
+    """Gradients against a wide model fixture: every BDGCN W gradient on the stored rows (`W_rows`) and in norm, every other
+    gradient in full."""
+    assert set(grads) == {k.split(":", 1)[1] for k in g if k.startswith(("grad:", "grad_rows:"))}
+    rows = g["W_rows"]
+    for k, v in grads.items():
+        v = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        if "grad_rows:" + k in g:
+            _rel_check(v[rows], g["grad_rows:" + k], tol, f"{what}/grad:{k} rows")
+            ref = float(g["grad_norm:" + k])
+            assert abs(float(np.linalg.norm(v.astype(np.float64))) - ref) <= tol * ref, f"{what}/grad:{k}: norm of the whole tensor"
+        else:
+            _rel_check(v, g["grad:" + k], tol, f"{what}/grad:{k}")
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# CPU
+# ------------------------------------------------------------------------------------------------------------------------------
+def test_wide_fixtures_exist_and_stay_out_of_the_other_sets():
+    layers, models = golden_names("wide_bdgcn_"), golden_names("wide_mpgcn_")
+    assert len(layers) == 4 and len(models) == 1
+    widths = {(int(load_golden(n)["C"]), int(load_golden(n)["H"])) for n in layers}
+    assert widths == {(64, 64), (64, 96), (32, 64), (128, 128)}
+    assert int(load_golden(models[0])["hidden"]) == 64
+    for prefix in ("bdgcn_", "big_bdgcn_", "many_bdgcn_", "mpgcn_"):
+        assert not set(layers + models) & set(golden_names(prefix))
+
+
+@pytest.mark.parametrize("name", golden_names("wide_bdgcn_"))
+def test_oracle_matches_reference_at_wide_channels(name):
+    g = layer_fixture(load_golden(name))
+    K, C, H = int(g["K"]), int(g["C"]), int(g["H"])
+    assert g["W"].shape == (K * K * C, H) and g["X"].shape[-1] == C
+    out = orc.bdgcn_forward(g["X"], _graph(g), g["W"], g["b"], "relu")
+    _rel_check(out, g["out"], FIXTURE_TOL, f"{name}: out")
+    dX, dW, db = orc.bdgcn_backward(g["X"], _graph(g), g["W"], g["b"], "relu", g["d_out"])
+    for a, k in ((dX, "dX"), (dW, "dW"), (db, "db")):
+        _rel_check(a, g[k], FIXTURE_TOL, f"{name}: {k}")
+    fac = orc.bdgcn_backward_factored(g["X"], _graph(g), g["W"], g["b"], "relu", g["d_out"])
+    for a, k in zip(fac, ("out", "dX", "dW", "db")):
+        _rel_check(a, g[k], FIXTURE_TOL, f"{name}: factored {k}")
+
+
+@pytest.mark.parametrize("name", golden_names("wide_mpgcn_"))
+def test_oracle_matches_reference_model_at_hidden_64(name):
+    g = load_golden(name)
+    y, grads = orc.mpgcn_forward_backward(_model_params(g), g["x_seq"], [g["G_static"], (g["G_o"], g["G_d"])], M=2, gcn_num_layers=3,
+                                          d_y=g["d_y"])
+    _rel_check(y, g["y"], FIXTURE_TOL, f"{name}: y")
+    _check_model_grads(grads, g, FIXTURE_TOL, name)
+
+
+@pytest.mark.parametrize("C,H,want", [(32, 32, 1), (64, 64, 1), (32, 64, 1), (64, 32, 1), (96, 128, 1), (256, 256, 1),
+                                      (16, 32, 0), (48, 48, 0), (64, 16, 0)])
+def test_tensor_path_accepts_multiples_of_32(C, H, want):
+    lib = _lib.load()
+    assert lib.mpgcn_bdgcn_precision_supported(2, 50, 3, C, H, 1) == want
+    assert ops.resolve_precision("auto", 2, 50, 3, C, H) == (_lib.PREC_FP16_TC if want else _lib.PREC_FP32)
+    if not want:
+        with pytest.raises(RuntimeError, match="multiples of 32"):
+            ops.resolve_precision("fp16", 2, 50, 3, C, H)
+
+
+def test_lstm_keeps_its_fp32_kernels_at_hidden_64():
+    lib = _lib.load()
+    assert lib.mpgcn_lstm_precision_supported(5, 64, 1) == 0 and lib.mpgcn_lstm_precision_supported(5, 64, 0) == 1
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# one layer through the C ABI at any width, the chunk layouts read back from the workspaces
+# ------------------------------------------------------------------------------------------------------------------------------
+def _offsets(parts):
+    """Byte offsets of consecutive 1024-byte aligned regions (bdgcn_tc.cu `take`) -> ({name: offset}, total)."""
+    off, res = 0, {}
+    for name, nbytes in parts:
+        off = (off + 1023) // 1024 * 1024
+        res[name] = off
+        off += nbytes
+    return res, (off + 1023) // 1024 * 1024
+
+
+def ws_layout(B, N, K, C, H, dyn, sms):
+    """The forward / backward workspace layouts of a whole layer (bdgcn_tc.cu fwd_layout / bwd_layout)."""
+    nz, Np = (B if dyn else 1), (N + 7) // 8 * 8
+    g16, rem = nz * K * N * Np * 2, nz * K * N * 4
+    fwd = _offsets([("x16", B * N * N * C * 2), ("gd16", g16), ("go16", g16), ("w16", 2 * K * K * C * H * 2), ("u16", B * K * N * N * H * 2),
+                    ("dd", rem), ("dgo", rem), ("dgo_masked", rem), ("z16", B * K * N * N * C * 2)])
+    rows, cols = K * C // 32, K * H // 32
+    total = B * -(-N * N // 64)
+    tiles = -(-rows // 4) * -(-cols // 8)
+    per = max(1, -(-total // max(1, sms // tiles)))
+    slices = -(-total // per)
+    bwd = _offsets([("dp16", B * N * N * H * 2), ("gd16", g16), ("go16", g16), ("v16", B * K * N * N * H * 2), ("y16", B * K * N * N * C * 2),
+                    ("wq16", K * K * C * H * 2), ("partials", slices * -(-rows // 4) * 128 * K * H * 4), ("scale", 64)])
+    return fwd, bwd
+
+
+def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn):
+    """fp16 forward + backward of one layer (ReLU) -> outputs and the intermediates in their logical layouts:
+    Z / Y [B][d][n][e][C], U / V [B][o][n][e][H], W16 [2][o][d][C][H], Wq16 [o][d][C][H]."""
+    lib = _lib.load()
+    dev = X.device
+    B, N, _, C = X.shape
+    K, H = Go.shape[-3], W.shape[1]
+    cC, cH = C // 32, H // 32
+    nz, Np = (B if dyn else 1), (N + 7) // 8 * 8
+    st = torch.cuda.current_stream().cuda_stream
+    (fo, ftot), (bo, btot) = ws_layout(B, N, K, C, H, dyn, torch.cuda.get_device_properties(dev).multi_processor_count)
+    assert ftot == lib.mpgcn_bdgcn_fwd_workspace_bytes(B, N, K, C, H, int(dyn), 1)
+    assert btot == lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, K, C, H, int(dyn), 1)
+    out = torch.full((B, N, N, H), math.nan, device=dev)
+    saved = _garbage(lib.mpgcn_bdgcn_saved_bytes(B, N, K, C, H, 1), dev)
+    ws = _garbage(ftot, dev)
+    _lib.check(lib.mpgcn_bdgcn_forward(X.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), bias.data_ptr(), 1, out.data_ptr(),
+                                       saved.data_ptr(), ws.data_ptr(), ws.numel(), B, N, K, C, H, 1, st), "forward")
+    r = dict(out=out)
+    if d_out is not None:
+        dX = torch.full((B, N, N, C), math.nan, device=dev)
+        dW = torch.full_like(W, math.nan)
+        db = torch.full((H,), math.nan, device=dev)
+        dx_amax = torch.full((1,), math.nan, device=dev)
+        wsb = _garbage(btot, dev)
+        _lib.check(lib.mpgcn_bdgcn_backward_ex(d_out.data_ptr(), out.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), 1,
+                                               saved.data_ptr(), dX.data_ptr(), dW.data_ptr(), db.data_ptr(), wsb.data_ptr(), wsb.numel(),
+                                               B, N, K, C, H, 1, None, dx_amax.data_ptr(), st), "backward_ex")
+        r.update(dX=dX, dW=dW, db=db, dx_amax=dx_amax)
+    torch.cuda.synchronize()
+
+    def h16(buf, o, *shape):
+        return buf[o:o + 2 * math.prod(shape)].view(torch.float16).view(*shape)
+
+    def f32(buf, o, *shape):
+        return buf[o:o + 4 * math.prod(shape)].view(torch.float32).view(*shape)
+
+    in_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, K, N, N, C)        # [B][d][lc][n][e][32] -> [B][d][n][e][C]
+    w16 = h16(ws, fo["w16"], 2, cH, K, K, cC, 32, 32).permute(0, 2, 3, 4, 5, 1, 6).reshape(2, K, K, C, H)
+    wq16 = h16(wsb, bo["wq16"], K, cC, K, cH, 32, 32).permute(2, 0, 1, 5, 3, 4).reshape(K, K, C, H) if d_out is not None else None
+    r.update(x16=h16(ws, fo["x16"], B, N, N, C), gd16=h16(ws, fo["gd16"], nz, K, N, Np), w16=w16,
+             u16=h16(ws, fo["u16"], B, cH, K, N, N, 32).permute(0, 2, 3, 4, 1, 5).reshape(B, K, N, N, H),
+             dd=f32(ws, fo["dd"], nz, K, N), z16=in_planes(saved.view(torch.float16).view(B, K, cC, N, N, 32)))
+    r["go16"], r["dgo"] = (h16(ws, fo["go16"], nz, K, N, Np), f32(ws, fo["dgo"], nz, K, N)) if dyn else (r["gd16"], r["dd"])
+    if d_out is not None:
+        r.update(dp16=h16(wsb, bo["dp16"], B, N, N, H), bgd16=h16(wsb, bo["gd16"], nz, K, N, Np),
+                 v16=h16(wsb, bo["v16"], B, K, cH, N, N, 32).permute(0, 1, 3, 4, 2, 5).reshape(B, K, N, N, H),
+                 y16=in_planes(h16(wsb, bo["y16"], B, K, cC, N, N, 32)), wq16=wq16, scale=f32(wsb, bo["scale"], 2))
+        r["bgo16"] = h16(wsb, bo["go16"], nz, K, N, Np) if dyn else r["bgd16"]
+    return r
+
+
+def check_stages_wide(r, X, Go, Gd, W, bias, d_out, dyn, kind):
+    """test_gpu_engine_stages.check_stages at any width: every stage of run_layer_wide's result against float64."""
+    B, N, _, C = X.shape
+    K, H = Go.shape[-3], W.shape[1]
+    nz = B if dyn else 1
+    Gd4, Go4 = Gd.view(nz, K, N, N), Go.view(nz, K, N, N)
+    W4 = W.view(K, K, C, H)
+    zb = (lambda b: b) if dyn else (lambda b: 0)
+    wf = (C + H) // 32                                    # memory budget of the float64 recomputation, in 32-channel units
+    res = {}
+
+    assert torch.equal(bits(r["x16"]), bits(f16_sat(X))), "x16"
+    for g16, G, what in ((r["gd16"], Gd4, "gd16"), (r["go16"], Go4, "go16")):
+        assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
+    hi, lo = hilo(W4)
+    assert torch.equal(bits(r["w16"][0]), bits(hi)) and torch.equal(bits(r["w16"][1]), bits(lo)), "w16 hi / lo in the mix's chunk order"
+    fired = 0
+    for name, G in (("dd", Gd4), ("dgo", Go4)):
+        want, near = diag_rule(G.reshape(nz * K, N, N).cpu().numpy())
+        got = r[name].reshape(nz * K, N).double().cpu().numpy()
+        assert not ((got != want) & ~near).any(), f"{name}: remainders differ from the tau = 1/16 rule"
+        fired = max(fired, int(np.count_nonzero(got)))
+    if kind == "diag":
+        assert fired >= 0.5 * nz * K * N, "the inputs were meant to make the remainder correction fire"
+
+    x16, gd16, go16 = r["x16"], r["gd16"][..., :N], r["go16"][..., :N]
+    dd, dgo, z16, u16, out = r["dd"], r["dgo"], r["z16"], r["u16"], r["out"]
+
+    bA, sA = Bound(N, True), Slope()
+    for b in range(B):
+        for d in range(K):
+            for ns in _chunks(N, N * 32 * wf):
+                base, corr, ab = fwd_a_ref(x16[b, ns], gd16[zb(b), d], dd[zb(b), d])
+                y = z16[b, d, ns]
+                bA.add(y, base + corr, ab)
+                sA.add(y.double() - base, corr)
+    res["FWD_A"], res["FWD_A remainder slope"] = bA, sA
+
+    bM, sM = Bound(2 * K * C, True), Slope()
+    for b in range(B):
+        for ns in _chunks(N, K * N * 32 * 4 * wf):
+            base, lpart, ab = mix_ref(z16[b, :, ns], hi, lo)
+            y = u16[b, :, ns]
+            bM.add(y, base + lpart, ab)
+            sM.add(y.double() - base, lpart)
+    res["FWD_MIX"], res["FWD_MIX lo slope"] = bM, sM
+
+    bB, sB = Bound(K * N + K + 1, False), Slope()
+    for b in range(B):
+        for es in _chunks(N, K * N * 32 * 4 * wf):
+            base, corr, ab = fwd_b_ref(go16[zb(b)], u16[b, :, :, es], dgo[zb(b)], bias)
+            y = out[b, :, es]
+            bB.add(y, torch.relu(base + corr), ab)
+            sB.add(y.double() - base, corr * (y > 0))
+    res["FWD_B"], res["FWD_B remainder slope"] = bB, sB
+    if d_out is None:
+        return res
+
+    amax = float(d_out.abs().max())
+    S, invS = expected_scale(amax)
+    assert (float(r["scale"][0]), float(r["scale"][1])) == (S, invS), "gradient scale"
+    d_pre = torch.where(out > 0, d_out, torch.zeros_like(d_out))
+    assert torch.equal(bits(r["dp16"]), bits(f16_sat(d_pre * S))), "dp16 != fp16_sat(dOut * [out > 0] * S)"
+    res["db"] = Bound(B * N * N, False).add(r["db"], d_pre.double().sum(dim=(0, 1, 2)), d_pre.double().abs().sum(dim=(0, 1, 2)))
+    for g16, G, what in ((r["bgd16"], Gd4, "backward gd16"), (r["bgo16"], Go4, "backward go16")):
+        assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
+    assert torch.equal(bits(r["wq16"]), bits(f16_sat(W4))), "wq16 != fp16(W) in the backward mix's chunk order"
+    wq = r["wq16"].permute(1, 0, 3, 2)                  # [d][o][h][c]
+    dp16, v16, y16 = r["dp16"], r["v16"], r["y16"]
+    bgd16, bgo16 = r["bgd16"][..., :N], r["bgo16"][..., :N]
+
+    bV = Bound(N, True)
+    for b in range(B):
+        for o in range(K):
+            for es in _chunks(N, N * 32 * 2 * wf):
+                ref, ab = contract("nm,meh->neh", bgo16[zb(b), o], dp16[b, :, es])
+                bV.add(v16[b, o, :, es], ref, ab)
+    res["BWD_V"] = bV
+
+    acc = torch.zeros(K, K, C, H, dtype=torch.float64, device=X.device)
+    aab = torch.zeros_like(acc)
+    for b in range(B):
+        for ns in _chunks(N, 2 * K * N * 32 * wf):
+            ref, ab = contract("dnel,oneh->odlh", z16[b, :, ns], v16[b, :, ns])
+            acc += ref
+            aab += ab
+    res["BWD_DW"] = Bound(B * N * N, False).add(r["dW"].view(K, K, C, H), acc * invS, aab * invS)
+
+    bY = Bound(H * K, True)
+    for b in range(B):
+        for ns in _chunks(N, 2 * K * N * 32 * wf):
+            ref, ab = contract("oneh,dohl->dnel", v16[b, :, ns], wq)
+            bY.add(y16[b, :, ns], ref, ab)
+    res["BWD_MIX"] = bY
+
+    bX = Bound(K * N, False)
+    for b in range(B):
+        for ns in _chunks(N, 2 * K * N * 32 * wf):
+            ref, ab = contract("dnel,dce->ncl", y16[b, :, ns], bgd16[zb(b)])
+            bX.add(r["dX"][b, ns], ref * invS, ab * invS)
+    res["BWD_DX"] = bX
+    assert float(r["dx_amax"][0]) == float(r["dX"].abs().max()), "dX_absmax hint != max|dX| over every chunk"
+    return res
+
+
+def _make_cases():
+    rows = []          # (C, H, N, K, B, dyn, kind, grad)
+    shapes = ([(C, H, 130, 3, 2, None) for C, H in ((64, 64), (32, 64), (64, 32), (96, 128), (128, 128))]
+              + [(64, 64, 130, K, 2, None) for K in (1, 9)]             # K = 9: 18 mix output planes in three groups
+              + [(64, 64, N, 3, 2, None) for N in (1, 65, 257)]         # tile edges
+              + [(32, 64, 65, 1, 2, None),                              # backward mix: 2 input planes in one k-block
+                 (64, 32, 65, 1, 2, None),                              # forward mix: the same
+                 (96, 128, 257, 1, 1, None),                            # 3 input planes in one k-block
+                 (128, 128, 1, 3, 2, None)]
+              + [(96, 128, 65, 9, 2, False),                            # 27 -> 36 planes: five mix groups, 7 x 5 dW tiles, W streamed
+                 (128, 128, 130, 9, 1, True),
+                 (64, 64, 257, 9, 3, True)])                            # odd batch
+    for i, (C, H, N, K, B, only) in enumerate(shapes):
+        for dyn in ((False, True) if only is None else (only,)):
+            kind = "diag" if (i + dyn) % 2 == 0 else "dense"
+            grad = 1e4 if (i + 2 * dyn) % 3 == 1 else 1e-5
+            rows.append((C, H, N, K, B, dyn, kind, grad))
+    return rows
+
+
+CASES = _make_cases()
+
+
+def test_stage_cases_cover_every_width_k_n_kind_and_scale():
+    assert {(c[0], c[1]) for c in CASES} == {(64, 64), (32, 64), (64, 32), (96, 128), (128, 128)}
+    assert {c[3] for c in CASES} == {1, 3, 9} and {c[2] for c in CASES} >= {1, 65, 130, 257}
+    assert {c[5] for c in CASES} == {False, True} and {c[6] for c in CASES} == {"diag", "dense"} and {c[7] for c in CASES} == {1e-5, 1e4}
+    for C, H in {(c[0], c[1]) for c in CASES}:
+        rows = [c for c in CASES if (c[0], c[1]) == (C, H)]
+        assert {c[5] for c in rows} == {False, True}, (C, H)
+
+
+def _inputs(C, H, N, K, B, dyn, kind, seed, dev):
+    rng = np.random.default_rng(seed)
+    nz = B if dyn else 1
+    mk = (lambda: diag_supports(rng, nz * K, N)) if kind == "diag" else (lambda: dense_supports(rng, nz * K, N))
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    X = t(np.tanh(rng.standard_normal((B, N, N, C))).astype(np.float32))
+    Gd = t(mk().reshape((B, K, N, N) if dyn else (K, N, N)))
+    Go = t(mk().reshape((B, K, N, N))) if dyn else Gd
+    W = t((rng.standard_normal((K * K * C, H)) * (2.0 / (K * K * C + H)) ** 0.5).astype(np.float32))
+    bias = t((rng.standard_normal(H) * 0.1).astype(np.float32))
+    return X, Go, Gd, W, bias
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("C,H,N,K,B,dyn,kind,grad", CASES)
+def test_every_stage_matches_float64_at_wide_channels(C, H, N, K, B, dyn, kind, grad, cuda_device):
+    X, Go, Gd, W, bias = _inputs(C, H, N, K, B, dyn, kind, 7919 * N + 31 * K + 2 * B + dyn + 3 * C + 5 * H, cuda_device)
+    d_out = torch.randn(B, N, N, H, device=cuda_device, generator=torch.Generator(cuda_device).manual_seed(N + K + C + H)) * grad
+    r = run_layer_wide(X, Go, Gd, W, bias, d_out, dyn)
+    tag = f"C={C} H={H} N={N} K={K} B={B} {'dyn' if dyn else 'static'}/{kind} |dOut|~{grad:g}"
+    _assert_and_record(check_stages_wide(r, X, Go, Gd, W, bias, d_out, dyn, kind), tag)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# GPU: end to end
+# ------------------------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", golden_names("wide_bdgcn_"))
+def test_layer_matches_reference_fixture_at_wide_channels(name, cuda_device):
+    g = layer_fixture(load_golden(name))
+    X, G, W, b, d_out = g["X"], _graph(g), g["W"], g["b"], g["d_out"]
+    for prec in ("fp32", "fp16"):
+        out, dX, dW, db = at_size._run_layer(X, G, W, b, d_out, prec, cuda_device)
+        _rel_check(out, g["out"], FWD_TOL[prec], f"{name}/{prec}/out vs reference")
+        if prec == "fp32":
+            for a, k in ((dX, "dX"), (dW, "dW"), (db, "db")):
+                _rel_check(a, g[k], BWD_TOL[prec], f"{name}/{prec}/{k} vs reference")
+        else:
+            f64 = lambda a: a.astype(np.float64)
+            refs = orc.bdgcn_backward_factored(f64(X), tuple(f64(a) for a in G) if isinstance(G, tuple) else f64(G), f64(W), f64(b), "relu",
+                                               f64(d_out), mask_from=out)[1:]
+            for a, ref, k in zip((dX, dW, db), refs, ("dX", "dW", "db")):
+                _rel_check(a, ref, BWD_TOL[prec], f"{name}/{prec}/{k} (engine mask)")
+                _rel_check(a, g[k], LOOSE_FP16_GRAD, f"{name}/{prec}/{k} vs reference", l2_only=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("N,dyn,kind", [(500, False, "rw"), (1000, True, "dense")])
+def test_layer_matches_oracle_at_size_at_64_channels(N, dyn, kind, cuda_device):
+    """test_gpu_at_size.test_layer_matches_oracle_at_size at C = H = 64, K = 3, B = 1: forward <= 1e-3 and every gradient <= 2e-3
+    against the factored oracle on the engine's ReLU mask, both kernel families."""
+    K, B, C = 3, 1, 64
+    rng = np.random.default_rng(1000 * N + 64 + dyn)
+    X = np.tanh(rng.standard_normal((B, N, N, C))).astype(np.float32)
+    G = (at_size._supports(rng, kind, K, N, B), at_size._supports(rng, kind, K, N, B)) if dyn else at_size._supports(rng, kind, K, N, 0)
+    W = (rng.standard_normal((K * K * C, C)) * (2.0 / (K * K * C + C)) ** 0.5).astype(np.float32)
+    b = (rng.standard_normal(C) * 0.1).astype(np.float32)
+    d_out = (rng.standard_normal((B, N, N, C)) * 1e-5).astype(np.float32)
+    out_o = orc.bdgcn_backward_factored(X, G, W, b, "relu", d_out)[0]
+    tag = f"layer C=H=64 N={N} K={K} {'dyn' if dyn else 'static'}/{kind}"
+    for prec in ("fp32", "fp16"):
+        out, dX, dW, db = at_size._run_layer(X, G, W, b, d_out, prec, cuda_device)
+        _rel_check(out, out_o, FWD_TOL[prec], f"{tag}/{prec}/out vs oracle")
+        refs = orc.bdgcn_backward_factored(X, G, W, b, "relu", d_out, mask_from=out)[1:]
+        for a, r, what in zip((dX, dW, db), refs, ("dX", "dW", "db")):
+            _rel_check(a, r, BWD_TOL[prec], f"{tag}/{prec}/{what} (engine mask)")
+
+
+def _model(N, K, hid, seed, dev):
+    torch.manual_seed(seed)
+    return shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=3, num_nodes=N,
+                      user_bias=True, activation=nn.ReLU).to(dev)
+
+
+def _set_layer_precision(model, prec):
+    """BDGCN layers on `prec`; the LSTM on its fp32 kernels (the tensor-core LSTM is hidden-32 only)."""
+    model.lstm_precision = "fp32"
+    for mod in model.modules():
+        if isinstance(mod, shim.BDGCN):
+            mod.precision = prec
+
+
+def _run_model(model, x_seq, G_list, d_y, prec):
+    _set_layer_precision(model, prec)
+    model.zero_grad(set_to_none=True)
+    y = model(x_seq=x_seq, G_list=G_list)
+    y.backward(d_y)
+    torch.cuda.synchronize()
+    return y.detach().clone(), {k: p.grad.detach().clone() for k, p in model.named_parameters()}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", golden_names("wide_mpgcn_"))
+def test_model_at_hidden_64_matches_reference_fixture(name, cuda_device):
+    """The whole model at hidden 64 (every BDGCN layer is 64 -> 64) against the reference: fp32 layers to 5e-5 / 2e-4 (as
+    test_gpu_parity.py; BDGCN W gradients on the fixture's rows and in norm); fp16 layers to 1e-3 in rel_L2 forward (its
+    rel_Linf recorded) and to 5e-3 in rel_L2 against the oracle's gradients on the engine's ReLU masks."""
+    g = load_golden(name)
+    K, hid = int(g["K"]), int(g["hidden"])
+    N = g["x_seq"].shape[2]
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda_device)
+    G_list = [t(g["G_static"]), (t(g["G_o"]), t(g["G_d"]))]
+    params = _model_params(g)
+    for prec in ("fp32", "fp16"):
+        model = _model(N, K, hid, 0, "cpu")
+        model.load_state_dict({k: torch.from_numpy(v) for k, v in params.items()})
+        model = model.to(cuda_device)
+        caps = {m: {"layers": [], "fc": None} for m in range(2)}
+        hooks = [layer.register_forward_hook(lambda mod, inp, out, m=m: caps[m]["layers"].append(out.detach().cpu().numpy()))
+                 for m in range(2) for layer in model.branch_models[m]['spatial']]
+        y, grads = _run_model(model, t(g["x_seq"]), G_list, t(g["d_y"]), prec)
+        for h in hooks:
+            h.remove()
+        if prec == "fp32":
+            _rel_check(y, g["y"], 5e-5, f"{name}/{prec}/y")
+            _check_model_grads(grads, g, 2e-4, f"{name}/{prec}")
+        else:
+            _rel_check(y, g["y"], FWD_TOL[prec], f"{name}/{prec}/y", l2_only=True)
+            for m in range(2):
+                fc = model.branch_models[m]['fc'][0]
+                caps[m]["fc"] = orc.fc_relu_forward(caps[m]["layers"][-1], fc.weight.detach().cpu().numpy(), fc.bias.detach().cpu().numpy())
+            _, grads_m = orc.mpgcn_forward_backward(params, g["x_seq"], [g["G_static"], (g["G_o"], g["G_d"])], M=2, gcn_num_layers=3,
+                                                    d_y=g["d_y"], masks=caps)
+            for k, v in grads.items():
+                _rel_check(v, grads_m[k], 5e-3, f"{name}/{prec}/grad:{k} (engine masks)", l2_only=True)
+
+
+@pytest.mark.gpu
+def test_model_at_hidden_64_fp16_matches_fp32(cuda_device):
+    """The whole model at hidden 64, N = 60, K = 3, static and dynamic graphs: the tensor-core layers against the fp32 layers.
+    The forward is bounded in rel_L2 (1e-3) and its rel_Linf recorded, as in test_gpu_many_supports.py; gradients to 8e-2 in
+    rel_L2 (another forward's ReLU mask).  The first seed whose fp32 run gives every parameter a gradient is used."""
+    dev = cuda_device
+    N, T, B, K = 60, 4, 2, 3
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    for seed in range(64, 2000, 100):
+        rng = np.random.default_rng(seed)
+        G_list = [t(at_size._supports(rng, "rw", K, N, 0)), (t(at_size._supports(rng, "rw", K, N, B)), t(at_size._supports(rng, "rw", K, N, B)))]
+        model = _model(N, K, 64, seed, dev)
+        x_seq = t((rng.random((B, T, N, N, 1)) * 8).astype(np.float32))
+        d_y = t(rng.standard_normal((B, 1, N, N, 1)).astype(np.float32))
+        y32, g32 = _run_model(model, x_seq, G_list, d_y, "fp32")
+        if all(float(g.abs().max()) > 0 for g in g32.values()):
+            break
+    else:
+        pytest.fail("no seed gives both branches a gradient")
+    y16, g16 = _run_model(model, x_seq, G_list, d_y, "fp16")
+    _rel_check(y16, y32, FWD_TOL["fp16"], f"model hidden 64 (seed {seed}): fp16 y vs fp32", l2_only=True)
+    for k, g in g32.items():
+        _rel_check(g16[k], g, LOOSE_FP16_GRAD, f"model hidden 64: fp16 grad:{k} vs fp32", l2_only=True)
+
+
+@pytest.mark.gpu
+def test_model_at_hidden_64_no_grad_allocates_no_stash_and_graph_rollout_equals_eager(cuda_device):
+    """Under torch.no_grad() the hidden-64 model keeps no Z stash (nor any other training state); the CUDA-graph rollout of
+    Model_Trainer.test's loop equals the eager loop bitwise."""
+    from mpgcn_b200 import rollout
+    dev = cuda_device
+    N, K, B, T, P = 47, 3, 2, 5, 3
+    model = _model(N, K, 64, 3, dev)
+    _set_layer_precision(model, "auto")
+    assert ops.resolve_precision("auto", B, N, K, 64, 64) == _lib.PREC_FP16_TC
+    G = torch.rand(K, N, N, device=dev) / N
+    dyn = (torch.rand(B, K, N, N, device=dev) / N, torch.rand(B, K, N, N, device=dev) / N)
+    x = torch.rand(B, T, N, N, 1, device=dev) * 8
+    ops.STASH_BYTES.clear()
+    with torch.no_grad():
+        y0 = model(x_seq=x, G_list=[G, dyn])
+    assert sum(ops.STASH_BYTES.values()) == 0, dict(ops.STASH_BYTES)
+    y1 = model(x_seq=x, G_list=[G, dyn])
+    assert ops.STASH_BYTES["bdgcn"] > 0 and torch.equal(y0, y1.detach())
+    eager = rollout.forecast(model, x, [G, dyn], P, use_cuda_graph=False)
+    graphed = rollout.forecast(model, x, [G, dyn], P, use_cuda_graph=True)
+    assert tuple(graphed.shape) == (B, P, N, N, 1)
+    assert torch.equal(eager, graphed)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("N,dyn", [(130, False), (258, True)])
+def test_row_shard_at_64_channels_sums_to_the_whole_layer(N, dyn, cuda_device):
+    """Row shard over 2 ranks at C = H = 64 on supports whose diagonal remainders fire: the fp16 partial pre-activations summed
+    equal the fp16 whole layer to 1e-5 (as test_gpu_shard.py at 32 channels)."""
+    dev = cuda_device
+    rng = np.random.default_rng(N + 64)
+    B, K, C, world = 2, 3, 64, 2
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    X = t(np.tanh(rng.standard_normal((B, N, N, C))).astype(np.float32))
+    shape = (B, K, N, N) if dyn else (K, N, N)
+    Gd = t(diag_supports(rng, (B if dyn else 1) * K, N).reshape(shape))
+    Go = t(diag_supports(rng, B * K, N).reshape(shape)) if dyn else Gd
+    W = t((rng.standard_normal((K * K * C, C)) * (2.0 / (K * K * C + C)) ** 0.5).astype(np.float32))
+    assert ops.resolve_precision("auto", B, N, K, C, C) == _lib.PREC_FP16_TC
+    cuda = shard.CudaEngine()
+    total = torch.zeros(B, N, N, C, dtype=torch.float64, device=dev)
+    for r in range(world):
+        plan = shard.ShardPlan("row", r, world, N, K)
+        pre, _ = cuda.forward_part(X[:, plan.row_lo:plan.row_hi].contiguous(), Go, Gd, dyn, W, N, plan.row_lo, K, K, 1, False)
+        total += pre.double()
+    whole, _ = abi.forward(X, Go, Gd, W, torch.zeros(C, device=dev), False, "fp16", want_saved=False)
+    _rel_check(total, whole.double(), 1e-5, f"row shard C=H=64 N={N} x{world} {'dyn' if dyn else 'static'}/diag fp16: sum of partials == whole")
