@@ -172,8 +172,8 @@ MPGCN_API int mpgcn_absmax(const float* x, long long n, float* out, void* stream
  *   w_ih [4C,1], w_hh [4C,C], b_ih [4C], b_hh [4C]   (gate order i,f,g,o)
  *   hT   [B*NN, C]
  * precision 0: fp32 CUDA-core kernels (C <= 64); precision 1: tensor-core gate GEMM with the recurrent h rounded to
- * fp16 as MMA operand, state and activations in fp32 (C == 32); x enters that GEMM as an fp16 hi + lo pair, exact to
- * ~22 bits for |x| < 65504 and saturating beyond. */
+ * fp16 as MMA operand, state and activations in fp32 (C = 32, 96 or 128; 1 <= T <= 256); x enters that GEMM as an fp16
+ * hi + lo pair, exact to ~22 bits for |x| < 65504 and saturating beyond. */
 MPGCN_API int mpgcn_lstm_precision_supported(int T, int C, int precision);
 MPGCN_API size_t mpgcn_lstm_bwd_workspace_bytes(int B, int T, long long NN, int C, int precision);
 MPGCN_API int mpgcn_lstm_last_forward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
@@ -203,8 +203,10 @@ MPGCN_API int mpgcn_lstm_last_backward_ex(const float* x_seq, const float* w_ih,
  * loss.backward(), Model_Trainer.py:114).  The forward additionally writes c_t and h_t of every step (fp16) into `saved`
  * (mpgcn_lstm_saved_bytes; 0 for precision 0, whose backward recomputes; 16-byte aligned; NULL = plain inference forward);
  * the backward walks that buffer once in reverse.  With saved == NULL the backward is mpgcn_lstm_last_backward_ex: it first
- * rebuilds that state in its workspace (mpgcn_lstm_bwd_workspace_bytes = 1 KB + the saved size); with saved != NULL the
- * workspace only needs 1024 bytes. */
+ * rebuilds that state in its workspace (mpgcn_lstm_bwd_workspace_bytes includes the saved size); with saved != NULL the
+ * workspace needs mpgcn_lstm_bwd_workspace_bytes - mpgcn_lstm_saved_bytes bytes: 1024 at C = 32, and at C = 96, 128 also
+ * the fp16 gate gradients of every cell and step (4C halves each), which a separate pass reduces to d_w_*.  The saved state
+ * takes 2C halves per cell and step (C = 32: 128-cell tiles; 96: 64-cell; 128: 48-cell). */
 MPGCN_API size_t mpgcn_lstm_saved_bytes(int B, int T, long long NN, int C, int precision);
 MPGCN_API int mpgcn_lstm_last_forward_train(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                                   float* hT, void* saved, size_t saved_bytes, int B, int T, long long NN, int C, int precision,

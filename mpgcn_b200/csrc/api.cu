@@ -281,14 +281,15 @@ int mpgcn_lstm_precision_supported(int T, int C, int precision) {
   return 0;
 }
 
+// sizes for the width of the tensor-core kernel; a width it does not run keeps the hidden-32 size these always returned
+static int lstm_tc_size_width(int C) { return lstm_tc_supported(1, C) ? C : 32; }
+
 size_t mpgcn_lstm_bwd_workspace_bytes(int B, int T, long long NN, int C, int precision) {
-  (void)C;
-  return precision == PREC_FP16_TC ? lstm_tc_bwd_workspace_bytes(B, T, NN) : 256;
+  return precision == PREC_FP16_TC ? lstm_tc_bwd_workspace_bytes(B, T, NN, lstm_tc_size_width(C)) : 256;
 }
 
 size_t mpgcn_lstm_saved_bytes(int B, int T, long long NN, int C, int precision) {
-  (void)C;
-  return precision == PREC_FP16_TC ? lstm_tc_saved_bytes(B, T, NN) : 0;
+  return precision == PREC_FP16_TC ? lstm_tc_saved_bytes(B, T, NN, lstm_tc_size_width(C)) : 0;
 }
 
 int mpgcn_lstm_last_forward_train(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
@@ -298,9 +299,9 @@ int mpgcn_lstm_last_forward_train(const float* x_seq, const float* w_ih, const f
   MPGCN_CHECK(mpgcn_lstm_precision_supported(T, C, precision), "lstm: precision %d does not support T=%d, hidden=%d", precision, T, C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (precision == PREC_FP16_TC) {
-    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN), "lstm forward: saved buffer too small (%zu < %zu)",
-                saved_bytes, lstm_tc_saved_bytes(B, T, NN));
-    return lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, B, T, NN, st);
+    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN, C), "lstm forward: saved buffer too small (%zu < %zu)",
+                saved_bytes, lstm_tc_saved_bytes(B, T, NN, C));
+    return lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, B, T, NN, C, st);
   }
   return lstm_last_forward(x_seq, w_ih, w_hh, b_ih, b_hh, hT, B, T, NN, C, st);
 }
@@ -340,9 +341,9 @@ int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const 
   MPGCN_CHECK(mpgcn_lstm_precision_supported(T, C, precision), "lstm: precision %d does not support T=%d, hidden=%d", precision, T, C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (precision == PREC_FP16_TC) {
-    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN), "lstm backward: saved buffer too small (%zu < %zu)",
-                saved_bytes, lstm_tc_saved_bytes(B, T, NN));
-    return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, workspace,
+    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN, C), "lstm backward: saved buffer too small (%zu < %zu)",
+                saved_bytes, lstm_tc_saved_bytes(B, T, NN, C));
+    return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, C, workspace,
                                  workspace_bytes, d_hT_absmax, st);
   }
   return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st);

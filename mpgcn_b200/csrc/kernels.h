@@ -99,16 +99,16 @@ int adj_process(const float* flow, float* supports, int B, int N, int kernel_typ
 size_t dyn_graph_workspace_bytes(int P, int N);
 int dyn_graph_build(const float* od_hist, int periods, float* o_g, float* d_g, int P, int N, void* ws, size_t ws_bytes, cudaStream_t st);
 
-// tensor-core LSTM (lstm_tc.cu): hidden size 32 only
+// tensor-core LSTM (lstm_tc.cu): hidden size C = 32, 96, 128
 bool lstm_tc_supported(int T, int C);
-size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN);
-size_t lstm_tc_saved_bytes(int B, int T, long long NN);
+size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C);
+size_t lstm_tc_saved_bytes(int B, int T, long long NN, int C);
 // saved (nullable): training state c_t, h_t written by the forward; the backward walks it instead of recomputing the forward
 int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                         void* saved, int B, int T, long long NN, cudaStream_t s);
+                         void* saved, int B, int T, long long NN, int C, cudaStream_t s);
 int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                           const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
-                          int B, int T, long long NN, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t s);
+                          int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t s);
 
 // ---- BDGCN layer orchestration ---------------------------------------------------------------
 struct BdgcnShape {

@@ -409,30 +409,551 @@ __global__ void copy_vec_kernel(const float* src, float* dst, int n) {
 
 }  // namespace lstm_tc
 
+// =======================================================================================
+// Hidden sizes H = 32 cH (cH = 3, 4: H = 96, 128).  Same semantics and numerics as above (fp16 hi + lo x and affine part,
+// h_{t-1} rounded to fp16 only as MMA operand, fp32 c / gate arguments / h_T, 7 SFU operations per unit and step,
+// power-of-two scaling of d_hT).  What changes with the width:
+//   * a warp owns 16 cells x one 32-unit slice of all four gates (128 gate columns, 64 fp32 accumulators per thread, the
+//     cell update thread-local as above); the cH warps of a 16-cell group exchange h_t through shared memory once per step
+//     (one named barrier per group and step).  A tile is CG groups (Dims::CG: 64 cells at H = 96, 48 at H = 128), CG * cH
+//     warps per CTA, one CTA per SM (the gate weights take 4H x (H + 24) halves of shared memory: 152 KB at H = 128).
+//   * Wx rows are kept in slice order r = 128 js + 32 gate + u (gate row j = gate H + 32 js + u), so a warp's B operand is
+//     one contiguous block of 128 rows, exactly as in the hidden-32 kernel.
+//   * backward: dWext [4H x (H + 16)] no longer fits a CTA's registers (74 K fp32 at H = 128).  The reverse walk writes the
+//     scaled fp16 gate gradients of every (tile, step) to the workspace and a separate tensor-core pass reduces
+//     dWext = sum da^T hx over cells and steps, reading h_{t-1} from the saved state.  The workspace is as large as twice the
+//     saved state; tiling the reduction inside the walk would need either 74 K fp32 of shared memory or a read-modify-write of
+//     a per-CTA fp32 partial every step.  dh_{t-1} = da_t W_hh reads W_hh from the same shared Wx block (ldmatrix.trans),
+//     since a transposed copy does not fit beside it; da_t is divided by the row scale s_j before it is rounded to fp16
+//     and the weight-gradient pass multiplies s_j back.
+// =======================================================================================
+namespace lstm_tcw {
+
+using lstm_tc::ex2_;
+using lstm_tc::rcp_;
+using lstm_tc::pack2;
+using lstm_tc::pack8;
+using lstm_tc::unpack8;
+using lstm_tc::x_base;
+using lstm_tc::x_cols;
+
+constexpr float kLn2 = 0.69314718055994531f;
+
+template <int CH>
+struct Dims {
+  // 16-cell groups per tile: 4 at H = 96 (12 warps, <= 168 registers per thread), 3 at H = 128 (12 warps; 16 warps would cap a
+  // thread at 128 registers, which the backward walk exceeds)
+  static constexpr int CG = CH == 4 ? 3 : 4;
+  static constexpr int CELLS = 16 * CG;
+  static constexpr int H = 32 * CH;
+  static constexpr int G4 = 4 * H;
+  static constexpr int KX = H + 16;            // operand row of a cell: h_{t-1} (H) | x columns (16, see lstm_tc::load_wx)
+  static constexpr int WX_LD = KX + 8;         // padded so that 8 consecutive rows fall in distinct 16-byte bank groups
+  static constexpr int H_LD = H + 8;           // h exchange tile row stride
+  static constexpr int DA_LD = G4 + 8;         // da tile row stride
+  static constexpr int NW = CG * CH;           // warps per CTA
+  static constexpr int THREADS = 32 * NW;
+  static constexpr int TILE_HALVES = CELLS * H * 2;     // saved c_t | h_t per (tile, step)
+  static constexpr size_t kFwdSmem = (size_t)(G4 * WX_LD + 2 * CELLS * H_LD) * sizeof(__half);
+  static constexpr size_t kBwdSmem = (size_t)(G4 * WX_LD + CELLS * DA_LD) * sizeof(__half) + (size_t)(CELLS * CH + G4) * sizeof(float);
+};
+
+// gate row j of slice-ordered row r (see above)
+template <int CH>
+__device__ __forceinline__ int gate_row(int r) { return (r & 127) / 32 * (32 * CH) + 32 * (r >> 7) + (r & 31); }
+__device__ __forceinline__ float row_scale(int r) { return ((r & 127) >> 5) == 2 ? -2.8853900817779268f : -1.4426950408889634f; }
+
+// Wx[r][k] = s_j * [ W_hh[j,:] | wih_hi  b_hi  wih_hi  wih_lo  b_lo  0 0 0 | 0 .. ], j = gate_row(r): lstm_tc::load_wx at width H
+template <int CH>
+__device__ void load_wx_w(__half* sWx, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh) {
+  using D = Dims<CH>;
+  constexpr int NCH = D::KX / 8;
+  for (int e = threadIdx.x; e < D::G4 * NCH; e += blockDim.x) {
+    const int r = e / NCH, ch = e % NCH, j = gate_row<CH>(r);
+    const float sc = row_scale(r);
+    float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (ch < D::H / 8) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = sc * w_hh[(size_t)j * D::H + ch * 8 + i];
+    } else if (ch == D::H / 8) {
+      const float wi = sc * w_ih[j], bb = sc * (b_ih[j] + b_hh[j]);
+      const float wi_hi = __half2float(__float2half_rn(wi)), b_hi = __half2float(__float2half_rn(bb));
+      v[0] = wi_hi; v[1] = b_hi; v[2] = wi_hi; v[3] = wi - wi_hi; v[4] = bb - b_hi;
+    }
+    *reinterpret_cast<uint4*>(sWx + r * D::WX_LD + ch * 8) = pack8(v);
+  }
+}
+
+// acc[nt] (nt = gate * 4 + jn) += hx_t . Wx^T for the warp's 16 cells and 128 gate columns.  a_h(kb, a) supplies the A fragment
+// of h-block kb < 2 cH; xw[h] are the x columns of row h (k-block 2 cH).  wx_addr: first of the warp's 128 Wx rows.
+template <int CH, class AH>
+__device__ __forceinline__ void gate_mma_w(float (&acc)[16][4], AH&& a_h, const uint32_t (&xw)[2], uint32_t wx_addr) {
+  using D = Dims<CH>;
+  const int lane = threadIdx.x & 31, mi = lane >> 3;
+#pragma unroll
+  for (int nt = 0; nt < 16; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+#pragma unroll
+  for (int kb = 0; kb <= 2 * CH; ++kb) {
+    uint32_t a[4];
+    if (kb < 2 * CH) a_h(kb, a);
+    else { a[0] = xw[0]; a[1] = xw[1]; a[2] = 0u; a[3] = 0u; }
+#pragma unroll
+    for (int pr = 0; pr < 8; ++pr) {
+      uint32_t b0, b1, b2, b3;
+      ldmatrix_x4(wx_addr + (uint32_t)(((16 * pr + 8 * (mi >> 1) + (lane & 7)) * D::WX_LD + 16 * kb + 8 * (mi & 1)) * 2), b0, b1, b2, b3);
+      mma_16816(acc[2 * pr], a, b0, b1);
+      mma_16816(acc[2 * pr + 1], a, b2, b3);
+    }
+  }
+}
+
+// Training state: per (tile, step) NW x 1024 halves, [warp][c | h][lane][16 halves] as in lstm_tc::save_off; warp = cg cH + js.
+template <int CH>
+__device__ __forceinline__ size_t save_off_w(long long tile, int T, int t, int warp, int kind, int lane) {
+  return ((size_t)tile * T + t) * Dims<CH>::TILE_HALVES + (size_t)warp * 1024 + (size_t)kind * 512 + (size_t)lane * 16;
+}
+
+// ---------------------------------------------------------------------------------------
+// forward
+// ---------------------------------------------------------------------------------------
+template <int CH, bool SAVE>
+__global__ void __launch_bounds__(Dims<CH>::THREADS, 1)
+lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
+                    const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
+                    long long cells, int T, long long NN) {
+  using D = Dims<CH>;
+  constexpr int CELLS = D::CELLS;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [G4][WX_LD], slice order
+  __half* sH = sWx + D::G4 * D::WX_LD;                     // 2 x [CELLS][H_LD]: h_t of the tile, double-buffered by step
+  load_wx_w<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const int cg = warp / CH, js = warp % CH;
+  const uint32_t wx_addr = smem_u32(sWx + js * 128 * D::WX_LD);
+  // this lane's ldmatrix row address in the h tile: row 16 cg + (lane & 15), column 8 (lane >> 4)
+  const uint32_t h_addr = smem_u32(sH + (cg * 16 + (lane & 15)) * D::H_LD + 8 * (lane >> 4));
+  const long long tiles = (cells + CELLS - 1) / CELLS;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    long long cell[2];
+    bool live[2];
+    size_t xb[2];
+    float xv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      cell[h] = tile * CELLS + cg * 16 + g + 8 * h;
+      live[h] = cell[h] < cells;
+      xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
+      xv[h] = live[h] ? x_seq[xb[h]] : 0.f;
+    }
+    float c[2][8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int s = 0; s < 8; ++s) c[h][s] = 0.f;
+    for (int t = 0; t < T; ++t) {
+      uint32_t xw[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) xw[h] = x_cols(xv[h], q);
+      // h_{t-1} was written to buffer t & 1 before the previous step's barrier; zero before the first step
+      const uint32_t hb = h_addr + (uint32_t)((t & 1) * CELLS * D::H_LD * 2);
+      float acc[16][4];
+      gate_mma_w<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
+        if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; }
+        else ldmatrix_x4(hb + 32 * kb, a[0], a[1], a[2], a[3]);
+      }, xw, wx_addr);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) xv[h] = (live[h] && t + 1 < T) ? x_seq[xb[h] + (size_t)(t + 1) * NN] : 0.f;
+      float hv[2][8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int s = 0; s < 8; ++s) {        // the hidden-32 cell update, see lstm_tc::lstm_fwd_tc_kernel
+          const int jn = s >> 1, k = 2 * h + (s & 1);
+          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
+          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
+          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
+          const float p = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
+          const float pig = ai * ag;
+          const float r = rcp_(pig * af);
+          const float gi = r * (ag * af);
+          const float gg = fmaf(r + r, ai * af, -1.f);
+          const float gf = r * pig;
+          c[h][s] = fmaf(gf, c[h][s], gi * gg);
+          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * c[h][s], 40.f));
+          const float r2 = rcp_(p * ac);
+          hv[h][s] = (r2 * ac) * fmaf(r2 + r2, p, -1.f);
+        }
+      }
+      if (SAVE) {
+        uint4* dc = reinterpret_cast<uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 0, lane));
+        uint4* dh = reinterpret_cast<uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 1, lane));
+        dc[0] = pack8(c[0]); dc[1] = pack8(c[1]);
+        dh[0] = pack8(hv[0]); dh[1] = pack8(hv[1]);
+      }
+      if (t + 1 < T) {
+        __half* sh = sH + ((t + 1) & 1) * CELLS * D::H_LD;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int jn = 0; jn < 4; ++jn)
+            *reinterpret_cast<uint32_t*>(sh + (cg * 16 + g + 8 * h) * D::H_LD + 32 * js + 8 * jn + 2 * q) = pack2(hv[h][2 * jn], hv[h][2 * jn + 1]);
+      } else if (hT != nullptr) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (live[h]) {
+#pragma unroll
+            for (int jn = 0; jn < 4; ++jn)
+              *reinterpret_cast<float2*>(hT + (size_t)cell[h] * D::H + 32 * js + 8 * jn + 2 * q) = make_float2(hv[h][2 * jn], hv[h][2 * jn + 1]);
+          }
+      }
+      // h_t is complete for the group; buffer (t + 1) & 1 is not written again before every warp has passed the next barrier
+      named_bar_sync(1 + cg, 32 * CH);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// backward from the saved c_t / h_t: reverse walk (dh, dc, dx and the gate gradients) ...
+// ---------------------------------------------------------------------------------------
+// Per step and warp: gates_t = hx_t x Wx^T (A = the group's saved h_{t-1}, read per k-block from global memory, + x columns);
+// the thread-local cell gradient; da'_t = da_t / s_j of the warp's 128 gate columns into the group's rows of the shared da
+// tile and into the workspace record of (tile, t) (rows = cells, 4H columns in slice order); after the group barrier
+// dh_{t-1}[slice] = da'_t x (s W_hh) over all 4H gates, and dx = sum of the cH slice partials in a fixed order.
+template <int CH>
+__global__ void __launch_bounds__(Dims<CH>::THREADS, 1)
+lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
+                         const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
+                         float* __restrict__ d_x, const __half* __restrict__ saved, __half* __restrict__ da_rec,
+                         const float* __restrict__ scale2, long long cells, int T, long long NN) {
+  using D = Dims<CH>;
+  constexpr int CELLS = D::CELLS;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [G4][WX_LD], slice order
+  __half* sDA = sWx + D::G4 * D::WX_LD;                    // [CELLS][DA_LD]: da'_t, columns in slice order
+  float* sDX = reinterpret_cast<float*>(sDA + CELLS * D::DA_LD);   // [CELLS][CH]: dx partial of each slice
+  float* s_wih = sDX + CELLS * CH;                         // [G4] by gate row j
+  load_wx_w<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
+  for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
+  __syncthreads();
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
+  const int cg = warp / CH, js = warp % CH;
+  const uint32_t wx_all = smem_u32(sWx), wx_addr = wx_all + (uint32_t)(js * 128 * D::WX_LD * 2);
+  const uint32_t da_addr = smem_u32(sDA + (cg * 16 + (lane & 15)) * D::DA_LD + 8 * (lane >> 4));
+  const long long tiles = (cells + CELLS - 1) / CELLS;
+  const float S = scale2[0], invS = scale2[1];
+
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    long long cell[2];
+    bool live[2];
+    size_t xb[2];
+    float dh[2][8], dc[2][8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      cell[h] = tile * CELLS + cg * 16 + g + 8 * h;
+      live[h] = cell[h] < cells;
+      xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
+#pragma unroll
+      for (int s = 0; s < 8; ++s) {
+        dh[h][s] = live[h] ? d_hT[(size_t)cell[h] * D::H + 32 * js + 8 * (s >> 1) + 2 * q + (s & 1)] * S : 0.f;
+        dc[h][s] = 0.f;
+      }
+    }
+    // the dx writer of the group (lanes 0..15 of slice 0) owns row 16 cg + lane
+    const long long dx_cell = tile * CELLS + cg * 16 + (lane & 15);
+    const bool dx_live = d_x != nullptr && js == 0 && lane < 16 && dx_cell < cells;
+    const size_t dx_base = dx_live ? x_base(dx_cell, T, NN) : 0;
+
+    for (int t = T - 1; t >= 0; --t) {
+      uint32_t xw[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) xw[h] = x_cols(live[h] ? x_seq[xb[h] + (size_t)t * NN] : 0.f, q);
+      // h_{t-1} of slice kb / 2 is the same lane's saved fragment of warp (cg, kb / 2): k-block kb = 2 sl + kk takes its
+      // words (h, 2 kk) and (h, 2 kk + 1), i.e. the uint2 number 2 h + kk of the 16 halves
+      const __half* hp = saved + (t > 0 ? save_off_w<CH>(tile, T, t - 1, cg * CH, 1, lane) : 0);
+      float acc[16][4];
+      gate_mma_w<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
+        if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; return; }
+        const uint2* p = reinterpret_cast<const uint2*>(hp + (kb >> 1) * 1024);
+        const uint2 r0 = __ldg(p + (kb & 1)), r1 = __ldg(p + 2 + (kb & 1));
+        a[0] = r0.x; a[1] = r1.x; a[2] = r0.y; a[3] = r1.y;
+      }, xw, wx_addr);
+
+      uint4 vc[2], vcp[2];
+      {
+        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 0, lane));
+        vc[0] = pc[0]; vc[1] = pc[1];
+        if (t > 0) {
+          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t - 1, warp, 0, lane));
+          vcp[0] = pcp[0]; vcp[1] = pcp[1];
+        } else {
+          vcp[0] = vcp[1] = make_uint4(0u, 0u, 0u, 0u);
+        }
+      }
+      uint32_t da[16][2];             // fp16 pairs of da' = da / s_j: gate column 8 nt + 2 q, +1 of row h, nt = gate * 4 + jn
+      float dx[2] = {0.f, 0.f};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float fc[8], fcp[8];
+        unpack8(vc[h], fc);
+        unpack8(vcp[h], fcp);
+        float di[8], df[8], dg[8], d_o[8];
+#pragma unroll
+        for (int s = 0; s < 8; ++s) {        // the hidden-32 cell gradient, see lstm_tc::lstm_bwd_saved_tc_kernel
+          const int jn = s >> 1, k = 2 * h + (s & 1);
+          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
+          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
+          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
+          const float ao = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
+          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * fc[s], 40.f));
+          const float pig = ai * ag;
+          const float r1 = rcp_(pig * af), r2 = rcp_(ao * ac);
+          const float gi = r1 * (ag * af), gg = fmaf(r1 + r1, ai * af, -1.f), gf = r1 * pig;
+          const float go = r2 * ac, tcv = fmaf(r2 + r2, ao, -1.f);
+          const float dhv = dh[h][s];
+          const float dcv = fmaf(dhv * go, fmaf(-tcv, tcv, 1.f), dc[h][s]);
+          d_o[s] = (dhv * tcv) * fmaf(-go, go, go);
+          di[s] = (dcv * gg) * fmaf(-gi, gi, gi);
+          df[s] = (dcv * fcp[s]) * fmaf(-gf, gf, gf);
+          dg[s] = (dcv * gi) * fmaf(-gg, gg, 1.f);
+          dc[h][s] = dcv * gf;
+          const int u = 32 * js + 8 * jn + 2 * q + (s & 1);
+          dx[h] += di[s] * s_wih[u] + df[s] * s_wih[D::H + u] + dg[s] * s_wih[2 * D::H + u] + d_o[s] * s_wih[3 * D::H + u];
+        }
+        // 1 / s: -ln 2 for i, f, o and -ln 2 / 2 for g
+#pragma unroll
+        for (int jn = 0; jn < 4; ++jn) {
+          da[jn][h] = pack2(-kLn2 * di[2 * jn], -kLn2 * di[2 * jn + 1]);
+          da[4 + jn][h] = pack2(-kLn2 * df[2 * jn], -kLn2 * df[2 * jn + 1]);
+          da[8 + jn][h] = pack2(-0.5f * kLn2 * dg[2 * jn], -0.5f * kLn2 * dg[2 * jn + 1]);
+          da[12 + jn][h] = pack2(-kLn2 * d_o[2 * jn], -kLn2 * d_o[2 * jn + 1]);
+        }
+        dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 1);
+        dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 2);
+      }
+      // every warp of the group has finished reading the previous step's da tile and dx partials
+      named_bar_sync(1 + cg, 32 * CH);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = cg * 16 + g + 8 * h;
+#pragma unroll
+        for (int nt = 0; nt < 16; ++nt) *reinterpret_cast<uint32_t*>(sDA + row * D::DA_LD + 128 * js + 8 * nt + 2 * q) = da[nt][h];
+        if (q == 0) sDX[row * CH + js] = dx[h];
+      }
+      named_bar_sync(1 + cg, 32 * CH);
+      if (dx_live) {
+        float v = 0.f;
+#pragma unroll
+        for (int sl = 0; sl < CH; ++sl) v += sDX[(cg * 16 + lane) * CH + sl];
+        d_x[dx_base + (size_t)t * NN] = v * invS;
+      }
+      {                                // the warp's 16 x 128 block of the da tile -> the (tile, t) record
+        __half* rec = da_rec + (((size_t)tile * T + t) * CELLS + cg * 16) * D::G4 + 128 * js;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int idx = 32 * i + lane, row = idx >> 4, ch = idx & 15;
+          *reinterpret_cast<uint4*>(rec + (size_t)row * D::G4 + 8 * ch) =
+              *reinterpret_cast<const uint4*>(sDA + (cg * 16 + row) * D::DA_LD + 128 * js + 8 * ch);
+        }
+      }
+      if (t > 0) {                    // dh_{t-1}[slice js] = da'_t x (s W_hh): B from Wx rows (k = gate row r), columns 32 js ..
+        float adh[4][4];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) adh[nt][0] = adh[nt][1] = adh[nt][2] = adh[nt][3] = 0.f;
+#pragma unroll 4
+        for (int kb = 0; kb < D::G4 / 16; ++kb) {
+          uint32_t a[4];
+          ldmatrix_x4(da_addr + 32 * kb, a[0], a[1], a[2], a[3]);
+#pragma unroll
+          for (int pr = 0; pr < 2; ++pr) {
+            uint32_t b0, b1, b2, b3;
+            ldmatrix_x4_trans(wx_all + (uint32_t)(((16 * kb + 8 * (mi & 1) + (lane & 7)) * D::WX_LD + 32 * js + 16 * pr + 8 * (mi >> 1)) * 2),
+                              b0, b1, b2, b3);
+            mma_16816(adh[2 * pr], a, b0, b1);
+            mma_16816(adh[2 * pr + 1], a, b2, b3);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int s = 0; s < 8; ++s) dh[h][s] = adh[s >> 1][2 * h + (s & 1)];
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// ... and the weight-gradient pass: dWext[r][k] = s_j * sum over (tile, t, cell) of da'[cell][r] hx_t[cell][k]
+// ---------------------------------------------------------------------------------------
+// CTA (js, split): the 128 gate rows of slice js, all H + 16 columns, over a contiguous range of (tile, t) records.  Per record
+// the da block and hx (h_{t-1} from the saved state, x columns) are staged in shared memory; warp w owns gate rows 16 w .. +15.
+constexpr int DW_THREADS = 256;
+constexpr int DW_DA_LD = 136;
+
+template <int CH>
+__global__ void __launch_bounds__(DW_THREADS)
+lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ saved, const __half* __restrict__ da_rec,
+                   float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, const float* __restrict__ scale2,
+                   long long cells, int T, long long NN) {
+  using D = Dims<CH>;
+  constexpr int CELLS = D::CELLS;
+  constexpr int HX_LD = D::KX + 8;
+  constexpr int NX = D::KX / 8;                 // n8 tiles of columns
+  __shared__ __align__(16) __half sDA[CELLS * DW_DA_LD];
+  __shared__ __align__(16) __half sHX[CELLS * HX_LD];
+  const int js = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
+  const long long tiles = (cells + CELLS - 1) / CELLS, records = tiles * T;
+  const long long per = (records + gridDim.y - 1) / gridDim.y;
+  const long long r0 = blockIdx.y * per, r1 = r0 + per < records ? r0 + per : records;
+  for (int e = threadIdx.x; e < CELLS; e += blockDim.x)          // constant zero columns H + 8 .. H + 15
+    *reinterpret_cast<uint4*>(sHX + e * HX_LD + D::H + 8) = make_uint4(0u, 0u, 0u, 0u);
+  const uint32_t da_addr = smem_u32(sDA), hx_addr = smem_u32(sHX);
+  float dw[NX][4];
+#pragma unroll
+  for (int nt = 0; nt < NX; ++nt) dw[nt][0] = dw[nt][1] = dw[nt][2] = dw[nt][3] = 0.f;
+
+  for (long long rec = r0; rec < r1; ++rec) {
+    const long long tile = rec / T;
+    const int t = (int)(rec - tile * T);
+    __syncthreads();                              // the previous record's tiles are no longer read
+    for (int e = threadIdx.x; e < CELLS * 16; e += blockDim.x) {
+      const int row = e >> 4, ch = e & 15;
+      *reinterpret_cast<uint4*>(sDA + row * DW_DA_LD + 8 * ch) =
+          __ldg(reinterpret_cast<const uint4*>(da_rec + ((size_t)rec * CELLS + row) * D::G4 + 128 * js + 8 * ch));
+    }
+    for (int e = threadIdx.x; e < D::NW * 64; e += blockDim.x) {    // saved h_{t-1}: (warp, lane, row half) -> 4 words
+      const int w = e >> 6, l = (e >> 1) & 31, h = e & 1;
+      const int row = (w / CH) * 16 + (l >> 2) + 8 * h, col = 32 * (w % CH) + 2 * (l & 3);
+      const uint4 v = t > 0 ? __ldg(reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t - 1, w, 1, l)) + h)
+                            : make_uint4(0u, 0u, 0u, 0u);
+      uint32_t* d = reinterpret_cast<uint32_t*>(sHX + row * HX_LD + col);
+      d[0] = v.x; d[4] = v.y; d[8] = v.z; d[12] = v.w;
+    }
+    for (int e = threadIdx.x; e < CELLS * 4; e += blockDim.x) {       // x columns H .. H + 7
+      const int row = e >> 2, qq = e & 3;
+      const long long cell = tile * CELLS + row;
+      const float x = cell < cells ? x_seq[x_base(cell, T, NN) + (size_t)t * NN] : 0.f;
+      *reinterpret_cast<uint32_t*>(sHX + row * HX_LD + D::H + 2 * qq) = x_cols(x, qq);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kc = 0; kc < CELLS / 16; ++kc) {
+      uint32_t a[4];
+      ldmatrix_x4_trans(da_addr + (uint32_t)(((16 * kc + 8 * (mi >> 1) + (lane & 7)) * DW_DA_LD + 16 * warp + 8 * (mi & 1)) * 2), a[0], a[1], a[2], a[3]);
+#pragma unroll
+      for (int pr = 0; pr < NX / 2; ++pr) {
+        uint32_t b0, b1, b2, b3;
+        ldmatrix_x4_trans(hx_addr + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * HX_LD + 16 * pr + 8 * (mi >> 1)) * 2), b0, b1, b2, b3);
+        mma_16816(dw[2 * pr], a, b0, b1);
+        mma_16816(dw[2 * pr + 1], a, b2, b3);
+      }
+    }
+  }
+  const float invS = scale2[1];
+#pragma unroll
+  for (int nt = 0; nt < NX; ++nt)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
+      const float v = dw[nt][i] * row_scale(r) * invS;
+      if (col < D::H) atomicAdd(&d_w_hh[(size_t)j * D::H + col], v);
+      else if (col == D::H || col == D::H + 2) atomicAdd(&d_w_ih[j], v);
+      else if (col == D::H + 1) atomicAdd(&d_b[j], v);
+    }
+}
+
+}  // namespace lstm_tcw
+
 // ---------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------
-bool lstm_tc_supported(int T, int C) { return C == 32 && T >= 1 && T <= 256; }
+bool lstm_tc_supported(int T, int C) { return (C == 32 || C == 96 || C == 128) && T >= 1 && T <= 256; }
 
-static int lstm_grid(long long cells, int per_sm) {
-  const long long tiles = (cells + lstm_tc::CELLS - 1) / lstm_tc::CELLS;
+static int lstm_grid(long long cells, int per_sm, int tile_cells = lstm_tc::CELLS) {
+  const long long tiles = (cells + tile_cells - 1) / tile_cells;
   long long g = (long long)per_sm * device_sm_count();
   return (int)(g < tiles ? g : tiles);
 }
 
-size_t lstm_tc_saved_bytes(int B, int T, long long NN) {
+// cells per tile of the wide kernels (lstm_tcw::Dims)
+static int lstm_tcw_cells(int C) { return C == 128 ? lstm_tcw::Dims<4>::CELLS : lstm_tcw::Dims<3>::CELLS; }
+static long long lstm_tcw_padded_cells(int B, long long NN, int C) {
+  const long long tc = lstm_tcw_cells(C);
+  return ((long long)B * NN + tc - 1) / tc * tc;
+}
+
+size_t lstm_tc_saved_bytes(int B, int T, long long NN, int C) {
+  if (C != 32)      // c_t | h_t of every cell (tiles padded) and step: 2 C halves, see lstm_tcw::save_off_w
+    return (size_t)lstm_tcw_padded_cells(B, NN, C) * T * 2 * C * sizeof(__half);
   const long long tiles = ((long long)B * NN + lstm_tc::CELLS - 1) / lstm_tc::CELLS;
   return (size_t)tiles * T * 8192 * sizeof(__half);      // see lstm_tc::save_off
 }
 
+// wide widths: the gate-gradient records of the reverse walk, 4 C halves per cell and step (lstm_tcw::lstm_bwd_walk_tcw_kernel)
+static size_t lstm_tcw_da_bytes(int B, int T, long long NN, int C) {
+  return (size_t)lstm_tcw_padded_cells(B, NN, C) * T * 4 * C * sizeof(__half);
+}
+
+// workspace of a backward that is handed the forward's saved state: the grad scale (1 KB) and, at the wide widths, the da records
+static size_t lstm_tc_bwd_saved_workspace_bytes(int B, int T, long long NN, int C) {
+  return 1024 + (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256));
+}
+
 // without a saved buffer from the forward, the backward first re-runs the (training) forward into its workspace
-size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN) { return 1024 + align_up(lstm_tc_saved_bytes(B, T, NN), 256); }
+size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) {
+  return lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C) + align_up(lstm_tc_saved_bytes(B, T, NN, C), 256);
+}
+
+template <int CH>
+static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
+                            void* saved, long long cells, int T, long long NN, cudaStream_t st) {
+  using D = lstm_tcw::Dims<CH>;
+  auto kern = saved ? lstm_tcw::lstm_fwd_tcw_kernel<CH, true> : lstm_tcw::lstm_fwd_tcw_kernel<CH, false>;
+  static DynSmemAttr attr_t = {}, attr_f = {};
+  if (int e = ensure_dyn_smem(kern, (int)D::kFwdSmem, saved ? attr_t : attr_f)) return e;
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
+  kern<<<lstm_grid(cells, 1, D::CELLS), D::THREADS, D::kFwdSmem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
+                                                                               cells, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int CH>
+static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, void* da_rec,
+                             const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+  using D = lstm_tcw::Dims<CH>;
+  static DynSmemAttr attr_b = {};
+  if (int e = ensure_dyn_smem(lstm_tcw::lstm_bwd_walk_tcw_kernel<CH>, (int)D::kBwdSmem, attr_b)) return e;
+  // walk: the gate recompute and dh_{t-1} (2 x 8 H (H + 1) per cell and step, as the hidden-32 count splits it) ...
+  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
+  lstm_tcw::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid(cells, 1, D::CELLS), D::THREADS, D::kBwdSmem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  // ... and the weight gradient (8 H (H + 1) / 2 more: 12 H (H + 1) in all)
+  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
+  long long splits = 4LL * device_sm_count() / CH;
+  if (splits > records) splits = records;
+  prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
+  lstm_tcw::lstm_dw_tcw_kernel<CH><<<dim3(CH, (unsigned)splits), lstm_tcw::DW_THREADS, 0, st>>>(
+      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2, cells, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
 
 int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                         void* saved, int B, int T, long long NN, cudaStream_t st) {
+                         void* saved, int B, int T, long long NN, int C_, cudaStream_t st) {
   using namespace lstm_tc;
   const long long cells = (long long)B * NN;
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm forward: saved buffer must be 16-byte aligned");
+  if (C_ == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
+  if (C_ == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
+  MPGCN_CHECK(C_ == C, "lstm forward: no tensor-core kernel for hidden=%d", C_);
   auto kern = saved ? lstm_fwd_tc_kernel<true> : lstm_fwd_tc_kernel<false>;
   prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)cells * T, st);
   kern<<<lstm_grid(cells, 2), FWD_THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells, T, NN);
@@ -443,18 +964,36 @@ int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_h
 
 int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                           const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
-                          int B, int T, long long NN, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
+                          int B, int T, long long NN, int C_, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
   using namespace lstm_tc;
   const long long cells = (long long)B * NN;
-  const size_t need = saved ? 1024 : lstm_tc_bwd_workspace_bytes(B, T, NN);
+  const size_t need = saved ? lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C_) : lstm_tc_bwd_workspace_bytes(B, T, NN, C_);
   MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, need);
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm backward: saved buffer must be 16-byte aligned");
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
+  MPGCN_CHECK(C_ == C || C_ == 96 || C_ == 128, "lstm backward: no tensor-core kernel for hidden=%d", C_);
   float* scale2 = static_cast<float*>(ws);
   if (saved == nullptr) {          // the caller kept no forward state: rebuild it (same kernel, same bits as the training forward)
-    void* tmp = static_cast<uint8_t*>(ws) + 1024;
-    if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, st)) return e;
+    void* tmp = static_cast<uint8_t*>(ws) + lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C_);
+    if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C_, st)) return e;
     saved = tmp;
+  }
+  if (C_ != C) {                   // wide widths: walk + weight-gradient pass; the da records follow the grad scale
+    const int G4w = 4 * C_;
+    void* da_rec = static_cast<uint8_t*>(ws) + 1024;
+    if (int e = grad_scale_prepare(d_hT, (size_t)cells * C_, scale2, d_hT_absmax, st)) return e;
+    MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4w, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4w * C_, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4w, st));
+    const int e = C_ == 96 ? lstm_backward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2,
+                                                  cells, T, NN, st)
+                           : lstm_backward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2,
+                                                  cells, T, NN, st);
+    if (e) return e;
+    prof_count(PROF_ELEMENTWISE);
+    copy_vec_kernel<<<(G4w + 127) / 128, 128, 0, st>>>(d_b_ih, d_b_hh, G4w);
+    MPGCN_CUDA(cudaGetLastError());
+    return 0;
   }
   if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
   MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4, st));

@@ -236,8 +236,19 @@ def resolve_lstm_precision(name, T, C) -> int:
         return _lib.PREC_FP16_TC if lib.mpgcn_lstm_precision_supported(T, C, _lib.PREC_FP16_TC) else _lib.PREC_FP32
     code = _PREC_NAMES[name]
     if not lib.mpgcn_lstm_precision_supported(T, C, code):
-        raise RuntimeError(f"LSTM precision {name!r} does not support T={T}, hidden={C} (tensor path needs hidden == 32)")
+        raise RuntimeError(f"LSTM precision {name!r} does not support T={T}, hidden={C} "
+                           "(tensor path needs hidden 32, 96 or 128 and 1 <= T <= 256; fp32 path needs hidden <= 64)")
     return code
+
+
+def lstm_engine_supports(name, T, C) -> bool:
+    """Whether `lstm_last` runs hidden size C over T steps at precision `name` (None / "auto" / "fp16" / "fp32").  "auto" resolves
+    to the fp32 kernels whenever the tensor-core ones do not apply, so the resolved kernel itself is asked, not only the name."""
+    try:
+        code = resolve_lstm_precision(name, T, C)
+    except RuntimeError:
+        return False
+    return bool(_lib.load().mpgcn_lstm_precision_supported(T, C, code))
 
 
 class _LSTMLastFn(torch.autograd.Function):
@@ -276,7 +287,9 @@ class _LSTMLastFn(torch.autograd.Function):
         g_bih, g_bhh = torch.empty_like(b_ih), torch.empty_like(b_hh)
         d_x = torch.empty_like(xc) if ctx.needs_input_grad[0] else None
         saved = ctx.lstm_saved
-        ws = _scratch(1024 if saved is not None else lib.mpgcn_lstm_bwd_workspace_bytes(B, T, NN, C, prec), dev)
+        # with the forward's state in hand the backward needs its workspace minus the room for rebuilding that state
+        ws_bytes = lib.mpgcn_lstm_bwd_workspace_bytes(B, T, NN, C, prec)
+        ws = _scratch(ws_bytes - saved.numel() if saved is not None else ws_bytes, dev)
         with torch.cuda.device(dev):
             _lib.check(lib.mpgcn_lstm_last_backward_saved(_ptr(xc), _ptr(w_ih), _ptr(w_hh), _ptr(b_ih), _ptr(b_hh), _ptr(d_hT), _ptr(g_wih),
                                                           _ptr(g_whh), _ptr(g_bih), _ptr(g_bhh), _ptr(d_x), _ptr(saved),
