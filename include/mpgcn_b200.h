@@ -171,7 +171,8 @@ MPGCN_API int mpgcn_absmax(const float* x, long long n, float* out, void* stream
  *   x_seq [B,T,NN] (= the model input [B,T,N,N,1] unchanged, NN = N*N)
  *   w_ih [4C,1], w_hh [4C,C], b_ih [4C], b_hh [4C]   (gate order i,f,g,o)
  *   hT   [B*NN, C]
- * precision 0: fp32 CUDA-core kernels (C <= 64); precision 1: tensor-core gate GEMM with the recurrent h rounded to
+ * precision 0: fp32 CUDA-core kernels (C <= 64, and T no longer than their backward's shared-memory stash holds: 15 steps at
+ * C = 64, 224 at 32, 8041 at 1; mpgcn_lstm_precision_supported answers it); precision 1: tensor-core gate GEMM with the recurrent h rounded to
  * fp16 as MMA operand, state and activations in fp32 (C = 32, 96 or 128; 1 <= T <= 256); x enters that GEMM as an fp16
  * hi + lo pair, exact to ~22 bits for |x| < 65504 and saturating beyond. */
 MPGCN_API int mpgcn_lstm_precision_supported(int T, int C, int precision);

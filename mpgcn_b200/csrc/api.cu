@@ -276,7 +276,7 @@ int mpgcn_dyn_graph_build(const float* od_history, int periods, float* o_graph, 
 }
 
 int mpgcn_lstm_precision_supported(int T, int C, int precision) {
-  if (precision == PREC_FP32_SIMT) return (T >= 1 && C >= 1 && C <= 64) ? 1 : 0;
+  if (precision == PREC_FP32_SIMT) return lstm_bwd_cells_per_block(T, C) >= 1 ? 1 : 0;     // the backward bounds T (DESIGN.md 6.4)
   if (precision == PREC_FP16_TC) return lstm_tc_supported(T, C) ? 1 : 0;
   return 0;
 }

@@ -82,6 +82,9 @@ int lstm_last_forward(const float* x_seq, const float* w_ih, const float* w_hh, 
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
                        long long NN, int C, cudaStream_t s);
+// cells per block of the backward, which keeps every recomputed step of its cells in shared memory; 0 where not even one cell
+// fits (T above 15 at hidden 64, 95 at 48, 224 at 32) or C is outside 1..64
+int lstm_bwd_cells_per_block(int T, int C);
 
 // FC head + branch mean (head_kernels.cu); g / dg are HOST arrays of M device pointers
 int head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,

@@ -252,6 +252,21 @@ __global__ void copy_kernel(const float* src, float* dst, int n) {
   if (i < n) dst[i] = src[i];
 }
 
+static constexpr size_t kBwdSmemBudget = 220 * 1024;
+
+// shared memory of lstm_bwd_kernel: weights and their gradient accumulators, then per cell T*(6C + 1) stash/x + 4C da + C dh
+static size_t lstm_bwd_fixed_bytes(int C) { return ((size_t)3 * 4 * C * C + 4 * 4 * (size_t)C) * sizeof(float); }
+static size_t lstm_bwd_per_cell_bytes(int T, int C) { return ((size_t)T * (6 * C + 1) + 5 * (size_t)C) * sizeof(float); }
+
+int lstm_bwd_cells_per_block(int T, int C) {
+  if (T < 1 || C < 1 || C > 64) return 0;
+  const size_t fixed = lstm_bwd_fixed_bytes(C);
+  if (fixed >= kBwdSmemBudget) return 0;
+  const size_t cells = (kBwdSmemBudget - fixed) / lstm_bwd_per_cell_bytes(T, C);
+  const size_t cap = 1024 / C < 16 ? 1024 / C : 16;
+  return (int)(cells < cap ? cells : cap);
+}
+
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
                        long long NN, int C, cudaStream_t st) {
@@ -259,19 +274,12 @@ int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh,
   MPGCN_CHECK(C >= 1 && C <= 64, "lstm backward: hidden size %d unsupported (1..64)", C);
   const long long cells = (long long)B * NN;
   const int G = 4 * C;
-  const size_t fixed = ((size_t)3 * G * C + 4 * (size_t)G) * sizeof(float);
-  const size_t budget = 220 * 1024;
-  MPGCN_CHECK(fixed < budget, "lstm backward: weights do not fit in shared memory");
-  // per cell: T*(6C + 1) stash/x + 4C da + C dh
-  const size_t per_cell = ((size_t)T * (6 * C + 1) + 5 * (size_t)C) * sizeof(float);
-  int CELLS = (int)((budget - fixed) / per_cell);
+  const int CELLS = lstm_bwd_cells_per_block(T, C);
   MPGCN_CHECK(CELLS >= 1, "lstm backward: sequence length %d too long for the shared-memory stash", T);
-  if (CELLS > 1024 / C) CELLS = 1024 / C;
-  if (CELLS > 16) CELLS = 16;
   const int threads = CELLS * C;
-  const size_t smem = fixed + (size_t)CELLS * per_cell;
+  const size_t smem = lstm_bwd_fixed_bytes(C) + (size_t)CELLS * lstm_bwd_per_cell_bytes(T, C);
   static DynSmemAttr attr = {};
-  if (int e = ensure_dyn_smem(lstm_bwd_kernel, (int)(budget + 4096), attr)) return e;
+  if (int e = ensure_dyn_smem(lstm_bwd_kernel, (int)(kBwdSmemBudget + 4096), attr)) return e;
   MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G, st));
   MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G * C, st));
   MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G, st));

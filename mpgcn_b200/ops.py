@@ -237,7 +237,8 @@ def resolve_lstm_precision(name, T, C) -> int:
     code = _PREC_NAMES[name]
     if not lib.mpgcn_lstm_precision_supported(T, C, code):
         raise RuntimeError(f"LSTM precision {name!r} does not support T={T}, hidden={C} "
-                           "(tensor path needs hidden 32, 96 or 128 and 1 <= T <= 256; fp32 path needs hidden <= 64)")
+                           "(tensor path needs hidden 32, 96 or 128 and 1 <= T <= 256; fp32 path needs hidden <= 64 and a T whose "
+                           "backward stash fits in shared memory, e.g. T <= 15 at hidden 64)")
     return code
 
 

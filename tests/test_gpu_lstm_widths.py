@@ -157,7 +157,9 @@ def test_lstm_saved_and_workspace_bytes_at_wide_hidden():
     assert lib.mpgcn_lstm_bwd_workspace_bytes(B, T, NN, 32, 1) == 1024 + lib.mpgcn_lstm_saved_bytes(B, T, NN, 32, 1)
 
 
-def test_lstm_precision_resolution_at_wide_hidden():
+def test_lstm_precision_resolution_at_wide_hidden_and_fp32_length_limit():
+    """Which kernel each precision name resolves to above and at hidden 64, and where "auto" leaves the LSTM to nn.LSTM: the
+    tensor-core kernels stop at T = 256, the fp32 kernels at the longest sequence their backward's shared-memory stash holds."""
     for C in WIDTHS:
         assert ops.resolve_lstm_precision("fp16", 12, C) == _lib.PREC_FP16_TC
         assert ops.resolve_lstm_precision("auto", 12, C) == _lib.PREC_FP16_TC
@@ -170,9 +172,11 @@ def test_lstm_precision_resolution_at_wide_hidden():
         ops.resolve_lstm_precision("fp16", 12, 64)
     assert not ops.lstm_engine_supports("fp16", 300, 128)
     # "auto" (the model's default) runs the engine only where a kernel applies: tensor cores at 32 / 96 / 128 with T <= 256, the
-    # fp32 kernels up to hidden 64; everywhere else the model keeps nn.LSTM
+    # fp32 kernels up to hidden 64 as long as their backward's shared-memory stash holds T steps (15 at hidden 64, 95 at 48, 224
+    # at 32); everywhere else the model keeps nn.LSTM
     for T, C, want in ((12, 32, True), (12, 48, True), (12, 64, True), (12, 96, True), (12, 128, True), (256, 128, True),
-                       (300, 128, False), (300, 96, False), (300, 64, True), (12, 80, False), (12, 160, False), (12, 256, False)):
+                       (300, 128, False), (300, 96, False), (300, 64, False), (15, 64, True), (16, 64, False), (95, 48, True),
+                       (96, 48, False), (256, 32, True), (300, 32, False), (12, 80, False), (12, 160, False), (12, 256, False)):
         assert ops.lstm_engine_supports("auto", T, C) == want, (T, C)
         assert ops.lstm_engine_supports(None, T, C) == want or ops.default_precision() != "auto", (T, C)
 
@@ -383,10 +387,11 @@ def test_model_at_hidden_128_no_grad_allocates_no_stash_and_graph_rollout_equals
 @pytest.mark.gpu
 @pytest.mark.parametrize("hid,T,prec,engine", [(96, 4, "fp32", False), (160, 4, None, False), (256, 4, "auto", False),
                                               (128, 300, None, False), (128, 300, "auto", False), (128, 4, None, True),
-                                              (96, 256, "auto", True)])
+                                              (96, 256, "auto", True), (64, 16, "auto", False), (64, 15, "auto", True)])
 def test_model_lstm_dispatch_above_hidden_64(hid, T, prec, engine, cuda_device, monkeypatch):
     """Above hidden 64 the model runs the engine LSTM only where a kernel applies (tensor cores at 96 / 128, T <= 256) and keeps
-    nn.LSTM everywhere else -- lstm_precision "fp32", other widths, longer sequences -- including under the default precision."""
+    nn.LSTM everywhere else -- lstm_precision "fp32", other widths, longer sequences -- including under the default precision.
+    At hidden 64 "auto" keeps nn.LSTM past the 15 steps the fp32 backward can hold."""
     monkeypatch.delenv("MPGCN_B200_PRECISION", raising=False)
     N = 5
     model = _model(N, 2, hid, 5, cuda_device)
