@@ -1,34 +1,59 @@
-// Per-OD-cell LSTM on tensor cores (hidden size 32), forward and BPTT backward.
+// Per-OD-cell LSTM on tensor cores at hidden sizes H = 32 CH (CH = 1, 3, 4: H = 32, 96, 128), forward and BPTT backward.
 //
-// Reference semantics: nn.LSTM(1, 32, 1, batch_first=True) over B*N*N independent cells with zero
-// initial state, last hidden state only (reference MPGCN.py: LSTM branch of MPGCN.forward); gate order i,f,g,o.
+// Reference semantics: nn.LSTM(1, H, 1, batch_first=True) over B*N*N independent cells with zero initial state, last hidden
+// state only (reference MPGCN.py: LSTM branch of MPGCN.forward); gate order i,f,g,o.
 //
-// Two kernels (details at each):
-//   lstm_fwd_tc_kernel<SAVE>     forward; SAVE additionally stores c_t, h_t (fp16) of every step for training
-//   lstm_bwd_saved_tc_kernel     backward from that saved state: one reverse walk
-// (a backward call that comes without saved state first re-runs the SAVE forward into its workspace)
-// Tile = 128 cells per CTA, 16 cells per warp.  The gate GEMM of a step, affine part and ex2 scaling included, is
-// [16 cells x 48] . [48 x 128 gates] of warp-level mma.sync m16n8k16 (fp16 operands, fp32 accumulators) whose accumulator is
-// the exponent argument of the activation.  In the m16n8 accumulator fragment a thread holds, for two cells, the same 8 hidden
-// units of all four gates, so the whole cell update is thread-local, and the new h_t is already the A fragment of the next
-// step's MMA: the recurrence never leaves registers.  The recurrence rounds h to fp16 only as MMA operand; c, the gate
-// arguments and the returned h_T stay fp32.  Activations cost 7 SFU operations per hidden unit and step.
+// One kernel family with three instances.  What they share is written once below: the tile geometry (Dims), the gate-weight
+// tile (load_wx), the gate GEMM of a step (gate_mma), the cell update (cell_update), the cell gradient (cell_grad) and the
+// saved-state layout (save_off).  A warp owns 16 cells x one 32-unit slice of all four gates; a tile is CG such 16-cell groups
+// of CH warps each.  The gate GEMM of a step, affine part and ex2 scaling included, is [16 cells x (H + 16)] . [(H + 16) x 128
+// gate columns] of warp-level mma.sync m16n8k16 (fp16 operands, fp32 accumulators) whose accumulator is the exponent argument
+// of the activation.  In the m16n8 accumulator fragment a thread holds, for two cells, the same 8 hidden units of all four
+// gates, so the whole cell update is thread-local.  h is rounded to fp16 only as MMA operand; c, the gate arguments and the
+// returned h_T stay fp32.  Activations cost 7 SFU operations per hidden unit and step.  The training forward (SAVE) also
+// stores c_t, h_t (fp16) of every step; a backward call that comes without that state first re-runs the SAVE forward into its
+// workspace.  The instances differ in how h_t and the weight gradient move between warps (details at each kernel):
+//   H = 32    lstm_fwd_tc_kernel<SAVE>, lstm_bwd_saved_tc_kernel.  A warp holds all 4H gate columns, so the new h_t is
+//             already the A fragment of the next step's MMA: the recurrence never leaves registers and a step needs no
+//             barrier.  128-cell tiles, 8 warps, 2 CTAs per SM in the forward.  The backward is one reverse walk that keeps
+//             dWext [128 x 48] in registers across every step and tile of the CTA and reads W_hh^T from its own shared copy.
+//   H = 96,   lstm_fwd_tcw_kernel<CH, SAVE>, lstm_bwd_walk_tcw_kernel<CH>, lstm_dw_tcw_kernel<CH>.  The CH warps of a group
+//   H = 128   exchange h_t through shared memory, one named barrier per group and step; one CTA per SM.  dWext fits neither
+//             in registers nor in shared memory, so the walk writes its gate gradients to the workspace and a separate pass
+//             reduces them.
 //
 // mma.sync m16n8k16 fragments (lane = 4 g + q): accumulator element (row g + 8 h, column 2 q + e) of an n8 tile is d[2 h + e];
 // A element (row g + 8 h, k 2 q + e + 8 kh) is half e of a[h + 2 kh]; B element (k 2 q + e + 8 kh, column g) is half e of b[kh].
-// Per thread: cell rows g, g + 8 of the warp's 16 (index h), units u = 8 jn + 2 q + e (slot s = 2 jn + e, jn < 4).
+// Per thread: cell rows g, g + 8 of the warp's 16 (index h), units u = 32 js + 8 jn + 2 q + e of the warp's slice js (slot
+// s = 2 jn + e, jn < 4).
 #include "kernels.h"
 
 namespace mpgcn {
 namespace lstm_tc {
 
-constexpr int C = 32;
-constexpr int G4 = 128;
-constexpr int CELLS = 128;
-constexpr int WX_LD = 56;       // Wx row stride in halves: 48 live k columns, padded so that 8 rows hit distinct banks
-constexpr int WT_LD = 136;      // W_hh^T row stride (128 gates + padding)
-constexpr int DA_LD = 136;      // da tile [128 cells][128 gates] row stride
-constexpr int HX_LD = 56;       // hx tile [128 cells][48 columns] row stride
+template <int CH>
+struct Dims {
+  // 16-cell groups per tile: 8 at H = 32 (8 warps; h stays in registers, so 2 CTAs fit an SM in the forward), 4 at H = 96 (12
+  // warps, <= 168 registers per thread), 3 at H = 128 (12 warps; 16 warps would cap a thread at 128 registers, which the
+  // backward walk exceeds)
+  static constexpr int CG = CH == 1 ? 8 : CH == 3 ? 4 : 3;
+  static constexpr int CELLS = 16 * CG;
+  static constexpr int H = 32 * CH;
+  static constexpr int G4 = 4 * H;
+  static constexpr int KX = H + 16;            // operand row of a cell: h_{t-1} (H) | x columns (16, see load_wx)
+  static constexpr int WX_LD = KX + 8;         // padded so that 8 consecutive rows fall in distinct 16-byte bank groups
+  static constexpr int HX_LD = KX + 8;         // staged operand rows of the weight-gradient GEMM
+  static constexpr int H_LD = H + 8;           // h exchange tile row stride
+  static constexpr int DA_LD = G4 + 8;         // da tile row stride
+  static constexpr int NW = CG * CH;           // warps per CTA
+  static constexpr int THREADS = 32 * NW;
+  static constexpr int FWD_CTAS_PER_SM = CH == 1 ? 2 : 1;
+  static constexpr int BWD_CTAS_PER_SM = 1;
+  static constexpr int TILE_HALVES = CELLS * H * 2;     // saved c_t | h_t per (tile, step)
+};
+
+constexpr int WT_LD = 136;      // H = 32 backward: W_hh^T row stride (128 gates + padding)
+constexpr float kLn2 = 0.69314718055994531f;
 
 // SFU primitives (2 ulp each); ex2 saturates to 0 / +inf and rcp(inf) = 0, which are the limits the activations need.
 __device__ __forceinline__ float ex2_(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -61,77 +86,154 @@ __device__ __forceinline__ void unpack8(const uint4& v, float* f) {
   }
 }
 
+// Wx rows are kept in slice order r = 128 js + 32 gate + u (gate row j = gate H + 32 js + u), so a warp's B operand is one
+// contiguous block of 128 rows; at H = 32 the order is the natural one.
+template <int CH>
+__device__ __forceinline__ int gate_row(int r) { return (r & 127) / 32 * (32 * CH) + 32 * (r >> 7) + (r & 31); }
+__device__ __forceinline__ float row_scale(int r) { return ((r & 127) >> 5) == 2 ? -2.8853900817779268f : -1.4426950408889634f; }
 
-// Wx[j][k] = s_j * [ W_hh[j,:] | wih_hi  b_hi  wih_hi  wih_lo  b_lo  0 0 0 | 0 .. ]  (k < 48; s_j = -log2 e for i, f, o and -2 log2 e
-// for g): with the operand row of a cell  hx_t = [ h_{t-1} (32) | x_hi  1  x_lo  x_hi  1  0 0 0 | 0 .. ]  the product hx_t . Wx[j]
-// is s_j * (W_hh h_{t-1} + w_ih x_t + b)_j; x, w_ih and b are split into fp16 hi + lo parts, so the affine part keeps ~22 bits.
+// Wx[r][k] = s_j * [ W_hh[j,:] | wih_hi  b_hi  wih_hi  wih_lo  b_lo  0 0 0 | 0 .. ]  (j = gate_row(r), k < H + 16; s_j = -log2 e
+// for i, f, o and -2 log2 e for g): with the operand row of a cell  hx_t = [ h_{t-1} (H) | x_hi  1  x_lo  x_hi  1  0 0 0 | 0 .. ]
+// the product hx_t . Wx[r] is s_j * (W_hh h_{t-1} + w_ih x_t + b)_j; x, w_ih and b are split into fp16 hi + lo parts, so the
+// affine part keeps ~22 bits.
+template <int CH>
 __device__ void load_wx(__half* sWx, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh) {
-  for (int e = threadIdx.x; e < G4 * 6; e += blockDim.x) {
-    const int j = e / 6, ch = e % 6;
-    const float sc = ((j >> 5) == 2) ? -2.8853900817779268f : -1.4426950408889634f;
+  using D = Dims<CH>;
+  constexpr int NCH = D::KX / 8;
+  for (int e = threadIdx.x; e < D::G4 * NCH; e += blockDim.x) {
+    const int r = e / NCH, ch = e % NCH, j = gate_row<CH>(r);
+    const float sc = row_scale(r);
     float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (ch < 4) {
+    if (ch < D::H / 8) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = sc * w_hh[j * C + ch * 8 + i];
-    } else if (ch == 4) {
+      for (int i = 0; i < 8; ++i) v[i] = sc * w_hh[(size_t)j * D::H + ch * 8 + i];
+    } else if (ch == D::H / 8) {
       const float wi = sc * w_ih[j], bb = sc * (b_ih[j] + b_hh[j]);
       const float wi_hi = __half2float(__float2half_rn(wi)), b_hi = __half2float(__float2half_rn(bb));
       v[0] = wi_hi; v[1] = b_hi; v[2] = wi_hi; v[3] = wi - wi_hi; v[4] = bb - b_hi;
     }
-    *reinterpret_cast<uint4*>(sWx + j * WX_LD + ch * 8) = pack8(v);
+    *reinterpret_cast<uint4*>(sWx + r * D::WX_LD + ch * 8) = pack8(v);
   }
 }
 
-// the x / 1 columns 32 + 2 q, 33 + 2 q of a cell's operand row (see load_wx)
+// the x / 1 columns H + 2 q, H + 1 + 2 q of a cell's operand row (see load_wx)
 __device__ __forceinline__ uint32_t x_cols(float x, int q) {
   const float x_hi = x_split_hi(x);
   return q == 0 ? pack2(x_hi, 1.f) : q == 1 ? pack2(x_split_lo(x, x_hi), x_hi) : q == 2 ? pack2(1.f, 0.f) : 0u;
 }
 
-// acc[nt] (nt = gate * 4 + jn) += hx_t . Wx^T for the warp's 16 cells.  hw: the thread's h_{t-1} as 8 fp16 pairs (word h * 4 + jn
-// holds units 8 jn + 2 q, +1 of cell row h) = the A fragments of k-blocks 0 and 1; xw[h]: the x columns of row h (k-block 2).
-__device__ __forceinline__ void gate_mma(float (&acc)[16][4], const uint32_t (&hw)[8], const uint32_t (&xw)[2], uint32_t wx_addr) {
-  const int lane = threadIdx.x & 31;
+// acc[nt] (nt = gate * 4 + jn) = hx_t . Wx^T for the warp's 16 cells and 128 gate columns.  a_h(kb, a) supplies the A fragment
+// of h-block kb < 2 CH; xw[h] are the x columns of row h (k-block 2 CH).  wx_addr: first of the warp's 128 Wx rows.
+template <int CH, class AH>
+__device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const uint32_t (&xw)[2], uint32_t wx_addr) {
+  using D = Dims<CH>;
+  const int lane = threadIdx.x & 31, mi = lane >> 3;
 #pragma unroll
   for (int nt = 0; nt < 16; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
 #pragma unroll
-  for (int kb = 0; kb < 3; ++kb) {
+  for (int kb = 0; kb <= 2 * CH; ++kb) {
     uint32_t a[4];
-    if (kb < 2) { a[0] = hw[2 * kb]; a[1] = hw[4 + 2 * kb]; a[2] = hw[2 * kb + 1]; a[3] = hw[4 + 2 * kb + 1]; }
+    if (kb < 2 * CH) a_h(kb, a);
     else { a[0] = xw[0]; a[1] = xw[1]; a[2] = 0u; a[3] = 0u; }
 #pragma unroll
     for (int pr = 0; pr < 8; ++pr) {
-      const int mi = lane >> 3;
       uint32_t b0, b1, b2, b3;
-      ldmatrix_x4(wx_addr + (uint32_t)(((16 * pr + 8 * (mi >> 1) + (lane & 7)) * WX_LD + 16 * kb + 8 * (mi & 1)) * 2), b0, b1, b2, b3);
+      ldmatrix_x4(wx_addr + (uint32_t)(((16 * pr + 8 * (mi >> 1) + (lane & 7)) * D::WX_LD + 16 * kb + 8 * (mi & 1)) * 2), b0, b1, b2, b3);
       mma_16816(acc[2 * pr], a, b0, b1);
       mma_16816(acc[2 * pr + 1], a, b2, b3);
     }
   }
 }
 
-// Training state written by the forward kernel and read by lstm_bwd_saved_tc_kernel: per (128-cell tile, step) 8192 halves,
-// [warp][c | h][lane][16 halves], the 16 halves of a thread in slot order h * 8 + s (its register fragment, stored as is).
-__device__ __forceinline__ size_t save_off(long long tile, int T, int t, int warp, int kind, int lane) {
-  return ((size_t)tile * T + t) * 8192 + (size_t)warp * 1024 + (size_t)kind * 512 + (size_t)lane * 16;
+// One step of the thread's 2 x 8 units: c (c_{t-1} -> c_t) in place and h_t into hv, from the gate accumulators.
+// Seven SFU operations per hidden unit (5 ex2 + 2 rcp): i, g, f share one reciprocal of the product of their three (1 + 2^arg)
+// terms, o and tanh(c) share another.  The accumulators are -log2e * pre (i, f, o) and -2 log2e * pre (g); arguments are
+// clamped from above at 40 (ex2(-big) = 0 is fine), so a triple product stays below 1.4e36; the clamp moves sigmoid / tanh by
+// < 1e-12.
+__device__ __forceinline__ void cell_update(const float (&acc)[16][4], float (&c)[2][8], float (&hv)[2][8]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int jn = s >> 1, k = 2 * h + (s & 1);
+      const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
+      const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
+      const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
+      const float p = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
+      const float pig = ai * ag;
+      const float r = rcp_(pig * af);
+      const float gi = r * (ag * af);                    // sigmoid(i)
+      const float gg = fmaf(r + r, ai * af, -1.f);       // tanh(g)
+      const float gf = r * pig;                          // sigmoid(f)
+      c[h][s] = fmaf(gf, c[h][s], gi * gg);
+      const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * c[h][s], 40.f));
+      const float r2 = rcp_(p * ac);
+      hv[h][s] = (r2 * ac) * fmaf(r2 + r2, p, -1.f);     // sigmoid(o) * tanh(c)
+    }
+  }
 }
 
-// ---------------------------------------------------------------------------------------
-// forward
-// ---------------------------------------------------------------------------------------
-constexpr int FWD_THREADS = 256;
+// The gate gradients of cell row h at one step of the reverse walk, from the gate accumulators recomputed from the saved
+// h_{t-1}, the saved c_t, c_{t-1} (vc, vcp) and the incoming dh, dc of the row's 8 units (dc becomes dc_{t-1} in place):
+// d[gate][s] for gates i, f, g, o.  Returns the thread's part of the row's dx = sum over its units u of d[.][s] w_ih[. H + u]
+// (s_wih: w_ih by gate row; js: the warp's unit slice).  The 7 SFU operations of cell_update.
+template <int CH>
+__device__ __forceinline__ float cell_grad(const float (&acc)[16][4], int h, const uint4& vc, const uint4& vcp, const float (&dh)[8],
+                                           float (&dc)[8], const float* s_wih, int js, int q, float (&d)[4][8]) {
+  constexpr int H = Dims<CH>::H;
+  float fc[8], fcp[8];
+  unpack8(vc, fc);
+  unpack8(vcp, fcp);
+  float dx = 0.f;
+#pragma unroll
+  for (int s = 0; s < 8; ++s) {
+    const int jn = s >> 1, k = 2 * h + (s & 1);
+    const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
+    const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
+    const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
+    const float ao = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
+    const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * fc[s], 40.f));
+    const float pig = ai * ag;
+    const float r1 = rcp_(pig * af), r2 = rcp_(ao * ac);
+    const float gi = r1 * (ag * af), gg = fmaf(r1 + r1, ai * af, -1.f), gf = r1 * pig;
+    const float go = r2 * ac, tcv = fmaf(r2 + r2, ao, -1.f);
+    const float dhv = dh[s];
+    const float dcv = fmaf(dhv * go, fmaf(-tcv, tcv, 1.f), dc[s]);
+    d[3][s] = (dhv * tcv) * fmaf(-go, go, go);
+    d[0][s] = (dcv * gg) * fmaf(-gi, gi, gi);
+    d[1][s] = (dcv * fcp[s]) * fmaf(-gf, gf, gf);
+    d[2][s] = (dcv * gi) * fmaf(-gg, gg, 1.f);
+    dc[s] = dcv * gf;
+    const int u = 32 * js + 8 * jn + 2 * q + (s & 1);
+    dx += d[0][s] * s_wih[u] + d[1][s] * s_wih[H + u] + d[2][s] * s_wih[2 * H + u] + d[3][s] * s_wih[3 * H + u];
+  }
+  return dx;
+}
 
+// Training state written by the forward kernels and read by the backward ones: per (tile, step) NW x 1024 halves,
+// [warp][c | h][lane][16 halves], the 16 halves of a thread in slot order h * 8 + s (its register fragment, stored as is);
+// warp = cg CH + js.
+template <int CH>
+__device__ __forceinline__ size_t save_off(long long tile, int T, int t, int warp, int kind, int lane) {
+  return ((size_t)tile * T + t) * Dims<CH>::TILE_HALVES + (size_t)warp * 1024 + (size_t)kind * 512 + (size_t)lane * 16;
+}
+
+// =======================================================================================
+// H = 32
+// =======================================================================================
+// forward: the thread's h_t, packed to fp16 pairs, is its A fragment of the next step's h k-blocks
 template <bool SAVE>
-__global__ void __launch_bounds__(FWD_THREADS, 2)
+__global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::FWD_CTAS_PER_SM)
 lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                    const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
                    long long cells, int T, long long NN) {
-  __shared__ __align__(16) __half sWx[G4 * WX_LD];
-  load_wx(sWx, w_ih, w_hh, b_ih, b_hh);
+  using D = Dims<1>;
+  __shared__ __align__(16) __half sWx[D::G4 * D::WX_LD];
+  load_wx<1>(sWx, w_ih, w_hh, b_ih, b_hh);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   const uint32_t wx_addr = smem_u32(sWx);
-  const long long tiles = (cells + CELLS - 1) / CELLS;
+  const long long tiles = (cells + D::CELLS - 1) / D::CELLS;
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     long long cell[2];
     bool live[2];
@@ -139,7 +241,7 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
     float xv[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      cell[h] = tile * CELLS + warp * 16 + g + 8 * h;
+      cell[h] = tile * D::CELLS + warp * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
       xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
       xv[h] = live[h] ? x_seq[xb[h]] : 0.f;
@@ -150,7 +252,7 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
 #pragma unroll
       for (int s = 0; s < 8; ++s) { c[h][s] = 0.f; hv[h][s] = 0.f; }
     for (int t = 0; t < T; ++t) {
-      uint32_t hw[8], xw[2];
+      uint32_t hw[8], xw[2];          // word h * 4 + jn: units 8 jn + 2 q, +1 of cell row h
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -158,36 +260,15 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
         xw[h] = x_cols(xv[h], q);
       }
       float acc[16][4];
-      gate_mma(acc, hw, xw, wx_addr);
+      gate_mma<1>(acc, [&](int kb, uint32_t (&a)[4]) {
+        a[0] = hw[2 * kb]; a[1] = hw[4 + 2 * kb]; a[2] = hw[2 * kb + 1]; a[3] = hw[4 + 2 * kb + 1];
+      }, xw, wx_addr);
 #pragma unroll
       for (int h = 0; h < 2; ++h) xv[h] = (live[h] && t + 1 < T) ? x_seq[xb[h] + (size_t)(t + 1) * NN] : 0.f;
-      // Seven SFU operations per hidden unit and step (5 ex2 + 2 rcp): i, g, f share one reciprocal of the product of their
-      // three (1 + 2^arg) terms, o and tanh(c) share another.  The accumulators are -log2e * pre (i, f, o) and -2 log2e * pre
-      // (g); arguments are clamped from above at 40 (ex2(-big) = 0 is fine), so a triple product stays below 1.4e36; the
-      // clamp moves sigmoid / tanh by < 1e-12.
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int s = 0; s < 8; ++s) {
-          const int jn = s >> 1, k = 2 * h + (s & 1);
-          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
-          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
-          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float p = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
-          const float pig = ai * ag;
-          const float r = rcp_(pig * af);
-          const float gi = r * (ag * af);                    // sigmoid(i)
-          const float gg = fmaf(r + r, ai * af, -1.f);       // tanh(g)
-          const float gf = r * pig;                          // sigmoid(f)
-          c[h][s] = fmaf(gf, c[h][s], gi * gg);
-          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * c[h][s], 40.f));
-          const float r2 = rcp_(p * ac);
-          hv[h][s] = (r2 * ac) * fmaf(r2 + r2, p, -1.f);     // sigmoid(o) * tanh(c)
-        }
-      }
+      cell_update(acc, c, hv);
       if (SAVE) {                     // training: c_t and h_t (fp16) for the backward kernel, see save_off()
-        uint4* dc = reinterpret_cast<uint4*>(saved + save_off(tile, T, t, warp, 0, lane));
-        uint4* dh = reinterpret_cast<uint4*>(saved + save_off(tile, T, t, warp, 1, lane));
+        uint4* dc = reinterpret_cast<uint4*>(saved + save_off<1>(tile, T, t, warp, 0, lane));
+        uint4* dh = reinterpret_cast<uint4*>(saved + save_off<1>(tile, T, t, warp, 1, lane));
         dc[0] = pack8(c[0]); dc[1] = pack8(c[1]);
         dh[0] = pack8(hv[0]); dh[1] = pack8(hv[1]);
       }
@@ -198,15 +279,13 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
         if (live[h]) {
 #pragma unroll
           for (int jn = 0; jn < 4; ++jn)
-            *reinterpret_cast<float2*>(hT + (size_t)cell[h] * C + 8 * jn + 2 * q) = make_float2(hv[h][2 * jn], hv[h][2 * jn + 1]);
+            *reinterpret_cast<float2*>(hT + (size_t)cell[h] * D::H + 8 * jn + 2 * q) = make_float2(hv[h][2 * jn], hv[h][2 * jn + 1]);
         }
     }
   }
 }
 
-// ---------------------------------------------------------------------------------------
 // backward from the forward kernel's saved c_t / h_t (training path)
-// ---------------------------------------------------------------------------------------
 // One reverse walk, no forward recompute: the gate pre-activations of step t depend only on the SAVED h_{t-1} and on x_t.
 // Per step and warp (16 cells), all on mma.sync:
 //     gates_t  = hx_t x Wx^T                (as in the forward; A = saved h_{t-1} fragment + x columns)
@@ -215,29 +294,31 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
 //     dWext   += da_t^T x hx_t              (128 gates x 48 columns over the tile's 128 cells; warp w owns gates 16 w .. 16 w + 15;
 //                                            columns 0..31 dW_hh, 32 + 34 dW_ih, 33 db)
 // da_t and hx_t go through double-buffered shared-memory tiles for that last product.
-constexpr int BWD_THREADS = 256;
-constexpr size_t kBwdSmem = (size_t)(G4 * WX_LD + C * WT_LD + 2 * CELLS * DA_LD + 2 * CELLS * HX_LD) * sizeof(__half) + G4 * sizeof(float);
+constexpr size_t kBwdSavedSmem = (size_t)(Dims<1>::G4 * Dims<1>::WX_LD + Dims<1>::H * WT_LD + 2 * Dims<1>::CELLS * Dims<1>::DA_LD +
+                                          2 * Dims<1>::CELLS * Dims<1>::HX_LD) * sizeof(__half) + Dims<1>::G4 * sizeof(float);
 
-__global__ void __launch_bounds__(BWD_THREADS, 1)
+__global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::BWD_CTAS_PER_SM)
 lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                          float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, float* __restrict__ d_x,
                          const __half* __restrict__ saved, const float* __restrict__ scale2, long long cells, int T, long long NN) {
+  using D = Dims<1>;
+  constexpr int C = D::H, CELLS = D::CELLS;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [128][WX_LD]
-  __half* sWT = sWx + G4 * WX_LD;                          // [32 units][WT_LD]: W_hh^T
+  __half* sWT = sWx + D::G4 * D::WX_LD;                    // [32 units][WT_LD]: W_hh^T
   __half* sDA = sWT + C * WT_LD;                           // 2 x [128 cells][DA_LD]
-  __half* sHX = sDA + 2 * CELLS * DA_LD;                   // 2 x [128 cells][HX_LD]
-  float* s_wih = reinterpret_cast<float*>(sHX + 2 * CELLS * HX_LD);
+  __half* sHX = sDA + 2 * CELLS * D::DA_LD;                // 2 x [128 cells][HX_LD]
+  float* s_wih = reinterpret_cast<float*>(sHX + 2 * CELLS * D::HX_LD);
 
-  load_wx(sWx, w_ih, w_hh, b_ih, b_hh);
-  for (int e = threadIdx.x; e < G4 * C; e += blockDim.x) {
+  load_wx<1>(sWx, w_ih, w_hh, b_ih, b_hh);
+  for (int e = threadIdx.x; e < D::G4 * C; e += blockDim.x) {
     const int j = e / C, u = e % C;
     sWT[u * WT_LD + j] = __float2half_rn(w_hh[e]);
   }
-  for (int j = threadIdx.x; j < G4; j += blockDim.x) s_wih[j] = w_ih[j];
+  for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
   for (int e = threadIdx.x; e < 2 * CELLS; e += blockDim.x)      // constant zero columns 40..47 of both hx buffers
-    *reinterpret_cast<uint4*>(sHX + e * HX_LD + 40) = make_uint4(0u, 0u, 0u, 0u);
+    *reinterpret_cast<uint4*>(sHX + e * D::HX_LD + 40) = make_uint4(0u, 0u, 0u, 0u);
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
@@ -269,11 +350,11 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
       // saved state: c_t, c_{t-1}, h_{t-1} (zero before the first step)
       uint4 vc[2], vcp[2], vhp[2];
       {
-        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off(tile, T, t, warp, 0, lane));
+        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t, warp, 0, lane));
         vc[0] = pc[0]; vc[1] = pc[1];
         if (t > 0) {
-          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off(tile, T, t - 1, warp, 0, lane));
-          const uint4* php = reinterpret_cast<const uint4*>(saved + save_off(tile, T, t - 1, warp, 1, lane));
+          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t - 1, warp, 0, lane));
+          const uint4* php = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t - 1, warp, 1, lane));
           vcp[0] = pcp[0]; vcp[1] = pcp[1]; vhp[0] = php[0]; vhp[1] = php[1];
         } else {
           vcp[0] = vcp[1] = vhp[0] = vhp[1] = make_uint4(0u, 0u, 0u, 0u);
@@ -288,47 +369,20 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
         xw[h] = x_cols(xt[h], q);
       }
       float acc[16][4];
-      gate_mma(acc, hw, xw, wx_addr);
+      gate_mma<1>(acc, [&](int kb, uint32_t (&a)[4]) {
+        a[0] = hw[2 * kb]; a[1] = hw[4 + 2 * kb]; a[2] = hw[2 * kb + 1]; a[3] = hw[4 + 2 * kb + 1];
+      }, xw, wx_addr);
 
       uint32_t da[16][2];             // fp16 pairs: gate column 8 nt + 2 q, +1 of row h, nt = gate * 4 + jn
-      float dx[2] = {0.f, 0.f};
+      float dx[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float fc[8], fcp[8];
-        unpack8(vc[h], fc);
-        unpack8(vcp[h], fcp);
-        float di[8], df[8], dg[8], d_o[8];
+        float d[4][8];
+        dx[h] = cell_grad<1>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, 0, q, d);
 #pragma unroll
-        for (int s = 0; s < 8; ++s) {
-          const int jn = s >> 1, k = 2 * h + (s & 1);
-          // accumulators are -log2e * pre (i, f, o) and -2 log2e * pre (g); clamp from above only (ex2(-big) = 0 is fine),
-          // which keeps the product of three (1 + 2^arg) terms below 1.4e36
-          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
-          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
-          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float ao = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
-          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * fc[s], 40.f));
-          const float pig = ai * ag;
-          const float r1 = rcp_(pig * af), r2 = rcp_(ao * ac);      // 7 SFU ops per unit: see the forward kernel
-          const float gi = r1 * (ag * af), gg = fmaf(r1 + r1, ai * af, -1.f), gf = r1 * pig;
-          const float go = r2 * ac, tcv = fmaf(r2 + r2, ao, -1.f);
-          const float dhv = dh[h][s];
-          const float dcv = fmaf(dhv * go, fmaf(-tcv, tcv, 1.f), dc[h][s]);
-          d_o[s] = (dhv * tcv) * fmaf(-go, go, go);
-          di[s] = (dcv * gg) * fmaf(-gi, gi, gi);
-          df[s] = (dcv * fcp[s]) * fmaf(-gf, gf, gf);
-          dg[s] = (dcv * gi) * fmaf(-gg, gg, 1.f);
-          dc[h][s] = dcv * gf;
-          const int u = 8 * jn + 2 * q + (s & 1);
-          dx[h] += di[s] * s_wih[u] + df[s] * s_wih[C + u] + dg[s] * s_wih[2 * C + u] + d_o[s] * s_wih[3 * C + u];
-        }
+        for (int jn = 0; jn < 4; ++jn)
 #pragma unroll
-        for (int jn = 0; jn < 4; ++jn) {
-          da[jn][h] = pack2(di[2 * jn], di[2 * jn + 1]);
-          da[4 + jn][h] = pack2(df[2 * jn], df[2 * jn + 1]);
-          da[8 + jn][h] = pack2(dg[2 * jn], dg[2 * jn + 1]);
-          da[12 + jn][h] = pack2(d_o[2 * jn], d_o[2 * jn + 1]);
-        }
+          for (int gt = 0; gt < 4; ++gt) da[4 * gt + jn][h] = pack2(d[gt][2 * jn], d[gt][2 * jn + 1]);
       }
       if (d_x != nullptr) {
 #pragma unroll
@@ -361,28 +415,28 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
       }
       // da_t and hx_t of the warp's cells into this step's buffers (last read two steps ago, before the previous step's barrier)
       const int buf = step & 1;
-      __half* sda = sDA + buf * CELLS * DA_LD;
-      __half* shx = sHX + buf * CELLS * HX_LD;
+      __half* sda = sDA + buf * CELLS * D::DA_LD;
+      __half* shx = sHX + buf * CELLS * D::HX_LD;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = warp * 16 + g + 8 * h;
 #pragma unroll
-        for (int nt = 0; nt < 16; ++nt) *reinterpret_cast<uint32_t*>(sda + row * DA_LD + 8 * nt + 2 * q) = da[nt][h];
+        for (int nt = 0; nt < 16; ++nt) *reinterpret_cast<uint32_t*>(sda + row * D::DA_LD + 8 * nt + 2 * q) = da[nt][h];
 #pragma unroll
-        for (int jn = 0; jn < 4; ++jn) *reinterpret_cast<uint32_t*>(shx + row * HX_LD + 8 * jn + 2 * q) = hw[4 * h + jn];
-        *reinterpret_cast<uint32_t*>(shx + row * HX_LD + 32 + 2 * q) = xw[h];
+        for (int jn = 0; jn < 4; ++jn) *reinterpret_cast<uint32_t*>(shx + row * D::HX_LD + 8 * jn + 2 * q) = hw[4 * h + jn];
+        *reinterpret_cast<uint32_t*>(shx + row * D::HX_LD + 32 + 2 * q) = xw[h];
       }
       __syncthreads();
       // dWext[16 warp .. +15][0..47] += da^T x hx over the tile's 128 cells
-      const uint32_t da_b = da_addr + (uint32_t)(buf * CELLS * DA_LD * 2), hx_b = hx_addr + (uint32_t)(buf * CELLS * HX_LD * 2);
+      const uint32_t da_b = da_addr + (uint32_t)(buf * CELLS * D::DA_LD * 2), hx_b = hx_addr + (uint32_t)(buf * CELLS * D::HX_LD * 2);
 #pragma unroll
       for (int kc = 0; kc < 8; ++kc) {
         uint32_t a[4];
-        ldmatrix_x4_trans(da_b + (uint32_t)(((16 * kc + 8 * (mi >> 1) + (lane & 7)) * DA_LD + 16 * warp + 8 * (mi & 1)) * 2), a[0], a[1], a[2], a[3]);
+        ldmatrix_x4_trans(da_b + (uint32_t)(((16 * kc + 8 * (mi >> 1) + (lane & 7)) * D::DA_LD + 16 * warp + 8 * (mi & 1)) * 2), a[0], a[1], a[2], a[3]);
 #pragma unroll
         for (int pr = 0; pr < 3; ++pr) {
           uint32_t b0, b1, b2, b3;
-          ldmatrix_x4_trans(hx_b + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * HX_LD + 16 * pr + 8 * (mi >> 1)) * 2), b0, b1, b2, b3);
+          ldmatrix_x4_trans(hx_b + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * D::HX_LD + 16 * pr + 8 * (mi >> 1)) * 2), b0, b1, b2, b3);
           mma_16816(dw[2 * pr], a, b0, b1);
           mma_16816(dw[2 * pr + 1], a, b2, b3);
         }
@@ -402,122 +456,27 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
     }
 }
 
-__global__ void copy_vec_kernel(const float* src, float* dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[i];
-}
-
-}  // namespace lstm_tc
-
 // =======================================================================================
-// Hidden sizes H = 32 cH (cH = 3, 4: H = 96, 128).  Same semantics and numerics as above (fp16 hi + lo x and affine part,
-// h_{t-1} rounded to fp16 only as MMA operand, fp32 c / gate arguments / h_T, 7 SFU operations per unit and step,
-// power-of-two scaling of d_hT).  What changes with the width:
-//   * a warp owns 16 cells x one 32-unit slice of all four gates (128 gate columns, 64 fp32 accumulators per thread, the
-//     cell update thread-local as above); the cH warps of a 16-cell group exchange h_t through shared memory once per step
-//     (one named barrier per group and step).  A tile is CG groups (Dims::CG: 64 cells at H = 96, 48 at H = 128), CG * cH
-//     warps per CTA, one CTA per SM (the gate weights take 4H x (H + 24) halves of shared memory: 152 KB at H = 128).
-//   * Wx rows are kept in slice order r = 128 js + 32 gate + u (gate row j = gate H + 32 js + u), so a warp's B operand is
-//     one contiguous block of 128 rows, exactly as in the hidden-32 kernel.
-//   * backward: dWext [4H x (H + 16)] no longer fits a CTA's registers (74 K fp32 at H = 128).  The reverse walk writes the
-//     scaled fp16 gate gradients of every (tile, step) to the workspace and a separate tensor-core pass reduces
-//     dWext = sum da^T hx over cells and steps, reading h_{t-1} from the saved state.  The workspace is as large as twice the
-//     saved state; tiling the reduction inside the walk would need either 74 K fp32 of shared memory or a read-modify-write of
-//     a per-CTA fp32 partial every step.  dh_{t-1} = da_t W_hh reads W_hh from the same shared Wx block (ldmatrix.trans),
-//     since a transposed copy does not fit beside it; da_t is divided by the row scale s_j before it is rounded to fp16
-//     and the weight-gradient pass multiplies s_j back.
+// H = 96, 128
 // =======================================================================================
-namespace lstm_tcw {
-
-using lstm_tc::ex2_;
-using lstm_tc::rcp_;
-using lstm_tc::pack2;
-using lstm_tc::pack8;
-using lstm_tc::unpack8;
-using lstm_tc::x_base;
-using lstm_tc::x_cols;
-
-constexpr float kLn2 = 0.69314718055994531f;
-
-template <int CH>
-struct Dims {
-  // 16-cell groups per tile: 4 at H = 96 (12 warps, <= 168 registers per thread), 3 at H = 128 (12 warps; 16 warps would cap a
-  // thread at 128 registers, which the backward walk exceeds)
-  static constexpr int CG = CH == 4 ? 3 : 4;
-  static constexpr int CELLS = 16 * CG;
-  static constexpr int H = 32 * CH;
-  static constexpr int G4 = 4 * H;
-  static constexpr int KX = H + 16;            // operand row of a cell: h_{t-1} (H) | x columns (16, see lstm_tc::load_wx)
-  static constexpr int WX_LD = KX + 8;         // padded so that 8 consecutive rows fall in distinct 16-byte bank groups
-  static constexpr int H_LD = H + 8;           // h exchange tile row stride
-  static constexpr int DA_LD = G4 + 8;         // da tile row stride
-  static constexpr int NW = CG * CH;           // warps per CTA
-  static constexpr int THREADS = 32 * NW;
-  static constexpr int TILE_HALVES = CELLS * H * 2;     // saved c_t | h_t per (tile, step)
-  static constexpr size_t kFwdSmem = (size_t)(G4 * WX_LD + 2 * CELLS * H_LD) * sizeof(__half);
-  static constexpr size_t kBwdSmem = (size_t)(G4 * WX_LD + CELLS * DA_LD) * sizeof(__half) + (size_t)(CELLS * CH + G4) * sizeof(float);
-};
-
-// gate row j of slice-ordered row r (see above)
-template <int CH>
-__device__ __forceinline__ int gate_row(int r) { return (r & 127) / 32 * (32 * CH) + 32 * (r >> 7) + (r & 31); }
-__device__ __forceinline__ float row_scale(int r) { return ((r & 127) >> 5) == 2 ? -2.8853900817779268f : -1.4426950408889634f; }
-
-// Wx[r][k] = s_j * [ W_hh[j,:] | wih_hi  b_hi  wih_hi  wih_lo  b_lo  0 0 0 | 0 .. ], j = gate_row(r): lstm_tc::load_wx at width H
-template <int CH>
-__device__ void load_wx_w(__half* sWx, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh) {
-  using D = Dims<CH>;
-  constexpr int NCH = D::KX / 8;
-  for (int e = threadIdx.x; e < D::G4 * NCH; e += blockDim.x) {
-    const int r = e / NCH, ch = e % NCH, j = gate_row<CH>(r);
-    const float sc = row_scale(r);
-    float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (ch < D::H / 8) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = sc * w_hh[(size_t)j * D::H + ch * 8 + i];
-    } else if (ch == D::H / 8) {
-      const float wi = sc * w_ih[j], bb = sc * (b_ih[j] + b_hh[j]);
-      const float wi_hi = __half2float(__float2half_rn(wi)), b_hi = __half2float(__float2half_rn(bb));
-      v[0] = wi_hi; v[1] = b_hi; v[2] = wi_hi; v[3] = wi - wi_hi; v[4] = bb - b_hi;
-    }
-    *reinterpret_cast<uint4*>(sWx + r * D::WX_LD + ch * 8) = pack8(v);
-  }
-}
-
-// acc[nt] (nt = gate * 4 + jn) += hx_t . Wx^T for the warp's 16 cells and 128 gate columns.  a_h(kb, a) supplies the A fragment
-// of h-block kb < 2 cH; xw[h] are the x columns of row h (k-block 2 cH).  wx_addr: first of the warp's 128 Wx rows.
-template <int CH, class AH>
-__device__ __forceinline__ void gate_mma_w(float (&acc)[16][4], AH&& a_h, const uint32_t (&xw)[2], uint32_t wx_addr) {
-  using D = Dims<CH>;
-  const int lane = threadIdx.x & 31, mi = lane >> 3;
-#pragma unroll
-  for (int nt = 0; nt < 16; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-#pragma unroll
-  for (int kb = 0; kb <= 2 * CH; ++kb) {
-    uint32_t a[4];
-    if (kb < 2 * CH) a_h(kb, a);
-    else { a[0] = xw[0]; a[1] = xw[1]; a[2] = 0u; a[3] = 0u; }
-#pragma unroll
-    for (int pr = 0; pr < 8; ++pr) {
-      uint32_t b0, b1, b2, b3;
-      ldmatrix_x4(wx_addr + (uint32_t)(((16 * pr + 8 * (mi >> 1) + (lane & 7)) * D::WX_LD + 16 * kb + 8 * (mi & 1)) * 2), b0, b1, b2, b3);
-      mma_16816(acc[2 * pr], a, b0, b1);
-      mma_16816(acc[2 * pr + 1], a, b2, b3);
-    }
-  }
-}
-
-// Training state: per (tile, step) NW x 1024 halves, [warp][c | h][lane][16 halves] as in lstm_tc::save_off; warp = cg cH + js.
-template <int CH>
-__device__ __forceinline__ size_t save_off_w(long long tile, int T, int t, int warp, int kind, int lane) {
-  return ((size_t)tile * T + t) * Dims<CH>::TILE_HALVES + (size_t)warp * 1024 + (size_t)kind * 512 + (size_t)lane * 16;
-}
+// A warp owns one 32-unit slice js of all four gates (128 of the 4H gate columns), and the CH warps of a 16-cell group cg
+// exchange h_t through shared memory once per step (one named barrier per group and step).  One CTA per SM: the gate weights
+// take 4H x (H + 24) halves of shared memory, 152 KB at H = 128.
+// Backward: dWext [4H x (H + 16)] no longer fits a CTA's registers (74 K fp32 at H = 128).  The reverse walk writes the scaled
+// fp16 gate gradients of every (tile, step) to the workspace and a separate tensor-core pass reduces dWext = sum da^T hx over
+// cells and steps, reading h_{t-1} from the saved state.  The workspace is as large as twice the saved state; tiling the
+// reduction inside the walk would need either 74 K fp32 of shared memory or a read-modify-write of a per-CTA fp32 partial every
+// step.  dh_{t-1} = da_t W_hh reads W_hh from the same shared Wx block (ldmatrix.trans), since a transposed copy does not fit
+// beside it; da_t is divided by the row scale s_j before it is rounded to fp16 and the weight-gradient pass multiplies s_j back.
 
 // ---------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------
+template <int CH>
+constexpr size_t kFwdWideSmem = (size_t)(Dims<CH>::G4 * Dims<CH>::WX_LD + 2 * Dims<CH>::CELLS * Dims<CH>::H_LD) * sizeof(__half);
+
 template <int CH, bool SAVE>
-__global__ void __launch_bounds__(Dims<CH>::THREADS, 1)
+__global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::FWD_CTAS_PER_SM)
 lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                     const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
                     long long cells, int T, long long NN) {
@@ -526,7 +485,7 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [G4][WX_LD], slice order
   __half* sH = sWx + D::G4 * D::WX_LD;                     // 2 x [CELLS][H_LD]: h_t of the tile, double-buffered by step
-  load_wx_w<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
+  load_wx<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   const int cg = warp / CH, js = warp % CH;
@@ -558,36 +517,17 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
       // h_{t-1} was written to buffer t & 1 before the previous step's barrier; zero before the first step
       const uint32_t hb = h_addr + (uint32_t)((t & 1) * CELLS * D::H_LD * 2);
       float acc[16][4];
-      gate_mma_w<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
+      gate_mma<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
         if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; }
         else ldmatrix_x4(hb + 32 * kb, a[0], a[1], a[2], a[3]);
       }, xw, wx_addr);
 #pragma unroll
       for (int h = 0; h < 2; ++h) xv[h] = (live[h] && t + 1 < T) ? x_seq[xb[h] + (size_t)(t + 1) * NN] : 0.f;
       float hv[2][8];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int s = 0; s < 8; ++s) {        // the hidden-32 cell update, see lstm_tc::lstm_fwd_tc_kernel
-          const int jn = s >> 1, k = 2 * h + (s & 1);
-          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
-          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
-          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float p = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
-          const float pig = ai * ag;
-          const float r = rcp_(pig * af);
-          const float gi = r * (ag * af);
-          const float gg = fmaf(r + r, ai * af, -1.f);
-          const float gf = r * pig;
-          c[h][s] = fmaf(gf, c[h][s], gi * gg);
-          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * c[h][s], 40.f));
-          const float r2 = rcp_(p * ac);
-          hv[h][s] = (r2 * ac) * fmaf(r2 + r2, p, -1.f);
-        }
-      }
+      cell_update(acc, c, hv);
       if (SAVE) {
-        uint4* dc = reinterpret_cast<uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 0, lane));
-        uint4* dh = reinterpret_cast<uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 1, lane));
+        uint4* dc = reinterpret_cast<uint4*>(saved + save_off<CH>(tile, T, t, warp, 0, lane));
+        uint4* dh = reinterpret_cast<uint4*>(saved + save_off<CH>(tile, T, t, warp, 1, lane));
         dc[0] = pack8(c[0]); dc[1] = pack8(c[1]);
         dh[0] = pack8(hv[0]); dh[1] = pack8(hv[1]);
       }
@@ -619,9 +559,13 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
 // Per step and warp: gates_t = hx_t x Wx^T (A = the group's saved h_{t-1}, read per k-block from global memory, + x columns);
 // the thread-local cell gradient; da'_t = da_t / s_j of the warp's 128 gate columns into the group's rows of the shared da
 // tile and into the workspace record of (tile, t) (rows = cells, 4H columns in slice order); after the group barrier
-// dh_{t-1}[slice] = da'_t x (s W_hh) over all 4H gates, and dx = sum of the cH slice partials in a fixed order.
+// dh_{t-1}[slice] = da'_t x (s W_hh) over all 4H gates, and dx = sum of the CH slice partials in a fixed order.
 template <int CH>
-__global__ void __launch_bounds__(Dims<CH>::THREADS, 1)
+constexpr size_t kWalkSmem = (size_t)(Dims<CH>::G4 * Dims<CH>::WX_LD + Dims<CH>::CELLS * Dims<CH>::DA_LD) * sizeof(__half) +
+                             (size_t)(Dims<CH>::CELLS * CH + Dims<CH>::G4) * sizeof(float);
+
+template <int CH>
+__global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::BWD_CTAS_PER_SM)
 lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                          float* __restrict__ d_x, const __half* __restrict__ saved, __half* __restrict__ da_rec,
@@ -633,7 +577,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
   __half* sDA = sWx + D::G4 * D::WX_LD;                    // [CELLS][DA_LD]: da'_t, columns in slice order
   float* sDX = reinterpret_cast<float*>(sDA + CELLS * D::DA_LD);   // [CELLS][CH]: dx partial of each slice
   float* s_wih = sDX + CELLS * CH;                         // [G4] by gate row j
-  load_wx_w<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
+  load_wx<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
   for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
   __syncthreads();
 
@@ -671,9 +615,9 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
       for (int h = 0; h < 2; ++h) xw[h] = x_cols(live[h] ? x_seq[xb[h] + (size_t)t * NN] : 0.f, q);
       // h_{t-1} of slice kb / 2 is the same lane's saved fragment of warp (cg, kb / 2): k-block kb = 2 sl + kk takes its
       // words (h, 2 kk) and (h, 2 kk + 1), i.e. the uint2 number 2 h + kk of the 16 halves
-      const __half* hp = saved + (t > 0 ? save_off_w<CH>(tile, T, t - 1, cg * CH, 1, lane) : 0);
+      const __half* hp = saved + (t > 0 ? save_off<CH>(tile, T, t - 1, cg * CH, 1, lane) : 0);
       float acc[16][4];
-      gate_mma_w<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
+      gate_mma<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
         if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; return; }
         const uint2* p = reinterpret_cast<const uint2*>(hp + (kb >> 1) * 1024);
         const uint2 r0 = __ldg(p + (kb & 1)), r1 = __ldg(p + 2 + (kb & 1));
@@ -682,53 +626,28 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
 
       uint4 vc[2], vcp[2];
       {
-        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t, warp, 0, lane));
+        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off<CH>(tile, T, t, warp, 0, lane));
         vc[0] = pc[0]; vc[1] = pc[1];
         if (t > 0) {
-          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t - 1, warp, 0, lane));
+          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off<CH>(tile, T, t - 1, warp, 0, lane));
           vcp[0] = pcp[0]; vcp[1] = pcp[1];
         } else {
           vcp[0] = vcp[1] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
       uint32_t da[16][2];             // fp16 pairs of da' = da / s_j: gate column 8 nt + 2 q, +1 of row h, nt = gate * 4 + jn
-      float dx[2] = {0.f, 0.f};
+      float dx[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float fc[8], fcp[8];
-        unpack8(vc[h], fc);
-        unpack8(vcp[h], fcp);
-        float di[8], df[8], dg[8], d_o[8];
+        float d[4][8];
+        dx[h] = cell_grad<CH>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, js, q, d);
 #pragma unroll
-        for (int s = 0; s < 8; ++s) {        // the hidden-32 cell gradient, see lstm_tc::lstm_bwd_saved_tc_kernel
-          const int jn = s >> 1, k = 2 * h + (s & 1);
-          const float ai = 1.f + ex2_(fminf(acc[jn][k], 40.f));
-          const float af = 1.f + ex2_(fminf(acc[4 + jn][k], 40.f));
-          const float ag = 1.f + ex2_(fminf(acc[8 + jn][k], 40.f));
-          const float ao = 1.f + ex2_(fminf(acc[12 + jn][k], 40.f));
-          const float ac = 1.f + ex2_(fminf(-2.8853900817779268f * fc[s], 40.f));
-          const float pig = ai * ag;
-          const float r1 = rcp_(pig * af), r2 = rcp_(ao * ac);
-          const float gi = r1 * (ag * af), gg = fmaf(r1 + r1, ai * af, -1.f), gf = r1 * pig;
-          const float go = r2 * ac, tcv = fmaf(r2 + r2, ao, -1.f);
-          const float dhv = dh[h][s];
-          const float dcv = fmaf(dhv * go, fmaf(-tcv, tcv, 1.f), dc[h][s]);
-          d_o[s] = (dhv * tcv) * fmaf(-go, go, go);
-          di[s] = (dcv * gg) * fmaf(-gi, gi, gi);
-          df[s] = (dcv * fcp[s]) * fmaf(-gf, gf, gf);
-          dg[s] = (dcv * gi) * fmaf(-gg, gg, 1.f);
-          dc[h][s] = dcv * gf;
-          const int u = 32 * js + 8 * jn + 2 * q + (s & 1);
-          dx[h] += di[s] * s_wih[u] + df[s] * s_wih[D::H + u] + dg[s] * s_wih[2 * D::H + u] + d_o[s] * s_wih[3 * D::H + u];
-        }
-        // 1 / s: -ln 2 for i, f, o and -ln 2 / 2 for g
+        for (int jn = 0; jn < 4; ++jn)
 #pragma unroll
-        for (int jn = 0; jn < 4; ++jn) {
-          da[jn][h] = pack2(-kLn2 * di[2 * jn], -kLn2 * di[2 * jn + 1]);
-          da[4 + jn][h] = pack2(-kLn2 * df[2 * jn], -kLn2 * df[2 * jn + 1]);
-          da[8 + jn][h] = pack2(-0.5f * kLn2 * dg[2 * jn], -0.5f * kLn2 * dg[2 * jn + 1]);
-          da[12 + jn][h] = pack2(-kLn2 * d_o[2 * jn], -kLn2 * d_o[2 * jn + 1]);
-        }
+          for (int gt = 0; gt < 4; ++gt) {
+            const float inv_s = gt == 2 ? -0.5f * kLn2 : -kLn2;     // 1 / s_j: -ln 2 for i, f, o and -ln 2 / 2 for g
+            da[4 * gt + jn][h] = pack2(inv_s * d[gt][2 * jn], inv_s * d[gt][2 * jn + 1]);
+          }
         dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 1);
         dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 2);
       }
@@ -798,7 +717,7 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
                    long long cells, int T, long long NN) {
   using D = Dims<CH>;
   constexpr int CELLS = D::CELLS;
-  constexpr int HX_LD = D::KX + 8;
+  constexpr int HX_LD = D::HX_LD;
   constexpr int NX = D::KX / 8;                 // n8 tiles of columns
   __shared__ __align__(16) __half sDA[CELLS * DW_DA_LD];
   __shared__ __align__(16) __half sHX[CELLS * HX_LD];
@@ -826,7 +745,7 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     for (int e = threadIdx.x; e < D::NW * 64; e += blockDim.x) {    // saved h_{t-1}: (warp, lane, row half) -> 4 words
       const int w = e >> 6, l = (e >> 1) & 31, h = e & 1;
       const int row = (w / CH) * 16 + (l >> 2) + 8 * h, col = 32 * (w % CH) + 2 * (l & 3);
-      const uint4 v = t > 0 ? __ldg(reinterpret_cast<const uint4*>(saved + save_off_w<CH>(tile, T, t - 1, w, 1, l)) + h)
+      const uint4 v = t > 0 ? __ldg(reinterpret_cast<const uint4*>(saved + save_off<CH>(tile, T, t - 1, w, 1, l)) + h)
                             : make_uint4(0u, 0u, 0u, 0u);
       uint32_t* d = reinterpret_cast<uint32_t*>(sHX + row * HX_LD + col);
       d[0] = v.x; d[4] = v.y; d[8] = v.z; d[12] = v.w;
@@ -864,36 +783,41 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     }
 }
 
-}  // namespace lstm_tcw
+__global__ void copy_vec_kernel(const float* src, float* dst, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = src[i];
+}
+
+}  // namespace lstm_tc
 
 // ---------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------
+using lstm_tc::Dims;
+
 bool lstm_tc_supported(int T, int C) { return (C == 32 || C == 96 || C == 128) && T >= 1 && T <= 256; }
 
-static int lstm_grid(long long cells, int per_sm, int tile_cells = lstm_tc::CELLS) {
-  const long long tiles = (cells + tile_cells - 1) / tile_cells;
-  long long g = (long long)per_sm * device_sm_count();
+template <int CH>
+static int lstm_grid(long long cells, int ctas_per_sm) {
+  const long long tiles = (cells + Dims<CH>::CELLS - 1) / Dims<CH>::CELLS;
+  long long g = (long long)ctas_per_sm * device_sm_count();
   return (int)(g < tiles ? g : tiles);
 }
 
-// cells per tile of the wide kernels (lstm_tcw::Dims)
-static int lstm_tcw_cells(int C) { return C == 128 ? lstm_tcw::Dims<4>::CELLS : lstm_tcw::Dims<3>::CELLS; }
-static long long lstm_tcw_padded_cells(int B, long long NN, int C) {
-  const long long tc = lstm_tcw_cells(C);
+// cells of B NN rounded up to whole tiles of the width's kernels
+static long long lstm_tc_padded_cells(int B, long long NN, int C) {
+  const long long tc = C == 32 ? Dims<1>::CELLS : C == 96 ? Dims<3>::CELLS : Dims<4>::CELLS;
   return ((long long)B * NN + tc - 1) / tc * tc;
 }
 
+// c_t | h_t of every cell (tiles padded) and step: 2 C halves, see lstm_tc::save_off
 size_t lstm_tc_saved_bytes(int B, int T, long long NN, int C) {
-  if (C != 32)      // c_t | h_t of every cell (tiles padded) and step: 2 C halves, see lstm_tcw::save_off_w
-    return (size_t)lstm_tcw_padded_cells(B, NN, C) * T * 2 * C * sizeof(__half);
-  const long long tiles = ((long long)B * NN + lstm_tc::CELLS - 1) / lstm_tc::CELLS;
-  return (size_t)tiles * T * 8192 * sizeof(__half);      // see lstm_tc::save_off
+  return (size_t)lstm_tc_padded_cells(B, NN, C) * T * 2 * C * sizeof(__half);
 }
 
-// wide widths: the gate-gradient records of the reverse walk, 4 C halves per cell and step (lstm_tcw::lstm_bwd_walk_tcw_kernel)
+// wide widths: the gate-gradient records of the reverse walk, 4 C halves per cell and step (lstm_tc::lstm_bwd_walk_tcw_kernel)
 static size_t lstm_tcw_da_bytes(int B, int T, long long NN, int C) {
-  return (size_t)lstm_tcw_padded_cells(B, NN, C) * T * 4 * C * sizeof(__half);
+  return (size_t)lstm_tc_padded_cells(B, NN, C) * T * 4 * C * sizeof(__half);
 }
 
 // workspace of a backward that is handed the forward's saved state: the grad scale (1 KB) and, at the wide widths, the da records
@@ -909,13 +833,31 @@ size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) {
 template <int CH>
 static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
                             void* saved, long long cells, int T, long long NN, cudaStream_t st) {
-  using D = lstm_tcw::Dims<CH>;
-  auto kern = saved ? lstm_tcw::lstm_fwd_tcw_kernel<CH, true> : lstm_tcw::lstm_fwd_tcw_kernel<CH, false>;
+  using D = Dims<CH>;
+  auto kern = saved ? lstm_tc::lstm_fwd_tcw_kernel<CH, true> : lstm_tc::lstm_fwd_tcw_kernel<CH, false>;
+  constexpr size_t smem = lstm_tc::kFwdWideSmem<CH>;
   static DynSmemAttr attr_t = {}, attr_f = {};
-  if (int e = ensure_dyn_smem(kern, (int)D::kFwdSmem, saved ? attr_t : attr_f)) return e;
+  if (int e = ensure_dyn_smem(kern, (int)smem, saved ? attr_t : attr_f)) return e;
   prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  kern<<<lstm_grid(cells, 1, D::CELLS), D::THREADS, D::kFwdSmem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
-                                                                               cells, T, NN);
+  kern<<<lstm_grid<CH>(cells, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT,
+                                                                           static_cast<__half*>(saved), cells, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// lstm_backward_h32 and lstm_backward_tcw<CH>: the kernels of one width's backward, run once the grad scale and the zeroed
+// weight gradients are in place.  da_rec: the gate-gradient records of the wide walk (the hidden-32 walk keeps them on chip).
+static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved,
+                             void* /*da_rec*/, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+  using D = Dims<1>;
+  if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
+  static DynSmemAttr attr_b = {};
+  if (int e = ensure_dyn_smem(lstm_tc::lstm_bwd_saved_tc_kernel, (int)lstm_tc::kBwdSavedSmem, attr_b)) return e;
+  prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)cells * T, st);
+  lstm_tc::lstm_bwd_saved_tc_kernel<<<lstm_grid<1>(cells, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -925,12 +867,13 @@ template <int CH>
 static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, void* da_rec,
                              const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
-  using D = lstm_tcw::Dims<CH>;
+  using D = Dims<CH>;
+  constexpr size_t smem = lstm_tc::kWalkSmem<CH>;
   static DynSmemAttr attr_b = {};
-  if (int e = ensure_dyn_smem(lstm_tcw::lstm_bwd_walk_tcw_kernel<CH>, (int)D::kBwdSmem, attr_b)) return e;
+  if (int e = ensure_dyn_smem(lstm_tc::lstm_bwd_walk_tcw_kernel<CH>, (int)smem, attr_b)) return e;
   // walk: the gate recompute and dh_{t-1} (2 x 8 H (H + 1) per cell and step, as the hidden-32 count splits it) ...
   prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  lstm_tcw::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid(cells, 1, D::CELLS), D::THREADS, D::kBwdSmem, st>>>(
+  lstm_tc::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid<CH>(cells, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(
       x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
@@ -939,7 +882,7 @@ static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float*
   long long splits = 4LL * device_sm_count() / CH;
   if (splits > records) splits = records;
   prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  lstm_tcw::lstm_dw_tcw_kernel<CH><<<dim3(CH, (unsigned)splits), lstm_tcw::DW_THREADS, 0, st>>>(
+  lstm_tc::lstm_dw_tcw_kernel<CH><<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, 0, st>>>(
       x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
@@ -947,16 +890,17 @@ static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float*
 }
 
 int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                         void* saved, int B, int T, long long NN, int C_, cudaStream_t st) {
-  using namespace lstm_tc;
+                         void* saved, int B, int T, long long NN, int C, cudaStream_t st) {
+  using D = Dims<1>;
   const long long cells = (long long)B * NN;
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm forward: saved buffer must be 16-byte aligned");
-  if (C_ == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
-  if (C_ == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
-  MPGCN_CHECK(C_ == C, "lstm forward: no tensor-core kernel for hidden=%d", C_);
-  auto kern = saved ? lstm_fwd_tc_kernel<true> : lstm_fwd_tc_kernel<false>;
+  if (C == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
+  if (C == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
+  MPGCN_CHECK(C == D::H, "lstm forward: no tensor-core kernel for hidden=%d", C);
+  auto kern = saved ? lstm_tc::lstm_fwd_tc_kernel<true> : lstm_tc::lstm_fwd_tc_kernel<false>;
   prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)cells * T, st);
-  kern<<<lstm_grid(cells, 2), FWD_THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells, T, NN);
+  kern<<<lstm_grid<1>(cells, D::FWD_CTAS_PER_SM), D::THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
+                                                                       cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -964,51 +908,30 @@ int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_h
 
 int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                           const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
-                          int B, int T, long long NN, int C_, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
-  using namespace lstm_tc;
+                          int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
   const long long cells = (long long)B * NN;
-  const size_t need = saved ? lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C_) : lstm_tc_bwd_workspace_bytes(B, T, NN, C_);
+  const size_t need = saved ? lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C) : lstm_tc_bwd_workspace_bytes(B, T, NN, C);
   MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, need);
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm backward: saved buffer must be 16-byte aligned");
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
-  MPGCN_CHECK(C_ == C || C_ == 96 || C_ == 128, "lstm backward: no tensor-core kernel for hidden=%d", C_);
+  MPGCN_CHECK(C == 32 || C == 96 || C == 128, "lstm backward: no tensor-core kernel for hidden=%d", C);
   float* scale2 = static_cast<float*>(ws);
+  void* da_rec = static_cast<uint8_t*>(ws) + 1024;   // wide widths: the da records follow the grad scale
   if (saved == nullptr) {          // the caller kept no forward state: rebuild it (same kernel, same bits as the training forward)
-    void* tmp = static_cast<uint8_t*>(ws) + lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C_);
-    if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C_, st)) return e;
+    void* tmp = static_cast<uint8_t*>(ws) + lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C);
+    if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C, st)) return e;
     saved = tmp;
   }
-  if (C_ != C) {                   // wide widths: walk + weight-gradient pass; the da records follow the grad scale
-    const int G4w = 4 * C_;
-    void* da_rec = static_cast<uint8_t*>(ws) + 1024;
-    if (int e = grad_scale_prepare(d_hT, (size_t)cells * C_, scale2, d_hT_absmax, st)) return e;
-    MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4w, st));
-    MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4w * C_, st));
-    MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4w, st));
-    const int e = C_ == 96 ? lstm_backward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2,
-                                                  cells, T, NN, st)
-                           : lstm_backward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2,
-                                                  cells, T, NN, st);
-    if (e) return e;
-    prof_count(PROF_ELEMENTWISE);
-    copy_vec_kernel<<<(G4w + 127) / 128, 128, 0, st>>>(d_b_ih, d_b_hh, G4w);
-    MPGCN_CUDA(cudaGetLastError());
-    return 0;
-  }
+  const int G4 = 4 * C;
   if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
   MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4, st));
   MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4 * C, st));
   MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4, st));
-  if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  static DynSmemAttr attr_b = {};
-  if (int e = ensure_dyn_smem(lstm_bwd_saved_tc_kernel, (int)kBwdSmem, attr_b)) return e;
-  prof_begin(PROF_LSTM_BWD, 12.0 * C * (C + 1) * (double)cells * T, st);
-  lstm_bwd_saved_tc_kernel<<<lstm_grid(cells, 1), BWD_THREADS, kBwdSmem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x,
-                                                                               static_cast<const __half*>(saved), scale2, cells, T, NN);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
+  auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
+  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2, cells, T, NN, st))
+    return e;
   prof_count(PROF_ELEMENTWISE);
-  copy_vec_kernel<<<1, G4, 0, st>>>(d_b_ih, d_b_hh, G4);
+  lstm_tc::copy_vec_kernel<<<(G4 + 127) / 128, 128, 0, st>>>(d_b_ih, d_b_hh, G4);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }

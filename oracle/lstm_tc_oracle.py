@@ -2,7 +2,7 @@
 
 Test infrastructure, numpy only.  It reproduces what the kernels round and nothing else:
 
-  * the gate weights `Wx` exactly as `load_wx` / `load_wx_w` build them: `s_j*W_hh` rounded to fp16, `s_j*w_ih` and `s_j*b`
+  * the gate weights `Wx` exactly as `load_wx` builds them: `s_j*W_hh` rounded to fp16, `s_j*w_ih` and `s_j*b`
     (b = b_ih + b_hh, formed in fp32) each split into an fp16 hi part and a separately fp16-rounded lo part, with
     `s_j = -log2 e` for the i, f, o gates and `-2 log2 e` for g;
   * the operand row of a cell as `x_cols` builds it, `[h_{t-1} | x_hi 1 x_lo x_hi 1]`, x saturated at +-65504;
@@ -18,8 +18,8 @@ GEMM read, since `pack2` / `pack8` round the same fp32 value) and emulates one r
 from the saved `h_{t-1}`, the power-of-two gradient scale S applied before the fp16 rounding of `da_t` (and at hidden 96 / 128
 the division by `s_j`), `dh_{t-1}` from the operands the kernel's dh GEMM reads, and `dWext = sum da_t^T hx_t`.
 
-Decoders map the kernels' buffers to [cell, t, unit] arrays: the saved state (`save_off` at hidden 32, `save_off_w` at 96 / 128;
-DESIGN.md section 5) and the gate-gradient records of the wide backward (`[tile][t][cell][4H]`, columns `128 js + 32 gate + u`).
+Decoders map the kernels' buffers to [cell, t, unit] arrays: the saved state (`save_off`, DESIGN.md section 5) and the
+gate-gradient records of the wide backward (`[tile][t][cell][4H]`, columns `128 js + 32 gate + u`).
 """
 import numpy as np
 
@@ -63,7 +63,7 @@ def x_split(x, exact=False, keep_xlo=True):
 
 
 def build_wx(w_ih, w_hh, b_ih, b_hh, exact=False, keep_wlo=True, keep_blo=True):
-    """Wx as load_wx builds it (natural gate-row order) -> dict of float64 arrays: whh [4C,C] = fp16(s_j W_hh), wi_hi, wi_lo,
+    """Wx as load_wx builds it, in natural gate-row order -> dict of float64 arrays: whh [4C,C] = fp16(s_j W_hh), wi_hi, wi_lo,
     b_hi, b_lo [4C], and s [4C] (float32 s_j)."""
     w_hh = np.asarray(w_hh, np.float32)
     C = w_hh.shape[1]
@@ -244,7 +244,7 @@ def tiles(cells, H):
 def decode_saved(buf, cells, T, H):
     """The training forward's saved state -> (c, h) [cells, T, H] float64.  buf: the fp16 buffer (numpy float16, at least
     tiles * T * CELLS * 2H halves).  Per (tile, step) the warps w = cg CH + js hold [c | h][lane][16 halves]; slot h2 * 8 + s of
-    lane l = 4 g + q is cell tile * CELLS + 16 cg + g + 8 h2 and unit 32 js + 8 (s >> 1) + 2 q + (s & 1) (save_off, save_off_w)."""
+    lane l = 4 g + q is cell tile * CELLS + 16 cg + g + 8 h2 and unit 32 js + 8 (s >> 1) + 2 q + (s & 1) (save_off)."""
     CH, CG, CELLS = dims(H)
     nt = tiles(cells, H)
     a = np.asarray(buf)[:nt * T * CELLS * 2 * H].reshape(nt, T, CG, CH, 2, 8, 4, 2, 4, 2)

@@ -182,7 +182,7 @@ def test_decoders_invert_the_kernel_layouts(H):
     rec = emu.decode_da_records(emu.encode_da_records(da, H), cells, T, H)
     assert np.array_equal(rec[:cells], da.astype(np.float64)) and not rec[cells:].any()
 
-    # the formulas of save_off / save_off_w and of the fragment: every half of the buffer lands on its (cell, t, unit)
+    # the formulas of save_off and of the fragment: every half of the buffer lands on its (cell, t, unit)
     nt = emu.tiles(cells, H)
     buf = np.arange(nt * T * CELLS * 2 * H, dtype=np.int64)
     tile, t, w, kind, lane, slot = np.unravel_index(buf, (nt, T, CG * CH, 2, 32, 16))
