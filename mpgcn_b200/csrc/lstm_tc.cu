@@ -13,10 +13,11 @@
 // returned h_T stay fp32.  Activations cost 7 SFU operations per hidden unit and step.  The training forward (SAVE) also
 // stores c_t, h_t (fp16) of every step; a backward call that comes without that state first re-runs the SAVE forward into its
 // workspace.  The instances differ in how h_t and the weight gradient move between warps (details at each kernel):
-//   H = 32    lstm_fwd_tc_kernel<SAVE>, lstm_bwd_saved_tc_kernel.  A warp holds all 4H gate columns, so the new h_t is
+//   H = 32    lstm_fwd_tc_kernel<SAVE>, lstm_bwd_saved_tc_kernel<DX>.  A warp holds all 4H gate columns, so the new h_t is
 //             already the A fragment of the next step's MMA: the recurrence never leaves registers and a step needs no
 //             barrier.  128-cell tiles, 8 warps, 2 CTAs per SM in the forward.  The backward is one reverse walk that keeps
-//             dWext [128 x 48] in registers across every step and tile of the CTA and reads W_hh^T from its own shared copy.
+//             dWext [128 x 48] in registers across every step and tile of the CTA and reads W_hh^T from its own shared copy;
+//             its warps share only the dWext operands, through a ring of shared tiles guarded by mbarriers.
 //   H = 96,   lstm_fwd_tcw_kernel<CH, SAVE>, lstm_bwd_walk_tcw_kernel<CH>, lstm_dw_tcw_kernel<CH>.  The CH warps of a group
 //   H = 128   exchange h_t through shared memory, one named barrier per group and step; one CTA per SM.  dWext fits neither
 //             in registers nor in shared memory, so the walk writes its gate gradients to the workspace and a separate pass
@@ -123,7 +124,8 @@ __device__ __forceinline__ uint32_t x_cols(float x, int q) {
 }
 
 // acc[nt] (nt = gate * 4 + jn) = hx_t . Wx^T for the warp's 16 cells and 128 gate columns.  a_h(kb, a) supplies the A fragment
-// of h-block kb < 2 CH; xw[h] are the x columns of row h (k-block 2 CH).  wx_addr: first of the warp's 128 Wx rows.
+// of h-block kb < 2 CH; xw[h] are the x columns H .. H + 7 of row h, the only nonzero columns of the last k-block, which
+// therefore runs as m16n8k8 (columns H + 8 .. H + 15 would add exact zeros).  wx_addr: first of the warp's 128 Wx rows.
 template <int CH, class AH>
 __device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const uint32_t (&xw)[2], uint32_t wx_addr) {
   using D = Dims<CH>;
@@ -131,10 +133,9 @@ __device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const ui
 #pragma unroll
   for (int nt = 0; nt < 16; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
 #pragma unroll
-  for (int kb = 0; kb <= 2 * CH; ++kb) {
+  for (int kb = 0; kb < 2 * CH; ++kb) {
     uint32_t a[4];
-    if (kb < 2 * CH) a_h(kb, a);
-    else { a[0] = xw[0]; a[1] = xw[1]; a[2] = 0u; a[3] = 0u; }
+    a_h(kb, a);
 #pragma unroll
     for (int pr = 0; pr < 8; ++pr) {
       uint32_t b0, b1, b2, b3;
@@ -142,6 +143,13 @@ __device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const ui
       mma_16816(acc[2 * pr], a, b0, b1);
       mma_16816(acc[2 * pr + 1], a, b2, b3);
     }
+  }
+#pragma unroll
+  for (int pr = 0; pr < 8; ++pr) {   // x columns: the k-half H .. H + 7 of n8 tiles 2 pr, 2 pr + 1
+    uint32_t b0, b1;
+    ldmatrix_x2(wx_addr + (uint32_t)(((16 * pr + 8 * (mi & 1) + (lane & 7)) * D::WX_LD + 32 * CH) * 2), b0, b1);
+    mma_1688(acc[2 * pr], xw[0], xw[1], b0);
+    mma_1688(acc[2 * pr + 1], xw[0], xw[1], b1);
   }
 }
 
@@ -175,9 +183,9 @@ __device__ __forceinline__ void cell_update(const float (&acc)[16][4], float (&c
 
 // The gate gradients of cell row h at one step of the reverse walk, from the gate accumulators recomputed from the saved
 // h_{t-1}, the saved c_t, c_{t-1} (vc, vcp) and the incoming dh, dc of the row's 8 units (dc becomes dc_{t-1} in place):
-// d[gate][s] for gates i, f, g, o.  Returns the thread's part of the row's dx = sum over its units u of d[.][s] w_ih[. H + u]
-// (s_wih: w_ih by gate row; js: the warp's unit slice).  The 7 SFU operations of cell_update.
-template <int CH>
+// d[gate][s] for gates i, f, g, o.  With DX, returns the thread's part of the row's dx = sum over its units u of
+// d[.][s] w_ih[. H + u] (s_wih: w_ih by gate row; js: the warp's unit slice); without, 0.  The 7 SFU operations of cell_update.
+template <int CH, bool DX>
 __device__ __forceinline__ float cell_grad(const float (&acc)[16][4], int h, const uint4& vc, const uint4& vcp, const float (&dh)[8],
                                            float (&dc)[8], const float* s_wih, int js, int q, float (&d)[4][8]) {
   constexpr int H = Dims<CH>::H;
@@ -204,8 +212,10 @@ __device__ __forceinline__ float cell_grad(const float (&acc)[16][4], int h, con
     d[1][s] = (dcv * fcp[s]) * fmaf(-gf, gf, gf);
     d[2][s] = (dcv * gi) * fmaf(-gg, gg, 1.f);
     dc[s] = dcv * gf;
-    const int u = 32 * js + 8 * jn + 2 * q + (s & 1);
-    dx += d[0][s] * s_wih[u] + d[1][s] * s_wih[H + u] + d[2][s] * s_wih[2 * H + u] + d[3][s] * s_wih[3 * H + u];
+    if (DX) {
+      const int u = 32 * js + 8 * jn + 2 * q + (s & 1);
+      dx += d[0][s] * s_wih[u] + d[1][s] * s_wih[H + u] + d[2][s] * s_wih[2 * H + u] + d[3][s] * s_wih[3 * H + u];
+    }
   }
   return dx;
 }
@@ -290,13 +300,26 @@ lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_
 // Per step and warp (16 cells), all on mma.sync:
 //     gates_t  = hx_t x Wx^T                (as in the forward; A = saved h_{t-1} fragment + x columns)
 //     dh_{t-1} = da_t x W_hh                (A = da_t straight from the gate-gradient registers, B = W_hh^T in shared memory)
-// and per step and CTA, after one barrier:
-//     dWext   += da_t^T x hx_t              (128 gates x 48 columns over the tile's 128 cells; warp w owns gates 16 w .. 16 w + 15;
+// and per step over the CTA's 128 cells:
+//     dWext   += da_t^T x hx_t              (128 gates x 40 nonzero columns; warp w owns gates 16 w .. 16 w + 15;
 //                                            columns 0..31 dW_hh, 32 + 34 dW_ih, 33 db)
-// da_t and hx_t go through double-buffered shared-memory tiles for that last product.
-constexpr size_t kBwdSavedSmem = (size_t)(Dims<1>::G4 * Dims<1>::WX_LD + Dims<1>::H * WT_LD + 2 * Dims<1>::CELLS * Dims<1>::DA_LD +
-                                          2 * Dims<1>::CELLS * Dims<1>::HX_LD) * sizeof(__half) + Dims<1>::G4 * sizeof(float);
+// The warps meet only in that last product, so no step waits for the whole CTA.  Its operands go through a ring of kBwdRing
+// da / hx tiles in shared memory: a warp waits on the slot's empty barrier, writes its 16 rows, arrives on the full barrier,
+// and then takes its product of the PREVIOUS step (waiting for that slot to be full, arriving on its empty barrier once read).
+// A warp can so run up to two steps ahead of the slowest, and one warp's product can overlap another's cell gradient.
+// The saved state and x of the walk stream in by cp.async, two steps ahead, into a per-warp ring of the same depth: entry k is
+// the (tile, t) of the walk's k-th step, a warp's own 2 KB c_t | h_t block of it (each thread copies, and later reads, exactly
+// its own 64 bytes, so its cp.async wait is the only synchronisation) and the x_t of the thread's two cells.  Step k reads
+// c_{t-1}, h_{t-1} from entry k + 1 and keeps c_{t-1} in registers as the c_t of the next step.
+// DX: the instance that also writes d_x (the host picks it from d_x != nullptr).
+constexpr int kBwdRing = 3;
+constexpr size_t kBwdSavedSmem =
+    (size_t)(Dims<1>::G4 * Dims<1>::WX_LD + Dims<1>::H * WT_LD + kBwdRing * Dims<1>::CELLS * (Dims<1>::DA_LD + Dims<1>::HX_LD)) * sizeof(__half) +
+    (size_t)kBwdRing * Dims<1>::NW * 2048 +                      // saved-state ring: [slot][warp][c h0, c h1, h h0, h h1][lane] uint4
+    (size_t)kBwdRing * Dims<1>::THREADS * 2 * sizeof(float) +    // x ring: [slot][thread][row h]
+    Dims<1>::G4 * sizeof(float) + 2 * kBwdRing * sizeof(uint64_t);
 
+template <bool DX>
 __global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::BWD_CTAS_PER_SM)
 lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
@@ -307,9 +330,13 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [128][WX_LD]
   __half* sWT = sWx + D::G4 * D::WX_LD;                    // [32 units][WT_LD]: W_hh^T
-  __half* sDA = sWT + C * WT_LD;                           // 2 x [128 cells][DA_LD]
-  __half* sHX = sDA + 2 * CELLS * D::DA_LD;                // 2 x [128 cells][HX_LD]
-  float* s_wih = reinterpret_cast<float*>(sHX + 2 * CELLS * D::HX_LD);
+  __half* sDA = sWT + C * WT_LD;                           // kBwdRing x [128 cells][DA_LD]
+  __half* sHX = sDA + kBwdRing * CELLS * D::DA_LD;         // kBwdRing x [128 cells][HX_LD]
+  uint4* sST = reinterpret_cast<uint4*>(sHX + kBwdRing * CELLS * D::HX_LD);
+  float* sX = reinterpret_cast<float*>(sST + kBwdRing * D::NW * 128);
+  float* s_wih = sX + kBwdRing * D::THREADS * 2;
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_wih + D::G4);     // da / hx slot written by all 8 warps
+  uint64_t* empty = full + kBwdRing;                               // da / hx slot read by all 8 warps
 
   load_wx<1>(sWx, w_ih, w_hh, b_ih, b_hh);
   for (int e = threadIdx.x; e < D::G4 * C; e += blockDim.x) {
@@ -317,18 +344,71 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
     sWT[u * WT_LD + j] = __float2half_rn(w_hh[e]);
   }
   for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
-  for (int e = threadIdx.x; e < 2 * CELLS; e += blockDim.x)      // constant zero columns 40..47 of both hx buffers
-    *reinterpret_cast<uint4*>(sHX + e * D::HX_LD + 40) = make_uint4(0u, 0u, 0u, 0u);
+  if (threadIdx.x == 0)
+    for (int s = 0; s < kBwdRing; ++s) { mbar_init(&full[s], D::NW); mbar_init(&empty[s], D::NW); }
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
   const uint32_t wx_addr = smem_u32(sWx), wt_addr = smem_u32(sWT), da_addr = smem_u32(sDA), hx_addr = smem_u32(sHX);
   const long long tiles = (cells + CELLS - 1) / CELLS;
   const float S = scale2[0], invS = scale2[1];
-  float dw[6][4];                     // dWext: gate 16 warp + g + 8 (i >> 1), column 8 nt + 2 q + (i & 1)
+  float dw[5][4];                     // dWext: gate 16 warp + g + 8 (i >> 1), column 8 nt + 2 q + (i & 1); columns 40..47 are 0
 #pragma unroll
-  for (int nt = 0; nt < 6; ++nt) dw[nt][0] = dw[nt][1] = dw[nt][2] = dw[nt][3] = 0.f;
-  int step = 0;                       // running step count across tiles: selects the da / hx buffer
+  for (int nt = 0; nt < 5; ++nt) dw[nt][0] = dw[nt][1] = dw[nt][2] = dw[nt][3] = 0.f;
+
+  // ---- the saved-state / x stream: entry (pf_tile, pf_t) is fetched next ----
+  long long pf_tile = blockIdx.x;
+  int pf_t = T - 1;
+  size_t pf_xb[2];
+  auto pf_cells = [&]() {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long cell = pf_tile * CELLS + warp * 16 + g + 8 * h;
+      pf_xb[h] = pf_tile < tiles && cell < cells ? x_base(cell, T, NN) : ~(size_t)0;
+    }
+  };
+  auto fetch = [&](int slot) {
+    if (pf_tile < tiles) {
+      const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off<1>(pf_tile, T, pf_t, warp, 0, lane));
+      const uint4* ph = reinterpret_cast<const uint4*>(saved + save_off<1>(pf_tile, T, pf_t, warp, 1, lane));
+      uint4* dst = sST + (slot * D::NW + warp) * 128 + lane;
+      cp_async16(dst, pc); cp_async16(dst + 32, pc + 1); cp_async16(dst + 64, ph); cp_async16(dst + 96, ph + 1);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (pf_xb[h] != ~(size_t)0) cp_async4(sX + (slot * D::THREADS + threadIdx.x) * 2 + h, x_seq + pf_xb[h] + (size_t)pf_t * NN);
+    }
+    cp_async_commit();
+    if (--pf_t < 0) { pf_t = T - 1; pf_tile += gridDim.x; pf_cells(); }
+  };
+  // ---- dWext[16 warp .. +15][0..47] += da^T x hx over the 128 cells of the step held in da / hx slot `slot` ----
+  auto dwext = [&](int slot, uint32_t phase) {
+    mbar_wait_inline(&full[slot], phase);
+    const uint32_t da_b = da_addr + (uint32_t)(slot * CELLS * D::DA_LD * 2), hx_b = hx_addr + (uint32_t)(slot * CELLS * D::HX_LD * 2);
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+      uint32_t a[4];
+      ldmatrix_x4_trans(da_b + (uint32_t)(((16 * kc + 8 * (mi >> 1) + (lane & 7)) * D::DA_LD + 16 * warp + 8 * (mi & 1)) * 2), a[0], a[1], a[2], a[3]);
+#pragma unroll
+      for (int pr = 0; pr < 2; ++pr) {
+        uint32_t b0, b1, b2, b3;
+        ldmatrix_x4_trans(hx_b + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * D::HX_LD + 16 * pr + 8 * (mi >> 1)) * 2), b0, b1, b2, b3);
+        mma_16816(dw[2 * pr], a, b0, b1);
+        mma_16816(dw[2 * pr + 1], a, b2, b3);
+      }
+      uint32_t b0, b1;                // columns 32..39; 40..47 are zero and never flushed
+      ldmatrix_x2_trans(hx_b + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * D::HX_LD + 32) * 2), b0, b1);
+      mma_16816(dw[4], a, b0, b1);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[slot]);
+  };
+
+  pf_cells();
+  fetch(0);
+  fetch(1);
+  int slot = 0, prev_slot = 0;        // ring slot of this step (k mod kBwdRing) and of the previous one
+  uint32_t phase = 0, prev_phase = 0; // (k / kBwdRing) & 1: the barrier phase of the slot's current use
+  bool have_prev = false;
 
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     long long cell[2];
@@ -339,35 +419,31 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
     for (int h = 0; h < 2; ++h) {
       cell[h] = tile * CELLS + warp * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
-      xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
+      xb[h] = DX && live[h] ? x_base(cell[h], T, NN) : 0;
 #pragma unroll
       for (int s = 0; s < 8; ++s) {
         dh[h][s] = live[h] ? d_hT[(size_t)cell[h] * C + 8 * (s >> 1) + 2 * q + (s & 1)] * S : 0.f;
         dc[h][s] = 0.f;
       }
     }
-    for (int t = T - 1; t >= 0; --t, ++step) {
-      // saved state: c_t, c_{t-1}, h_{t-1} (zero before the first step)
-      uint4 vc[2], vcp[2], vhp[2];
-      {
-        const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t, warp, 0, lane));
-        vc[0] = pc[0]; vc[1] = pc[1];
-        if (t > 0) {
-          const uint4* pcp = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t - 1, warp, 0, lane));
-          const uint4* php = reinterpret_cast<const uint4*>(saved + save_off<1>(tile, T, t - 1, warp, 1, lane));
-          vcp[0] = pcp[0]; vcp[1] = pcp[1]; vhp[0] = php[0]; vhp[1] = php[1];
-        } else {
-          vcp[0] = vcp[1] = vhp[0] = vhp[1] = make_uint4(0u, 0u, 0u, 0u);
-        }
+    uint4 vc[2];                      // c_t: read from the stream at the tile's first step, then carried from c_{t-1}
+    for (int t = T - 1; t >= 0; --t) {
+      fetch(slot == 0 ? kBwdRing - 1 : slot - 1);   // entry k + 2 into the slot of entry k - 1, last read in the previous step
+      cp_async_wait<1>();                           // entries k and k + 1 have landed
+      const uint4* st0 = sST + (slot * D::NW + warp) * 128 + lane;
+      const uint4* st1 = sST + ((slot + 1 == kBwdRing ? 0 : slot + 1) * D::NW + warp) * 128 + lane;
+      if (t == T - 1) { vc[0] = st0[0]; vc[1] = st0[32]; }
+      // saved state: c_{t-1}, h_{t-1} (zero before the first step)
+      uint4 vcp[2], vhp[2];
+      if (t > 0) {
+        vcp[0] = st1[0]; vcp[1] = st1[32]; vhp[0] = st1[64]; vhp[1] = st1[96];
+      } else {
+        vcp[0] = vcp[1] = vhp[0] = vhp[1] = make_uint4(0u, 0u, 0u, 0u);
       }
       const uint32_t hw[8] = {vhp[0].x, vhp[0].y, vhp[0].z, vhp[0].w, vhp[1].x, vhp[1].y, vhp[1].z, vhp[1].w};
-      float xt[2];
       uint32_t xw[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        xt[h] = live[h] ? x_seq[xb[h] + (size_t)t * NN] : 0.f;
-        xw[h] = x_cols(xt[h], q);
-      }
+      for (int h = 0; h < 2; ++h) xw[h] = x_cols(live[h] ? sX[(slot * D::THREADS + threadIdx.x) * 2 + h] : 0.f, q);
       float acc[16][4];
       gate_mma<1>(acc, [&](int kb, uint32_t (&a)[4]) {
         a[0] = hw[2 * kb]; a[1] = hw[4 + 2 * kb]; a[2] = hw[2 * kb + 1]; a[3] = hw[4 + 2 * kb + 1];
@@ -378,13 +454,13 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float d[4][8];
-        dx[h] = cell_grad<1>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, 0, q, d);
+        dx[h] = cell_grad<1, DX>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, 0, q, d);
 #pragma unroll
         for (int jn = 0; jn < 4; ++jn)
 #pragma unroll
           for (int gt = 0; gt < 4; ++gt) da[4 * gt + jn][h] = pack2(d[gt][2 * jn], d[gt][2 * jn + 1]);
       }
-      if (d_x != nullptr) {
+      if (DX) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float v = dx[h];
@@ -413,10 +489,10 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
 #pragma unroll
           for (int s = 0; s < 8; ++s) dh[h][s] = adh[s >> 1][2 * h + (s & 1)];
       }
-      // da_t and hx_t of the warp's cells into this step's buffers (last read two steps ago, before the previous step's barrier)
-      const int buf = step & 1;
-      __half* sda = sDA + buf * CELLS * D::DA_LD;
-      __half* shx = sHX + buf * CELLS * D::HX_LD;
+      // da_t and hx_t of the warp's cells into this step's slot, once every warp has read the step that last used it
+      mbar_wait_inline(&empty[slot], phase ^ 1u);
+      __half* sda = sDA + slot * CELLS * D::DA_LD;
+      __half* shx = sHX + slot * CELLS * D::HX_LD;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = warp * 16 + g + 8 * h;
@@ -426,23 +502,18 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
         for (int jn = 0; jn < 4; ++jn) *reinterpret_cast<uint32_t*>(shx + row * D::HX_LD + 8 * jn + 2 * q) = hw[4 * h + jn];
         *reinterpret_cast<uint32_t*>(shx + row * D::HX_LD + 32 + 2 * q) = xw[h];
       }
-      __syncthreads();
-      // dWext[16 warp .. +15][0..47] += da^T x hx over the tile's 128 cells
-      const uint32_t da_b = da_addr + (uint32_t)(buf * CELLS * D::DA_LD * 2), hx_b = hx_addr + (uint32_t)(buf * CELLS * D::HX_LD * 2);
-#pragma unroll
-      for (int kc = 0; kc < 8; ++kc) {
-        uint32_t a[4];
-        ldmatrix_x4_trans(da_b + (uint32_t)(((16 * kc + 8 * (mi >> 1) + (lane & 7)) * D::DA_LD + 16 * warp + 8 * (mi & 1)) * 2), a[0], a[1], a[2], a[3]);
-#pragma unroll
-        for (int pr = 0; pr < 3; ++pr) {
-          uint32_t b0, b1, b2, b3;
-          ldmatrix_x4_trans(hx_b + (uint32_t)(((16 * kc + 8 * (mi & 1) + (lane & 7)) * D::HX_LD + 16 * pr + 8 * (mi >> 1)) * 2), b0, b1, b2, b3);
-          mma_16816(dw[2 * pr], a, b0, b1);
-          mma_16816(dw[2 * pr + 1], a, b2, b3);
-        }
-      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&full[slot]);
+      if (have_prev) dwext(prev_slot, prev_phase);  // the previous step's product, in step order
+      have_prev = true;
+      prev_slot = slot;
+      prev_phase = phase;
+      if (++slot == kBwdRing) { slot = 0; phase ^= 1u; }
+      vc[0] = vcp[0];
+      vc[1] = vcp[1];
     }
   }
+  if (have_prev) dwext(prev_slot, prev_phase);
   // ---- flush the weight-gradient accumulator ----
 #pragma unroll
   for (int nt = 0; nt < 5; ++nt)
@@ -640,7 +711,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float d[4][8];
-        dx[h] = cell_grad<CH>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, js, q, d);
+        dx[h] = cell_grad<CH, true>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, js, q, d);
 #pragma unroll
         for (int jn = 0; jn < 4; ++jn)
 #pragma unroll
@@ -853,10 +924,11 @@ static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float*
                              void* /*da_rec*/, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
   using D = Dims<1>;
   if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  static DynSmemAttr attr_b = {};
-  if (int e = ensure_dyn_smem(lstm_tc::lstm_bwd_saved_tc_kernel, (int)lstm_tc::kBwdSavedSmem, attr_b)) return e;
+  auto kern = d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true> : lstm_tc::lstm_bwd_saved_tc_kernel<false>;
+  static DynSmemAttr attr_x = {}, attr_n = {};
+  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, d_x ? attr_x : attr_n)) return e;
   prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  lstm_tc::lstm_bwd_saved_tc_kernel<<<lstm_grid<1>(cells, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
+  kern<<<lstm_grid<1>(cells, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
       x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
