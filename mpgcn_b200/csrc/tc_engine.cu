@@ -200,6 +200,29 @@ namespace tc {
 
 static const int kMaxSmem = 232448;   // 227 KB opt-in limit per CTA on sm_90
 
+// Store map of a contraction output: element (ch, i, r, z) at base + z*sZ + i*sI + r*sR + ch, dims (32, m_valid, r_valid, Z),
+// box one chunk of 64 rows, in the swizzle the epilogue writes its store buffer with (a 64- or 128-byte row).  TMA clips every
+// box at these dims, which is what bounds a partial tile.
+static int make_out_map(CUtensorMap* m, const void* base, bool f16, const Epilogue& ep, int Z) {
+  EncodeTiledFn fn = get_encode_fn();
+  MPGCN_CHECK(fn != nullptr, "cuTensorMapEncodeTiled is not available (no CUDA driver?)");
+  const uint64_t es = f16 ? 2 : 4;
+  cuuint64_t dims[4] = {32, (cuuint64_t)ep.m_valid, (cuuint64_t)ep.r_valid, (cuuint64_t)Z};
+  cuuint64_t str[3] = {(cuuint64_t)ep.sI * es, (cuuint64_t)ep.sR * es, (cuuint64_t)ep.sZ * es};
+  cuuint32_t box[4] = {32, 64, 1, 1};
+  cuuint32_t one[4] = {1, 1, 1, 1};
+  for (int i = 0; i < 3; ++i)
+    MPGCN_CHECK(str[i] % 16 == 0 && str[i] < (1ull << 40), "output stride %llu of dim %d is not a multiple of 16 bytes",
+                (unsigned long long)str[i], i + 1);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0, "output pointer must be 16-byte aligned");
+  CUresult r = fn(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(base), dims, str, box,
+                  one, CU_TENSOR_MAP_INTERLEAVE_NONE, f16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MPGCN_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (output) failed (%d): dims=(32,%d,%d,%d) strides=(%llu,%llu,%llu)", (int)r,
+              ep.m_valid, ep.r_valid, Z, (unsigned long long)str[0], (unsigned long long)str[1], (unsigned long long)str[2]);
+  return 0;
+}
+
 template <int AK, int BK>
 static int launch_impl(GemmParams& p, cudaStream_t stream) {
   using C = Cfg<AK, BK>;
@@ -208,13 +231,20 @@ static int launch_impl(GemmParams& p, cudaStream_t stream) {
   MPGCN_CHECK(p.R >= 1 && p.R <= 8, "R=%d out of range", p.R);
   const size_t b_stage = (size_t)p.R * BK * 64;
   const int nres = p.b_res_reps * p.kb_total;
+  MPGCN_CHECK(p.ep.out != nullptr && p.ep.m_valid > 0 && p.ep.r_valid > 0, "contraction without an output");
+  if (int e = make_out_map(&p.out_map, p.ep.out, p.ep.out_f16 != 0, p.ep, p.Z)) return e;
+  const bool shadow = !p.ep.out_f16 && p.ep.out16 != nullptr;
+  if (shadow)
+    if (int e = make_out_map(&p.out16_map, p.ep.out16, true, p.ep, p.Z)) return e;
+  p.st_bytes = p.ep.out_f16 ? 64 * 64 : shadow ? 64 * 128 + 64 * 64 : 64 * 128;
+  const size_t fixed = smem_bytes(0, p.R, BK, 0, 0, p.st_bytes);      // everything but the ring
   int stages;
   if (nres) {
     MPGCN_CHECK(p.NT == 1 && p.kb_per_seg == 1 && !p.split_k && p.bm.z_mul == 0, "resident B needs a tile-independent B operand");
-    MPGCN_CHECK((size_t)nres * b_stage + 2 * (size_t)C::A_STAGE + kEpiBytes + 1536 <= (size_t)kMaxSmem, "resident B operand does not fit in shared memory");
-    stages = (int)((kMaxSmem - 1024 - 512 - kEpiBytes - (size_t)nres * b_stage) / (size_t)C::A_STAGE);
+    MPGCN_CHECK(fixed + (size_t)nres * b_stage + 2 * (size_t)C::A_STAGE <= (size_t)kMaxSmem, "resident B operand does not fit in shared memory");
+    stages = (int)((kMaxSmem - fixed - (size_t)nres * b_stage) / (size_t)C::A_STAGE);
   } else {
-    stages = (int)((kMaxSmem - 1024 - 512 - kEpiBytes) / ((size_t)C::A_STAGE + b_stage));
+    stages = (int)((kMaxSmem - fixed) / ((size_t)C::A_STAGE + b_stage));
   }
   // small stages (channel mixes, 8 KB of A per k-block) are HBM-latency bound: keep >= 128 KB of loads in flight per SM
   const int max_stages = ((size_t)C::A_STAGE + (nres ? 0 : b_stage) <= 16384) ? 16 : 8;
@@ -223,7 +253,7 @@ static int launch_impl(GemmParams& p, cudaStream_t stream) {
   p.stages = stages;
   // always request the full opt-in budget: exactly one CTA per SM
   const size_t smem = kMaxSmem;
-  MPGCN_CHECK(smem_bytes(C::A_STAGE, p.R, BK, stages, nres) <= smem, "internal: smem budget");
+  MPGCN_CHECK(smem_bytes(C::A_STAGE, p.R, BK, stages, nres, p.st_bytes) <= smem, "internal: smem budget");
   const long long tiles = (long long)p.MT * p.NT * p.Z;
   MPGCN_CHECK(tiles > 0 && tiles < (1ll << 31), "bad tile count %lld", tiles);
   MPGCN_CHECK(p.kb_total > 0 && p.kb_per_seg > 0, "empty contraction");

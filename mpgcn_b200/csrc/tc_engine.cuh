@@ -14,8 +14,11 @@
 //     B       : always [k][chunk r][32 ch], 64-byte rows, SWIZZLE_64B, MN-major
 // * warpgroups 0 and 1 = MMA + epilogue of rows 0..63 / 64..127 of the tile.  Thread 0 also issues the TMA loads: it fills
 //   the ring, then refills each stage as soon as both warpgroups released it, so loads run up to `stages` k-blocks (into the
-//   next tile as well) ahead of the MMAs.  A separate producer warp would push the CTA past 256 threads and so cap the
-//   registers at 168 per thread, below what the accumulator tile needs.
+//   next tile as well) ahead of the MMAs.  (A separate producer warp takes the CTA past 256 threads, which caps registers at
+//   168 per thread unless setmaxnreg hands the consumers up to 232; that split has not been tried.)
+// * the epilogue writes each 64-row x 32-channel chunk of the result, converted, into one of two shared-memory store buffers
+//   per warpgroup and stores it by TMA (cp.async.bulk.tensor, bulk-group completion): the stores drain while the next tile's
+//   MMAs run, and partial tiles are clipped by the output tensor map.
 //
 // Reference math being evaluated: BDGCN.forward of the reference MPGCN.py, in the factored order of SURVEY.md section 7.1.
 #pragma once
@@ -59,12 +62,17 @@ struct Epilogue {
 struct alignas(64) GemmParams {
   CUtensorMap a_map;
   CUtensorMap b_map;
+  // the output as (32 ch, m_valid rows, r_valid chunks, Z) with the strides of `ep`, box one chunk of 64 rows; and its fp16
+  // shadow.  Set by launch_contract from `ep`.
+  CUtensorMap out_map;
+  CUtensorMap out16_map;
   OperandMap am, bm;
   int MT, NT, Z;             // tile grid: tile id = (z * NT + nt) * MT + mt
   int R;                     // 32-column chunks per tile
   int kb_total, kb_per_seg;  // k-blocks over all segments / per segment
   int split_k, kb_per_slice; // split-K: z is a k-slice [z*kb_per_slice, ...)
   int stages;
+  int st_bytes;              // one store buffer: a chunk of 64 rows in the output type (+ 4 KB fp16 shadow); set by launch_contract
   // resident B (channel mixes): the whole B operand -- b_res_reps * kb_total tiles, index rep * kb_total + kb -- is loaded
   // once per CTA and every A k-block is multiplied by its b_res_reps tiles (the fp16 hi / lo halves of W); 0 = B streams
   // through the ring with A.  Needs NT == 1, kb_per_seg == 1, no split-K, a z-independent B map.
@@ -77,8 +85,6 @@ struct alignas(64) GemmParams {
 
 constexpr int kConsumerWGs = 2;                        // 64 tile rows each
 constexpr int kThreads1 = 128 * kConsumerWGs;          // 256 threads: the 128 x 256 fp32 accumulator tile needs ~250 registers
-constexpr int kEpiRow = 40;                            // staging-row stride (floats): conflict-free 8-byte fragment writes
-constexpr size_t kEpiBytes = (size_t)kConsumerWGs * 2 * 64 * kEpiRow * sizeof(float);   // two chunks per consumer warpgroup
 
 template <int AK, int BK>
 struct Cfg {
@@ -104,10 +110,11 @@ struct Cfg {
   static_assert(BK % 16 == 0, "wgmma K is 16 for fp16");
 };
 
-__host__ __device__ inline size_t smem_bytes(int a_stage, int R, int BK, int stages, int b_resident_tiles = 0) {
+// shared memory of one CTA: the operand ring (or A ring + resident B), two store buffers of st_bytes per consumer warpgroup
+__host__ __device__ inline size_t smem_bytes(int a_stage, int R, int BK, int stages, int b_resident_tiles, int st_bytes) {
   const size_t b_stage = (size_t)R * BK * 64;
-  return 1024 /*align slack*/ + (size_t)stages * a_stage + (size_t)(b_resident_tiles ? b_resident_tiles : stages) * b_stage + kEpiBytes +
-         512 /*barriers, bias*/;
+  return 1024 /*align slack*/ + (size_t)stages * a_stage + (size_t)(b_resident_tiles ? b_resident_tiles : stages) * b_stage +
+         (size_t)2 * kConsumerWGs * st_bytes + 512 /*barriers, bias*/;
 }
 
 #ifdef __CUDACC__
@@ -128,53 +135,7 @@ __device__ __forceinline__ void decode_tile(const GemmParams& p, int t, int& mt,
   }
 }
 
-// one full 32-byte L2 sector per lane, as two back-to-back 16-byte stores (the widest global store of sm_90)
-__device__ __forceinline__ void st_global_256(void* ptr, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t a4, uint32_t a5,
-                                              uint32_t a6, uint32_t a7) {
-  uint4* d = reinterpret_cast<uint4*>(ptr);
-  d[0] = make_uint4(a0, a1, a2, a3);
-  d[1] = make_uint4(a4, a5, a6, a7);
-}
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) { return f2h2_sat_bits(a, b); }   // an fp16 operand never holds inf
-
-__device__ __forceinline__ void store_chunk(const Epilogue& ep, float alpha, const float* sbias, long long off,
-                                            uint32_t (&acc)[32], float& amax) {
-  float v[32];
-#pragma unroll
-  for (int c = 0; c < 32; ++c) {
-    float x = __uint_as_float(acc[c]) * alpha;
-    if (ep.bias) x += sbias[c];
-    if (ep.relu) x = fmaxf(x, 0.f);
-    v[c] = x;
-  }
-  if (ep.absmax_out) {
-#pragma unroll
-    for (int c = 0; c < 32; ++c) amax = fmaxf(amax, fabsf(v[c]));
-  }
-  if (ep.out_f16) {        // 64 bytes per row and chunk: two 32-byte stores
-    __half* dst = reinterpret_cast<__half*>(ep.out) + off;
-#pragma unroll
-    for (int q = 0; q < 2; ++q)
-      st_global_256(dst + 16 * q, pack_h2(v[16 * q + 0], v[16 * q + 1]), pack_h2(v[16 * q + 2], v[16 * q + 3]),
-                    pack_h2(v[16 * q + 4], v[16 * q + 5]), pack_h2(v[16 * q + 6], v[16 * q + 7]), pack_h2(v[16 * q + 8], v[16 * q + 9]),
-                    pack_h2(v[16 * q + 10], v[16 * q + 11]), pack_h2(v[16 * q + 12], v[16 * q + 13]), pack_h2(v[16 * q + 14], v[16 * q + 15]));
-  } else {                 // 128 bytes per row and chunk: four 32-byte stores
-    float* dst = reinterpret_cast<float*>(ep.out) + off;
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      st_global_256(dst + 8 * q, __float_as_uint(v[8 * q + 0]), __float_as_uint(v[8 * q + 1]), __float_as_uint(v[8 * q + 2]),
-                    __float_as_uint(v[8 * q + 3]), __float_as_uint(v[8 * q + 4]), __float_as_uint(v[8 * q + 5]),
-                    __float_as_uint(v[8 * q + 6]), __float_as_uint(v[8 * q + 7]));
-    if (ep.out16) {
-      __half* d16 = ep.out16 + off;
-#pragma unroll
-      for (int q = 0; q < 2; ++q)
-        st_global_256(d16 + 16 * q, pack_h2(v[16 * q + 0], v[16 * q + 1]), pack_h2(v[16 * q + 2], v[16 * q + 3]),
-                      pack_h2(v[16 * q + 4], v[16 * q + 5]), pack_h2(v[16 * q + 6], v[16 * q + 7]), pack_h2(v[16 * q + 8], v[16 * q + 9]),
-                      pack_h2(v[16 * q + 10], v[16 * q + 11]), pack_h2(v[16 * q + 12], v[16 * q + 13]), pack_h2(v[16 * q + 14], v[16 * q + 15]));
-    }
-  }
-}
 
 template <int AK, int BK>
 __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_constant__ GemmParams p) {
@@ -189,8 +150,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
   const int NRES = p.b_res_reps * p.kb_total;       // resident B tiles (0: B goes through the ring)
   uint8_t* sA = smem;
   uint8_t* sB = sA + (size_t)S * A_STAGE;
-  float* sEpi = reinterpret_cast<float*>(sB + (size_t)(NRES ? NRES : S) * B_STAGE);
-  uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + kEpiBytes);
+  uint8_t* sStore = sB + (size_t)(NRES ? NRES : S) * B_STAGE;     // 2 store buffers per consumer warpgroup
+  uint64_t* full = reinterpret_cast<uint64_t*>(sStore + (size_t)2 * kConsumerWGs * p.st_bytes);
   uint64_t* empty = full + S;
   uint64_t* bres_full = empty + S;
   float* sbias = reinterpret_cast<float*>(bres_full + 1);
@@ -201,6 +162,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.a_map);
     tma_prefetch_desc(&p.b_map);
+    tma_prefetch_desc(&p.out_map);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 4 * kConsumerWGs);     // one arrival per warp
@@ -284,7 +246,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
     const float alpha = p.ep.alpha_dev ? p.ep.alpha * __ldg(p.ep.alpha_dev) : p.ep.alpha;
     const uint64_t a_hi = gmma_desc_hi(C::A_SBO, C::A_LAYOUT);
     const uint64_t b_hi = gmma_desc_hi(C::B_SBO, GMMA_SW64);
-    float* stg = sEpi + (size_t)wg * 2 * 64 * kEpiRow;
+    uint32_t st_seq = 0;                // store buffers used so far by this warpgroup: buffer st_seq & 1 is next
     float amax = 0.f;
     float acc[128];
     int stage = 0;
@@ -345,84 +307,113 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
         if (threadIdx.x == 0) produce();
         __syncwarp();
       }
-      // ---- epilogue: two chunks at a time through the staging buffer, then one thread per (row, chunk) as a 32-channel row ----
-      const int half = tw >> 6, rr = tw & 63;
-      const int i = mt * 128 + wg * 64 + rr;
-      const long long base = (long long)z * p.ep.sZ + (long long)i * p.ep.sI;
+      // ---- epilogue: chunk by chunk straight from the accumulator fragment into a store buffer in the output's layout, which
+      // one thread then writes out by TMA.  The MMAs of the next tile start while that store is in flight.  Per element the
+      // same operations as a row-wise pass, in the same order: correction FMAs by segment, * alpha, + bias, ReLU, conversion.
+      const int row0 = mt * 128 + wg * 64;     // first output row of this warpgroup; the tensor maps clip rows >= m_valid
+      int ii[2];
+      long long cbase[2] = {0, 0};
+      const float* dsrc[2] = {nullptr, nullptr};   // delta of segment 0 of row ii[h]: segment sg at dsrc[h][sg * m_valid]
       // the remainders of the first 8 segments stay in registers for the whole tile; those of segments 8.. (more than 8
       // supports) are re-read per chunk, 8 at a time
-      float dl[8];
-      long long cbase = 0;
-      const float* dsrc = nullptr;    // delta of segment 0 of this row: segment sg at dsrc[sg * m_valid]
-      bool any_corr = false;
-      if (p.ep.corr_src != nullptr) {
-        const int zA = ((z / p.am.z_div) % p.am.z_mod) * p.am.z_mul;
-        const int zB = ((z / p.bm.z_div) % p.bm.z_mod) * p.bm.z_mul;
-        cbase = (long long)zB * p.ep.cZ + (long long)i * p.ep.cI;
-        dsrc = p.ep.corr_delta + (long long)zA * p.ep.corr_nseg * p.ep.m_valid + i;
+      float dl[2][8];
+      bool any_corr[2] = {false, false};
 #pragma unroll
-        for (int sgi = 0; sgi < 8; ++sgi) {
-          dl[sgi] = (sgi < p.ep.corr_nseg && i < p.ep.m_valid) ? __ldg(dsrc + (long long)sgi * p.ep.m_valid) : 0.f;
-          any_corr |= (dl[sgi] != 0.f);
+      for (int h = 0; h < 2; ++h) {
+        ii[h] = row0 + 16 * wq + g + 8 * h;
+        if (p.ep.corr_src != nullptr) {
+          const int zA = ((z / p.am.z_div) % p.am.z_mod) * p.am.z_mul;
+          const int zB = ((z / p.bm.z_div) % p.bm.z_mod) * p.bm.z_mul;
+          cbase[h] = (long long)zB * p.ep.cZ + (long long)ii[h] * p.ep.cI;
+          dsrc[h] = p.ep.corr_delta + (long long)zA * p.ep.corr_nseg * p.ep.m_valid + ii[h];
+#pragma unroll
+          for (int sgi = 0; sgi < 8; ++sgi) {
+            dl[h][sgi] = (sgi < p.ep.corr_nseg && ii[h] < p.ep.m_valid) ? __ldg(dsrc[h] + (long long)sgi * p.ep.m_valid) : 0.f;
+            any_corr[h] |= (dl[h][sgi] != 0.f);
+          }
+          for (int sg = 8; sg < p.ep.corr_nseg && !any_corr[h] && ii[h] < p.ep.m_valid; ++sg)
+            any_corr[h] = __ldg(dsrc[h] + (long long)sg * p.ep.m_valid) != 0.f;
+        } else {
+#pragma unroll
+          for (int sgi = 0; sgi < 8; ++sgi) dl[h][sgi] = 0.f;
         }
-        for (int sg = 8; sg < p.ep.corr_nseg && !any_corr && i < p.ep.m_valid; ++sg) any_corr = __ldg(dsrc + (long long)sg * p.ep.m_valid) != 0.f;
       }
 #pragma unroll
-      for (int j0 = 0; j0 < 8; j0 += 2) {
-        if (j0 < R) {
-          // accumulator fragment: acc[16 j + 4 jj + 2 h + e] = D[row 16 wq + g + 8 h][column 32 j + 8 jj + 2 q + e]
-#pragma unroll
-          for (int s = 0; s < 2; ++s) {
-            if (j0 + s < R) {
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                  *reinterpret_cast<float2*>(stg + (s * 64 + 16 * wq + g + 8 * h) * kEpiRow + 8 * jj + 2 * q) =
-                      make_float2(acc[16 * (j0 + s) + 4 * jj + 2 * h], acc[16 * (j0 + s) + 4 * jj + 2 * h + 1]);
-            }
-          }
-          named_bar_sync(1 + wg, 128);
-          const int j = j0 + half;
+      for (int j = 0; j < 8; ++j) {
+        if (j < R) {
           const int r = nt * R + j;
-          if (j < R && i < p.ep.m_valid && r < p.ep.r_valid) {
-            uint32_t regs[32];
+          // accumulator fragment: acc[16 j + 4 jj + 2 h + e] = D[row 16 wq + g + 8 h][column 32 j + 8 jj + 2 q + e]
+          float v[16];
 #pragma unroll
-            for (int c = 0; c < 32; c += 4) {
-              const float4 v = *reinterpret_cast<const float4*>(stg + (half * 64 + rr) * kEpiRow + c);
-              regs[c] = __float_as_uint(v.x); regs[c + 1] = __float_as_uint(v.y);
-              regs[c + 2] = __float_as_uint(v.z); regs[c + 3] = __float_as_uint(v.w);
-            }
+          for (int c = 0; c < 16; ++c) v[c] = acc[16 * j + c];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!any_corr[h] || ii[h] >= p.ep.m_valid || r >= p.ep.r_valid) continue;
             // segments in groups of 8 (one group for <= 8 supports), in segment order
-            for (int sg0 = 0; any_corr && sg0 < p.ep.corr_nseg; sg0 += 8) {
+            for (int sg0 = 0; sg0 < p.ep.corr_nseg; sg0 += 8) {
               float dg[8];
 #pragma unroll
               for (int sgi = 0; sgi < 8; ++sgi)
-                dg[sgi] = sg0 == 0 ? dl[sgi] : (sg0 + sgi < p.ep.corr_nseg ? __ldg(dsrc + (long long)(sg0 + sgi) * p.ep.m_valid) : 0.f);
+                dg[sgi] = sg0 == 0 ? dl[h][sgi] : (sg0 + sgi < p.ep.corr_nseg ? __ldg(dsrc[h] + (long long)(sg0 + sgi) * p.ep.m_valid) : 0.f);
 #pragma unroll
               for (int sgi = 0; sgi < 8; ++sgi) {
                 if (sg0 + sgi < p.ep.corr_nseg && dg[sgi] != 0.f) {
-                  const uint4* src = reinterpret_cast<const uint4*>(p.ep.corr_src + cbase + (long long)(sg0 + sgi) * p.ep.cSeg + (long long)r * p.ep.cR);
+                  const __half2* src = reinterpret_cast<const __half2*>(p.ep.corr_src + cbase[h] + (long long)(sg0 + sgi) * p.ep.cSeg +
+                                                                        (long long)r * p.ep.cR) + q;
 #pragma unroll
-                  for (int qq = 0; qq < 4; ++qq) {
-                    const uint4 v = __ldg(src + qq);
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                      const float2 f = __half22float2(h2[e]);
-                      regs[8 * qq + 2 * e] = __float_as_uint(fmaf(dg[sgi], f.x, __uint_as_float(regs[8 * qq + 2 * e])));
-                      regs[8 * qq + 2 * e + 1] = __float_as_uint(fmaf(dg[sgi], f.y, __uint_as_float(regs[8 * qq + 2 * e + 1])));
-                    }
+                  for (int jj = 0; jj < 4; ++jj) {
+                    const float2 f = __half22float2(__ldg(src + 4 * jj));
+                    v[4 * jj + 2 * h] = fmaf(dg[sgi], f.x, v[4 * jj + 2 * h]);
+                    v[4 * jj + 2 * h + 1] = fmaf(dg[sgi], f.y, v[4 * jj + 2 * h + 1]);
                   }
                 }
               }
             }
-            store_chunk(p.ep, alpha, sbias, base + (long long)r * p.ep.sR, regs, amax);
           }
+#pragma unroll
+          for (int c = 0; c < 16; ++c) {
+            float x = v[c] * alpha;
+            if (p.ep.bias) x += sbias[8 * (c >> 2) + 2 * q + (c & 1)];
+            if (p.ep.relu) x = fmaxf(x, 0.f);
+            v[c] = x;
+          }
+          if (p.ep.absmax_out && r < p.ep.r_valid) {
+#pragma unroll
+            for (int c = 0; c < 16; ++c)
+              if (ii[(c >> 1) & 1] < p.ep.m_valid) amax = fmaxf(amax, fabsf(v[c]));
+          }
+          // store buffer of this chunk: [64 rows][32 channels], 128-byte rows SWIZZLE_128B (fp32) or 64-byte rows SWIZZLE_64B
+          // (fp16), the fp16 shadow of an fp32 output 8 KB behind; conflict-free fragment writes
+          uint8_t* buf = sStore + (size_t)(wg * 2 + (st_seq & 1)) * p.st_bytes;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t rho = 16 * wq + g + 8 * h;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const uint32_t o16 = (rho * 64 + 16 * jj + 4 * q) ^ (((rho >> 1) & 3) << 4);
+              const uint32_t h2 = pack_h2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
+              if (p.ep.out_f16) {
+                *reinterpret_cast<uint32_t*>(buf + o16) = h2;
+              } else {
+                const uint32_t o32 = (rho * 128 + 32 * jj + 8 * q) ^ ((rho & 7) << 4);
+                *reinterpret_cast<float2*>(buf + o32) = make_float2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
+                if (p.ep.out16) *reinterpret_cast<uint32_t*>(buf + 8192 + o16) = h2;
+              }
+            }
+          }
+          fence_proxy_async_smem();                 // the generic-proxy writes above, before the TMA engine reads them
+          if (tw == 0) bulk_wait_read<0>();         // the other buffer's store has read it: it may be rewritten after the barrier
           named_bar_sync(1 + wg, 128);
+          if (tw == 0) {
+            tma_store_4d(&p.out_map, buf, 0, row0, r, z);
+            if (!p.ep.out_f16 && p.ep.out16) tma_store_4d(&p.out16_map, buf + 8192, 0, row0, r, z);
+            bulk_commit();
+          }
+          ++st_seq;
         }
       }
     }
+    if (tw == 0) bulk_wait_all();                   // shared memory must outlive the last stores
     if (p.ep.absmax_out) {
       for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
       if (lane == 0) atomicMax(reinterpret_cast<unsigned int*>(p.ep.absmax_out), __float_as_uint(amax));
