@@ -154,7 +154,8 @@ MPGCN_API int mpgcn_relu_backward(const float* d_out, const float* out, int act,
  *   rows_reduce_bias_act:  out[b,r,e,h] = act( sum_j partials[j][b, row0 + r, e, h] + bias[h] )   out [B,rows,N,H]
  *        = reduce-scatter of the partial pre-activations (each rank reads ITS rows from every rank) + MPGCN.py:47-49;
  *   relu_backward_scatter: d_pre = d_out * [out > 0] (d_out, out [B,rows,N,H]) stored to rows [row0, row0 + rows) of EVERY dsts[j];
- *        db[h] = sum d_pre (nullable)   = ReLU mask + all-gather of dPre. */
+ *        db[h] = sum d_pre (nullable)   = ReLU mask + all-gather of dPre.
+ * rows_reduce_bias_act takes any H >= 1, relu_backward_scatter and its fp16 flavour any 1 <= H <= 1024. */
 MPGCN_API int mpgcn_rows_reduce_bias_act(float* out, const float* const* partials, int g, const float* bias, int act, int B, int N, int row0,
                                int rows, int H, void* stream);
 MPGCN_API int mpgcn_relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N,

@@ -228,9 +228,7 @@ int mpgcn_absmax(const float* x, long long n, float* out, void* stream) {
 
 int mpgcn_relu_backward(const float* d_out, const float* out, int act, float* d_pre, float* db, long long n, int H, void* stream) {
   MPGCN_CHECK(d_out && d_pre && n >= 1 && (act == 0 || (act == 1 && out)), "mpgcn_relu_backward: bad argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, st));
-  return relu_bwd_prep(d_out, out, act, nullptr, d_pre, db, (size_t)n, H, nullptr, st);
+  return relu_bwd_prep(d_out, out, act, nullptr, d_pre, db, (size_t)n, H, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int mpgcn_adj_num_supports(int kernel_type, int K) { return adj_num_supports(kernel_type, K); }

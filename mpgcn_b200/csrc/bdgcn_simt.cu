@@ -113,7 +113,6 @@ int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* ou
 
   const float* dP = d_out;         // a partial call receives dPre itself (every origin row m, already masked)
   if (!s.partial) {
-    if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, st));
     if (int e = relu_bwd_prep(d_out, out, s.act, nullptr, dPre, db, (size_t)s.B * NN * H, (int)H, nullptr, st)) return e;
     dP = dPre;
   }
@@ -150,7 +149,7 @@ int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* ou
     if (int e = simt_sgemm(p, st)) return e;
   }
   if (dX) {
-    if (int e = permute_w_bwd(W, nullptr, Wq, (int)Ko, (int)Kd, (int)C, (int)H, st)) return e;
+    if (int e = permute_w_bwd(W, Wq, (int)Ko, (int)Kd, (int)C, (int)H, st)) return e;
     {  // Y[b,d] (rows x l) = sum_o V[b,o] (rows x h) * Wq[d,o] (h x l)
       SgemmParams p{};
       p.A = V; p.B = Wq; p.D = Y;

@@ -479,10 +479,7 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
     if (int e = mask_delta_rows(go.delta, masked, g_planes(s, s.Ko), s.N, s.row0, s.R, st)) return e;
     delta_o = masked;
   }
-  const size_t wn = (size_t)s.Ko * s.Kd * s.C * s.H;
-  if (s.H == 32) {      // the mix's W order [(hc,o)][(d,lc,l)][h] is then W's own [o][d][c][h]
-    if (int e = cvt_f32_to_f16_hilo(W, w16, w16 + wn, wn, st)) return e;
-  } else if (int e = permute_w_mix(W, w16, w16 + wn, s.Ko, s.Kd, s.C, s.H, st)) return e;
+  if (int e = permute_w_mix(W, w16, w16 + (size_t)s.Ko * s.Kd * s.C * s.H, s.Ko, s.Kd, s.C, s.H, st)) return e;
   if (int e = run_fwd_a(s, gd.g16, x16, z16, gd.delta, st)) return e;
   if (int e = run_mix(s, z16, w16, 2, u16, PROF_FWD_MIX, s.Kd * (s.C / 32), s.Ko * (s.H / 32), st)) return e;
   if (int e = run_fwd_b(s, go.g16, u16, bias, out, static_cast<__half*>(ex.out_f16), delta_o, st)) return e;
@@ -522,7 +519,6 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
   } else {
     __half* dp16_ws = reinterpret_cast<__half*>(wb + L.dp16);
     float* scale2_ws = reinterpret_cast<float*>(wb + L.scale);
-    if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * s.H, st));
     if (int e = grad_scale_prepare(d_out, (size_t)s.B * NNfull * s.H, scale2_ws, ex.d_out_absmax, st)) return e;
     if (ex.out_f16 != nullptr && act) {
       if (int e = relu_bwd_prep_f16mask(d_out, static_cast<const __half*>(ex.out_f16), act, dp16_ws, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st)) return e;
@@ -543,9 +539,7 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
   if (int e = reduce_dw_partials(partials, dW, slices, mt, s.Ko, s.Kd, s.C, s.H, scale2 + 1, st)) return e;
   if (dX) {
     if (ex.dx_absmax) MPGCN_CUDA(cudaMemsetAsync(ex.dx_absmax, 0, sizeof(float), st));
-    if (s.C == 32) {    // the mix's W order [(d,lc)][(o,hc,h)][l] is then permute_w_bwd's [d][o][h][l]
-      if (int e = permute_w_bwd(W, wq16, nullptr, s.Ko, s.Kd, 32, s.H, st)) return e;
-    } else if (int e = permute_w_mix(W, wq16, nullptr, s.Ko, s.Kd, s.C, s.H, st)) return e;
+    if (int e = permute_w_mix(W, wq16, nullptr, s.Ko, s.Kd, s.C, s.H, st)) return e;
     if (int e = run_mix(s, v16, wq16, 1, y16, PROF_BWD_MIX, s.Ko * (s.H / 32), s.Kd * (s.C / 32), st)) return e;
     if (int e = run_bwd_dx(s, gd.g16, y16, dX, scale2 + 1, ex.dx_absmax, st)) return e;
   }

@@ -35,26 +35,25 @@ struct SgemmParams {
 };
 int simt_sgemm(const SgemmParams& p, cudaStream_t stream);
 
-// ---- elementwise / layout helpers (prep_kernels.cu) ---------------------------------------
+// ---- elementwise / layout helpers (simt_kernels.cu) ---------------------------------------
 int cvt_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t s);
-// hi = fp16(x), lo = fp16(x - hi): x == hi + lo to ~22 bits
-int cvt_f32_to_f16_hilo(const float* src, __half* hi, __half* lo, size_t n, cudaStream_t s);
 // delta[p*N + i] = G[p][i][i] - float(fp16(G[p][i][i])) for `planes` N x N matrices
 int support_diag_delta(const float* G, float* delta, size_t planes, int N, cudaStream_t s);
 // [rows][cols] fp32 -> [rows][ld] fp16 (ld >= cols, padding zeroed)
 int cvt_f32_to_f16_padded(const float* src, __half* dst, size_t rows, int cols, int ld, cudaStream_t s);
-// d_pre = d_out * (out > 0) (relu) or d_out; fp16 and/or fp32 output; db[h] += sum (db may be null; pre-zeroed)
+// d_pre = d_out * (out > 0) (relu) or d_out, 1 <= H <= 1024; exactly one output: fp32, or fp16(scale[0] * d_pre) (scale: device
+// scalar); db[h] = sum d_pre (nullable)
 int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d_pre16, float* d_pre32, float* db, size_t n, int H,
                   const float* scale, cudaStream_t s);
-// the same with the ReLU mask taken from an fp16 copy of the forward output (tensor-core path: fp16 d_pre only, H % 4 == 0)
+// the same with the ReLU mask taken from an fp16 copy of the forward output (tensor-core path: fp16 d_pre only)
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d_pre16, float* db, size_t n, int H,
                           const float* scale, cudaStream_t s);
 // scale2[0] = S = 2^k with S*max|d_out| in [16,32), scale2[1] = 1/S (S = 1 for an all-zero or non-finite input).
 // fp16 has 5 exponent bits: realistic gradients (MSE mean over B*N*N cells ~ 1e-7) must be rescaled before the cast.
 // absmax_hint: optional device scalar already holding max|d_out| (produced by the epilogue that wrote d_out): skips the pass
 int grad_scale_prepare(const float* d_out, size_t n, float* scale2, const float* absmax_hint, cudaStream_t s);
-// W[o][d][l][h] fp32 (o < Ko, d < Kd) -> Wq[d][o][h][l] (fp16 and/or fp32)
-int permute_w_bwd(const float* W, __half* wq16, float* wq32, int Ko, int Kd, int C, int H, cudaStream_t s);
+// W[o][d][l][h] fp32 (o < Ko, d < Kd) -> Wq[d][o][h][l] fp32
+int permute_w_bwd(const float* W, float* wq32, int Ko, int Kd, int C, int H, cudaStream_t s);
 // W[o][d][c][h] fp32 -> the fp16 W operand of a tensor-core channel mix (bdgcn_tc.cu), C and H multiples of 32, c = 32 lc + l,
 // h = 32 hc + h':  lo != null: forward, hi / lo = fp16 split as [(hc,o)][(d,lc)][l][h'];  lo == null: backward, [(d,lc)][(o,hc)][h'][l]
 int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s);
@@ -65,7 +64,8 @@ int mask_delta_rows(const float* delta, float* out, size_t planes, int N, int ro
 // x[i] = act(x[i] + bias[i % H]) in place (bias nullable; act 0 none / 1 ReLU): the epilogue a partial layer call leaves out
 int bias_act_inplace(float* x, const float* bias, int act, size_t n, int H, cudaStream_t s);
 // exchange steps of the origin-row shard fused into elementwise kernels over peer memory (parts / dsts: HOST arrays of g <= 8 DEVICE
-// pointers to [B][N][N][H] buffers, the rank's own and its peers' NVLink-mapped ones)
+// pointers to [B][N][N][H] buffers, the rank's own and its peers' NVLink-mapped ones); rows_reduce_bias_act takes any H >= 1, the
+// relu_backward_scatter pair any 1 <= H <= 1024
 int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int H,
                          cudaStream_t s);
 // the same with the fp16 cast of the tensor-core path folded in: scale2 = [S, 1/S] from the GLOBAL max|d_out| (device scalar), values
@@ -85,6 +85,8 @@ int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh,
 // cells per block of the backward, which keeps every recomputed step of its cells in shared memory; 0 where not even one cell
 // fits (T above 15 at hidden 64, 95 at 48, 224 at 32) or C is outside 1..64
 int lstm_bwd_cells_per_block(int T, int C);
+// d_b_hh = d_b_ih (n = 4C floats): the last step of both LSTM backwards, whose gate bias gradients are the same sum
+int lstm_copy_bias_grad(const float* d_b_ih, float* d_b_hh, int n, cudaStream_t st);
 
 // FC head + branch mean (head_kernels.cu); g / dg are HOST arrays of M device pointers
 int head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,

@@ -251,6 +251,12 @@ __global__ void copy_kernel(const float* src, float* dst, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = src[i];
 }
+int lstm_copy_bias_grad(const float* d_b_ih, float* d_b_hh, int n, cudaStream_t st) {
+  prof_count(PROF_ELEMENTWISE);
+  copy_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_b_ih, d_b_hh, n);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
 
 static constexpr size_t kBwdSmemBudget = 220 * 1024;
 
@@ -291,10 +297,7 @@ int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh,
                                                            NN, C, CELLS);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
-  prof_count(PROF_ELEMENTWISE);
-  copy_kernel<<<(G + 255) / 256, 256, 0, st>>>(d_b_ih, d_b_hh, G);   // d(b_ih) == d(b_hh)
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  return lstm_copy_bias_grad(d_b_ih, d_b_hh, G, st);
 }
 
 }  // namespace mpgcn

@@ -854,11 +854,6 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     }
 }
 
-__global__ void copy_vec_kernel(const float* src, float* dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[i];
-}
-
 }  // namespace lstm_tc
 
 // ---------------------------------------------------------------------------------------
@@ -1002,10 +997,7 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
   if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2, cells, T, NN, st))
     return e;
-  prof_count(PROF_ELEMENTWISE);
-  lstm_tc::copy_vec_kernel<<<(G4 + 127) / 128, 128, 0, st>>>(d_b_ih, d_b_hh, G4);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  return lstm_copy_bias_grad(d_b_ih, d_b_hh, G4, st);
 }
 
 }  // namespace mpgcn

@@ -7,6 +7,9 @@
 // the fp16 tensor path).  It is NOT a CPU fallback: everything here runs on the GPU.
 #include "kernels.h"
 
+#include <algorithm>
+#include <type_traits>
+
 namespace mpgcn {
 
 // ---------------------------------------------------------------------------------------
@@ -158,23 +161,6 @@ int cvt_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t s) {
   return 0;
 }
 
-__global__ void cvt_f16_hilo_kernel(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float x = src[i];
-    const __half h = f2h_sat(x);
-    hi[i] = h;
-    lo[i] = f2h_sat(x - __half2float(h));
-  }
-}
-int cvt_f32_to_f16_hilo(const float* src, __half* hi, __half* lo, size_t n, cudaStream_t s) {
-  if (n == 0) return 0;
-  prof_count(PROF_ELEMENTWISE);
-  cvt_f16_hilo_kernel<<<grid_for(n, 256), 256, 0, s>>>(src, hi, lo, n);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
 // delta[p][i] = G_p[i,i] - fp16(G_p[i,i]) where the diagonal entry DOMINATES its column (G_ii^2 > kDiagTau * sum_{c != i} G_ci^2),
 // else 0.  The contraction epilogues add delta * (the diagonal operand row) back, which removes the one rounding error that
 // matters when a support is close to the identity (Chebyshev / random-walk T_k of a sparse graph); for a dense support the
@@ -231,150 +217,143 @@ int cvt_f32_to_f16_padded(const float* src, __half* dst, size_t rows, int cols, 
   return 0;
 }
 
-// d_pre = d_out * [out > 0];  db[h] += sum over cells.  Thread's channel is fixed because the
-// grid stride is a multiple of H.
-__global__ void relu_bwd_prep_kernel(const float* __restrict__ d_out, const float* __restrict__ out, int relu,
-                                     __half* __restrict__ d16, float* __restrict__ d32, float* __restrict__ db, size_t n, int H,
-                                     const float* __restrict__ scale) {
-  const float S = scale ? __ldg(scale) : 1.f;
-  extern __shared__ float s_db[];   // [blockDim.x]
-  const size_t stride = (size_t)gridDim.x * blockDim.x;   // multiple of H by construction
-  float local = 0.f;
-  const size_t first = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (size_t i = first; i < n; i += stride) {
-    float g = d_out[i];
-    if (relu && !(out[i] > 0.f)) g = 0.f;
-    if (d16) d16[i] = f2h_sat(g * S);
-    if (d32) d32[i] = g;
-    local += g;
-  }
-  if (db) {
-    s_db[threadIdx.x] = local;
-    __syncthreads();
-    if ((int)threadIdx.x < H) {
-      // threads t, t+H, t+2H, ... of this block share channel (first % H)
-      float sum = 0.f;
-      for (int t = threadIdx.x; t < (int)blockDim.x; t += H) sum += s_db[t];
-      const int ch = (int)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) % H);
-      atomicAdd(&db[ch], sum);
-    }
+// ---- ReLU backward: d_pre = d_out * [out > 0] (or d_out), stored as fp32 or as fp16(S * d_pre) into g <= 8 destinations, and the
+// per-channel bias gradient db[h] = sum d_pre.  The local pass of a layer backward is one sample and one destination; the row
+// shard's all-gather (relu_backward_scatter[_f16]) writes rows [row0, row0 + rows) of every rank's [B][N][N][H] buffer.
+enum class Mask { None, F32, F16 };   // ReLU mask source: none (linear layer), the fp32 forward output, or its fp16 copy
+template <class T>
+struct PeerPtrs { T* p[8]; };
+
+// V consecutive values at p <-> V floats in registers; V = 4 is one 16-byte (fp32) or 8-byte (fp16) access
+__device__ __forceinline__ void ld_v(const float* p, float (&v)[1]) { v[0] = *p; }
+__device__ __forceinline__ void ld_v(const float* p, float (&v)[4]) {
+  const float4 t = *reinterpret_cast<const float4*>(p);
+  v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+__device__ __forceinline__ void ld_v(const __half* p, float (&v)[1]) { v[0] = __half2float(*p); }
+__device__ __forceinline__ void ld_v(const __half* p, float (&v)[4]) {
+  const uint2 t = *reinterpret_cast<const uint2*>(p);
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
+  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+}
+// read once: streaming loads
+__device__ __forceinline__ void ld_cs_v(const float* p, float (&v)[1]) { v[0] = __ldcs(p); }
+__device__ __forceinline__ void ld_cs_v(const float* p, float (&v)[4]) {
+  const float4 t = __ldcs(reinterpret_cast<const float4*>(p));
+  v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+// fp32 stores the value, fp16 stores fp16(S * value) (saturating).  __stwb is the default store; a plain assignment through the
+// cast pointer compiles to 4-byte stores here.
+__device__ __forceinline__ void st_v(float* p, const float (&v)[1], float) { *p = v[0]; }
+__device__ __forceinline__ void st_v(float* p, const float (&v)[4], float) { __stwb(reinterpret_cast<float4*>(p), make_float4(v[0], v[1], v[2], v[3])); }
+__device__ __forceinline__ void st_v(__half* p, const float (&v)[1], float S) { *p = f2h_sat(v[0] * S); }
+__device__ __forceinline__ void st_v(__half* p, const float (&v)[4], float S) {
+  const __half2 a = __halves2half2(f2h_sat(v[0] * S), f2h_sat(v[1] * S)), b = __halves2half2(f2h_sat(v[2] * S), f2h_sat(v[3] * S));
+  __stwb(reinterpret_cast<uint2*>(p), make_uint2(*reinterpret_cast<const unsigned int*>(&a), *reinterpret_cast<const unsigned int*>(&b)));
+}
+
+// db[c] += the block's partial sums of channel c.  The block is a multiple of H / V threads with at least H of them, so thread t
+// owns channels V * (t % (H / V)) .. + V - 1 for its whole grid-stride loop; thread c < H adds the partials of channel c in thread order.
+template <int V>
+__device__ __forceinline__ void block_bias_grad(const float (&local)[V], float* db, int H) {
+  extern __shared__ float s_db[];   // [V][blockDim.x]
+  const int nt = blockDim.x;
+#pragma unroll
+  for (int e = 0; e < V; ++e) s_db[e * nt + threadIdx.x] = local[e];
+  __syncthreads();
+  if ((int)threadIdx.x < H) {
+    const int q = threadIdx.x / V, e = threadIdx.x % V;
+    float sum = 0.f;
+    for (int t = q; t < nt; t += H / V) sum += s_db[e * nt + t];
+    atomicAdd(&db[threadIdx.x], sum);
   }
 }
 
-// Same, four channels per thread (float4 loads, one 8-byte fp16 store): H % 4 == 0, H / 4 divides the block size, so a
-// thread keeps its four channels across the grid-stride loop.
-__global__ void relu_bwd_prep_vec4_kernel(const float4* __restrict__ d_out, const float4* __restrict__ out, int relu,
-                                          uint2* __restrict__ d16, float4* __restrict__ d32, float* __restrict__ db, size_t n4, int H4,
-                                          const float* __restrict__ scale) {
-  const float S = scale ? __ldg(scale) : 1.f;
-  extern __shared__ float s_db[];   // [4][blockDim.x]
-  const size_t stride = (size_t)gridDim.x * blockDim.x;   // multiple of H4 by construction
-  float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 g = d_out[i];
-    if (relu) {
-      const float4 o = out[i];
-      g.x = o.x > 0.f ? g.x : 0.f; g.y = o.y > 0.f ? g.y : 0.f;
-      g.z = o.z > 0.f ? g.z : 0.f; g.w = o.w > 0.f ? g.w : 0.f;
+// grid.y = sample b: d_out[b * n + i] -> dst[j][b * full + off + i] for i < n; S = scale[0] for an fp16 destination.  At most
+// 32 registers, so that 2048 threads fit on an SM: a streaming kernel needs every load in flight it can get.
+template <int V, Mask M, class T>
+__global__ void __launch_bounds__(1024, 2) relu_bwd_kernel(const float* __restrict__ d_out, const void* __restrict__ mask, PeerPtrs<T> dst, int g, float* __restrict__ db,
+                                const float* __restrict__ scale, size_t n, size_t full, size_t off, int H) {
+  using MaskT = std::conditional_t<M == Mask::F16, __half, float>;
+  const float S = std::is_same<T, __half>::value ? __ldg(scale) : 1.f;
+  const size_t b = blockIdx.y;
+  float local[V] = {};
+  for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; i < n; i += (size_t)gridDim.x * blockDim.x * V) {
+    float v[V];
+    ld_v(d_out + b * n + i, v);
+    if constexpr (M != Mask::None) {
+      float o[V];
+      ld_v(static_cast<const MaskT*>(mask) + b * n + i, o);
+#pragma unroll
+      for (int e = 0; e < V; ++e) v[e] = o[e] > 0.f ? v[e] : 0.f;
     }
-    if (d16) {
-      const __half2 a = __halves2half2(f2h_sat(g.x * S), f2h_sat(g.y * S)), b = __halves2half2(f2h_sat(g.z * S), f2h_sat(g.w * S));
-      d16[i] = make_uint2(*reinterpret_cast<const unsigned int*>(&a), *reinterpret_cast<const unsigned int*>(&b));
-    }
-    if (d32) d32[i] = g;
-    l0 += g.x; l1 += g.y; l2 += g.z; l3 += g.w;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (j < g) st_v(dst.p[j] + b * full + off + i, v, S);
+#pragma unroll
+    for (int e = 0; e < V; ++e) local[e] += v[e];
   }
-  if (db) {
-    const int nt = blockDim.x;
-    s_db[threadIdx.x] = l0; s_db[nt + threadIdx.x] = l1; s_db[2 * nt + threadIdx.x] = l2; s_db[3 * nt + threadIdx.x] = l3;
-    __syncthreads();
-    if ((int)threadIdx.x < 4 * H4) {       // one thread per channel: quad q = channel / 4, component e = channel % 4
-      const int q = threadIdx.x >> 2, e = threadIdx.x & 3;
-      float sum = 0.f;
-      for (int t = q; t < nt; t += H4) sum += s_db[e * nt + t];
-      const int quad0 = (int)(((size_t)blockIdx.x * blockDim.x) % H4);      // channel quad of thread 0 of this block
-      atomicAdd(&db[((q + quad0) % H4) * 4 + e], sum);
-    }
-  }
+  if (db) block_bias_grad<V>(local, db, H);
 }
 
-__global__ void relu_bwd_prep_f16mask_kernel(const float4* __restrict__ d_out, const uint2* __restrict__ out16, int relu,
-                                             uint2* __restrict__ d16, float* __restrict__ db, size_t n4, int H4,
-                                             const float* __restrict__ scale) {
-  const float S = scale ? __ldg(scale) : 1.f;
-  extern __shared__ float s_db[];   // [4][blockDim.x]
-  const size_t stride = (size_t)gridDim.x * blockDim.x;   // multiple of H4 by construction
-  float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 g = d_out[i];
-    if (relu) {
-      const uint2 o = out16[i];
-      const float2 o01 = __half22float2(*reinterpret_cast<const __half2*>(&o.x)), o23 = __half22float2(*reinterpret_cast<const __half2*>(&o.y));
-      g.x = o01.x > 0.f ? g.x : 0.f; g.y = o01.y > 0.f ? g.y : 0.f;
-      g.z = o23.x > 0.f ? g.z : 0.f; g.w = o23.y > 0.f ? g.w : 0.f;
-    }
-    const __half2 a = __halves2half2(f2h_sat(g.x * S), f2h_sat(g.y * S)), b = __halves2half2(f2h_sat(g.z * S), f2h_sat(g.w * S));
-    d16[i] = make_uint2(*reinterpret_cast<const unsigned int*>(&a), *reinterpret_cast<const unsigned int*>(&b));
-    l0 += g.x; l1 += g.y; l2 += g.z; l3 += g.w;
-  }
-  if (db) {
-    const int nt = blockDim.x;
-    s_db[threadIdx.x] = l0; s_db[nt + threadIdx.x] = l1; s_db[2 * nt + threadIdx.x] = l2; s_db[3 * nt + threadIdx.x] = l3;
-    __syncthreads();
-    if ((int)threadIdx.x < 4 * H4) {
-      const int q = threadIdx.x >> 2, e = threadIdx.x & 3;
-      float sum = 0.f;
-      for (int t = q; t < nt; t += H4) sum += s_db[e * nt + t];
-      const int quad0 = (int)(((size_t)blockIdx.x * blockDim.x) % H4);
-      atomicAdd(&db[((q + quad0) % H4) * 4 + e], sum);
-    }
-  }
+static bool aligned(const void* p, size_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// Block size of the elementwise kernels that keep a thread's channels fixed: a multiple of H / V threads (the grid stride then is
+// one too), at least one thread per channel, 256 for every H / V that divides 256.
+static int channel_block(int H, int V) {
+  const int HV = H / V;
+  return HV * std::max(256 / HV, V);
 }
 
-// block size of the four-channel kernels: a multiple of H / 4 (a thread keeps its channel quad across the grid-stride loop) with
-// at least one thread per channel for the bias-gradient reduction; 256 for every H <= 256 whose quad count divides 256
-static int quad_block(int H) {
-  const int H4 = H / 4;
-  return H4 * (256 / H4 > 4 ? 256 / H4 : 4);
+// One relu_bwd_kernel launch over B samples of n elements; V = 4 when H, n, full, off are multiples of 4 and every pointer is aligned
+// for the vector access, else V = 1.  The exchange steps (PROF_EXCHANGE) are timed, the local pass is counted.
+template <Mask M, class T>
+static int relu_bwd_launch(const float* d_out, const void* mask, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s) {
+  MPGCN_CHECK(H >= 1 && H <= 1024, "relu backward: H=%d unsupported (1..1024)", H);
+  MPGCN_CHECK(g >= 1 && g <= 8, "relu backward: %d ranks unsupported (1..8)", g);
+  constexpr bool f16 = std::is_same<T, __half>::value;
+  MPGCN_CHECK(!f16 || scale != nullptr, "relu backward: an fp16 destination needs its scale");
+  bool vec = H % 4 == 0 && (n | full | off) % 4 == 0 && aligned(d_out, 16) && (M == Mask::None || aligned(mask, M == Mask::F16 ? 8 : 16));
+  PeerPtrs<T> pp{};
+  for (int j = 0; j < g; ++j) {
+    MPGCN_CHECK(dsts[j] != nullptr, "relu backward: destination %d is null", j);
+    pp.p[j] = dsts[j];
+    vec = vec && aligned(dsts[j], 4 * sizeof(T));
+  }
+  if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, s));
+  const int V = vec ? 4 : 1, threads = channel_block(H, V);
+  const dim3 grid(grid_for(n / V, threads), (unsigned)B);
+  const size_t smem = (size_t)V * threads * sizeof(float);
+  if (tag == PROF_EXCHANGE) prof_begin(tag, 0.0, s);
+  else prof_count(tag);
+  if (vec) relu_bwd_kernel<4, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, scale, n, full, off, H);
+  else relu_bwd_kernel<1, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, scale, n, full, off, H);
+  prof_end(s);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+// the same with the ReLU mask taken from the fp32 forward output (act 1) or no mask (act 0)
+template <class T>
+static int relu_bwd_launch(const float* d_out, const float* out, int act, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s) {
+  return act ? relu_bwd_launch<Mask::F32>(d_out, out, dsts, g, db, scale, B, n, full, off, H, tag, s)
+             : relu_bwd_launch<Mask::None>(d_out, nullptr, dsts, g, db, scale, B, n, full, off, H, tag, s);
 }
 
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d16, float* db, size_t n, int H, const float* scale,
                           cudaStream_t s) {
   if (n == 0) return 0;
-  MPGCN_CHECK(H % 4 == 0 && H >= 4 && H <= 1024 && n % 4 == 0, "relu_bwd_prep_f16mask: H=%d / n=%zu unsupported", H, n);
-  MPGCN_CHECK(((reinterpret_cast<uintptr_t>(d_out) & 15) | (reinterpret_cast<uintptr_t>(out16) & 7) | (reinterpret_cast<uintptr_t>(d16) & 7)) == 0,
-              "relu_bwd_prep_f16mask: misaligned pointer");
-  const int threads = quad_block(H);
-  prof_count(PROF_ELEMENTWISE);
-  relu_bwd_prep_f16mask_kernel<<<grid_for(n / 4, threads), threads, 4 * threads * sizeof(float), s>>>(
-      reinterpret_cast<const float4*>(d_out), reinterpret_cast<const uint2*>(out16), relu, reinterpret_cast<uint2*>(d16), db, n / 4, H / 4, scale);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  if (!relu) return relu_bwd_launch<Mask::None>(d_out, nullptr, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
+  return relu_bwd_launch<Mask::F16>(d_out, out16, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
 }
 
 int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d16, float* d32, float* db, size_t n, int H,
                   const float* scale, cudaStream_t s) {
   if (n == 0) return 0;
-  MPGCN_CHECK(H >= 1 && H <= 1024, "relu_bwd_prep: H=%d unsupported", H);
-  const bool aligned = ((reinterpret_cast<uintptr_t>(d_out) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(d32)) & 15) == 0 &&
-                       (reinterpret_cast<uintptr_t>(d16) & 7) == 0;
-  if (H % 4 == 0 && 256 % (H / 4) == 0 && n % 4 == 0 && aligned) {
-    const int threads = quad_block(H);
-    unsigned blocks = grid_for(n / 4, threads);
-    prof_count(PROF_ELEMENTWISE);
-    relu_bwd_prep_vec4_kernel<<<blocks, threads, 4 * threads * sizeof(float), s>>>(
-        reinterpret_cast<const float4*>(d_out), reinterpret_cast<const float4*>(out), relu, reinterpret_cast<uint2*>(d16),
-        reinterpret_cast<float4*>(d32), db, n / 4, H / 4, scale);
-    MPGCN_CUDA(cudaGetLastError());
-    return 0;
-  }
-  int threads = (256 / H) * H;          // multiple of H so each thread keeps one channel
-  if (threads == 0) threads = H;
-  unsigned blocks = grid_for(n, threads);
-  prof_count(PROF_ELEMENTWISE);
-  relu_bwd_prep_kernel<<<blocks, threads, threads * sizeof(float), s>>>(d_out, out, relu, d16, d32, db, n, H, scale);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  MPGCN_CHECK((d16 == nullptr) != (d32 == nullptr), "relu_bwd_prep: exactly one of the fp16 and fp32 outputs");
+  if (d16) return relu_bwd_launch(d_out, out, relu, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
+  return relu_bwd_launch(d_out, out, relu, &d32, 1, db, nullptr, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
 }
 
 // max |x| over a tensor as the bit pattern of a non-negative float (monotone as unsigned int)
@@ -411,8 +390,7 @@ int grad_scale_prepare(const float* d_out, size_t n, float* scale2, const float*
   return 0;
 }
 
-__global__ void permute_w_bwd_kernel(const float* __restrict__ W, __half* __restrict__ q16, float* __restrict__ q32, int Ko, int Kd, int C,
-                                     int H) {
+__global__ void permute_w_bwd_kernel(const float* __restrict__ W, float* __restrict__ q32, int Ko, int Kd, int C, int H) {
   const int total = Ko * Kd * C * H;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     // destination index i = ((d*Ko + o)*H + h)*C + l
@@ -420,15 +398,13 @@ __global__ void permute_w_bwd_kernel(const float* __restrict__ W, __half* __rest
     const int h = (i / C) % H;
     const int o = (i / (C * H)) % Ko;
     const int d = i / (C * H * Ko);
-    const float v = W[((size_t)(o * Kd + d) * C + l) * H + h];
-    if (q16) q16[i] = f2h_sat(v);
-    if (q32) q32[i] = v;
+    q32[i] = W[((size_t)(o * Kd + d) * C + l) * H + h];
   }
 }
 
-int permute_w_bwd(const float* W, __half* wq16, float* wq32, int Ko, int Kd, int C, int H, cudaStream_t s) {
+int permute_w_bwd(const float* W, float* wq32, int Ko, int Kd, int C, int H, cudaStream_t s) {
   prof_count(PROF_ELEMENTWISE);
-  permute_w_bwd_kernel<<<grid_for((size_t)Ko * Kd * C * H, 256), 256, 0, s>>>(W, wq16, wq32, Ko, Kd, C, H);
+  permute_w_bwd_kernel<<<grid_for((size_t)Ko * Kd * C * H, 256), 256, 0, s>>>(W, wq32, Ko, Kd, C, H);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }
@@ -502,190 +478,93 @@ int mask_delta_rows(const float* delta, float* out, size_t planes, int N, int ro
   return 0;
 }
 
-// in place: x = act(x + bias[channel]); H % 4 == 0 and 16-byte alignment take the float4 path
-__global__ void bias_act_vec4_kernel(float4* __restrict__ x, const float* __restrict__ bias, int act, size_t n4, int H4) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 v = x[i];
-    if (bias) {
-      const float4 b = reinterpret_cast<const float4*>(bias)[i % H4];
-      v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
-    }
-    if (act) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-    x[i] = v;
-  }
-}
-__global__ void bias_act_kernel(float* __restrict__ x, const float* __restrict__ bias, int act, size_t n, int H) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float v = x[i] + (bias ? bias[i % H] : 0.f);
-    x[i] = act ? fmaxf(v, 0.f) : v;
-  }
-}
 // ---- exchange steps of the origin-row shard, fused into elementwise kernels over PEER memory (NVLink P2P loads / stores) ----
-struct PeerPtrs { float* p[8]; };
-
-// out[b][r][e][h] = act( sum_j part[j][b][row0 + r][e][h] + bias[h] ): the reduce-scatter of the partial pre-activations -- every rank
-// reads ITS rows out of all g partial buffers (its own and, over NVLink, the peers') -- fused with the bias / activation epilogue
-// (reference MPGCN.py:47-49).  grid.y = sample; x4 = float4 index inside the sample's slab.
-__global__ void rows_reduce_bias_act_kernel(float4* __restrict__ out, PeerPtrs parts, int g, const float* __restrict__ bias, int act,
-                                            size_t slab4 /*rows*N*H/4*/, size_t full4 /*N*N*H/4*/, size_t off4 /*row0*N*H/4*/, int H4) {
+// out[b][i] = act( sum_j parts[j][b * full + off + i] + bias[i % H] ) for i < n; grid.y = sample b.  For the row shard's reduce-scatter
+// of the partial pre-activations, every rank reads ITS rows out of all g partial buffers (its own and, over NVLink, the peers') and
+// applies the bias / activation epilogue (reference MPGCN.py:47-49).  bias_act_inplace is g = 1, parts[0] == out: out and parts
+// alias, hence no __restrict__ on them.
+template <int V>
+__global__ void reduce_bias_act_kernel(float* out, PeerPtrs<const float> parts, int g, const float* __restrict__ bias, int act, size_t n,
+                                       size_t full, size_t off, int H) {
   const size_t b = blockIdx.y;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < slab4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; i < n; i += (size_t)gridDim.x * blockDim.x * V) {
+    float acc[V];
+    ld_cs_v(parts.p[0] + b * full + off + i, acc);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 1; j < 8; ++j) {
       if (j < g) {
-        const float4 v = __ldcs(reinterpret_cast<const float4*>(parts.p[j]) + b * full4 + off4 + i);      // read once: streaming
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+        float v[V];
+        ld_cs_v(parts.p[j] + b * full + off + i, v);
+#pragma unroll
+        for (int e = 0; e < V; ++e) acc[e] += v[e];
       }
     }
     if (bias) {
-      const float4 bb = reinterpret_cast<const float4*>(bias)[i % H4];
-      acc.x += bb.x; acc.y += bb.y; acc.z += bb.z; acc.w += bb.w;
+      float bb[V];
+      ld_v(bias + i % H, bb);
+#pragma unroll
+      for (int e = 0; e < V; ++e) acc[e] += bb[e];
     }
-    if (act) { acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f); }
-    out[b * slab4 + i] = acc;
+    if (act)
+#pragma unroll
+      for (int e = 0; e < V; ++e) acc[e] = fmaxf(acc[e], 0.f);
+    st_v(out + b * n + i, acc, 1.f);
   }
 }
-int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int H,
-                         cudaStream_t s) {
+// B samples of n outputs, 256 threads; V = 4 when H, n, full, off are multiples of 4 and every pointer is 16-byte aligned
+static int reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, size_t n, size_t full, size_t off,
+                           int H, ProfTag tag, cudaStream_t s) {
   MPGCN_CHECK(g >= 1 && g <= 8, "rows_reduce: %d ranks unsupported (1..8)", g);
-  MPGCN_CHECK(H % 4 == 0 && row0 >= 0 && rows >= 1 && row0 + rows <= N, "rows_reduce: bad slab rows [%d, %d) of %d, H=%d", row0, row0 + rows, N, H);
-  PeerPtrs pp{};
+  MPGCN_CHECK(H >= 1, "bias_act: H=%d", H);
+  bool vec = H % 4 == 0 && (n | full | off) % 4 == 0 && aligned(out, 16) && aligned(bias, 16);
+  PeerPtrs<const float> pp{};
   for (int j = 0; j < g; ++j) {
-    MPGCN_CHECK(parts[j] != nullptr && (reinterpret_cast<uintptr_t>(parts[j]) & 15) == 0, "rows_reduce: partial buffer %d null or misaligned", j);
-    pp.p[j] = const_cast<float*>(parts[j]);
+    MPGCN_CHECK(parts[j] != nullptr, "rows_reduce: partial buffer %d is null", j);
+    pp.p[j] = parts[j];
+    vec = vec && aligned(parts[j], 16);
   }
-  const size_t slab4 = (size_t)rows * N * H / 4, full4 = (size_t)N * N * H / 4, off4 = (size_t)row0 * N * H / 4;
-  dim3 grid(grid_for(slab4, 256), (unsigned)B);
-  prof_begin(PROF_EXCHANGE, 0.0, s);
-  rows_reduce_bias_act_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<float4*>(out), pp, g, bias, act, slab4, full4, off4, H / 4);
+  const dim3 grid(grid_for(vec ? n / 4 : n, 256), (unsigned)B);
+  if (tag == PROF_EXCHANGE) prof_begin(tag, 0.0, s);
+  else prof_count(tag);
+  if (vec) reduce_bias_act_kernel<4><<<grid, 256, 0, s>>>(out, pp, g, bias, act, n, full, off, H);
+  else reduce_bias_act_kernel<1><<<grid, 256, 0, s>>>(out, pp, g, bias, act, n, full, off, H);
   prof_end(s);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// d_pre = d_out * [out > 0] (or d_out), written to rows [row0, row0 + rows) of EVERY destination buffer [B][N][N][H] -- the rank's own
-// and, over NVLink, the peers': the all-gather of dPre fused with the ReLU mask; db[h] += sum d_pre.  H4 divides the block size,
-// so a thread keeps its four channels.
-__global__ void relu_backward_scatter_kernel(const float4* __restrict__ d_out, const float4* __restrict__ out, int act, PeerPtrs dst, int g,
-                                             float* __restrict__ db, size_t slab4, size_t full4, size_t off4, int H4) {
-  extern __shared__ float s_db[];   // [4][blockDim.x]
-  const size_t b = blockIdx.y;
-  float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < slab4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 gq = d_out[b * slab4 + i];
-    if (act) {
-      const float4 o = out[b * slab4 + i];
-      gq.x = o.x > 0.f ? gq.x : 0.f; gq.y = o.y > 0.f ? gq.y : 0.f; gq.z = o.z > 0.f ? gq.z : 0.f; gq.w = o.w > 0.f ? gq.w : 0.f;
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (j < g) reinterpret_cast<float4*>(dst.p[j])[b * full4 + off4 + i] = gq;
-    l0 += gq.x; l1 += gq.y; l2 += gq.z; l3 += gq.w;
-  }
-  if (db) {
-    const int nt = blockDim.x;
-    s_db[threadIdx.x] = l0; s_db[nt + threadIdx.x] = l1; s_db[2 * nt + threadIdx.x] = l2; s_db[3 * nt + threadIdx.x] = l3;
-    __syncthreads();
-    if ((int)threadIdx.x < 4 * H4) {       // one thread per channel: quad q = channel / 4, component e = channel % 4
-      const int q = threadIdx.x >> 2, e = threadIdx.x & 3;
-      float sum = 0.f;
-      for (int t = q; t < nt; t += H4) sum += s_db[e * nt + t];      // threads t = q (mod H4) own quad q (the grid stride is a multiple of H4)
-      atomicAdd(&db[q * 4 + e], sum);
-    }
-  }
-}
-int relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N, int row0, int rows,
-                          int H, cudaStream_t s) {
-  MPGCN_CHECK(g >= 1 && g <= 8, "relu_backward_scatter: %d ranks unsupported (1..8)", g);
-  MPGCN_CHECK(H % 4 == 0 && 256 % (H / 4) == 0 && 4 * (H / 4) <= 256, "relu_backward_scatter: H=%d unsupported", H);
-  MPGCN_CHECK(row0 >= 0 && rows >= 1 && row0 + rows <= N, "relu_backward_scatter: bad slab rows [%d, %d) of %d", row0, row0 + rows, N);
-  PeerPtrs pp{};
-  for (int j = 0; j < g; ++j) {
-    MPGCN_CHECK(dsts[j] != nullptr && (reinterpret_cast<uintptr_t>(dsts[j]) & 15) == 0, "relu_backward_scatter: destination %d null or misaligned", j);
-    pp.p[j] = dsts[j];
-  }
-  if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, s));
-  const size_t slab4 = (size_t)rows * N * H / 4, full4 = (size_t)N * N * H / 4, off4 = (size_t)row0 * N * H / 4;
-  dim3 grid(grid_for(slab4, 256), (unsigned)B);
-  prof_begin(PROF_EXCHANGE, 0.0, s);
-  relu_backward_scatter_kernel<<<grid, 256, 4 * 256 * sizeof(float), s>>>(reinterpret_cast<const float4*>(d_out), reinterpret_cast<const float4*>(out),
-                                                                         act, pp, g, db, slab4, full4, off4, H / 4);
-  prof_end(s);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
-struct PeerPtrs16 { __half* p[8]; };
-__global__ void relu_backward_scatter_f16_kernel(const float4* __restrict__ d_out, const float4* __restrict__ out, int act, PeerPtrs16 dst, int g,
-                                                 float* __restrict__ db, const float* __restrict__ scale2, size_t slab4, size_t full4, size_t off4,
-                                                 int H4) {
-  extern __shared__ float s_db[];   // [4][blockDim.x]
-  const float S = __ldg(scale2);
-  const size_t b = blockIdx.y;
-  float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < slab4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 gq = d_out[b * slab4 + i];
-    if (act) {
-      const float4 o = out[b * slab4 + i];
-      gq.x = o.x > 0.f ? gq.x : 0.f; gq.y = o.y > 0.f ? gq.y : 0.f; gq.z = o.z > 0.f ? gq.z : 0.f; gq.w = o.w > 0.f ? gq.w : 0.f;
-    }
-    const __half2 lo = __halves2half2(f2h_sat(gq.x * S), f2h_sat(gq.y * S)), hi = __halves2half2(f2h_sat(gq.z * S), f2h_sat(gq.w * S));
-    const uint2 pk = make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (j < g) reinterpret_cast<uint2*>(dst.p[j])[b * full4 + off4 + i] = pk;
-    l0 += gq.x; l1 += gq.y; l2 += gq.z; l3 += gq.w;
-  }
-  if (db) {
-    const int nt = blockDim.x;
-    s_db[threadIdx.x] = l0; s_db[nt + threadIdx.x] = l1; s_db[2 * nt + threadIdx.x] = l2; s_db[3 * nt + threadIdx.x] = l3;
-    __syncthreads();
-    if ((int)threadIdx.x < 4 * H4) {
-      const int q = threadIdx.x >> 2, e = threadIdx.x & 3;
-      float sum = 0.f;
-      for (int t = q; t < nt; t += H4) sum += s_db[e * nt + t];
-      atomicAdd(&db[q * 4 + e], sum);
-    }
-  }
-}
-int relu_backward_scatter_f16(const float* d_out, const float* out, int act, __half* const* dsts, int g, float* db, const float* absmax,
-                              float* scale2, int B, int N, int row0, int rows, int H, cudaStream_t s) {
-  MPGCN_CHECK(g >= 1 && g <= 8, "relu_backward_scatter_f16: %d ranks unsupported (1..8)", g);
-  MPGCN_CHECK(H % 4 == 0 && 256 % (H / 4) == 0 && 4 * (H / 4) <= 256, "relu_backward_scatter_f16: H=%d unsupported", H);
-  MPGCN_CHECK(row0 >= 0 && rows >= 1 && row0 + rows <= N, "relu_backward_scatter_f16: bad slab rows [%d, %d) of %d", row0, row0 + rows, N);
-  MPGCN_CHECK(absmax != nullptr && scale2 != nullptr, "relu_backward_scatter_f16: absmax / scale2 are required");
-  PeerPtrs16 pp{};
-  for (int j = 0; j < g; ++j) {
-    MPGCN_CHECK(dsts[j] != nullptr && (reinterpret_cast<uintptr_t>(dsts[j]) & 7) == 0, "relu_backward_scatter_f16: destination %d null or misaligned", j);
-    pp.p[j] = dsts[j];
-  }
-  if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, s));
-  prof_count(PROF_ELEMENTWISE);
-  make_scale_kernel<<<1, 1, 0, s>>>(scale2, absmax);
-  const size_t slab4 = (size_t)rows * N * H / 4, full4 = (size_t)N * N * H / 4, off4 = (size_t)row0 * N * H / 4;
-  dim3 grid(grid_for(slab4, 256), (unsigned)B);
-  prof_begin(PROF_EXCHANGE, 0.0, s);
-  relu_backward_scatter_f16_kernel<<<grid, 256, 4 * 256 * sizeof(float), s>>>(reinterpret_cast<const float4*>(d_out), reinterpret_cast<const float4*>(out),
-                                                                             act, pp, g, db, scale2, slab4, full4, off4, H / 4);
-  prof_end(s);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-int absmax_f32(const float* x, size_t n, float* out, cudaStream_t s) {
-  MPGCN_CUDA(cudaMemsetAsync(out, 0, sizeof(float), s));
-  prof_count(PROF_ELEMENTWISE);
-  absmax_kernel<<<grid_for(n, 256), 256, 0, s>>>(x, n, reinterpret_cast<unsigned int*>(out));
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }
 
 int bias_act_inplace(float* x, const float* bias, int act, size_t n, int H, cudaStream_t s) {
-  MPGCN_CHECK(H >= 1, "bias_act: H=%d", H);
+  return reduce_bias_act(x, &x, 1, bias, act, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
+}
+
+int rows_reduce_bias_act(float* out, const float* const* parts, int g, const float* bias, int act, int B, int N, int row0, int rows, int H,
+                         cudaStream_t s) {
+  MPGCN_CHECK(H >= 1 && row0 >= 0 && rows >= 1 && row0 + rows <= N, "rows_reduce: bad slab rows [%d, %d) of %d, H=%d", row0, row0 + rows, N, H);
+  return reduce_bias_act(out, parts, g, bias, act, B, (size_t)rows * N * H, (size_t)N * N * H, (size_t)row0 * N * H, H, PROF_EXCHANGE, s);
+}
+
+// d_pre = d_out * [out > 0] (or d_out), written to rows [row0, row0 + rows) of EVERY destination buffer [B][N][N][H] -- the rank's own
+// and, over NVLink, the peers': the all-gather of dPre fused with the ReLU mask; db[h] = sum d_pre.
+int relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N, int row0, int rows,
+                          int H, cudaStream_t s) {
+  MPGCN_CHECK(row0 >= 0 && rows >= 1 && row0 + rows <= N, "relu_backward_scatter: bad slab rows [%d, %d) of %d", row0, row0 + rows, N);
+  return relu_bwd_launch(d_out, out, act, dsts, g, db, nullptr, B, (size_t)rows * N * H, (size_t)N * N * H, (size_t)row0 * N * H, H,
+                         PROF_EXCHANGE, s);
+}
+// the same storing fp16(S * d_pre), S from the global max|d_out|
+int relu_backward_scatter_f16(const float* d_out, const float* out, int act, __half* const* dsts, int g, float* db, const float* absmax,
+                              float* scale2, int B, int N, int row0, int rows, int H, cudaStream_t s) {
+  MPGCN_CHECK(row0 >= 0 && rows >= 1 && row0 + rows <= N, "relu_backward_scatter_f16: bad slab rows [%d, %d) of %d", row0, row0 + rows, N);
+  MPGCN_CHECK(absmax != nullptr && scale2 != nullptr, "relu_backward_scatter_f16: absmax / scale2 are required");
   prof_count(PROF_ELEMENTWISE);
-  const bool vec = (H % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(bias)) & 15) == 0;
-  if (vec) bias_act_vec4_kernel<<<grid_for(n / 4, 256), 256, 0, s>>>(reinterpret_cast<float4*>(x), bias, act, n / 4, H / 4);
-  else bias_act_kernel<<<grid_for(n, 256), 256, 0, s>>>(x, bias, act, n, H);
+  make_scale_kernel<<<1, 1, 0, s>>>(scale2, absmax);
+  return relu_bwd_launch(d_out, out, act, dsts, g, db, scale2, B, (size_t)rows * N * H, (size_t)N * N * H, (size_t)row0 * N * H, H,
+                         PROF_EXCHANGE, s);
+}
+int absmax_f32(const float* x, size_t n, float* out, cudaStream_t s) {
+  MPGCN_CUDA(cudaMemsetAsync(out, 0, sizeof(float), s));
+  prof_count(PROF_ELEMENTWISE);
+  absmax_kernel<<<grid_for(n, 256), 256, 0, s>>>(x, n, reinterpret_cast<unsigned int*>(out));
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }

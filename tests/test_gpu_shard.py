@@ -111,19 +111,42 @@ def test_row_shard_fp16_partials_on_dominant_diagonals_sum_to_the_whole_layer(N,
     _check(total, whole, 1e-5, f"row shard N={N} x{world} {'dyn' if dyn else 'static'}/diag fp16: sum of partials == fp16 whole layer")
 
 
+def _bits(t):
+    return t.view(torch.int16 if t.dtype == torch.float16 else torch.int32)
+
+
+def _masked(d, out):
+    return torch.where(out > 0, d, torch.zeros_like(d))
+
+
+def _check_db(db, d_pre, what):
+    """db [H] against the float64 per-channel sum of d_pre [..., H], relative to the sum of magnitudes"""
+    x = d_pre.double().reshape(-1, d_pre.shape[-1])
+    err = (db.double() - x.sum(0)).abs()
+    assert bool((err <= 2e-6 * x.abs().sum(0) + 1e-30).all()), f"{what}: db error {float(err.max()):.3e}"
+
+
 def test_bias_act_and_relu_backward_kernels(cuda_device):
-    torch.manual_seed(0)
-    x = torch.randn(3, 17, 19, 32, device=cuda_device)
-    b = torch.randn(32, device=cuda_device)
+    """`mpgcn_bias_act` and `mpgcn_relu_backward` at widths 1 .. 1024; offset 1 places the tensors one float past a 16-byte boundary,
+    which takes the scalar kernels"""
     eng = shard.CudaEngine()
-    want = torch.relu(x + b)
-    got = eng.bias_act(x.clone(), b, 1)
-    assert torch.equal(got, want)
-    assert torch.equal(eng.bias_act(x.clone(), None, 0), x)
-    d = torch.randn_like(x)
-    d_pre, db = eng.relu_backward(d, want, 1, True)
-    assert torch.equal(d_pre, d * (want > 0))
-    torch.testing.assert_close(db, (d * (want > 0)).reshape(-1, 32).sum(0), rtol=1e-4, atol=1e-4)
+    for H, offset in ((1, 0), (3, 0), (32, 0), (96, 0), (1024, 0), (32, 1)):
+        torch.manual_seed(H)
+        shape = (3, 17, 19, H)
+
+        def at(t):      # a copy of t starting `offset` floats into its allocation
+            v = torch.empty(t.numel() + offset, device=cuda_device)[offset:].view(t.shape)
+            return v.copy_(t)
+
+        x = torch.randn(shape, device=cuda_device)
+        b = torch.randn(H, device=cuda_device)
+        want = torch.relu(x + b)
+        assert torch.equal(_bits(eng.bias_act(at(x), b, 1)), _bits(want)), f"H={H} offset={offset}: bias + ReLU"
+        assert torch.equal(_bits(eng.bias_act(at(x), None, 0)), _bits(x)), f"H={H} offset={offset}: identity"
+        d = torch.randn_like(x)
+        d_pre, db = eng.relu_backward(at(d), at(want), 1, True)
+        assert torch.equal(_bits(d_pre), _bits(_masked(d, want))), f"H={H} offset={offset}: masked dOut"
+        _check_db(db, _masked(d, want), f"H={H} offset={offset}")
 
 
 @pytest.mark.parametrize("kind,peer", [("row", True), ("row", False), ("k", False)])
@@ -153,40 +176,47 @@ def test_sharded_model_nccl_world2(kind, peer, tmp_path):
 def test_peer_exchange_kernels_on_one_gpu(cuda_device):
     """`mpgcn_rows_reduce_bias_act`, `mpgcn_relu_backward_scatter(_f16)` and the prepared-fp16-dPre entry of `backward_part`, with the g
     "ranks'" buffers all on one GPU (the kernels only see pointers): reduce-scatter + bias + ReLU, mask + all-gather, and the fp16
-    flavour bit-identical to the fp32 route through the library's own cast."""
+    flavour bit-identical to the fp32 route through the library's own cast.  The exchange steps at layer widths 32, 96 (an LSTM
+    width) and 100 (not a multiple of 32); the fp16 backward_part at 32."""
     dev = cuda_device
-    torch.manual_seed(3)
-    B, N, H, g, K = 2, 136, 32, 4, 3
-    rows = N // g
+    B, N, g, K = 2, 136, 4, 3
+    rows, r = N // g, 2
     eng = shard.CudaEngine()
-    parts = [torch.randn(B, N, N, H, device=dev) for _ in range(g)]
-    bias = torch.randn(H, device=dev)
-    for r in range(g):
-        out = eng.rows_reduce_bias_act([p.data_ptr() for p in parts], B, N, r * rows, rows, H, bias, 1, dev)
-        want = torch.relu(torch.stack([p[:, r * rows:(r + 1) * rows] for p in parts]).sum(0) + bias)
-        torch.testing.assert_close(out, want, rtol=1e-6, atol=1e-6)
-    # scatter (fp32): every destination receives the masked rows, nothing else is touched
-    r = 2
-    d_out = torch.randn(B, rows, N, H, device=dev) * 1e-5
-    out_slab = torch.relu(torch.randn(B, rows, N, H, device=dev))
-    dsts = [torch.full((B, N, N, H), 7.0, device=dev) for _ in range(g)]
-    db = eng.relu_backward_scatter(d_out, out_slab, 1, [d.data_ptr() for d in dsts], N, r * rows, True)
-    want = d_out * (out_slab > 0)
-    for d in dsts:
-        assert torch.equal(d[:, r * rows:(r + 1) * rows], want)
-        assert float((d[:, :r * rows] - 7.0).abs().max()) == 0.0 and float((d[:, (r + 1) * rows:] - 7.0).abs().max()) == 0.0
-    torch.testing.assert_close(db, want.reshape(-1, H).sum(0), rtol=1e-4, atol=1e-9)
-    # scatter (fp16): S = 2^k with S * absmax in [16, 32)
-    amax = eng.absmax(d_out)
-    assert float(amax) == float(d_out.abs().max())
-    dsts16 = [torch.zeros(B, N, N, H, device=dev, dtype=torch.float16) for _ in range(g)]
-    db16, scale2 = eng.relu_backward_scatter_f16(d_out, out_slab, 1, [d.data_ptr() for d in dsts16], N, r * rows, True, amax)
-    S = float(scale2[0])
-    assert 16.0 <= S * float(amax) < 32.0 and abs(np.log2(S) - round(np.log2(S))) < 1e-9 and float(scale2[1]) == 1.0 / S
-    for d in dsts16:
-        assert torch.equal(d[:, r * rows:(r + 1) * rows], (want * S).to(torch.float16))
-    torch.testing.assert_close(db16, db, rtol=1e-5, atol=1e-9)
+    for H in (32, 96, 100):
+        torch.manual_seed(3)
+        parts = [torch.randn(B, N, N, H, device=dev) for _ in range(g)]
+        bias = torch.randn(H, device=dev)
+        for rr in range(g):
+            out = eng.rows_reduce_bias_act([p.data_ptr() for p in parts], B, N, rr * rows, rows, H, bias, 1, dev)
+            want = torch.relu(torch.stack([p[:, rr * rows:(rr + 1) * rows] for p in parts]).sum(0) + bias)
+            torch.testing.assert_close(out, want, rtol=1e-6, atol=1e-6, msg=lambda m: f"H={H} rows_reduce_bias_act: {m}")
+        del parts
+        # scatter (fp32): every destination receives the masked rows, nothing else is touched
+        d_out = torch.randn(B, rows, N, H, device=dev) * 1e-5
+        out_slab = torch.relu(torch.randn(B, rows, N, H, device=dev))
+        dsts = [torch.full((B, N, N, H), 7.0, device=dev) for _ in range(g)]
+        db = eng.relu_backward_scatter(d_out, out_slab, 1, [d.data_ptr() for d in dsts], N, r * rows, True)
+        want = _masked(d_out, out_slab)
+        for d in dsts:
+            assert torch.equal(_bits(d[:, r * rows:(r + 1) * rows]), _bits(want)), f"H={H}: scattered rows"
+            assert float((d[:, :r * rows] - 7.0).abs().max()) == 0.0 and float((d[:, (r + 1) * rows:] - 7.0).abs().max()) == 0.0, \
+                f"H={H}: rows outside the slab were written"
+        _check_db(db, want, f"H={H} scatter")
+        del dsts
+        # scatter (fp16): S = 2^k with S * absmax in [16, 32)
+        amax = eng.absmax(d_out)
+        assert float(amax) == float(d_out.abs().max())
+        dsts16 = [torch.zeros(B, N, N, H, device=dev, dtype=torch.float16) for _ in range(g)]
+        db16, scale2 = eng.relu_backward_scatter_f16(d_out, out_slab, 1, [d.data_ptr() for d in dsts16], N, r * rows, True, amax)
+        S = float(scale2[0])
+        assert 16.0 <= S * float(amax) < 32.0 and abs(np.log2(S) - round(np.log2(S))) < 1e-9 and float(scale2[1]) == 1.0 / S
+        for d in dsts16:
+            assert torch.equal(_bits(d[:, r * rows:(r + 1) * rows]), _bits((want * S).to(torch.float16))), f"H={H}: fp16 scattered rows"
+        _check_db(db16, want, f"H={H} scatter_f16")
+        torch.testing.assert_close(db16, db, rtol=1e-5, atol=1e-9)
     # backward_part fed the prepared fp16 dPre == backward_part casting the fp32 dPre itself (same S, same bits)
+    H = 32
+    out_slab = torch.relu(torch.randn(B, rows, N, H, device=dev))
     X = torch.tanh(torch.randn(B, rows, N, 32, device=dev))
     G = torch.randn(K, N, N, device=dev) / N ** 0.5
     W = torch.randn(K * K * 32, 32, device=dev) * 0.05
