@@ -1,4 +1,5 @@
-"""Worker of tests/test_shard_gloo.py: one rank of a world-2 gloo run of the sharded model (CPU stand-in engine)."""
+"""Worker of tests/test_shard_gloo.py: one rank of a world-2 gloo run of the sharded model (CPU stand-in engine).
+Arguments: kind, output path[, lstm_hidden_dim, gcn_hidden_dim] (both 8 by default)."""
 import os
 import sys
 
@@ -15,12 +16,12 @@ from mpgcn_b200 import dist as mdist, shard  # noqa: E402
 from shard_standin import TorchEngine  # noqa: E402
 
 
-def main(kind, out_path):
+def main(kind, out_path, lstm_hid=8, gcn_hid=8):
     rank, world = mdist.init_from_env("gloo")
     shard._ENGINE = TorchEngine()
-    N, K, T, B, hid = 8, 3, 3, 2, 8
+    N, K, T, B = 8, 3, 3, 2
     torch.manual_seed(0)
-    model = shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=3,
+    model = shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=lstm_hid, lstm_num_layers=1, gcn_hidden_dim=gcn_hid, gcn_num_layers=3,
                        num_nodes=N, user_bias=True, activation=nn.ReLU)
     with torch.no_grad():                       # non-zero biases so that the bias gradient path is exercised
         for p in model.parameters():
@@ -59,4 +60,4 @@ def main(kind, out_path):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1], sys.argv[2])
+    main(sys.argv[1], sys.argv[2], *(int(a) for a in sys.argv[3:5]))

@@ -11,6 +11,7 @@ Ko*cH chunks (DESIGN.md section 5).
     from the workspaces; the layer against the fixtures and the factored oracle at size; the whole model at hidden 64; a row
     shard.
 """
+import ctypes
 import math
 
 import numpy as np
@@ -130,61 +131,124 @@ def test_lstm_keeps_its_fp32_kernels_at_hidden_64():
 # ------------------------------------------------------------------------------------------------------------------------------
 # one layer through the C ABI at any width, the chunk layouts read back from the workspaces
 # ------------------------------------------------------------------------------------------------------------------------------
-def _offsets(parts):
-    """Byte offsets of consecutive 1024-byte aligned regions (bdgcn_tc.cu `take`) -> ({name: offset}, total)."""
-    off, res = 0, {}
-    for name, nbytes in parts:
-        off = (off + 1023) // 1024 * 1024
-        res[name] = off
-        off += nbytes
-    return res, (off + 1023) // 1024 * 1024
+class Layout(dict):
+    """name -> byte offset of consecutive regions, each starting at a multiple of `align` (bdgcn_tc.cu `take`: 1024; bdgcn_simt.cu
+    `Carver`: 256); .size[name] = its bytes, .total = the workspace size the library asks for (`slack` bytes added)."""
+
+    def __init__(self, parts, align=1024, slack=0):
+        super().__init__()
+        self.size, off = {}, 0
+        for name, nbytes in parts:
+            off = -(-off // align) * align
+            self[name], self.size[name] = off, nbytes
+            off += nbytes
+        self.total = -(-off // align) * align + slack
 
 
-def ws_layout(B, N, K, C, H, dyn, sms):
-    """The forward / backward workspace layouts of a whole layer (bdgcn_tc.cu fwd_layout / bwd_layout)."""
-    nz, Np = (B if dyn else 1), (N + 7) // 8 * 8
-    g16, rem = nz * K * N * Np * 2, nz * K * N * 4
-    fwd = _offsets([("x16", B * N * N * C * 2), ("gd16", g16), ("go16", g16), ("w16", 2 * K * K * C * H * 2), ("u16", B * K * N * N * H * 2),
-                    ("dd", rem), ("dgo", rem), ("dgo_masked", rem), ("z16", B * K * N * N * C * 2)])
-    rows, cols = K * C // 32, K * H // 32
-    total = B * -(-N * N // 64)
+def dw_slices(B, R, N, rows, cols, sms):
+    """Split-K slices of BWD_DW (bdgcn_tc.cu dw_slices): rows = Kd*cC, cols = Ko*cH chunks, 64-row k-blocks per sample slab"""
+    total = B * -(-R * N // 64)
     tiles = -(-rows // 4) * -(-cols // 8)
     per = max(1, -(-total // max(1, sms // tiles)))
-    slices = -(-total // per)
-    bwd = _offsets([("dp16", B * N * N * H * 2), ("gd16", g16), ("go16", g16), ("v16", B * K * N * N * H * 2), ("y16", B * K * N * N * C * 2),
-                    ("wq16", K * K * C * H * 2), ("partials", slices * -(-rows // 4) * 128 * K * H * 4), ("scale", 64)])
+    return -(-total // per)
+
+
+def part_ws_layout(B, N, C, H, dyn, R, row0, Ko, Kd, sms):
+    """The forward / backward workspace layouts of a layer part (bdgcn_tc.cu fwd_layout / bwd_layout): origin rows [row0, row0 + R)
+    (the layout does not depend on row0), Ko origin and Kd destination supports.  The whole layer is R = N, Ko = Kd = K."""
+    nz, Np, RN = (B if dyn else 1), (N + 7) // 8 * 8, R * N
+    g16, rem = (lambda K: nz * K * N * Np * 2), (lambda K: nz * K * N * 4)
+    fwd = Layout([("x16", B * RN * C * 2), ("gd16", g16(Kd)), ("go16", g16(Ko)), ("w16", 2 * Ko * Kd * C * H * 2), ("u16", B * Ko * RN * H * 2),
+                  ("dd", rem(Kd)), ("dgo", rem(Ko)), ("dgo_masked", rem(Ko)), ("z16", B * Kd * RN * C * 2)])
+    rows, cols = Kd * C // 32, Ko * H // 32
+    slices = dw_slices(B, R, N, rows, cols, sms)
+    bwd = Layout([("dp16", B * N * N * H * 2), ("gd16", g16(Kd)), ("go16", g16(Ko)), ("v16", B * Ko * RN * H * 2), ("y16", B * Kd * RN * C * 2),
+                  ("wq16", Ko * Kd * C * H * 2), ("partials", slices * -(-rows // 4) * 128 * Ko * H * 4), ("scale", 64)])
     return fwd, bwd
 
 
-def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn):
-    """fp16 forward + backward of one layer (ReLU) -> outputs and the intermediates in their logical layouts:
-    Z / Y [B][d][n][e][C], U / V [B][o][n][e][H], W16 [2][o][d][C][H], Wq16 [o][d][C][H]."""
+def ws_layout(B, N, K, C, H, dyn, sms):
+    """The forward / backward workspace layouts of a whole layer."""
+    return part_ws_layout(B, N, C, H, dyn, N, 0, K, K, sms)
+
+
+def simt_ws_layout(B, N, C, H, R, Ko, Kd):
+    """The fp32 family's workspaces (bdgcn_simt.cu `Carver`): forward U (Z lives in `saved`; its region serves only a call without
+    one); backward dPre (whole layer: a part reads the caller's), V, Y, Wq [d][o][h][l].  The size functions add 256 / 1024 bytes."""
+    RN = R * N
+    fwd = Layout([("u", B * Ko * RN * H * 4), ("z", B * Kd * RN * C * 4)], 256, 256)
+    bwd = Layout([("dpre", B * N * N * H * 4), ("v", B * Ko * RN * H * 4), ("y", B * Kd * RN * C * 4), ("wq", Ko * Kd * C * H * 4)], 256, 1024)
+    return fwd, bwd
+
+
+def _nan_alloc(nbytes, dev, what):
+    return _garbage(nbytes, dev)
+
+
+def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn, row0=None, prec=1, alloc=_nan_alloc, d_pre16=None):
+    """Forward + backward of one layer (ReLU) or, with row0 set, of one PART of a layer (mpgcn_bdgcn_forward_part / _backward_part):
+    X is then the slab [B,R,N,C] of origin rows [row0, row0 + R), Go / Gd hold the part's Ko / Kd supports, W its [Ko*Kd*C, H]
+    slice, `out` receives the raw partial pre-activation and d_out is dPre -- or d_pre16 = (fp16 dPre, [S, 1/S]) as
+    mpgcn_relu_backward_scatter_f16 leaves them, passed in the extras.  prec 1: the tensor-core family, 0: the fp32 one.
+    Every buffer the library writes comes from alloc(nbytes, device, what) (uint8, prefilled).
+    -> outputs and the intermediates in their logical layouts (n < R): Z / Y [B][d][n][e][C], U / V [B][o][n][e][H], dP [B][m][e][H];
+    tensor cores: W16 [2][o][d][C][H], Wq16 [o][d][C][H] and the fp16 operand copies; fp32: Wq [d][o][H][C] as stored."""
     lib = _lib.load()
     dev = X.device
-    B, N, _, C = X.shape
-    K, H = Go.shape[-3], W.shape[1]
-    cC, cH = C // 32, H // 32
+    B, R, N, C = X.shape
+    Ko, Kd, H = Go.shape[-3], Gd.shape[-3], W.shape[1]
+    part, backward = row0 is not None, d_out is not None or d_pre16 is not None
     nz, Np = (B if dyn else 1), (N + 7) // 8 * 8
     st = torch.cuda.current_stream().cuda_stream
-    (fo, ftot), (bo, btot) = ws_layout(B, N, K, C, H, dyn, torch.cuda.get_device_properties(dev).multi_processor_count)
-    assert ftot == lib.mpgcn_bdgcn_fwd_workspace_bytes(B, N, K, C, H, int(dyn), 1)
-    assert btot == lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, K, C, H, int(dyn), 1)
-    out = torch.full((B, N, N, H), math.nan, device=dev)
-    saved = _garbage(lib.mpgcn_bdgcn_saved_bytes(B, N, K, C, H, 1), dev)
-    ws = _garbage(ftot, dev)
-    _lib.check(lib.mpgcn_bdgcn_forward(X.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), bias.data_ptr(), 1, out.data_ptr(),
-                                       saved.data_ptr(), ws.data_ptr(), ws.numel(), B, N, K, C, H, 1, st), "forward")
-    r = dict(out=out)
-    if d_out is not None:
-        dX = torch.full((B, N, N, C), math.nan, device=dev)
+    if part:
+        pdesc = _lib.BdgcnPart(row0, R, Ko, Kd)
+        pp = ctypes.addressof(pdesc)
+        n_saved = lib.mpgcn_bdgcn_part_saved_bytes(B, N, C, H, prec, pp)
+        n_ws = lib.mpgcn_bdgcn_part_fwd_workspace_bytes(B, N, C, H, int(dyn), prec, pp)
+        n_wsb = lib.mpgcn_bdgcn_part_bwd_workspace_bytes(B, N, C, H, int(dyn), prec, pp)
+    else:
+        assert R == N and Ko == Kd
+        n_saved = lib.mpgcn_bdgcn_saved_bytes(B, N, Ko, C, H, prec)
+        n_ws = lib.mpgcn_bdgcn_fwd_workspace_bytes(B, N, Ko, C, H, int(dyn), prec)
+        n_wsb = lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, Ko, C, H, int(dyn), prec)
+    if prec == 1:
+        fo, bo = part_ws_layout(B, N, C, H, dyn, R, row0 or 0, Ko, Kd, torch.cuda.get_device_properties(dev).multi_processor_count)
+    else:
+        fo, bo = simt_ws_layout(B, N, C, H, R, Ko, Kd)
+    assert (fo.total, bo.total) == (n_ws, n_wsb), f"workspace layouts {(fo.total, bo.total)} != library sizes {(n_ws, n_wsb)}"
+    assert n_saved == B * Kd * R * N * C * (2 if prec == 1 else 4)
+    out_b = alloc(4 * B * N * N * H, dev, "out")
+    out = out_b.view(torch.float32).view(B, N, N, H)
+    saved = alloc(n_saved, dev, "saved")
+    ws = alloc(n_ws, dev, "forward workspace")
+    if part:
+        _lib.check(lib.mpgcn_bdgcn_forward_part(X.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), out.data_ptr(),
+                                                saved.data_ptr(), ws.data_ptr(), n_ws, B, N, C, H, prec, pp, None, st), "forward_part")
+    else:
+        _lib.check(lib.mpgcn_bdgcn_forward(X.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), bias.data_ptr(), 1, out.data_ptr(),
+                                           saved.data_ptr(), ws.data_ptr(), n_ws, B, N, Ko, C, H, prec, st), "forward")
+    r = dict(out=out, layouts=(fo, bo), bufs=dict(out=out_b, saved=saved, ws=ws))
+    if backward:
+        dX_b = alloc(4 * B * R * N * C, dev, "dX")
+        dX = dX_b.view(torch.float32).view(B, R, N, C)
         dW = torch.full_like(W, math.nan)
-        db = torch.full((H,), math.nan, device=dev)
-        dx_amax = torch.full((1,), math.nan, device=dev)
-        wsb = _garbage(btot, dev)
-        _lib.check(lib.mpgcn_bdgcn_backward_ex(d_out.data_ptr(), out.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), 1,
-                                               saved.data_ptr(), dX.data_ptr(), dW.data_ptr(), db.data_ptr(), wsb.data_ptr(), wsb.numel(),
-                                               B, N, K, C, H, 1, None, dx_amax.data_ptr(), st), "backward_ex")
-        r.update(dX=dX, dW=dW, db=db, dx_amax=dx_amax)
+        wsb = alloc(n_wsb, dev, "backward workspace")
+        if part:
+            ex = _lib.BdgcnExtras()
+            if d_pre16 is not None:
+                ex.d_pre_f16, ex.d_pre_scale2 = d_pre16[0].data_ptr(), d_pre16[1].data_ptr()
+            _lib.check(lib.mpgcn_bdgcn_backward_part(None if d_pre16 is not None else d_out.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn),
+                                                     W.data_ptr(), saved.data_ptr(), dX.data_ptr(), dW.data_ptr(), wsb.data_ptr(), n_wsb, B, N, C,
+                                                     H, prec, pp, ctypes.addressof(ex), st), "backward_part")
+        else:
+            db = torch.full((H,), math.nan, device=dev)
+            dx_amax = torch.full((1,), math.nan, device=dev)
+            _lib.check(lib.mpgcn_bdgcn_backward_ex(d_out.data_ptr(), out.data_ptr(), Go.data_ptr(), Gd.data_ptr(), int(dyn), W.data_ptr(), 1,
+                                                   saved.data_ptr(), dX.data_ptr(), dW.data_ptr(), db.data_ptr(), wsb.data_ptr(), n_wsb,
+                                                   B, N, Ko, C, H, prec, None, dx_amax.data_ptr(), st), "backward_ex")
+            r.update(db=db, dx_amax=dx_amax)
+        r.update(dX=dX, dW=dW)
+        r["bufs"].update(dX=dX_b, wsb=wsb)
     torch.cuda.synchronize()
 
     def h16(buf, o, *shape):
@@ -193,123 +257,177 @@ def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn):
     def f32(buf, o, *shape):
         return buf[o:o + 4 * math.prod(shape)].view(torch.float32).view(*shape)
 
-    in_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, K, N, N, C)        # [B][d][lc][n][e][32] -> [B][d][n][e][C]
-    w16 = h16(ws, fo["w16"], 2, cH, K, K, cC, 32, 32).permute(0, 2, 3, 4, 5, 1, 6).reshape(2, K, K, C, H)
-    wq16 = h16(wsb, bo["wq16"], K, cC, K, cH, 32, 32).permute(2, 0, 1, 5, 3, 4).reshape(K, K, C, H) if d_out is not None else None
-    r.update(x16=h16(ws, fo["x16"], B, N, N, C), gd16=h16(ws, fo["gd16"], nz, K, N, Np), w16=w16,
-             u16=h16(ws, fo["u16"], B, cH, K, N, N, 32).permute(0, 2, 3, 4, 1, 5).reshape(B, K, N, N, H),
-             dd=f32(ws, fo["dd"], nz, K, N), z16=in_planes(saved.view(torch.float16).view(B, K, cC, N, N, 32)))
-    r["go16"], r["dgo"] = (h16(ws, fo["go16"], nz, K, N, Np), f32(ws, fo["dgo"], nz, K, N)) if dyn else (r["gd16"], r["dd"])
-    if d_out is not None:
-        r.update(dp16=h16(wsb, bo["dp16"], B, N, N, H), bgd16=h16(wsb, bo["gd16"], nz, K, N, Np),
-                 v16=h16(wsb, bo["v16"], B, K, cH, N, N, 32).permute(0, 1, 3, 4, 2, 5).reshape(B, K, N, N, H),
-                 y16=in_planes(h16(wsb, bo["y16"], B, K, cC, N, N, 32)), wq16=wq16, scale=f32(wsb, bo["scale"], 2))
-        r["bgo16"] = h16(wsb, bo["go16"], nz, K, N, Np) if dyn else r["bgd16"]
+    if prec != 1:
+        r.update(z=saved.view(torch.float32).view(B, Kd, R, N, C), u=f32(ws, fo["u"], B, Ko, R, N, H))
+        if backward:
+            r.update(v=f32(wsb, bo["v"], B, Ko, R, N, H), y=f32(wsb, bo["y"], B, Kd, R, N, C), wq=f32(wsb, bo["wq"], Kd, Ko, H, C))
+            if not part:
+                r["dpre"] = f32(wsb, bo["dpre"], B, N, N, H)
+        return r
+    cC, cH = C // 32, H // 32
+    in_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, Kd, R, N, C)      # [B][d][lc][n][e][32] -> [B][d][n][e][C]
+    out_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, Ko, R, N, H)     # [B][o][hc][n][e][32] -> [B][o][n][e][H]
+    r.update(x16=h16(ws, fo["x16"], B, R, N, C), gd16=h16(ws, fo["gd16"], nz, Kd, N, Np), dd=f32(ws, fo["dd"], nz, Kd, N),
+             w16=h16(ws, fo["w16"], 2, cH, Ko, Kd, cC, 32, 32).permute(0, 2, 3, 4, 5, 1, 6).reshape(2, Ko, Kd, C, H),
+             u=h16(ws, fo["u16"], B, cH, Ko, R, N, 32).permute(0, 2, 3, 4, 1, 5).reshape(B, Ko, R, N, H),
+             z=in_planes(saved.view(torch.float16).view(B, Kd, cC, R, N, 32)))
+    # G_o gets its own fp16 copy (and remainders) unless it is the G_d buffer with as many planes: nothing writes go16 / dgo then
+    r["own_go"] = own_go = Go.data_ptr() != Gd.data_ptr() or Ko != Kd
+    r["go16"], r["dgo"] = (h16(ws, fo["go16"], nz, Ko, N, Np), f32(ws, fo["dgo"], nz, Ko, N)) if own_go else (r["gd16"], r["dd"])
+    if R < N:
+        r["dgo_masked"] = f32(ws, fo["dgo_masked"], nz, Ko, N)
+    if backward:
+        prepared = d_pre16 is not None
+        r.update(dp=d_pre16[0] if prepared else h16(wsb, bo["dp16"], B, N, N, H), scale=d_pre16[1] if prepared else f32(wsb, bo["scale"], 2),
+                 bgd16=h16(wsb, bo["gd16"], nz, Kd, N, Np), v=out_planes(h16(wsb, bo["v16"], B, Ko, cH, R, N, 32)),
+                 y=in_planes(h16(wsb, bo["y16"], B, Kd, cC, R, N, 32)),
+                 wq16=h16(wsb, bo["wq16"], Kd, cC, Ko, cH, 32, 32).permute(2, 0, 1, 5, 3, 4).reshape(Ko, Kd, C, H))
+        r["bgo16"] = h16(wsb, bo["go16"], nz, Ko, N, Np) if own_go else r["bgd16"]
     return r
 
 
-def check_stages_wide(r, X, Go, Gd, W, bias, d_out, dyn, kind):
-    """test_gpu_engine_stages.check_stages at any width: every stage of run_layer_wide's result against float64."""
-    B, N, _, C = X.shape
-    K, H = Go.shape[-3], W.shape[1]
+def _dims(X, Go, Gd, W, dyn):
+    B, R, N, C = X.shape
+    Ko, Kd, H = Go.shape[-3], Gd.shape[-3], W.shape[1]
     nz = B if dyn else 1
-    Gd4, Go4 = Gd.view(nz, K, N, N), Go.view(nz, K, N, N)
-    W4 = W.view(K, K, C, H)
+    wf = max(1, -(-(C + H) // 32))        # memory budget of the float64 recomputation, in 32-channel units
+    return B, R, N, C, H, Ko, Kd, nz, Go.reshape(nz, Ko, N, N), Gd.reshape(nz, Kd, N, N), W.view(Ko, Kd, C, H), wf
+
+
+def forward_stages(r, X, Go, Gd, W, bias, dyn, kind, row0=None, prec=1):
+    """The forward stages of run_layer_wide's result against float64 -> {stage: Bound or Slope}.  The fp32 family is the same algebra
+    with no operand conversions, no remainders, no `lo` half of W and fp32 intermediates."""
+    B, R, N, C, H, Ko, Kd, nz, Go4, Gd4, W4, wf = _dims(X, Go, Gd, W, dyn)
+    part, row0, fp16 = row0 is not None, row0 or 0, prec == 1
     zb = (lambda b: b) if dyn else (lambda b: 0)
-    wf = (C + H) // 32                                    # memory budget of the float64 recomputation, in 32-channel units
     res = {}
+    if fp16:
+        assert torch.equal(bits(r["x16"]), bits(f16_sat(X))), "x16"
+        for g16, G, what in ((r["gd16"], Gd4, "gd16"), (r["go16"], Go4, "go16")):
+            assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
+        hi, lo = hilo(W4)
+        assert torch.equal(bits(r["w16"][0]), bits(hi)) and torch.equal(bits(r["w16"][1]), bits(lo)), "w16 hi / lo in the mix's chunk order"
+        fired = 0.0
+        for name, G in (("dd", Gd4), ("dgo", Go4)):
+            P = G.shape[1]
+            want, near = diag_rule(G.reshape(nz * P, N, N).cpu().numpy())
+            got = r[name].reshape(nz * P, N).double().cpu().numpy()
+            assert not ((got != want) & ~near).any(), f"{name}: remainders differ from the tau = 1/16 rule"
+            fired = max(fired, np.count_nonzero(got) / (nz * P * N))
+        if kind == "diag":
+            assert fired >= 0.5, "the inputs were meant to make the remainder correction fire"
+        dgo = r["dgo"]
+        if "dgo_masked" in r:                 # a row slab: the origin remainders act on the slab's own rows m only
+            m = r["dgo_masked"]
+            assert torch.equal(bits(m[..., row0:row0 + R]), bits(dgo[..., row0:row0 + R])), "dgo_masked != dgo on the slab rows"
+            assert not bits(m[..., :row0]).any() and not bits(m[..., row0 + R:]).any(), "dgo_masked != 0 outside the slab rows"
+            dgo = m
+        x, gd, go, dd = r["x16"], r["gd16"][..., :N], r["go16"][..., :N], r["dd"]
+    else:
+        x, gd, go, hi, lo = X, Gd4, Go4, W4, torch.zeros_like(W4)
+        dd, dgo = torch.zeros(nz, Kd, N, device=X.device), torch.zeros(nz, Ko, N, device=X.device)
+    z, u, out = r["z"], r["u"], r["out"]
 
-    assert torch.equal(bits(r["x16"]), bits(f16_sat(X))), "x16"
-    for g16, G, what in ((r["gd16"], Gd4, "gd16"), (r["go16"], Go4, "go16")):
-        assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
-    hi, lo = hilo(W4)
-    assert torch.equal(bits(r["w16"][0]), bits(hi)) and torch.equal(bits(r["w16"][1]), bits(lo)), "w16 hi / lo in the mix's chunk order"
-    fired = 0
-    for name, G in (("dd", Gd4), ("dgo", Go4)):
-        want, near = diag_rule(G.reshape(nz * K, N, N).cpu().numpy())
-        got = r[name].reshape(nz * K, N).double().cpu().numpy()
-        assert not ((got != want) & ~near).any(), f"{name}: remainders differ from the tau = 1/16 rule"
-        fired = max(fired, int(np.count_nonzero(got)))
-    if kind == "diag":
-        assert fired >= 0.5 * nz * K * N, "the inputs were meant to make the remainder correction fire"
-
-    x16, gd16, go16 = r["x16"], r["gd16"][..., :N], r["go16"][..., :N]
-    dd, dgo, z16, u16, out = r["dd"], r["dgo"], r["z16"], r["u16"], r["out"]
-
-    bA, sA = Bound(N, True), Slope()
+    bA, sA = Bound(N, fp16), Slope()
     for b in range(B):
-        for d in range(K):
-            for ns in _chunks(N, N * 32 * wf):
-                base, corr, ab = fwd_a_ref(x16[b, ns], gd16[zb(b), d], dd[zb(b), d])
-                y = z16[b, d, ns]
+        for d in range(Kd):
+            for ns in _chunks(R, N * 32 * wf):
+                base, corr, ab = fwd_a_ref(x[b, ns], gd[zb(b), d], dd[zb(b), d])
+                y = z[b, d, ns]
                 bA.add(y, base + corr, ab)
                 sA.add(y.double() - base, corr)
-    res["FWD_A"], res["FWD_A remainder slope"] = bA, sA
+    res["FWD_A"] = bA
 
-    bM, sM = Bound(2 * K * C, True), Slope()
+    bM, sM = Bound((2 if fp16 else 1) * Kd * C, fp16), Slope()
     for b in range(B):
-        for ns in _chunks(N, K * N * 32 * 4 * wf):
-            base, lpart, ab = mix_ref(z16[b, :, ns], hi, lo)
-            y = u16[b, :, ns]
+        for ns in _chunks(R, (Ko + Kd) * N * 32 * 2 * wf):
+            base, lpart, ab = mix_ref(z[b, :, ns], hi, lo)
+            y = u[b, :, ns]
             bM.add(y, base + lpart, ab)
             sM.add(y.double() - base, lpart)
-    res["FWD_MIX"], res["FWD_MIX lo slope"] = bM, sM
+    res["FWD_MIX"] = bM
 
-    bB, sB = Bound(K * N + K + 1, False), Slope()
+    # FWD_B: a part's output is the raw partial sum over (o, n in the slab) for every m (no bias, no ReLU)
+    bB, sB = Bound(Ko * R + Ko + 1, False), Slope()
     for b in range(B):
-        for es in _chunks(N, K * N * 32 * 4 * wf):
-            base, corr, ab = fwd_b_ref(go16[zb(b)], u16[b, :, :, es], dgo[zb(b)], bias)
+        for es in _chunks(N, Ko * R * 32 * 4 * wf):
+            base, corr, ab = fwd_b_ref(go[zb(b), :, row0:row0 + R], u[b, :, :, es], dgo[zb(b)], None if part else bias, row0)
             y = out[b, :, es]
-            bB.add(y, torch.relu(base + corr), ab)
-            sB.add(y.double() - base, corr * (y > 0))
-    res["FWD_B"], res["FWD_B remainder slope"] = bB, sB
-    if d_out is None:
-        return res
+            bB.add(y, base + corr if part else torch.relu(base + corr), ab)
+            sB.add(y.double() - base, corr if part else corr * (y > 0))
+    res["FWD_B"] = bB
+    if fp16:
+        res.update({"FWD_A remainder slope": sA, "FWD_MIX lo slope": sM, "FWD_B remainder slope": sB})
+    return res
 
-    amax = float(d_out.abs().max())
-    S, invS = expected_scale(amax)
-    assert (float(r["scale"][0]), float(r["scale"][1])) == (S, invS), "gradient scale"
-    d_pre = torch.where(out > 0, d_out, torch.zeros_like(d_out))
-    assert torch.equal(bits(r["dp16"]), bits(f16_sat(d_pre * S))), "dp16 != fp16_sat(dOut * [out > 0] * S)"
-    res["db"] = Bound(B * N * N, False).add(r["db"], d_pre.double().sum(dim=(0, 1, 2)), d_pre.double().abs().sum(dim=(0, 1, 2)))
-    for g16, G, what in ((r["bgd16"], Gd4, "backward gd16"), (r["bgo16"], Go4, "backward go16")):
-        assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
-    assert torch.equal(bits(r["wq16"]), bits(f16_sat(W4))), "wq16 != fp16(W) in the backward mix's chunk order"
-    wq = r["wq16"].permute(1, 0, 3, 2)                  # [d][o][h][c]
-    dp16, v16, y16 = r["dp16"], r["v16"], r["y16"]
-    bgd16, bgo16 = r["bgd16"][..., :N], r["bgo16"][..., :N]
 
-    bV = Bound(N, True)
+def backward_stages(r, X, Go, Gd, W, d_out, dyn, row0=None, prec=1, amax=None):
+    """The backward stages of run_layer_wide's result against float64 -> {stage: Bound}.  d_out: dOut of a whole layer (ReLU), dPre
+    of a part; amax: the max|dPre| the gradient scale comes from (default max|d_out|; a prepared dPre takes a global one)."""
+    B, R, N, C, H, Ko, Kd, nz, Go4, Gd4, W4, wf = _dims(X, Go, Gd, W, dyn)
+    part, row0, fp16 = row0 is not None, row0 or 0, prec == 1
+    zb = (lambda b: b) if dyn else (lambda b: 0)
+    res = {}
+    d_pre = d_out if part else torch.where(r["out"] > 0, d_out, torch.zeros_like(d_out))
+    if fp16:
+        S, invS = expected_scale(float(d_out.abs().max()) if amax is None else amax)
+        assert (float(r["scale"][0]), float(r["scale"][1])) == (S, invS), "gradient scale"
+        assert torch.equal(bits(r["dp"]), bits(f16_sat(d_pre * S))), "dP16 != fp16_sat(S dPre)"
+        for g16, G, what in ((r["bgd16"], Gd4, "backward gd16"), (r["bgo16"], Go4, "backward go16")):
+            assert torch.equal(bits(g16[..., :N]), bits(f16_sat(G))) and not bits(g16[..., N:]).any(), what
+        assert torch.equal(bits(r["wq16"]), bits(f16_sat(W4))), "wq16 != fp16(W) in the backward mix's chunk order"
+        dp, bgd, bgo, wq = r["dp"], r["bgd16"][..., :N], r["bgo16"][..., :N], r["wq16"].permute(1, 0, 3, 2)      # wq: [d][o][h][c]
+    else:
+        S = invS = 1.0
+        if not part:
+            assert torch.equal(r["dpre"], d_pre), "dPre != dOut * [out > 0]"
+        assert torch.equal(bits(r["wq"]), bits(W4.permute(1, 0, 3, 2).contiguous())), "Wq != W as [d][o][h][c]"
+        dp, bgd, bgo, wq = d_pre, Gd4, Go4, r["wq"]
+    if not part:
+        res["db"] = Bound(B * N * N, False).add(r["db"], d_pre.double().sum(dim=(0, 1, 2)), d_pre.double().abs().sum(dim=(0, 1, 2)))
+    v, y = r["v"], r["y"]
+
+    bV = Bound(N, fp16)
     for b in range(B):
-        for o in range(K):
-            for es in _chunks(N, N * 32 * 2 * wf):
-                ref, ab = contract("nm,meh->neh", bgo16[zb(b), o], dp16[b, :, es])
-                bV.add(v16[b, o, :, es], ref, ab)
+        for o in range(Ko):
+            for es in _chunks(N, (N + R) * 32 * 2 * wf):
+                ref, ab = contract("nm,meh->neh", bgo[zb(b), o, row0:row0 + R], dp[b, :, es])
+                bV.add(v[b, o, :, es], ref, ab)
     res["BWD_V"] = bV
 
-    acc = torch.zeros(K, K, C, H, dtype=torch.float64, device=X.device)
+    acc = torch.zeros(Ko, Kd, C, H, dtype=torch.float64, device=X.device)
     aab = torch.zeros_like(acc)
     for b in range(B):
-        for ns in _chunks(N, 2 * K * N * 32 * wf):
-            ref, ab = contract("dnel,oneh->odlh", z16[b, :, ns], v16[b, :, ns])
+        for ns in _chunks(R, 2 * (Ko + Kd) * N * 32 * wf):
+            ref, ab = contract("dnel,oneh->odlh", r["z"][b, :, ns], v[b, :, ns])
             acc += ref
             aab += ab
-    res["BWD_DW"] = Bound(B * N * N, False).add(r["dW"].view(K, K, C, H), acc * invS, aab * invS)
+    res["BWD_DW"] = Bound(B * R * N, False).add(r["dW"].view(Ko, Kd, C, H), acc * invS, aab * invS)
 
-    bY = Bound(H * K, True)
+    bY = Bound(H * Ko, fp16)
     for b in range(B):
-        for ns in _chunks(N, 2 * K * N * 32 * wf):
-            ref, ab = contract("oneh,dohl->dnel", v16[b, :, ns], wq)
-            bY.add(y16[b, :, ns], ref, ab)
+        for ns in _chunks(R, 2 * (Ko + Kd) * N * 32 * wf):
+            ref, ab = contract("oneh,dohl->dnel", v[b, :, ns], wq)
+            bY.add(y[b, :, ns], ref, ab)
     res["BWD_MIX"] = bY
 
-    bX = Bound(K * N, False)
+    bX = Bound(Kd * N, False)
     for b in range(B):
-        for ns in _chunks(N, 2 * K * N * 32 * wf):
-            ref, ab = contract("dnel,dce->ncl", y16[b, :, ns], bgd16[zb(b)])
+        for ns in _chunks(R, 2 * Kd * N * 32 * wf):
+            ref, ab = contract("dnel,dce->ncl", y[b, :, ns], bgd[zb(b)])
             bX.add(r["dX"][b, ns], ref * invS, ab * invS)
     res["BWD_DX"] = bX
-    assert float(r["dx_amax"][0]) == float(r["dX"].abs().max()), "dX_absmax hint != max|dX| over every chunk"
+    if not part:      # the max|dX| hint: exact on the tensor cores, 0 ("unknown") from the fp32 kernels
+        assert float(r["dx_amax"][0]) == (float(r["dX"].abs().max()) if fp16 else 0.0), "dX_absmax hint"
+    return res
+
+
+def check_stages_wide(r, X, Go, Gd, W, bias, d_out, dyn, kind, row0=None, prec=1):
+    """test_gpu_engine_stages.check_stages at any width, for a whole layer or a part (row0 set), for either kernel family: every
+    stage of run_layer_wide's result against float64."""
+    res = forward_stages(r, X, Go, Gd, W, bias, dyn, kind, row0, prec)
+    if d_out is not None:
+        res.update(backward_stages(r, X, Go, Gd, W, d_out, dyn, row0, prec))
     return res
 
 

@@ -165,12 +165,19 @@ def mix_ref(z, hi, lo):
             torch.einsum("dnel,odlh->oneh", z.abs(), hi.double().abs() + lo.double().abs()))
 
 
-def fwd_b_ref(g, u, delta, bias):
-    """pre[m,e,h] = sum_{o,n} g[o,n,m] u[o,n,e,h] + bias[h] + sum_o delta[o,m] u[o,m,e,h]      u: all n, a range of e"""
-    g, u, delta, bias = g.double(), u.double(), delta.double(), bias.double()
-    base = torch.einsum("onm,oneh->meh", g, u) + bias
-    corr = torch.einsum("om,omeh->meh", delta, u)
-    return base, corr, torch.einsum("onm,oneh->meh", g.abs(), u.abs()) + corr.abs() + bias.abs()
+def fwd_b_ref(g, u, delta, bias, row0=0):
+    """pre[m,e,h] = sum_{o,n} g[o,n,m] u[o,n,e,h] + bias[h] + sum_o delta[o,m] u[o,m-row0,e,h]      u: every row n of the slab of
+    origin rows [row0, row0 + R) (the whole layer: R = N), a range of e; g: those rows of G_o; the remainder term only for m in
+    the slab; bias None: a raw partial"""
+    g, u, delta = g.double(), u.double(), delta.double()
+    R = u.shape[1]
+    base = torch.einsum("onm,oneh->meh", g, u)
+    corr = torch.zeros_like(base)
+    corr[row0:row0 + R] = torch.einsum("on,oneh->neh", delta[:, row0:row0 + R], u)
+    ab = torch.einsum("onm,oneh->meh", g.abs(), u.abs()) + corr.abs()
+    if bias is not None:
+        base, ab = base + bias.double(), ab + bias.double().abs()
+    return base, corr, ab
 
 
 def contract(eq, a, b):

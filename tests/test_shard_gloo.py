@@ -32,6 +32,17 @@ def test_shard_plan_partitions():
 def test_sharded_model_world2_matches_whole_model_oracle(kind, tmp_path):
     """row / k: world 2.  rowhyb: world 4 = 2 batch groups x 2 row ranks (the exchange stays inside a group; gradients are summed
     over all ranks and averaged over the groups)."""
+    _run_and_check(kind, tmp_path, 8, 8)
+
+
+@pytest.mark.parametrize("kind", ["row", "k"])
+def test_sharded_model_with_lstm_hidden_unlike_gcn_hidden_matches_whole_model_oracle(kind, tmp_path):
+    """lstm_hidden_dim 8, gcn_hidden_dim 12: the first BDGCN layer of each branch has C != H, so the K shard's weight slice
+    W.view(K, K, C, H)[:, d_lo:d_hi] and the row shard's exchanges of H-channel tensors fed by C-channel slabs are checked."""
+    _run_and_check(kind, tmp_path, 8, 12)
+
+
+def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
     nproc = 4 if kind == "rowhyb" else 2
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
@@ -40,16 +51,16 @@ def test_sharded_model_world2_matches_whole_model_oracle(kind, tmp_path):
     procs = []
     for r in range(nproc):
         env = dict(os.environ, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(r), WORLD_SIZE=str(nproc))
-        procs.append(subprocess.Popen([sys.executable, worker, kind, str(tmp_path / f"r{r}.pt")], env=env))
+        procs.append(subprocess.Popen([sys.executable, worker, kind, str(tmp_path / f"r{r}.pt"), str(lstm_hid), str(gcn_hid)], env=env))
     for p in procs:
         assert p.wait(timeout=300) == 0
     res = [torch.load(tmp_path / f"r{r}.pt") for r in range(nproc)]
     # the same model / inputs as the worker builds, evaluated whole by the oracle
     sys.path.insert(0, os.path.dirname(HERE))
     import MPGCN as shim
-    N, K, T, B, hid = 8, 3, 3, 2, 8
+    N, K, T, B = 8, 3, 3, 2
     torch.manual_seed(0)
-    model = shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=3,
+    model = shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=lstm_hid, lstm_num_layers=1, gcn_hidden_dim=gcn_hid, gcn_num_layers=3,
                        num_nodes=N, user_bias=True, activation=nn.ReLU)
     with torch.no_grad():
         for p in model.parameters():
