@@ -218,6 +218,32 @@ MPGCN_API int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_
                                    const void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes, int B, int T,
                                    long long NN, int C, int precision, const float* d_hT_absmax, void* stream);
 
+/* Stacked LSTM: nn.LSTM(input_size=1, hidden=C, num_layers=L, batch_first) over the B*NN OD cells with zero initial state,
+ * last hidden state of the top layer only (reference MPGCN.py:69,80-87,100-104 with lstm_num_layers = L).  Tensor cores
+ * (precision 1) at C = 32 and 96, L >= 2, 1 <= T <= 256; mpgcn_lstm_stack_supported answers it (L = 1: the single-layer
+ * query, whose entry points are mpgcn_lstm_last_*).  Per-layer parameters are HOST arrays of L device pointers in nn.LSTM's
+ * layout: w_ih[0] [4C,1], w_ih[l > 0] [4C,C], w_hh[l] [4C,C], b_ih[l], b_hh[l] [4C]; the gradients likewise.
+ * Forward: with saved != NULL (mpgcn_lstm_stack_saved_bytes, 256-byte aligned) the training state c_t, h_t of every layer
+ * and step; with saved == NULL an inference forward that keeps only the h sequence of the layer below in the workspace
+ * (mpgcn_lstm_stack_fwd_workspace_bytes; unused in training).  Backward from that saved state (there is no recomputing
+ * flavour): workspace from mpgcn_lstm_stack_bwd_workspace_bytes, d_x [B,T,NN] or NULL, d_hT_absmax as in
+ * mpgcn_lstm_last_backward_ex.  All buffers 256-byte aligned.  Backward workspace layout: [S, 1/S] (1024 B), the fp32 sequence
+ * d(h^{l-1}_t) handed from walk to walk (C floats per cell and step, DESIGN.md 6.4), then the fp16 gate-gradient records of one layer, reused
+ * by every layer; a workspace with L - 1 more record regions (each of the size the query counts) keeps every layer's records. */
+MPGCN_API int mpgcn_lstm_stack_supported(int T, int C, int L, int precision);
+MPGCN_API size_t mpgcn_lstm_stack_saved_bytes(int B, int T, long long NN, int C, int L, int precision);
+MPGCN_API size_t mpgcn_lstm_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision);
+MPGCN_API size_t mpgcn_lstm_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision);
+MPGCN_API int mpgcn_lstm_stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh,
+                                       const float* const* b_ih, const float* const* b_hh, float* hT, void* saved, size_t saved_bytes,
+                                       void* workspace, size_t workspace_bytes, int B, int T, long long NN, int C, int precision,
+                                       void* stream);
+MPGCN_API int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh,
+                                        const float* const* b_ih, const float* const* b_hh, const float* d_hT, float* const* d_w_ih,
+                                        float* const* d_w_hh, float* const* d_b_ih, float* const* d_b_hh, float* d_x, const void* saved,
+                                        size_t saved_bytes, void* workspace, size_t workspace_bytes, int B, int T, long long NN, int C,
+                                        int precision, const float* d_hT_absmax, void* stream);
+
 /* Dynamic origin / destination graphs from the OD history = DataInput.construct_dyn_G (reference Data_Container_OD.py:39-59).
  *   od_history [periods * P, N, N]  the first periods*P days of the (un-normalised) OD tensor, P = perceived period (7)
  *   o_graph, d_graph [P, N, N]      slot t: A_t = mean_k od_history[t + k P];

@@ -15,7 +15,7 @@ and the trainer runs unchanged on our kernels.  What is kept identical to the re
     (reference MPGCN.py:26-42, 95-96).
 
 What differs: the arithmetic.  No einsum / cat / cuDNN -- `BDGCN.forward` is one call of
-`ops.bdgcn` (factored 2K-contraction engine) and the per-cell LSTM is `ops.lstm_last`, which reads
+`ops.bdgcn` (factored 2K-contraction engine) and the per-cell LSTM is `ops.lstm_module_last`, which reads
 `x_seq` in place, assumes the zero initial state the reference always passes (MPGCN.py:80-87,98) and
 never materialises the `[B*N*N, T, C]` output sequence.
 """
@@ -105,17 +105,7 @@ class MPGCN(nn.Module):
         return [(weight.new_zeros(shape), weight.new_zeros(shape)) for _ in range(self.M)]
 
     def _temporal(self, lstm: nn.LSTM, x_seq: torch.Tensor) -> torch.Tensor:
-        B, T, N, _, I = x_seq.shape
-        # under "auto" the engine runs wherever one of its kernels applies; up to hidden 64 an explicit precision always goes to the
-        # engine, which refuses a shape it cannot run; above that the tensor-core kernel runs hidden 96 and 128
-        explicit = self.lstm_precision not in (None, "auto") and lstm.hidden_size <= 64
-        if I == 1 and lstm.num_layers == 1 and (explicit or ops.lstm_engine_supports(self.lstm_precision, T, lstm.hidden_size)):
-            return ops.lstm_last(x_seq, lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0, precision=self.lstm_precision)
-        # configurations without an engine kernel: input_dim > 1 or stacked layers (Model_Trainer.py:49-51 hard-codes input_dim=1,
-        # 1 layer), hidden sizes above 64 other than 96 / 128, sequences longer than 256 steps above hidden 64, sequences whose
-        # fp32 backward does not fit in shared memory (T > 15 at hidden 64, DESIGN.md 6.4), and fp32 above 64
-        lstm_in = x_seq.permute(0, 2, 3, 1, 4).reshape(B * N * N, T, I)
-        return lstm(lstm_in)[0][:, -1, :]
+        return ops.lstm_module_last(lstm, x_seq, self.lstm_precision)
 
     def forward(self, x_seq: torch.Tensor, G_list: list):
         """x_seq (B, T, N, N, 1); G_list: per branch a static (K,N,N) tensor or a dynamic tuple.  -> (B, 1, N, N, 1)"""

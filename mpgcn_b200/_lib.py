@@ -80,6 +80,17 @@ _SIGS = {
     "mpgcn_relu_backward": (ctypes.c_int, [_c_f, _c_f, ctypes.c_int, _c_f, _c_f, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
     "mpgcn_lstm_last_backward": (ctypes.c_int, [_c_f] * 12 + [ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int,
                                                 ctypes.c_int, ctypes.c_void_p]),
+    "mpgcn_lstm_stack_supported": (ctypes.c_int, [ctypes.c_int] * 4),
+    "mpgcn_lstm_stack_saved_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "mpgcn_lstm_stack_fwd_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int,
+                                                                ctypes.c_int]),
+    "mpgcn_lstm_stack_bwd_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int,
+                                                                ctypes.c_int]),
+    "mpgcn_lstm_stack_forward": (ctypes.c_int, [_c_f, ctypes.c_int] + [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f, _c_f, ctypes.c_size_t, _c_f,
+                                 ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "mpgcn_lstm_stack_backward": (ctypes.c_int, [_c_f, ctypes.c_int] + [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f] +
+                                  [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f, _c_f, ctypes.c_size_t, _c_f, ctypes.c_size_t, ctypes.c_int,
+                                  ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, _c_f, ctypes.c_void_p]),
 }
 ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)

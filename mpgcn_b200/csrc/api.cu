@@ -347,4 +347,56 @@ int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const 
   return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st);
 }
 
+int mpgcn_lstm_stack_supported(int T, int C, int L, int precision) {
+  if (L == 1) return mpgcn_lstm_precision_supported(T, C, precision);
+  return precision == PREC_FP16_TC && lstm_tc_stack_supported(T, C, L) ? 1 : 0;
+}
+
+size_t mpgcn_lstm_stack_saved_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_saved_bytes(B, T, NN, C, L) : 0;
+}
+size_t mpgcn_lstm_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_fwd_workspace_bytes(B, T, NN, C, L) : 0;
+}
+size_t mpgcn_lstm_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_bwd_workspace_bytes(B, T, NN, C, L) : 0;
+}
+
+static int check_stack(const char* what, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                       const float* const* b_hh, int B, int T, long long NN, int C, int precision) {
+  MPGCN_CHECK(L >= 2, "%s: L=%d (a single layer is mpgcn_lstm_last_*)", what, L);
+  MPGCN_CHECK(w_ih && w_hh && b_ih && b_hh, "%s: null pointer argument", what);
+  for (int l = 0; l < L; ++l) MPGCN_CHECK(w_ih[l] && w_hh[l] && b_ih[l] && b_hh[l], "%s: null pointer argument (layer %d)", what, l);
+  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "%s: empty input", what);
+  MPGCN_CHECK(mpgcn_lstm_stack_supported(T, C, L, precision), "%s: precision %d does not support T=%d, hidden=%d, L=%d", what, precision, T,
+              C, L);
+  return 0;
+}
+
+int mpgcn_lstm_stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                             const float* const* b_hh, float* hT, void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes,
+                             int B, int T, long long NN, int C, int precision, void* stream) {
+  if (int e = check_stack("mpgcn_lstm_stack_forward", L, w_ih, w_hh, b_ih, b_hh, B, T, NN, C, precision)) return e;
+  MPGCN_CHECK(x_seq && hT, "mpgcn_lstm_stack_forward: null pointer argument");
+  MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_stack_saved_bytes(B, T, NN, C, L),
+              "lstm stack forward: saved buffer too small (%zu < %zu)", saved_bytes, lstm_tc_stack_saved_bytes(B, T, NN, C, L));
+  return lstm_stack_forward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, workspace, workspace_bytes, B, T, NN, C,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                              const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
+                              float* const* d_b_hh, float* d_x, const void* saved, size_t saved_bytes, void* workspace,
+                              size_t workspace_bytes, int B, int T, long long NN, int C, int precision, const float* d_hT_absmax,
+                              void* stream) {
+  if (int e = check_stack("mpgcn_lstm_stack_backward", L, w_ih, w_hh, b_ih, b_hh, B, T, NN, C, precision)) return e;
+  MPGCN_CHECK(x_seq && d_hT && d_w_ih && d_w_hh && d_b_ih && d_b_hh && saved, "mpgcn_lstm_stack_backward: null pointer argument");
+  for (int l = 0; l < L; ++l)
+    MPGCN_CHECK(d_w_ih[l] && d_w_hh[l] && d_b_ih[l] && d_b_hh[l], "mpgcn_lstm_stack_backward: null pointer argument (layer %d)", l);
+  MPGCN_CHECK(saved_bytes >= lstm_tc_stack_saved_bytes(B, T, NN, C, L), "lstm stack backward: saved buffer too small (%zu < %zu)",
+              saved_bytes, lstm_tc_stack_saved_bytes(B, T, NN, C, L));
+  return lstm_stack_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, workspace, workspace_bytes,
+                                B, T, NN, C, d_hT_absmax, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -32,7 +32,7 @@
 namespace mpgcn {
 namespace lstm_tc {
 
-template <int CH>
+template <int CH, bool UP = false>
 struct Dims {
   // 16-cell groups per tile: 8 at H = 32 (8 warps; h stays in registers, so 2 CTAs fit an SM in the forward), 4 at H = 96 (12
   // warps, <= 168 registers per thread), 3 at H = 128 (12 warps; 16 warps would cap a thread at 128 registers, which the
@@ -41,7 +41,9 @@ struct Dims {
   static constexpr int CELLS = 16 * CG;
   static constexpr int H = 32 * CH;
   static constexpr int G4 = 4 * H;
-  static constexpr int KX = H + 16;            // operand row of a cell: h_{t-1} (H) | x columns (16, see load_wx)
+  // operand row of a cell: h_{t-1} (H) | x columns (16, see load_wx); UP, a stacked layer above the first:
+  // h_{t-1} (H) | h^{l-1}_t (H) | bias columns (16)
+  static constexpr int KX = (UP ? 2 * H : H) + 16;
   static constexpr int WX_LD = KX + 8;         // padded so that 8 consecutive rows fall in distinct 16-byte bank groups
   static constexpr int HX_LD = KX + 8;         // staged operand rows of the weight-gradient GEMM
   static constexpr int H_LD = H + 8;           // h exchange tile row stride
@@ -97,9 +99,11 @@ __device__ __forceinline__ float row_scale(int r) { return ((r & 127) >> 5) == 2
 // for i, f, o and -2 log2 e for g): with the operand row of a cell  hx_t = [ h_{t-1} (H) | x_hi  1  x_lo  x_hi  1  0 0 0 | 0 .. ]
 // the product hx_t . Wx[r] is s_j * (W_hh h_{t-1} + w_ih x_t + b)_j; x, w_ih and b are split into fp16 hi + lo parts, so the
 // affine part keeps ~22 bits.
-template <int CH>
+// UP (a stacked layer l > 0, w_ih [4H][H]): Wx[r] = s_j * [ W_hh[j,:] | W_ih[j,:] | b_hi  b_lo  0 .. ] against the operand row
+// [ h_{t-1} | h^{l-1}_t | 1  1  0 .. ]: W_ih is a single fp16 like W_hh, since its operand h^{l-1}_t is one too.
+template <int CH, bool UP = false>
 __device__ void load_wx(__half* sWx, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh) {
-  using D = Dims<CH>;
+  using D = Dims<CH, UP>;
   constexpr int NCH = D::KX / 8;
   for (int e = threadIdx.x; e < D::G4 * NCH; e += blockDim.x) {
     const int r = e / NCH, ch = e % NCH, j = gate_row<CH>(r);
@@ -108,6 +112,14 @@ __device__ void load_wx(__half* sWx, const float* w_ih, const float* w_hh, const
     if (ch < D::H / 8) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = sc * w_hh[(size_t)j * D::H + ch * 8 + i];
+    } else if constexpr (UP) {
+      if (ch < 2 * D::H / 8) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = sc * w_ih[(size_t)j * D::H + ch * 8 - D::H + i];
+      } else if (ch == 2 * D::H / 8) {
+        const float bb = sc * (b_ih[j] + b_hh[j]), b_hi = __half2float(__float2half_rn(bb));
+        v[0] = b_hi; v[1] = bb - b_hi;
+      }
     } else if (ch == D::H / 8) {
       const float wi = sc * w_ih[j], bb = sc * (b_ih[j] + b_hh[j]);
       const float wi_hi = __half2float(__float2half_rn(wi)), b_hi = __half2float(__float2half_rn(bb));
@@ -122,18 +134,21 @@ __device__ __forceinline__ uint32_t x_cols(float x, int q) {
   const float x_hi = x_split_hi(x);
   return q == 0 ? pack2(x_hi, 1.f) : q == 1 ? pack2(x_split_lo(x, x_hi), x_hi) : q == 2 ? pack2(1.f, 0.f) : 0u;
 }
+// UP: the bias columns 2 H + 2 q, 2 H + 1 + 2 q
+__device__ __forceinline__ uint32_t bias_cols(int q) { return q == 0 ? pack2(1.f, 1.f) : 0u; }
 
 // acc[nt] (nt = gate * 4 + jn) = hx_t . Wx^T for the warp's 16 cells and 128 gate columns.  a_h(kb, a) supplies the A fragment
-// of h-block kb < 2 CH; xw[h] are the x columns H .. H + 7 of row h, the only nonzero columns of the last k-block, which
-// therefore runs as m16n8k8 (columns H + 8 .. H + 15 would add exact zeros).  wx_addr: first of the warp's 128 Wx rows.
-template <int CH, class AH>
+// of h-block kb < 2 CH (UP: kb < 4 CH, h^{l-1}_t from kb = 2 CH); xw[h] are the x columns H .. H + 7 of row h (UP: the bias
+// columns 2 H .. 2 H + 7), the only nonzero columns of the last k-block, which therefore runs as m16n8k8 (its upper 8 columns
+// would add exact zeros).  wx_addr: first of the warp's 128 Wx rows.
+template <int CH, bool UP = false, class AH>
 __device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const uint32_t (&xw)[2], uint32_t wx_addr) {
-  using D = Dims<CH>;
+  using D = Dims<CH, UP>;
   const int lane = threadIdx.x & 31, mi = lane >> 3;
 #pragma unroll
   for (int nt = 0; nt < 16; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
 #pragma unroll
-  for (int kb = 0; kb < 2 * CH; ++kb) {
+  for (int kb = 0; kb < (D::KX - 16) / 16; ++kb) {
     uint32_t a[4];
     a_h(kb, a);
 #pragma unroll
@@ -147,7 +162,7 @@ __device__ __forceinline__ void gate_mma(float (&acc)[16][4], AH&& a_h, const ui
 #pragma unroll
   for (int pr = 0; pr < 8; ++pr) {   // x columns: the k-half H .. H + 7 of n8 tiles 2 pr, 2 pr + 1
     uint32_t b0, b1;
-    ldmatrix_x2(wx_addr + (uint32_t)(((16 * pr + 8 * (mi & 1) + (lane & 7)) * D::WX_LD + 32 * CH) * 2), b0, b1);
+    ldmatrix_x2(wx_addr + (uint32_t)(((16 * pr + 8 * (mi & 1) + (lane & 7)) * D::WX_LD + D::KX - 16) * 2), b0, b1);
     mma_1688(acc[2 * pr], xw[0], xw[1], b0);
     mma_1688(acc[2 * pr + 1], xw[0], xw[1], b1);
   }
@@ -226,6 +241,28 @@ __device__ __forceinline__ float cell_grad(const float (&acc)[16][4], int h, con
 template <int CH>
 __device__ __forceinline__ size_t save_off(long long tile, int T, int t, int warp, int kind, int lane) {
   return ((size_t)tile * T + t) * Dims<CH>::TILE_HALVES + (size_t)warp * 1024 + (size_t)kind * 512 + (size_t)lane * 16;
+}
+
+// A stacked layer reads the h_t of the layer below from a sequence whose warp blocks lie `ld` halves apart: the training state
+// (base saved + 512, ld 1024: the h half of save_off) or the h-only sequence an inference forward hands up (ld 512).  The tiles
+// of every layer of one width are the same, so a lane's fragment there is its own A fragment.
+template <int CH>
+__device__ __forceinline__ size_t h_off(long long tile, int T, int t, int warp, int lane, int ld) {
+  return (((size_t)tile * T + t) * Dims<CH>::NW + warp) * (size_t)ld + (size_t)lane * 16;
+}
+// A fragment of h k-block kb < 2 CH of a 16-cell group from its first warp's fragment hp: slice kb / 2 is the same lane's
+// fragment of warp kb / 2 of the group; k-block kb = 2 sl + kk takes its words (h, 2 kk) and (h, 2 kk + 1), i.e. the uint2
+// number 2 h + kk of the 16 halves
+__device__ __forceinline__ void a_from_seq(const __half* hp, int ld, int kb, uint32_t (&a)[4]) {
+  const uint2* p = reinterpret_cast<const uint2*>(hp + (kb >> 1) * ld);
+  const uint2 r0 = __ldg(p + (kb & 1)), r1 = __ldg(p + 2 + (kb & 1));
+  a[0] = r0.x; a[1] = r1.x; a[2] = r0.y; a[3] = r1.y;
+}
+// gradient sequence between the walks of a stack, fp32 in the walk's register fragment: per (tile, step, warp, lane) the 16
+// values dh[h][s] of the thread (scaled by S); the walk of layer l writes d(h^{l-1}_t) there, the walk of layer l - 1 adds it
+template <int CH>
+__device__ __forceinline__ size_t dseq_off(long long tile, int T, int t, int warp, int lane) {
+  return (((size_t)tile * T + t) * Dims<CH>::NW + warp) * 512 + (size_t)lane * 16;
 }
 
 // =======================================================================================
@@ -543,20 +580,25 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
 // ---------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------
-template <int CH>
-constexpr size_t kFwdWideSmem = (size_t)(Dims<CH>::G4 * Dims<CH>::WX_LD + 2 * Dims<CH>::CELLS * Dims<CH>::H_LD) * sizeof(__half);
+template <int CH, bool UP = false>
+constexpr size_t kFwdWideSmem = (size_t)(Dims<CH, UP>::G4 * Dims<CH, UP>::WX_LD + 2 * Dims<CH>::CELLS * Dims<CH>::H_LD) * sizeof(__half);
 
-template <int CH, bool SAVE>
+// Layers of a stack (lstm_stack_forward_tc) run this kernel at every width, hidden 32 as CH = 1:
+//   UP     the input is h^{l-1}_t of the layer below from h_in (see h_off) instead of x_seq: in training its saved state + 512
+//          (ld 1024), in inference its h-only sequence (ld 512);
+//   HSEQ   an inference layer below the top also writes h_t of every step to h_seq (h_off, ld 512) for the layer above.
+template <int CH, bool SAVE, bool UP = false, bool HSEQ = false>
 __global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::FWD_CTAS_PER_SM)
 lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                     const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
-                    long long cells, int T, long long NN) {
-  using D = Dims<CH>;
+                    long long cells, int T, long long NN, const __half* __restrict__ h_in, __half* __restrict__ h_seq) {
+  using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
+  constexpr int IN_LD = SAVE ? 1024 : 512;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [G4][WX_LD], slice order
   __half* sH = sWx + D::G4 * D::WX_LD;                     // 2 x [CELLS][H_LD]: h_t of the tile, double-buffered by step
-  load_wx<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
+  load_wx<CH, UP>(sWx, w_ih, w_hh, b_ih, b_hh);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   const int cg = warp / CH, js = warp % CH;
@@ -573,8 +615,8 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
     for (int h = 0; h < 2; ++h) {
       cell[h] = tile * CELLS + cg * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
-      xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
-      xv[h] = live[h] ? x_seq[xb[h]] : 0.f;
+      xb[h] = !UP && live[h] ? x_base(cell[h], T, NN) : 0;
+      xv[h] = !UP && live[h] ? x_seq[xb[h]] : 0.f;
     }
     float c[2][8];
 #pragma unroll
@@ -584,22 +626,30 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
     for (int t = 0; t < T; ++t) {
       uint32_t xw[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) xw[h] = x_cols(xv[h], q);
+      for (int h = 0; h < 2; ++h) xw[h] = UP ? bias_cols(q) : x_cols(xv[h], q);
       // h_{t-1} was written to buffer t & 1 before the previous step's barrier; zero before the first step
       const uint32_t hb = h_addr + (uint32_t)((t & 1) * CELLS * D::H_LD * 2);
+      const __half* hin = UP ? h_in + h_off<CH>(tile, T, t, cg * CH, lane, IN_LD) : nullptr;
       float acc[16][4];
-      gate_mma<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
-        if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; }
+      gate_mma<CH, UP>(acc, [&](int kb, uint32_t (&a)[4]) {
+        if (UP && kb >= 2 * CH) a_from_seq(hin, IN_LD, kb - 2 * CH, a);
+        else if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; }
         else ldmatrix_x4(hb + 32 * kb, a[0], a[1], a[2], a[3]);
       }, xw, wx_addr);
+      if (!UP) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) xv[h] = (live[h] && t + 1 < T) ? x_seq[xb[h] + (size_t)(t + 1) * NN] : 0.f;
+        for (int h = 0; h < 2; ++h) xv[h] = (live[h] && t + 1 < T) ? x_seq[xb[h] + (size_t)(t + 1) * NN] : 0.f;
+      }
       float hv[2][8];
       cell_update(acc, c, hv);
       if (SAVE) {
         uint4* dc = reinterpret_cast<uint4*>(saved + save_off<CH>(tile, T, t, warp, 0, lane));
         uint4* dh = reinterpret_cast<uint4*>(saved + save_off<CH>(tile, T, t, warp, 1, lane));
         dc[0] = pack8(c[0]); dc[1] = pack8(c[1]);
+        dh[0] = pack8(hv[0]); dh[1] = pack8(hv[1]);
+      }
+      if (HSEQ) {
+        uint4* dh = reinterpret_cast<uint4*>(h_seq + h_off<CH>(tile, T, t, warp, lane, 512));
         dh[0] = pack8(hv[0]); dh[1] = pack8(hv[1]);
       }
       if (t + 1 < T) {
@@ -631,25 +681,60 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
 // the thread-local cell gradient; da'_t = da_t / s_j of the warp's 128 gate columns into the group's rows of the shared da
 // tile and into the workspace record of (tile, t) (rows = cells, 4H columns in slice order); after the group barrier
 // dh_{t-1}[slice] = da'_t x (s W_hh) over all 4H gates, and dx = sum of the CH slice partials in a fixed order.
-template <int CH>
-constexpr size_t kWalkSmem = (size_t)(Dims<CH>::G4 * Dims<CH>::WX_LD + Dims<CH>::CELLS * Dims<CH>::DA_LD) * sizeof(__half) +
+// In a stack (hidden 32 as CH = 1):
+//   DHIN   a layer below the top: dh_t = the recurrent part + d(h_t) of the layer above, read from d_seq (dseq_off) at step t;
+//          d_hT is not read;
+//   UP     a layer above the first: the input columns are h^{l-1}_t from h_in (the lower layer's saved state + 512) and the
+//          walk also writes d(h^{l-1}_t) = da'_t x (s W_ih) to d_seq -- the dh_{t-1} product over the W_ih columns of Wx; no dx.
+//          A middle layer reads and writes d_seq in place: each thread reads its own 16 values of a step before it writes them.
+template <int CH, bool UP = false>
+constexpr size_t kWalkSmem = (size_t)(Dims<CH, UP>::G4 * Dims<CH, UP>::WX_LD + Dims<CH>::CELLS * Dims<CH>::DA_LD) * sizeof(__half) +
                              (size_t)(Dims<CH>::CELLS * CH + Dims<CH>::G4) * sizeof(float);
 
-template <int CH>
+// dh[slice js] of the warp's 16 cells = da'_t x (s W) with W the 4H x H block of Wx columns col0 .. col0 + H - 1 (W_hh at 0,
+// W_ih at H in a stacked layer): B from Wx rows (k = gate row r), columns col0 + 32 js ..
+template <int CH, bool UP>
+__device__ __forceinline__ void da_times_w(uint32_t da_addr, uint32_t wx_all, int col0, int lane, int mi, int js, float (&dh)[2][8]) {
+  using D = Dims<CH, UP>;
+  float adh[4][4];
+#pragma unroll
+  for (int nt = 0; nt < 4; ++nt) adh[nt][0] = adh[nt][1] = adh[nt][2] = adh[nt][3] = 0.f;
+#pragma unroll (UP ? 2 : 4)
+  for (int kb = 0; kb < D::G4 / 16; ++kb) {
+    uint32_t a[4];
+    ldmatrix_x4(da_addr + 32 * kb, a[0], a[1], a[2], a[3]);
+#pragma unroll
+    for (int pr = 0; pr < 2; ++pr) {
+      uint32_t b0, b1, b2, b3;
+      ldmatrix_x4_trans(wx_all + (uint32_t)(((16 * kb + 8 * (mi & 1) + (lane & 7)) * D::WX_LD + col0 + 32 * js + 16 * pr + 8 * (mi >> 1)) * 2),
+                        b0, b1, b2, b3);
+      mma_16816(adh[2 * pr], a, b0, b1);
+      mma_16816(adh[2 * pr + 1], a, b2, b3);
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int s = 0; s < 8; ++s) dh[h][s] = adh[s >> 1][2 * h + (s & 1)];
+}
+
+template <int CH, bool UP = false, bool DHIN = false>
 __global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::BWD_CTAS_PER_SM)
 lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                          float* __restrict__ d_x, const __half* __restrict__ saved, __half* __restrict__ da_rec,
-                         const float* __restrict__ scale2, long long cells, int T, long long NN) {
-  using D = Dims<CH>;
+                         const float* __restrict__ scale2, long long cells, int T, long long NN, const __half* __restrict__ h_in,
+                         float* __restrict__ d_seq) {
+  using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sWx = reinterpret_cast<__half*>(smem_raw);       // [G4][WX_LD], slice order
   __half* sDA = sWx + D::G4 * D::WX_LD;                    // [CELLS][DA_LD]: da'_t, columns in slice order
   float* sDX = reinterpret_cast<float*>(sDA + CELLS * D::DA_LD);   // [CELLS][CH]: dx partial of each slice
   float* s_wih = sDX + CELLS * CH;                         // [G4] by gate row j
-  load_wx<CH>(sWx, w_ih, w_hh, b_ih, b_hh);
-  for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
+  load_wx<CH, UP>(sWx, w_ih, w_hh, b_ih, b_hh);
+  if (!UP)
+    for (int j = threadIdx.x; j < D::G4; j += blockDim.x) s_wih[j] = w_ih[j];
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
@@ -671,24 +756,35 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
       xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
 #pragma unroll
       for (int s = 0; s < 8; ++s) {
-        dh[h][s] = live[h] ? d_hT[(size_t)cell[h] * D::H + 32 * js + 8 * (s >> 1) + 2 * q + (s & 1)] * S : 0.f;
+        // (a top layer reads S here rather than keep it in a register across tiles: it has none to spare)
+        dh[h][s] = !DHIN && live[h] ? d_hT[(size_t)cell[h] * D::H + 32 * js + 8 * (s >> 1) + 2 * q + (s & 1)] * (UP ? __ldg(scale2) : S) : 0.f;
         dc[h][s] = 0.f;
       }
     }
     // the dx writer of the group (lanes 0..15 of slice 0) owns row 16 cg + lane
     const long long dx_cell = tile * CELLS + cg * 16 + (lane & 15);
-    const bool dx_live = d_x != nullptr && js == 0 && lane < 16 && dx_cell < cells;
+    const bool dx_live = !UP && d_x != nullptr && js == 0 && lane < 16 && dx_cell < cells;
     const size_t dx_base = dx_live ? x_base(dx_cell, T, NN) : 0;
 
     for (int t = T - 1; t >= 0; --t) {
+      if (DHIN) {                     // d(h_t) from the layer above
+        const float4* p = reinterpret_cast<const float4*>(d_seq + dseq_off<CH>(tile, T, t, warp, lane));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float4 v = p[i];
+          dh[i >> 1][4 * (i & 1)] += v.x; dh[i >> 1][4 * (i & 1) + 1] += v.y;
+          dh[i >> 1][4 * (i & 1) + 2] += v.z; dh[i >> 1][4 * (i & 1) + 3] += v.w;
+        }
+      }
       uint32_t xw[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) xw[h] = x_cols(live[h] ? x_seq[xb[h] + (size_t)t * NN] : 0.f, q);
-      // h_{t-1} of slice kb / 2 is the same lane's saved fragment of warp (cg, kb / 2): k-block kb = 2 sl + kk takes its
-      // words (h, 2 kk) and (h, 2 kk + 1), i.e. the uint2 number 2 h + kk of the 16 halves
+      for (int h = 0; h < 2; ++h) xw[h] = UP ? bias_cols(q) : x_cols(live[h] ? x_seq[xb[h] + (size_t)t * NN] : 0.f, q);
+      // h_{t-1} of the group from the saved state (a_from_seq); UP: then h^{l-1}_t of the layer below
       const __half* hp = saved + (t > 0 ? save_off<CH>(tile, T, t - 1, cg * CH, 1, lane) : 0);
+      const __half* hin = UP ? h_in + h_off<CH>(tile, T, t, cg * CH, lane, 1024) : nullptr;
       float acc[16][4];
-      gate_mma<CH>(acc, [&](int kb, uint32_t (&a)[4]) {
+      gate_mma<CH, UP>(acc, [&](int kb, uint32_t (&a)[4]) {
+        if (UP && kb >= 2 * CH) { a_from_seq(hin, 1024, kb - 2 * CH, a); return; }
         if (t == 0) { a[0] = a[1] = a[2] = a[3] = 0u; return; }
         const uint2* p = reinterpret_cast<const uint2*>(hp + (kb >> 1) * 1024);
         const uint2 r0 = __ldg(p + (kb & 1)), r1 = __ldg(p + 2 + (kb & 1));
@@ -711,7 +807,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float d[4][8];
-        dx[h] = cell_grad<CH, true>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, js, q, d);
+        dx[h] = cell_grad<CH, !UP>(acc, h, vc[h], vcp[h], dh[h], dc[h], s_wih, js, q, d);
 #pragma unroll
         for (int jn = 0; jn < 4; ++jn)
 #pragma unroll
@@ -719,8 +815,10 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
             const float inv_s = gt == 2 ? -0.5f * kLn2 : -kLn2;     // 1 / s_j: -ln 2 for i, f, o and -ln 2 / 2 for g
             da[4 * gt + jn][h] = pack2(inv_s * d[gt][2 * jn], inv_s * d[gt][2 * jn + 1]);
           }
-        dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 1);
-        dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 2);
+        if (!UP) {
+          dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 1);
+          dx[h] += __shfl_xor_sync(0xffffffffu, dx[h], 2);
+        }
       }
       // every warp of the group has finished reading the previous step's da tile and dx partials
       named_bar_sync(1 + cg, 32 * CH);
@@ -729,7 +827,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
         const int row = cg * 16 + g + 8 * h;
 #pragma unroll
         for (int nt = 0; nt < 16; ++nt) *reinterpret_cast<uint32_t*>(sDA + row * D::DA_LD + 128 * js + 8 * nt + 2 * q) = da[nt][h];
-        if (q == 0) sDX[row * CH + js] = dx[h];
+        if (!UP && q == 0) sDX[row * CH + js] = dx[h];
       }
       named_bar_sync(1 + cg, 32 * CH);
       if (dx_live) {
@@ -747,11 +845,18 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
               *reinterpret_cast<const uint4*>(sDA + (cg * 16 + row) * D::DA_LD + 128 * js + 8 * ch);
         }
       }
+      if (UP) {                       // d(h^{l-1}_t) into d_seq, while dh (consumed by cell_grad) holds nothing
+        da_times_w<CH, UP>(da_addr, wx_all, D::H, lane, mi, js, dh);
+        float4* p = reinterpret_cast<float4*>(d_seq + dseq_off<CH>(tile, T, t, warp, lane));
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          p[i] = make_float4(dh[i >> 1][4 * (i & 1)], dh[i >> 1][4 * (i & 1) + 1], dh[i >> 1][4 * (i & 1) + 2], dh[i >> 1][4 * (i & 1) + 3]);
+      }
       if (t > 0) {                    // dh_{t-1}[slice js] = da'_t x (s W_hh): B from Wx rows (k = gate row r), columns 32 js ..
         float adh[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) adh[nt][0] = adh[nt][1] = adh[nt][2] = adh[nt][3] = 0.f;
-#pragma unroll 4
+#pragma unroll (UP ? 2 : 4)
         for (int kb = 0; kb < D::G4 / 16; ++kb) {
           uint32_t a[4];
           ldmatrix_x4(da_addr + 32 * kb, a[0], a[1], a[2], a[3]);
@@ -776,29 +881,46 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
 // ---------------------------------------------------------------------------------------
 // ... and the weight-gradient pass: dWext[r][k] = s_j * sum over (tile, t, cell) of da'[cell][r] hx_t[cell][k]
 // ---------------------------------------------------------------------------------------
-// CTA (js, split): the 128 gate rows of slice js, all H + 16 columns, over a contiguous range of (tile, t) records.  Per record
-// the da block and hx (h_{t-1} from the saved state, x columns) are staged in shared memory; warp w owns gate rows 16 w .. +15.
+// CTA (js, split): the 128 gate rows of slice js, all KX columns, over a contiguous range of (tile, t) records.  Per record
+// the da block and hx (h_{t-1} from the saved state, x columns; UP: h_{t-1}, h^{l-1}_t from h_in = the lower layer's saved
+// state + 512, bias columns) are staged in shared memory; warp w owns gate rows 16 w .. +15.
 constexpr int DW_THREADS = 256;
 constexpr int DW_DA_LD = 136;
+// the staged tiles; above the 48 KB of static shared memory (hidden 32 in a stack) they are dynamic
+template <int CH, bool UP = false>
+constexpr size_t kDwSmem = (size_t)Dims<CH>::CELLS * (DW_DA_LD + Dims<CH, UP>::HX_LD) * sizeof(__half);
 
-template <int CH>
+template <int CH, bool UP = false>
 __global__ void __launch_bounds__(DW_THREADS)
 lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ saved, const __half* __restrict__ da_rec,
                    float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, const float* __restrict__ scale2,
-                   long long cells, int T, long long NN) {
-  using D = Dims<CH>;
+                   long long cells, int T, long long NN, const __half* __restrict__ h_in) {
+  using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
   constexpr int HX_LD = D::HX_LD;
   constexpr int NX = D::KX / 8;                 // n8 tiles of columns
-  __shared__ __align__(16) __half sDA[CELLS * DW_DA_LD];
-  __shared__ __align__(16) __half sHX[CELLS * HX_LD];
+  __half* sDA;
+  __half* sHX;
+  if constexpr (kDwSmem<CH, UP> <= 48 * 1024) {
+    __shared__ __align__(16) __half s_da[CELLS * DW_DA_LD];
+    __shared__ __align__(16) __half s_hx[CELLS * HX_LD];
+    sDA = s_da;
+    sHX = s_hx;
+  } else {
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    sDA = reinterpret_cast<__half*>(smem_raw);
+    sHX = sDA + CELLS * DW_DA_LD;
+  }
   const int js = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
   const long long tiles = (cells + CELLS - 1) / CELLS, records = tiles * T;
   const long long per = (records + gridDim.y - 1) / gridDim.y;
   const long long r0 = blockIdx.y * per, r1 = r0 + per < records ? r0 + per : records;
-  for (int e = threadIdx.x; e < CELLS; e += blockDim.x)          // constant zero columns H + 8 .. H + 15
-    *reinterpret_cast<uint4*>(sHX + e * HX_LD + D::H + 8) = make_uint4(0u, 0u, 0u, 0u);
+  for (int e = threadIdx.x; e < CELLS; e += blockDim.x)          // constant zero columns KX - 8 .. KX - 1
+    *reinterpret_cast<uint4*>(sHX + e * HX_LD + D::KX - 8) = make_uint4(0u, 0u, 0u, 0u);
+  if (UP)
+    for (int e = threadIdx.x; e < CELLS * 4; e += blockDim.x)     // constant bias columns 2 H .. 2 H + 7
+      *reinterpret_cast<uint32_t*>(sHX + (e >> 2) * HX_LD + 2 * D::H + 2 * (e & 3)) = bias_cols(e & 3);
   const uint32_t da_addr = smem_u32(sDA), hx_addr = smem_u32(sHX);
   float dw[NX][4];
 #pragma unroll
@@ -821,11 +943,21 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
       uint32_t* d = reinterpret_cast<uint32_t*>(sHX + row * HX_LD + col);
       d[0] = v.x; d[4] = v.y; d[8] = v.z; d[12] = v.w;
     }
-    for (int e = threadIdx.x; e < CELLS * 4; e += blockDim.x) {       // x columns H .. H + 7
-      const int row = e >> 2, qq = e & 3;
-      const long long cell = tile * CELLS + row;
-      const float x = cell < cells ? x_seq[x_base(cell, T, NN) + (size_t)t * NN] : 0.f;
-      *reinterpret_cast<uint32_t*>(sHX + row * HX_LD + D::H + 2 * qq) = x_cols(x, qq);
+    if (UP) {
+      for (int e = threadIdx.x; e < D::NW * 64; e += blockDim.x) {  // h^{l-1}_t, the same way into columns H ..
+        const int w = e >> 6, l = (e >> 1) & 31, h = e & 1;
+        const int row = (w / CH) * 16 + (l >> 2) + 8 * h, col = D::H + 32 * (w % CH) + 2 * (l & 3);
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(h_in + h_off<CH>(tile, T, t, w, l, 1024)) + h);
+        uint32_t* d = reinterpret_cast<uint32_t*>(sHX + row * HX_LD + col);
+        d[0] = v.x; d[4] = v.y; d[8] = v.z; d[12] = v.w;
+      }
+    } else {
+      for (int e = threadIdx.x; e < CELLS * 4; e += blockDim.x) {     // x columns H .. H + 7
+        const int row = e >> 2, qq = e & 3;
+        const long long cell = tile * CELLS + row;
+        const float x = cell < cells ? x_seq[x_base(cell, T, NN) + (size_t)t * NN] : 0.f;
+        *reinterpret_cast<uint32_t*>(sHX + row * HX_LD + D::H + 2 * qq) = x_cols(x, qq);
+      }
     }
     __syncthreads();
 #pragma unroll
@@ -849,6 +981,10 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
       const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
       const float v = dw[nt][i] * row_scale(r) * invS;
       if (col < D::H) atomicAdd(&d_w_hh[(size_t)j * D::H + col], v);
+      else if (UP) {
+        if (col < 2 * D::H) atomicAdd(&d_w_ih[(size_t)j * D::H + col - D::H], v);
+        else if (col == 2 * D::H) atomicAdd(&d_b[j], v);     // (column 2 H + 1, against b_lo, is the same sum)
+      }
       else if (col == D::H || col == D::H + 2) atomicAdd(&d_w_ih[j], v);
       else if (col == D::H + 1) atomicAdd(&d_b[j], v);
     }
@@ -906,7 +1042,7 @@ static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* 
   if (int e = ensure_dyn_smem(kern, (int)smem, saved ? attr_t : attr_f)) return e;
   prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
   kern<<<lstm_grid<CH>(cells, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT,
-                                                                           static_cast<__half*>(saved), cells, T, NN);
+                                                                           static_cast<__half*>(saved), cells, T, NN, nullptr, nullptr);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -941,7 +1077,8 @@ static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float*
   // walk: the gate recompute and dh_{t-1} (2 x 8 H (H + 1) per cell and step, as the hidden-32 count splits it) ...
   prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
   lstm_tc::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid<CH>(cells, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, T, NN);
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, T, NN,
+      nullptr, nullptr);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   // ... and the weight gradient (8 H (H + 1) / 2 more: 12 H (H + 1) in all)
@@ -950,7 +1087,7 @@ static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float*
   if (splits > records) splits = records;
   prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
   lstm_tc::lstm_dw_tcw_kernel<CH><<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, 0, st>>>(
-      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2, cells, T, NN);
+      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2, cells, T, NN, nullptr);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -998,6 +1135,192 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2, cells, T, NN, st))
     return e;
   return lstm_copy_bias_grad(d_b_ih, d_b_hh, G4, st);
+}
+
+// ---------------------------------------------------------------------------------------
+// stacked LSTM (L >= 2 layers): every layer on the wide kernels, hidden 32 as CH = 1
+// ---------------------------------------------------------------------------------------
+// Hidden 32 and 96 only: an upper layer's gate weights, 4H x (2H + 24) halves, take 22 KB and 162 KB of shared memory; at 128
+// they would take 280 KB, more than a CTA has.
+bool lstm_tc_stack_supported(int T, int C, int L) { return L >= 2 && (C == 32 || C == 96) && T >= 1 && T <= 256; }
+
+// training state of the stack: one lstm_tc_saved_bytes block per layer (multiples of 256 bytes)
+size_t lstm_tc_stack_saved_bytes(int B, int T, long long NN, int C, int L) { return (size_t)L * lstm_tc_saved_bytes(B, T, NN, C); }
+
+// the h-only sequence (C halves per cell and step) an inference layer hands to the layer above
+static size_t lstm_tc_hseq_bytes(int B, int T, long long NN, int C) {
+  return align_up((size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(__half), 256);
+}
+
+// inference forward: the h sequences of two consecutive layers (one for L = 2)
+size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L) {
+  return (L >= 3 ? 2 : 1) * lstm_tc_hseq_bytes(B, T, NN, C);
+}
+
+// backward: the grad scale (1 KB), the fp32 gradient sequence d(h^{l-1}_t) between consecutive walks (lstm_tc::dseq_off) and
+// the da records of one layer (the layers run one after another).  A workspace with room for L da regions keeps every
+// layer's records (layer l in region l) instead of reusing one, so that they can be read back after the call.
+static size_t lstm_tc_stack_dseq_bytes(int B, int T, long long NN, int C) {
+  return align_up((size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(float), 256);
+}
+size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int /*L*/) {
+  return 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
+}
+
+template <int CH, bool SAVE, bool UP, bool HSEQ>
+static int stack_fwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
+                           void* saved, const void* h_in, void* h_seq, long long cells, int T, long long NN, cudaStream_t st) {
+  using D = Dims<CH>;
+  auto kern = lstm_tc::lstm_fwd_tcw_kernel<CH, SAVE, UP, HSEQ>;
+  constexpr size_t smem = lstm_tc::kFwdWideSmem<CH, UP>;
+  static DynSmemAttr attr = {};
+  if (int e = ensure_dyn_smem(kern, (int)smem, attr)) return e;
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * ((UP ? 2 : 1) * D::H + 1) * (double)cells * T, st);
+  kern<<<lstm_grid<CH>(cells, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
+                                                                           cells, T, NN, static_cast<const __half*>(h_in),
+                                                                           static_cast<__half*>(h_seq));
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int CH>
+static int stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                         const float* const* b_hh, float* hT, void* saved, void* ws, int B, int T, long long NN, cudaStream_t st) {
+  const int C = 32 * CH;
+  const long long cells = (long long)B * NN;
+  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C), hseq_bytes = lstm_tc_hseq_bytes(B, T, NN, C);
+  auto lsaved = [&](int l) { return static_cast<uint8_t*>(saved) + (size_t)l * layer_bytes; };
+  auto hbuf = [&](int l) { return static_cast<uint8_t*>(ws) + (size_t)(l & 1) * hseq_bytes; };   // inference: h of layer l
+  for (int l = 0; l < L; ++l) {
+    const bool top = l == L - 1;
+    float* out = top ? hT : nullptr;
+    int e;
+    if (saved) {       // training: every layer keeps c_t | h_t; the layer above reads the h half
+      if (l == 0) e = stack_fwd_layer<CH, true, false, false>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], out, lsaved(0), nullptr, nullptr,
+                                                           cells, T, NN, st);
+      else e = stack_fwd_layer<CH, true, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], out, lsaved(l), lsaved(l - 1) + 1024, nullptr, cells, T, NN, st);
+    } else if (l == 0) {
+      e = stack_fwd_layer<CH, false, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, nullptr, nullptr, hbuf(0), cells, T,
+                                                  NN, st);
+    } else if (!top) {
+      e = stack_fwd_layer<CH, false, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, nullptr, hbuf(l - 1), hbuf(l),
+                                                 cells, T, NN, st);
+    } else {
+      e = stack_fwd_layer<CH, false, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], hT, nullptr, hbuf(l - 1), nullptr, cells,
+                                                  T, NN, st);
+    }
+    if (e) return e;
+  }
+  return 0;
+}
+
+template <int CH, bool UP, bool DHIN>
+static int stack_bwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* d_hT,
+                           float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, const void* h_in, void* da_rec,
+                           float* d_seq, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+  using D = Dims<CH>;
+  constexpr int KH = UP ? 2 * D::H : D::H;     // the input and recurrent columns of the gate GEMM
+  auto walk = lstm_tc::lstm_bwd_walk_tcw_kernel<CH, UP, DHIN>;
+  constexpr size_t smem = lstm_tc::kWalkSmem<CH, UP>;
+  static DynSmemAttr attr_w = {};
+  if (int e = ensure_dyn_smem(walk, (int)smem, attr_w)) return e;
+  // the walk and the weight gradient, counted as the single layer's are, with the gate GEMM KH + 1 deep: 8 H (KH + 1) ...
+  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (KH + 1) * (double)cells * T, st);
+  walk<<<lstm_grid<CH>(cells, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x,
+                                                                           static_cast<const __half*>(saved), static_cast<__half*>(da_rec),
+                                                                           scale2, cells, T, NN, static_cast<const __half*>(h_in), d_seq);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  // ... and the weight gradient
+  auto dw = lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
+  constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
+  static DynSmemAttr attr_d = {};
+  if (dw_smem)
+    if (int e = ensure_dyn_smem(dw, (int)dw_smem, attr_d)) return e;
+  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
+  long long splits = 4LL * device_sm_count() / CH;
+  if (splits > records) splits = records;
+  prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (KH + 1) * (double)cells * T, st);      // ... and 4 H (KH + 1)
+  dw<<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, dw_smem, st>>>(x_seq, static_cast<const __half*>(saved),
+                                                                       static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2,
+                                                                       cells, T, NN, static_cast<const __half*>(h_in));
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int CH>
+static int stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                          const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b,
+                          float* d_x, const void* saved, uint8_t* da_rec, size_t da_stride, float* d_seq, const float* scale2, int B,
+                          int T, long long NN, cudaStream_t st) {
+  const long long cells = (long long)B * NN;
+  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, 32 * CH);
+  auto lsaved = [&](int l) { return static_cast<const uint8_t*>(saved) + (size_t)l * layer_bytes; };
+  for (int l = L - 1; l >= 0; --l) {    // top-down: the walk of layer l leaves d(h^{l-1}_t) in d_seq for layer l - 1
+    const bool top = l == L - 1;
+    uint8_t* rec = da_rec + (size_t)l * da_stride;
+    int e;
+    if (l == 0)
+      e = stack_bwd_layer<CH, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, d_w_ih[0], d_w_hh[0], d_b[0], d_x, lsaved(0),
+                                           nullptr, rec, d_seq, scale2, cells, T, NN, st);
+    else if (top)
+      e = stack_bwd_layer<CH, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], d_hT, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
+                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, scale2, cells, T, NN, st);
+    else
+      e = stack_bwd_layer<CH, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
+                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, scale2, cells, T, NN, st);
+    if (e) return e;
+  }
+  return 0;
+}
+
+int lstm_stack_forward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                          const float* const* b_hh, float* hT, void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN, int C,
+                          cudaStream_t st) {
+  MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
+  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack forward: saved buffer must be 256-byte aligned");
+  if (saved == nullptr) {
+    const size_t need = lstm_tc_stack_fwd_workspace_bytes(B, T, NN, C, L);
+    MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm stack forward: workspace too small (%zu < %zu)", ws_bytes, need);
+    MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack forward: workspace must be 256-byte aligned");
+  }
+  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, B, T, NN, st)
+                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, B, T, NN, st);
+}
+
+int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
+                           float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,
+                           int C, const float* d_hT_absmax, cudaStream_t st) {
+  MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
+  const size_t need = lstm_tc_stack_bwd_workspace_bytes(B, T, NN, C, L);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm stack backward: workspace too small (%zu < %zu)", ws_bytes, need);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack backward: saved buffer must be 256-byte aligned");
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack backward: workspace must be 256-byte aligned");
+  const long long cells = (long long)B * NN;
+  float* scale2 = static_cast<float*>(ws);
+  float* d_seq = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024);
+  uint8_t* da_rec = static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C);
+  const size_t da_region = align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
+  const size_t da_stride = ws_bytes >= need + (size_t)(L - 1) * da_region ? da_region : 0;     // every layer's records, or one region
+  // one gradient scale S for the whole stack, from max|d_hT|: every walk keeps dh, dc and d_seq in units of S
+  if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
+  const int G4 = 4 * C;
+  for (int l = 0; l < L; ++l) {
+    MPGCN_CUDA(cudaMemsetAsync(d_w_ih[l], 0, sizeof(float) * G4 * (l == 0 ? 1 : C), st));
+    MPGCN_CUDA(cudaMemsetAsync(d_w_hh[l], 0, sizeof(float) * G4 * C, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
+  }
+  const int e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
+                                            scale2, B, T, NN, st)
+                        : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
+                                            scale2, B, T, NN, st);
+  if (e) return e;
+  for (int l = 0; l < L; ++l)
+    if (int e2 = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e2;
+  return 0;
 }
 
 }  // namespace mpgcn

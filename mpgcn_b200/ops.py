@@ -2,6 +2,8 @@
 
     bdgcn(X, G, W, b, activation)  <->  reference BDGCN.forward           (MPGCN.py:24-50)
     lstm_last(x_seq, w_ih, w_hh, b_ih, b_hh)  <->  nn.LSTM(...)[:, -1, :]  (MPGCN.py:69,100-104)
+    lstm_stack(x_seq, params, precision)      <->  the same with num_layers = L >= 2
+    lstm_module_last(lstm, x_seq, precision)  <->  either of them, or the module itself where the engine has no kernel
 
 PyTorch supplies device memory, the current stream and the autograd tape; all arithmetic is in
 libmpgcn_b200.so.
@@ -69,7 +71,7 @@ def _scratch(nbytes: int, device) -> torch.Tensor:
 # accepts the hint only if the gradient it receives is that very memory, unmodified (gradient accumulation from a second
 # consumer arrives in a different buffer or with a bumped version).  Purely an optimisation: a missed hint costs one pass.
 _VIEW_NODES = ("ViewBackward", "UnsafeViewBackward", "ReshapeAliasBackward", "AliasBackward")
-_OUR_NODES = ("_BDGCNFnBackward", "_LSTMLastFnBackward")
+_OUR_NODES = ("_BDGCNFnBackward", "_LSTMLastFnBackward", "_LSTMStackFnBackward")
 
 
 def _producer_node(t):
@@ -304,6 +306,120 @@ def lstm_last(x_seq: torch.Tensor, w_ih, w_hh, b_ih, b_hh, precision=None) -> to
     """h_T of a 1-layer, input-size-1 LSTM run over every OD cell of x_seq [B,T,N,N,1] -> [B*N*N, C]."""
     _require_cuda(x_seq, "x_seq")
     return _LSTMLastFn.apply(x_seq, w_ih, w_hh, b_ih, b_hh, precision, torch.is_grad_enabled())
+
+
+def lstm_stack_supports(name, T, C, L) -> bool:
+    """Whether `lstm_stack` runs L >= 2 layers of hidden size C over T steps at precision `name`: the tensor-core kernels at
+    hidden 32 and 96 ("auto" or "fp16"); there are no fp32 stacked kernels."""
+    name = default_precision() if name is None else name
+    if name not in _PREC_NAMES:
+        raise ValueError(f"unknown precision {name!r}; expected one of {sorted(_PREC_NAMES)}")
+    code = _lib.PREC_FP16_TC if name == "auto" else _PREC_NAMES[name]
+    return bool(_lib.load().mpgcn_lstm_stack_supported(T, C, L, code))
+
+
+def lstm_runs_on_engine(lstm: torch.nn.LSTM, T: int, precision) -> bool:
+    """Whether `lstm_module_last` runs this nn.LSTM module over T steps on the engine rather than calling the module itself.
+    One layer: under "auto" wherever one of the engine's kernels applies; up to hidden 64 an explicit precision always goes
+    to the engine, which refuses a shape it cannot run; above that the tensor-core kernel runs hidden 96 and 128.  L >= 2
+    layers: the tensor-core kernels at hidden 32 and 96 (at 128 an upper layer's gate weights do not fit a CTA's shared
+    memory, DESIGN.md 6.4), with no dropout between the layers in training; anything else stays with the module, as do
+    modules the engine does not compute: without biases, bidirectional, projected, or not batch_first."""
+    if lstm.input_size != 1 or not lstm.bias or lstm.bidirectional or lstm.proj_size or not lstm.batch_first:
+        return False
+    C, L = lstm.hidden_size, lstm.num_layers
+    if L == 1:
+        explicit = precision not in (None, "auto") and C <= 64
+        return explicit or lstm_engine_supports(precision, T, C)
+    if lstm.dropout > 0 and lstm.training:
+        return False
+    return lstm_stack_supports(precision, T, C, L)
+
+
+def lstm_module_last(lstm: torch.nn.LSTM, x_seq: torch.Tensor, precision=None) -> torch.Tensor:
+    """h_T of the top layer of `lstm` (batch_first, zero initial state) over every OD cell of x_seq [B,T,N,N,I] -> [B*N*N, C]."""
+    B, T, N, N2, I = x_seq.shape
+    L = lstm.num_layers
+    if lstm_runs_on_engine(lstm, T, precision):
+        if L == 1:
+            return lstm_last(x_seq, lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0, precision=precision)
+        params = [getattr(lstm, f"{k}_l{l}") for l in range(L) for k in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]
+        return lstm_stack(x_seq, params)
+    # configurations without an engine kernel: input_dim > 1 (Model_Trainer.py:49-51 hard-codes input_dim=1), hidden sizes
+    # above 64 other than 96 / 128, sequences longer than 256 steps above hidden 64, sequences whose fp32 backward does not fit
+    # in shared memory (T > 15 at hidden 64, DESIGN.md 6.4), fp32 above 64, and stacks other than those above
+    lstm_in = x_seq.permute(0, 2, 3, 1, 4).reshape(B * N * N2, T, I)
+    return lstm(lstm_in)[0][:, -1, :]
+
+
+def _ptr_array(ts):
+    import ctypes
+    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+class _LSTMStackFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, grad_mode: bool, x_seq, *params):
+        lib = _lib.load()
+        B, T = x_seq.shape[0], x_seq.shape[1]
+        NN = x_seq[0, 0].numel()
+        L, C = len(params) // 4, params[1].shape[1]
+        prec = _lib.PREC_FP16_TC
+        xc = _f32c(x_seq)
+        ps = [_f32c(t) for t in params]
+        hT = torch.empty((B * NN, C), dtype=torch.float32, device=x_seq.device)
+        # training: every layer keeps c_t / h_t of every step; inference keeps only the h sequence of the layer below (workspace)
+        need = grad_mode and any(ctx.needs_input_grad[1:])
+        saved = torch.empty(lib.mpgcn_lstm_stack_saved_bytes(B, T, NN, C, L, prec), dtype=torch.uint8, device=x_seq.device) if need else None
+        STASH_BYTES["lstm"] += saved.numel() if saved is not None else 0
+        ws = None if need else _scratch(lib.mpgcn_lstm_stack_fwd_workspace_bytes(B, T, NN, C, L, prec), x_seq.device)
+        with torch.cuda.device(x_seq.device):
+            _lib.check(lib.mpgcn_lstm_stack_forward(_ptr(xc), L, *[_ptr_array(ps[k::4]) for k in range(4)], _ptr(hT), _ptr(saved),
+                                                    saved.numel() if saved is not None else 0, _ptr(ws), ws.numel() if ws is not None else 0,
+                                                    B, T, NN, C, prec, _stream()), "lstm_stack_forward")
+        ctx.dims = (B, T, NN, C, L, prec)
+        ctx.lstm_saved = saved
+        ctx.save_for_backward(xc, *ps)
+        return hT
+
+    @staticmethod
+    def backward(ctx, d_hT):
+        lib = _lib.load()
+        xc, *ps = ctx.saved_tensors
+        B, T, NN, C, L, prec = ctx.dims
+        if ctx.lstm_saved is None:
+            raise RuntimeError("mpgcn_b200.lstm_stack: backward called but forward ran without requires_grad inputs")
+        hint = _take_hint(ctx, d_hT) if (d_hT.dtype == torch.float32 and d_hT.is_contiguous()) else None
+        d_hT = _f32c(d_hT)
+        dev = xc.device
+        grads = [torch.empty_like(p) for p in ps]
+        d_x = torch.empty_like(xc) if ctx.needs_input_grad[1] else None
+        saved = ctx.lstm_saved
+        ws = _scratch(lib.mpgcn_lstm_stack_bwd_workspace_bytes(B, T, NN, C, L, prec), dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.mpgcn_lstm_stack_backward(_ptr(xc), L, *[_ptr_array(ps[k::4]) for k in range(4)], _ptr(d_hT),
+                                                     *[_ptr_array(grads[k::4]) for k in range(4)], _ptr(d_x), _ptr(saved), saved.numel(),
+                                                     _ptr(ws), ws.numel(), B, T, NN, C, prec, _ptr(hint), _stream()), "lstm_stack_backward")
+        ctx.lstm_saved = None
+        return (None, d_x, *grads)
+
+
+def lstm_stack(x_seq: torch.Tensor, params) -> torch.Tensor:
+    """h_T of the top layer of an L-layer, input-size-1 LSTM run over every OD cell of x_seq [B,T,N,N,1] -> [B*N*N, C];
+    params: [w_ih, w_hh, b_ih, b_hh] of layer 0, then of layer 1, ... (nn.LSTM's *_l0, *_l1, ...).  Tensor cores only."""
+    _require_cuda(x_seq, "x_seq")
+    if len(params) < 8 or len(params) % 4:
+        raise ValueError(f"lstm_stack: expected 4 parameters per layer and at least 2 layers, got {len(params)}")
+    if x_seq.dim() < 3 or (x_seq.dim() == 5 and x_seq.shape[-1] != 1):
+        raise ValueError(f"lstm_stack: x_seq must be [B,T,N,N,1] (input size 1), got {tuple(x_seq.shape)}")
+    C = params[1].shape[-1]
+    for i, p in enumerate(params):
+        l, k = divmod(i, 4)
+        want = ((4 * C, 1 if l == 0 else C), (4 * C, C), (4 * C,), (4 * C,))[k]
+        if tuple(p.shape) != want or not p.is_floating_point() or p.device != x_seq.device:
+            raise ValueError(f"lstm_stack: parameter {i} (layer {l}) must be a float tensor of shape {want} on {x_seq.device}, "
+                             f"got {tuple(p.shape)} {p.dtype} on {p.device}")
+    return _LSTMStackFn.apply(torch.is_grad_enabled(), x_seq, *params)
 
 
 class _HeadFn(torch.autograd.Function):

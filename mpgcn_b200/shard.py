@@ -175,7 +175,7 @@ class CudaEngine:
         return db, scale2
 
     def lstm_last(self, x_seq, lstm, precision):
-        return ops.lstm_last(x_seq, lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0, precision=precision)
+        return ops.lstm_module_last(lstm, x_seq, precision)
 
     def head(self, feats, w, b):
         return ops.fc_relu_mean(feats, w, b)

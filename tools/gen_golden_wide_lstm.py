@@ -74,10 +74,10 @@ def gen_lstm():
         print("wrote", name)
 
 
-def _gen_one_model(ref_mpgcn, ref_gcn, seed, N, K, gk, T, B, hid):
+def _gen_one_model(ref_mpgcn, ref_gcn, seed, N, K, gk, T, B, hid, lstm_num_layers=1):
     rng = np.random.default_rng(seed)
     torch.manual_seed(seed)
-    model = ref_mpgcn.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=3,
+    model = ref_mpgcn.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=lstm_num_layers, gcn_hidden_dim=hid, gcn_num_layers=3,
                             num_nodes=N, user_bias=True, activation=torch.nn.ReLU)
     params = wide_model_params(seed, {k: v.shape for k, v in model.state_dict().items()})
     model.load_state_dict({k: torch.from_numpy(v) for k, v in params.items()})
