@@ -113,6 +113,19 @@ MPGCN_API int mpgcn_bdgcn_backward_ex(const float* d_out, const float* out, cons
                             const void* saved, float* dX, float* dW, float* db, void* workspace, size_t workspace_bytes, int B, int N,
                             int K, int C, int H, int precision, const float* d_out_absmax, float* dX_absmax, void* stream);
 
+/* Gradient with respect to the supports (learnable G): mpgcn_bdgcn_backward_x plus
+ *     dG_o[n,m] = sum_{b,e,h} U_o[b,n,e,h] dPre[b,m,e,h]   (U_o = sum_d (G_d-transformed X)_d W[o,d], recomputed from `saved`)
+ *     dG_d[c,e] = sum_{b,n,l} X[b,n,c,l] Y_d[b,n,e,l]      (Y_d = sum_o (G_o dPre)_o W[o,d]^T)
+ * static supports (G_o == G_d == G [K,N,N]): dG_o receives dL/dG [K,N,N] = dG_o + dG_d summed over the batch; dG_d must be NULL.
+ * dynamic supports: dG_o [B,K,N,N] and dG_d [B,K,N,N], either of them NULL when not wanted.  X [B,N,N,C] is the forward's input;
+ * dX, dW and db are bitwise those of mpgcn_bdgcn_backward_x on the same arguments (the dG stages run after its stages).  Adds
+ * 2 K B N^3 (C + H) flops.  workspace: mpgcn_bdgcn_support_grad_workspace_bytes (at least the backward's). */
+MPGCN_API size_t mpgcn_bdgcn_support_grad_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision);
+MPGCN_API int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const float* G_o, const float* G_d, int dynamic, const float* W,
+                                  int act, const void* saved, float* dX, float* dW, float* db, void* workspace, size_t workspace_bytes,
+                                  int B, int N, int K, int C, int H, int precision, const mpgcn_bdgcn_extras* extras, const float* X,
+                                  float* dG_o, float* dG_d, void* stream);
+
 /* ---- PARTS of a layer: what one GPU evaluates when a layer is sharded (SURVEY.md section 8(e)) -----------------------------------
  * The reference has no multi-GPU code; these entry points are the engine's own addition behind the same BDGCN.forward math
  * (MPGCN.py:24-50).  A part is described by

@@ -40,6 +40,7 @@ class BDGCN(nn.Module):
         self.use_bias = use_bias
         self.activation = activation() if activation is not None else None     # a class, as in the reference (MPGCN.py:13)
         self.precision = None          # None -> ops.default_precision(); or "auto" / "fp16" / "fp32"
+        self.support_grad = False      # True: a G that requires grad gets dL/dG (opt-in: it doubles the layer's N^3 backward work)
         self.init_params()
 
     def init_params(self, b_init=0.0):
@@ -63,7 +64,8 @@ class BDGCN(nn.Module):
             raise NotImplementedError
         assert X.dim() == 4 and X.shape[1] == X.shape[2] == G[0].shape[-1] and X.shape[3] == self.input_dim
         fused_relu = isinstance(self.activation, nn.ReLU)
-        out = ops.bdgcn(X, G, self.W, self.b if self.use_bias else None, relu=fused_relu, precision=self.precision)
+        out = ops.bdgcn(X, G, self.W, self.b if self.use_bias else None, relu=fused_relu, precision=self.precision,
+                        support_grad=self.support_grad)
         if self.activation is not None and not fused_relu:  # any other activation: unfused epilogue
             out = self.activation(out)
         return out

@@ -91,6 +91,9 @@ _SIGS = {
     "mpgcn_lstm_stack_backward": (ctypes.c_int, [_c_f, ctypes.c_int] + [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f] +
                                   [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f, _c_f, ctypes.c_size_t, _c_f, ctypes.c_size_t, ctypes.c_int,
                                   ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, _c_f, ctypes.c_void_p]),
+    "mpgcn_bdgcn_support_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 7),
+    "mpgcn_bdgcn_backward_supports": (ctypes.c_int, [_c_f, _c_f, _c_f, _c_f, ctypes.c_int, _c_f, ctypes.c_int, _c_f, _c_f, _c_f, _c_f, _c_f,
+                                                     ctypes.c_size_t] + [ctypes.c_int] * 6 + [ctypes.c_void_p, _c_f, _c_f, _c_f, ctypes.c_void_p]),
 }
 ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)
@@ -145,7 +148,7 @@ def check(code: int, what: str) -> None:
 
 
 PROFILE_TAGS = ("FWD_A", "FWD_MIX", "FWD_B", "BWD_V", "BWD_DW", "BWD_MIX", "BWD_DX", "SIMT_GEMM", "ELEMENTWISE", "LSTM_FWD", "LSTM_BWD",
-                "LAYER_FWD", "LAYER_BWD", "HEAD", "EXCHANGE")
+                "LAYER_FWD", "LAYER_BWD", "HEAD", "EXCHANGE", "BWD_DG")
 REGION_TAGS = ("LAYER_FWD", "LAYER_BWD", "HEAD")      # whole C-ABI calls (their `launches` count calls, not kernels)
 
 

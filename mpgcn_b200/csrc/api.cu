@@ -132,6 +132,36 @@ int mpgcn_bdgcn_backward_x(const float* d_out, const float* out, const float* G_
   return bdgcn_backward_simt(s, d_out, out, G_o, G_d, W, saved, dX, dW, db, workspace, workspace_bytes, st);
 }
 
+size_t mpgcn_bdgcn_support_grad_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision) {
+  const BdgcnShape s = mk(B, N, K, C, H, dynamic, 0);
+  if (check_shape(s, precision)) return 0;
+  return precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s);
+}
+
+int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const float* G_o, const float* G_d, int dynamic, const float* W, int act,
+                                  const void* saved, float* dX, float* dW, float* db, void* workspace, size_t workspace_bytes, int B, int N,
+                                  int K, int C, int H, int precision, const mpgcn_bdgcn_extras* extras, const float* X, float* dG_o,
+                                  float* dG_d, void* stream) {
+  const BdgcnShape s = mk(B, N, K, C, H, dynamic ? 1 : 0, act);
+  if (int e = check_shape(s, precision)) return e;
+  const bool have_out16 = extras && extras->out_f16 && precision == PREC_FP16_TC;
+  MPGCN_CHECK(d_out && (out || have_out16) && X && G_o && G_d && W && saved && dW && workspace,
+              "mpgcn_bdgcn_backward_supports: null pointer argument");
+  MPGCN_CHECK(dynamic || (dG_o && !dG_d), "mpgcn_bdgcn_backward_supports: static supports take their gradient in dG_o; dG_d must be NULL");
+  MPGCN_CHECK(!extras || !extras->d_pre_f16, "mpgcn_bdgcn_backward_supports: a prepared fp16 dPre belongs to a layer part");
+  const size_t need = precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s);
+  MPGCN_CHECK(workspace_bytes >= need, "mpgcn_bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  // the supports' own gradient adds 2 K B N^3 (C + H) to the backward's flops
+  const double dg_flops = 2.0 * s.K * s.B * (double)s.N * s.N * s.N * (s.C + s.H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfRegion region(PROF_LAYER_BWD, layer_flops(s, true) + dg_flops, st);
+  if (precision == PREC_FP16_TC)
+    return bdgcn_backward_supports_tc(s, d_out, out, X, G_o, G_d, W, saved, dX, dW, db, dG_o, dG_d, workspace, workspace_bytes,
+                                      to_extras(extras), st);
+  if (extras && extras->dX_absmax) MPGCN_CUDA(cudaMemsetAsync(extras->dX_absmax, 0, sizeof(float), st));      // "unknown"
+  return bdgcn_backward_supports_simt(s, d_out, out, X, G_o, G_d, W, saved, dX, dW, db, dG_o, dG_d, workspace, workspace_bytes, st);
+}
+
 int mpgcn_bdgcn_backward_ex(const float* d_out, const float* out, const float* G_o, const float* G_d, int dynamic, const float* W, int act,
                             const void* saved, float* dX, float* dW, float* db, void* workspace, size_t workspace_bytes, int B, int N,
                             int K, int C, int H, int precision, const float* d_out_absmax, float* dX_absmax, void* stream) {

@@ -11,6 +11,8 @@
 //     dW[o,d,l,h]  = sum_{b,n,e} Z[b,d,n,e,l] V[b,o,n,e,h]
 //     Y[b,d,n,e,l] = sum_{o,h} V[b,o,n,e,h] W[o,d,l,h]
 //     dX[b,n,c,l]  = sum_{d,e} Y[b,d,n,e,l] G_d[c,e]
+//   support gradients (opt-in; U recomputed from the Z stash)
+//     dG_o[n,m] = sum_{b,e,h} U_o[b,n,e,h] dPre[b,m,e,h]     dG_d[c,e] = sum_{b,n,l} X[b,n,c,l] Y_d[b,n,e,l]
 #include "kernels.h"
 
 namespace mpgcn {
@@ -98,8 +100,13 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
   return 0;
 }
 
-int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st) {
+size_t simt_sgrad_ws_bytes(const BdgcnShape& s) {
+  return simt_bwd_ws_bytes(s) + 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256);
+}
+
+// form_y: form Y even without dX (the support gradient reads it)
+static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
+                              const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, bool form_y, cudaStream_t st) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   MPGCN_CHECK(Z != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
@@ -148,7 +155,7 @@ int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* ou
     p.ksplit = (int)ks; p.alpha = 1.f;
     if (int e = simt_sgemm(p, st)) return e;
   }
-  if (dX) {
+  if (dX || form_y) {
     if (int e = permute_w_bwd(W, Wq, (int)Ko, (int)Kd, (int)C, (int)H, st)) return e;
     {  // Y[b,d] (rows x l) = sum_o V[b,o] (rows x h) * Wq[d,o] (h x l)
       SgemmParams p{};
@@ -164,7 +171,7 @@ int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* ou
       p.ksplit = 1; p.alpha = 1.f;
       if (int e = simt_sgemm(p, st)) return e;
     }
-    {  // dX[b,n] (c x l) = sum_d G_d (c x e) * Y[b,d,n] (e x l)
+    if (dX) {  // dX[b,n] (c x l) = sum_d G_d (c x e) * Y[b,d,n] (e x l)
       SgemmParams p{};
       p.A = Gd; p.B = Y; p.D = dX;
       p.M = (int)N; p.N = (int)C; p.K = (int)N;
@@ -177,6 +184,88 @@ int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* ou
       p.d_sz[0] = RN * C; p.d_sz[1] = N * C;
       p.ksplit = 1; p.alpha = 1.f;
       if (int e = simt_sgemm(p, st)) return e;
+    }
+  }
+  return 0;
+}
+
+}  // namespace mpgcn
+
+namespace mpgcn {
+
+int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
+                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st) {
+  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, false, st);
+}
+
+int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
+                                 const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
+                                 size_t ws_bytes, cudaStream_t st) {
+  MPGCN_CHECK(s.whole(), "support gradients: whole layers only");
+  MPGCN_CHECK(ws_bytes >= simt_sgrad_ws_bytes(s), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes,
+              simt_sgrad_ws_bytes(s));
+  const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
+  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, want_d, st)) return e;
+  const long long N = s.N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
+  const float* Z = static_cast<const float*>(saved);
+  Carver cv(ws, ws_bytes);                          // the backward's regions, then U
+  const float* dPre = cv.take<float>((size_t)s.B * NN * H);
+  cv.take<float>((size_t)s.B * Ko * NN * H);
+  const float* Y = cv.take<float>((size_t)s.B * Kd * NN * C);
+  cv.take<float>((size_t)Ko * Kd * C * H);
+  float* U = cv.take<float>((size_t)s.B * Ko * NN * H);
+  MPGCN_CHECK(cv.ok(), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, cv.off);
+  if (dGo) {
+    {  // U[b,o] (rows x h) = sum_d Z[b,d] (rows x l) * W[o,d] (l x h), as the forward
+      SgemmParams p{};
+      p.A = Z; p.B = W; p.D = U;
+      p.M = (int)NN; p.N = (int)H; p.K = (int)C;
+      p.a_si = C; p.a_sk = 1; p.b_sk = H; p.b_sj = 1; p.d_si = H;
+      p.nseg = (int)Kd; p.a_sseg = NN * C; p.b_sseg = C * H;
+      p.Z0 = s.B; p.Z1 = (int)Ko; p.Z2 = 1;
+      p.a_sz[0] = Kd * NN * C;
+      p.b_sz[1] = Kd * C * H;
+      p.d_sz[0] = Ko * NN * H; p.d_sz[1] = NN * H;
+      p.ksplit = 1; p.alpha = 1.f;
+      if (int e = simt_sgemm(p, st)) return e;
+    }
+    {  // dG_o (n x m) = sum_b U[b,o] (n x (e,h)) * dPre[b]^T ((e,h) x m): one k-segment per sample when the supports are static
+      SgemmParams p{};
+      p.A = U; p.B = dPre; p.D = dGo;
+      p.M = (int)N; p.N = (int)N; p.K = (int)(N * H);
+      p.a_si = N * H; p.a_sk = 1; p.b_sk = 1; p.b_sj = N * H; p.d_si = N;
+      if (s.dynamic) {
+        p.nseg = 1; p.Z0 = s.B; p.Z1 = (int)Ko; p.Z2 = 1;
+        p.a_sz[0] = Ko * NN * H; p.a_sz[1] = NN * H; p.b_sz[0] = NN * H; p.d_sz[0] = Ko * NN; p.d_sz[1] = NN;
+      } else {
+        p.nseg = s.B; p.a_sseg = Ko * NN * H; p.b_sseg = NN * H; p.Z0 = (int)Ko; p.Z1 = 1; p.Z2 = 1;
+        p.a_sz[0] = NN * H; p.d_sz[0] = NN;
+      }
+      p.ksplit = 1; p.alpha = 1.f;
+      if (int e = simt_sgemm(p, st)) return e;
+    }
+  }
+  if (want_d) {
+    // dG_d (c x e) = sum_n X[b,n] (c x l) * Y[b,d,n]^T (l x e): one k-segment per origin row n; static supports add every sample
+    // (one launch each) into the dG_o result, the stack's one gradient
+    SgemmParams p{};
+    p.M = (int)N; p.N = (int)N; p.K = (int)C;
+    p.a_si = C; p.a_sk = 1; p.b_sk = 1; p.b_sj = C; p.d_si = N;
+    p.nseg = (int)N; p.a_sseg = N * C; p.b_sseg = N * C;
+    p.ksplit = 1; p.alpha = 1.f;
+    if (s.dynamic) {
+      p.A = X; p.B = Y; p.D = dGd;
+      p.Z0 = s.B; p.Z1 = (int)Kd; p.Z2 = 1;
+      p.a_sz[0] = NN * C; p.b_sz[0] = Kd * NN * C; p.b_sz[1] = NN * C; p.d_sz[0] = Kd * NN; p.d_sz[1] = NN;
+      if (int e = simt_sgemm(p, st)) return e;
+    } else {
+      p.Z0 = (int)Kd; p.Z1 = 1; p.Z2 = 1;
+      p.b_sz[0] = NN * C; p.d_sz[0] = NN;
+      p.D = dGo; p.Cin = dGo; p.beta = 1.f; p.c_sz[0] = NN;
+      for (int b = 0; b < s.B; ++b) {
+        p.A = X + (size_t)b * NN * C; p.B = Y + (size_t)b * Kd * NN * C;
+          if (int e = simt_sgemm(p, st)) return e;
+      }
     }
   }
   return 0;

@@ -18,6 +18,10 @@
 //     BWD_DW  dW = Z^T V            A_MN64  (Z, Kd cC chunks)  B = V16 (Ko cH chunks)   split-K
 //     BWD_MIX Y = sum_o V_o W[o,d]^T  A_K64 (V plane)        B = Wq16                              Ko cH -> Kd cC planes
 //     BWD_DX  dX = sum_d Y_d x2 G_d^T A_K128 (G_d [c][e])    B = Y16 chunk lc (l, e, n, (b,d))     one launch per lc
+//   support gradients (opt-in, after the stages above; X16 [B][n][c][C] cast again, U16 recomputed from the Z stash by FWD_MIX)
+//     BWD_DGO dG_o[n][m] = sum_{b,e,h} U_o[b,n,e,h] dPre[b,m,e,h]   A_K64 (U16 plane, k = (e, 32))   B K-major = dP16 [m][(e, 32 hc)]
+//     BWD_DGD dG_d[c][e] = sum_{b,n,l} X[b,n,c,l] Y_d[b,n,e,l]     A_K64 (X16 [c][(lc, 32)])        B K-major = Y16 [e][32] per (b,d,lc,n)
+//             one split-K launch per output plane into fp32 partials [slice][N][32 ceil(N/32)], each reduced (x 1/S) into dG
 // The N^3 contractions act on each channel on its own, so a chunk is a 32-channel layer to them; the chunk planes are laid out
 // so that the per-chunk launch addresses them through a base offset and strides (plane index (b*K + d)*cC + lc of Z16 / Y16
 // and (b*Ko + o)*cH + hc of V16 are affine in the launch's z = b*K + d; U16 keeps FWD_B's flat (o, n) contraction per chunk).
@@ -171,6 +175,27 @@ static BwdLayout bwd_layout(const BdgcnShape& s) {
   return L;
 }
 size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s).total; }
+
+// support-gradient workspace: the backward's, then X16, U16, the forward's fp16 W split and the dG partials
+struct SgradLayout { size_t x16, u16, w16, partials, total; };
+static int dg_chunks(const BdgcnShape& s) { return ceil_div(s.N, 32); }                 // 32-column chunks of a dG row
+static int dg_r(const BdgcnShape& s) { return dg_chunks(s) < 8 ? dg_chunks(s) : 8; }   // chunks per tile
+static int dg_max_slices(const BdgcnShape& s) {
+  const int tiles = ceil_div(s.N, 128) * ceil_div(dg_chunks(s), dg_r(s));
+  const int want = device_sm_count() / tiles;
+  return want < 1 ? 1 : want;
+}
+static SgradLayout sgrad_layout(const BdgcnShape& s) {
+  SgradLayout L;
+  size_t off = bwd_layout(s).total;
+  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2);
+  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
+  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2);
+  L.partials = take(off, (size_t)dg_max_slices(s) * s.N * 32 * dg_chunks(s) * 4);
+  L.total = align_up(off, 1024);
+  return L;
+}
+size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return sgrad_layout(s).total; }
 
 // which: 0 x16, 1 gd16, 2 go16, 3 w16, 4 u16 (forward); 10 dp16, 11 gd16, 12 go16, 13 v16, 14 y16, 15 wq16, 16 partials,
 // 17 number of dW slices (not an offset)
@@ -486,9 +511,10 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
   return 0;
 }
 
-int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                      const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
-                      cudaStream_t st) {
+// form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it)
+static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
+                            const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
+                            bool form_y, cudaStream_t st) {
   MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
               s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
@@ -537,11 +563,137 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
   int slices = 0, mt = 0;
   if (int e = run_bwd_dw(s, z16, v16, partials, &slices, &mt, st)) return e;
   if (int e = reduce_dw_partials(partials, dW, slices, mt, s.Ko, s.Kd, s.C, s.H, scale2 + 1, st)) return e;
-  if (dX) {
-    if (ex.dx_absmax) MPGCN_CUDA(cudaMemsetAsync(ex.dx_absmax, 0, sizeof(float), st));
+  if (dX || form_y) {
+    if (dX && ex.dx_absmax) MPGCN_CUDA(cudaMemsetAsync(ex.dx_absmax, 0, sizeof(float), st));
     if (int e = permute_w_mix(W, wq16, nullptr, s.Ko, s.Kd, s.C, s.H, st)) return e;
     if (int e = run_mix(s, v16, wq16, 1, y16, PROF_BWD_MIX, s.Ko * (s.H / 32), s.Kd * (s.C / 32), st)) return e;
-    if (int e = run_bwd_dx(s, gd.g16, y16, dX, scale2 + 1, ex.dx_absmax, st)) return e;
+    if (dX) { if (int e = run_bwd_dx(s, gd.g16, y16, dX, scale2 + 1, ex.dx_absmax, st)) return e; }
+  }
+  return 0;
+}
+
+int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
+                      const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
+                      cudaStream_t st) {
+  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, false, st);
+}
+
+// One support-gradient contraction into the partials [slice][N][ldp] (ldp = 32 ceil(N/32): a 32-column chunk never runs into
+// the next row), then reduced into dG [N][N].  A is K-major SW64 (one 32-wide k block per k-block), B K-major.
+static int run_dg(const BdgcnShape& s, GemmParams& p, int kb_total, int kb_per_seg, double flops, float* partials, float* dG,
+                  const float* inv_scale, int accumulate, cudaStream_t st) {
+  const int N = s.N, ldp = 32 * dg_chunks(s);
+  int per = ceil_div(kb_total, dg_max_slices(s));
+  if (per < 1) per = 1;
+  const int slices = ceil_div(kb_total, per);
+  p.R = dg_r(s); p.MT = ceil_div(N, 128); p.NT = ceil_div(dg_chunks(s), p.R); p.Z = slices;
+  p.kb_total = kb_total; p.kb_per_seg = kb_per_seg;
+  p.split_k = 1; p.kb_per_slice = per;
+  p.ep.out = partials; p.ep.out_f16 = 0;
+  p.ep.sZ = (long long)N * ldp; p.ep.sI = ldp; p.ep.sR = 32;
+  p.ep.m_valid = N; p.ep.r_valid = dg_chunks(s);
+  prof_set_next(PROF_BWD_DG, flops);
+  if (int e = tc::launch_contract_bkm(p, st)) return e;
+  return reduce_dg_partials(partials, dG, slices, N, ldp, inv_scale, accumulate, st);
+}
+
+// BWD_DGO, output plane o (sample b, or every sample summed when b < 0):
+//   dG_o[n][m] = sum_{(b,) hc, e, h} U16[b][hc][o][n][e][h] dP16[b][m][e][32 hc + h]      k-block = (segment (b,) hc; e), 32 h
+static int run_bwd_dgo(const BdgcnShape& s, const __half* u16, const __half* dp16, int b, int o, float* partials, float* dG,
+                       const float* inv_scale, cudaStream_t st) {
+  const int N = s.N, H = s.H, cH = s.H / 32, Ko = s.Ko;
+  const long long NN = (long long)N * N;
+  const long long plane0 = (long long)(b < 0 ? 0 : b) * cH * Ko + o;           // U16 plane (b*cH + hc)*Ko + o
+  GemmParams p;
+  init_params(p);
+  {   // U16 planes [n][(e, h)] from plane0 on: dims ((e,h), n, plane)
+    const uint64_t dims[4] = {(uint64_t)N * 32, (uint64_t)N, (uint64_t)((long long)s.B * cH * Ko - plane0), 1};
+    const uint64_t str[3] = {(uint64_t)N * 64, (uint64_t)NN * 64, (uint64_t)NN * 64 * (uint64_t)((long long)s.B * cH * Ko - plane0)};
+    const uint32_t box[4] = {32, 128, 1, 1};
+    if (int e = make_tmap_f16(&p.a_map, u16 + plane0 * NN * 32, 4, dims, str, box, TMAP_SW64)) return e;
+  }
+  {   // dP16 [b][m][e][H]: dims (h, m, e, b), a box of 32 h x 32 R rows m
+    const long long nb = b < 0 ? s.B : 1;
+    const uint64_t dims[4] = {(uint64_t)H, (uint64_t)N, (uint64_t)N, (uint64_t)nb};
+    const uint64_t str[3] = {(uint64_t)N * H * 2, (uint64_t)H * 2, (uint64_t)NN * H * 2};
+    const uint32_t box[4] = {32, (uint32_t)(32 * dg_r(s)), 1, 1};
+    if (int e = make_tmap_f16(&p.b_map, dp16 + (b < 0 ? 0 : (long long)b * NN * H), 4, dims, str, box, TMAP_SW64)) return e;
+  }
+  const int nseg = (b < 0 ? s.B : 1) * cH;              // segment = (b,) hc
+  p.am = omap(1, 1, 0, Ko, 0);                           // plane0 + seg * Ko; k = e * 32
+  p.bm = omap(1, 1, 0, 0, 32, cH, 1);                    // h = 32 (seg % cH); b = seg / cH; e = k-block in the segment
+  const double flops = 2.0 * (b < 0 ? s.B : 1) * (double)NN * N * H;
+  return run_dg(s, p, nseg * N, N, flops, partials, dG, inv_scale, 0, st);
+}
+
+// BWD_DGD, output plane d (sample b, or every sample summed when b < 0), added to dG when `accumulate`:
+//   dG_d[c][e] = sum_{(b,) n, l} X16[b][n][c][l] Y16[b][d][lc][n][e][l - 32 lc]      k-block = (segment (b,) n; lc), 32 l
+static int run_bwd_dgd(const BdgcnShape& s, const __half* x16, const __half* y16, int b, int d, float* partials, float* dG,
+                       const float* inv_scale, int accumulate, cudaStream_t st) {
+  const int N = s.N, C = s.C, cC = s.C / 32, Kd = s.Kd;
+  const long long NN = (long long)N * N;
+  GemmParams p;
+  init_params(p);
+  {   // X16 [(b,) n][c][C]: dims (C, c, (b,n))
+    const long long planes = (long long)(b < 0 ? s.B : 1) * N;
+    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)N, (uint64_t)planes, 1};
+    const uint64_t str[3] = {(uint64_t)C * 2, (uint64_t)N * C * 2, (uint64_t)N * C * 2 * (uint64_t)planes};
+    const uint32_t box[4] = {32, 128, 1, 1};
+    if (int e = make_tmap_f16(&p.a_map, x16 + (b < 0 ? 0 : (long long)b * NN * C), 4, dims, str, box, TMAP_SW64)) return e;
+  }
+  {   // Y16 [b][d][lc][n][e][32] from plane (b*Kd + d)*cC on: dims (l, e, lc, flat (b, n) = b*Kd*cC*N + n), a box of 32 l x 32 R rows e
+    const long long plane0 = ((long long)(b < 0 ? 0 : b) * Kd + d) * cC;
+    const uint64_t flat = (uint64_t)(((long long)s.B * Kd * cC - plane0) * N);
+    const uint64_t dims[4] = {32, (uint64_t)N, (uint64_t)cC, flat};
+    const uint64_t str[3] = {64, (uint64_t)NN * 64, (uint64_t)N * 64};
+    const uint32_t box[4] = {32, (uint32_t)(32 * dg_r(s)), 1, 1};
+    if (int e = make_tmap_f16(&p.b_map, y16 + plane0 * NN * 32, 4, dims, str, box, TMAP_SW64)) return e;
+  }
+  const int nseg = (b < 0 ? s.B : 1) * N;                // segment = (b,) n
+  p.am = omap(1, 1, 0, 1, 0);                            // X plane b*N + n = seg; k = lc * 32
+  p.bm = omap(1, 1, 0, 1, 0, N, Kd * cC * N);            // flat n + b*Kd*cC*N; lc = k-block in the segment
+  const double flops = 2.0 * (b < 0 ? s.B : 1) * (double)NN * N * C;
+  return run_dg(s, p, nseg * cC, cC, flops, partials, dG, inv_scale, accumulate, st);
+}
+
+int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
+                               const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
+                               size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st) {
+  MPGCN_CHECK(s.whole(), "support gradients: whole layers only");
+  MPGCN_CHECK(ex.d_pre_f16 == nullptr, "support gradients: a prepared fp16 dPre belongs to a layer part");
+  const SgradLayout S = sgrad_layout(s);
+  MPGCN_CHECK(ws_bytes >= S.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, S.total);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(X) & 15) == 0, "bdgcn_backward_supports: X must be 16-byte aligned");
+  const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
+  if (int e = backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, want_d, st)) return e;
+  const BwdLayout L = bwd_layout(s);
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  const __half* z16 = static_cast<const __half*>(saved);
+  const __half* dp16 = reinterpret_cast<const __half*>(wb + L.dp16);
+  const __half* y16 = reinterpret_cast<const __half*>(wb + L.y16);
+  const float* inv_scale = reinterpret_cast<const float*>(wb + L.scale) + 1;
+  __half* x16 = reinterpret_cast<__half*>(wb + S.x16);
+  __half* u16 = reinterpret_cast<__half*>(wb + S.u16);
+  __half* w16 = reinterpret_cast<__half*>(wb + S.w16);
+  float* partials = reinterpret_cast<float*>(wb + S.partials);
+  const size_t NN = (size_t)s.N * s.N;
+  if (dGo) {   // U16 again, as the forward formed it (FWD_MIX of the saved Z16)
+    if (int e = permute_w_mix(W, w16, w16 + (size_t)s.Ko * s.Kd * s.C * s.H, s.Ko, s.Kd, s.C, s.H, st)) return e;
+    if (int e = run_mix(s, z16, w16, 2, u16, PROF_BWD_DG, s.Kd * (s.C / 32), s.Ko * (s.H / 32), st)) return e;
+    for (int b = s.dynamic ? 0 : -1; b < (s.dynamic ? s.B : 0); ++b)
+      for (int o = 0; o < s.Ko; ++o) {
+        float* dst = dGo + ((size_t)(b < 0 ? 0 : b) * s.Ko + o) * NN;
+        if (int e = run_bwd_dgo(s, u16, dp16, b, o, partials, dst, inv_scale, st)) return e;
+      }
+  }
+  if (want_d) {
+    if (int e = cvt_f32_to_f16(X, x16, (size_t)s.B * NN * s.C, st)) return e;
+    float* base = s.dynamic ? dGd : dGo;                   // static supports: G_d is G_o, one gradient
+    for (int b = s.dynamic ? 0 : -1; b < (s.dynamic ? s.B : 0); ++b)
+      for (int d = 0; d < s.Kd; ++d) {
+        float* dst = base + ((size_t)(b < 0 ? 0 : b) * s.Kd + d) * NN;
+        if (int e = run_bwd_dgd(s, x16, y16, b, d, partials, dst, inv_scale, s.dynamic ? 0 : 1, st)) return e;
+      }
   }
   return 0;
 }

@@ -226,6 +226,7 @@ enum ProfTag {
   // regions, not kernels: a whole C-ABI call (every kernel of it, the gaps between them included); they count calls, not launches
   PROF_LAYER_FWD, PROF_LAYER_BWD, PROF_HEAD,
   PROF_EXCHANGE,      // kernels: the peer-memory exchange steps of the row shard (rows_reduce_bias_act, relu_backward_scatter[_f16])
+  PROF_BWD_DG,        // kernels: the support gradient of the tensor-core path (U16 recompute, BWD_DGO / BWD_DGD, their reductions)
   PROF_NUM_TAGS
 };
 constexpr int PROF_FIRST_REGION_TAG = PROF_LAYER_FWD;

@@ -59,6 +59,8 @@ int permute_w_bwd(const float* W, float* wq32, int Ko, int Kd, int C, int H, cud
 int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s);
 // dW[o][d][c][h] = sum_slices P[slice][d*C + c][o*H + h]   (P: [slice][MT*128 rows][Ko*H]; o < Ko, d < Kd)
 int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, int C, int H, const float* inv_scale, cudaStream_t s);
+// dG[n][m] (+)= inv_scale * sum_slices P[slice][n][m]   (P: [slice][N][ldp]; n, m < N; accumulate: add to dG)
+int reduce_dg_partials(const float* P, float* dG, int slices, int N, int ldp, const float* inv_scale, int accumulate, cudaStream_t s);
 // out[p][i] = (row0 <= i < row0 + rows) ? delta[p][i] : 0   (diagonal remainders restricted to an origin-row slab)
 int mask_delta_rows(const float* delta, float* out, size_t planes, int N, int row0, int rows, cudaStream_t s);
 // x[i] = act(x[i] + bias[i % H]) in place (bias nullable; act 0 none / 1 ReLU): the epilogue a partial layer call leaves out
@@ -169,5 +171,15 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
                       cudaStream_t st);
+// the backward plus the support gradients (whole layer): static supports get dGo [K][N][N] = dG_o + dG_d summed over the batch
+// (dGd unused), dynamic ones dGo [B][K][N][N] and dGd [B][K][N][N] (either nullable).  dX / dW / db are those of the backward.
+size_t tc_sgrad_ws_bytes(const BdgcnShape& s);
+size_t simt_sgrad_ws_bytes(const BdgcnShape& s);
+int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
+                               const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
+                               size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st);
+int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
+                                 const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
+                                 size_t ws_bytes, cudaStream_t st);
 
 }  // namespace mpgcn

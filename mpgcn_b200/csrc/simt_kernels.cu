@@ -465,6 +465,25 @@ int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, in
   return 0;
 }
 
+__global__ void reduce_dg_kernel(const float* __restrict__ P, float* __restrict__ dG, int slices, int N, int ldp,
+                                 const float* __restrict__ inv_scale, int accumulate) {
+  const float a = inv_scale ? __ldg(inv_scale) : 1.f;
+  const size_t total = (size_t)N * N, slice = (size_t)N * ldp;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t r = i / N, c = i % N;
+    float sum = 0.f;
+    for (int s = 0; s < slices; ++s) sum += P[s * slice + r * ldp + c];
+    dG[i] = accumulate ? fmaf(sum, a, dG[i]) : sum * a;
+  }
+}
+
+int reduce_dg_partials(const float* P, float* dG, int slices, int N, int ldp, const float* inv_scale, int accumulate, cudaStream_t s) {
+  prof_count(PROF_BWD_DG);
+  reduce_dg_kernel<<<grid_for((size_t)N * N, 256), 256, 0, s>>>(P, dG, slices, N, ldp, inv_scale, accumulate);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
 __global__ void mask_delta_rows_kernel(const float* __restrict__ delta, float* __restrict__ out, size_t total, int N, int row0, int rows) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int r = (int)(i % N) - row0;

@@ -223,14 +223,15 @@ static int make_out_map(CUtensorMap* m, const void* base, bool f16, const Epilog
   return 0;
 }
 
-template <int AK, int BK>
+template <int AK, int BK, bool BKM = false>
 static int launch_impl(GemmParams& p, cudaStream_t stream) {
   using C = Cfg<AK, BK>;
   static DynSmemAttr attr = {};
-  if (int e = ensure_dyn_smem(contract_kernel<AK, BK>, kMaxSmem, attr)) return e;
+  if (int e = ensure_dyn_smem(contract_kernel<AK, BK, BKM>, kMaxSmem, attr)) return e;
   MPGCN_CHECK(p.R >= 1 && p.R <= 8, "R=%d out of range", p.R);
   const size_t b_stage = (size_t)p.R * BK * 64;
   const int nres = p.b_res_reps * p.kb_total;
+  MPGCN_CHECK(!BKM || nres == 0, "a K-major B operand streams through the ring");
   MPGCN_CHECK(p.ep.out != nullptr && p.ep.m_valid > 0 && p.ep.r_valid > 0, "contraction without an output");
   if (int e = make_out_map(&p.out_map, p.ep.out, p.ep.out_f16 != 0, p.ep, p.Z)) return e;
   const bool shadow = !p.ep.out_f16 && p.ep.out16 != nullptr;
@@ -262,7 +263,7 @@ static int launch_impl(GemmParams& p, cudaStream_t stream) {
   double fl = 0;
   prof_take_next(&tag, &fl);
   prof_begin(tag, fl, stream);
-  contract_kernel<AK, BK><<<grid, kThreads1, smem, stream>>>(p);
+  contract_kernel<AK, BK, BKM><<<grid, kThreads1, smem, stream>>>(p);
   prof_end(stream);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -278,6 +279,8 @@ int launch_contract(int ak, int bk, GemmParams& p, cudaStream_t stream) {
   set_error("no contraction kernel for A kind %d, BK %d", ak, bk);
   return 1;
 }
+
+int launch_contract_bkm(GemmParams& p, cudaStream_t stream) { return launch_impl<A_K64, 32, true>(p, stream); }
 
 }  // namespace tc
 }  // namespace mpgcn

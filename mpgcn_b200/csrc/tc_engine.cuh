@@ -11,7 +11,9 @@
 //     A_K128  : A is [m][k], k contiguous      (G_o for  V = G_o x1 dPre ; G_d for dX)
 //     A_K64   : A is [m][32], one 32-wide k block per plane (channel mixes Z->U, V->Y)
 //     A_MN64  : A is [k][chunk][32]            (Z for the weight gradient dW = Z^T V)
-//     B       : always [k][chunk r][32 ch], 64-byte rows, SWIZZLE_64B, MN-major
+//     B       : [k][chunk r][32 ch], 64-byte rows, SWIZZLE_64B, MN-major; or, with BKM (A_K64, BK = 32 only), K-major
+//               [32 r rows][32 k], 64-byte rows, SWIZZLE_64B (the support-gradient products dG = U dPre^T and X Y^T, whose
+//               reduction runs over the channels: both operands have it contiguous)
 // * warpgroups 0 and 1 = MMA + epilogue of rows 0..63 / 64..127 of the tile.  Thread 0 also issues the TMA loads: it fills
 //   the ring, then refills each stage as soon as both warpgroups released it, so loads run up to `stages` k-blocks (into the
 //   next tile as well) ahead of the MMAs.  (A separate producer warp takes the CTA past 256 threads, which caps registers at
@@ -137,9 +139,10 @@ __device__ __forceinline__ void decode_tile(const GemmParams& p, int t, int& mt,
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) { return f2h2_sat_bits(a, b); }   // an fp16 operand never holds inf
 
-template <int AK, int BK>
+template <int AK, int BK, bool BKM = false>
 __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_constant__ GemmParams p) {
   using C = Cfg<AK, BK>;
+  static_assert(!BKM || (AK == A_K64 && BK == 32), "a K-major B tile is one 32-wide k block, paired with a K-major SW64 A");
   constexpr int A_STAGE = C::A_STAGE;
   const int R = p.R;
   const int B_STAGE = R * BK * 64;
@@ -212,7 +215,9 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
     } else {                      // A_MN64: dims (ch, k, chunk, z), 4 chunks per tile
       tma_load_4d(a_dst, &p.a_map, &full[p_stage], 0, kA, p_mt * 4, zA);
     }
-    if (!NRES)                    // dims (ch, k, r, z); a resident B was loaded once up front
+    if constexpr (BKM)            // dims (k within the block, n row, k-block, z): the segment's k offset selects a 32-wide chunk
+      tma_load_4d(b_dst, &p.b_map, &full[p_stage], p_sb_lo * p.bm.k_seg, p_nt * R * 32, p_kk, zB);
+    else if (!NRES)               // dims (ch, k, r, z); a resident B was loaded once up front
       tma_load_4d(b_dst, &p.b_map, &full[p_stage], 0, kB, p_nt * R, zB);
     if (++p_stage == S) { p_stage = 0; p_phase ^= 1u; }
     if (++p_kk == p.kb_per_seg) {
@@ -274,8 +279,9 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k) {
               const uint64_t ad = gmma_desc(a_hi, a_addr + C::a_koff(k), C::A_LBO);
-              const uint64_t bd = gmma_desc(b_hi, b_addr + k * C::B_KSTEP, C::B_LBO);
-              wgmma_n<RW, C::A_MN ? 1 : 0, 1>(acc, ad, bd, (first && k == 0) ? 0 : 1);
+              // K-major B: the k-th 16 halves of each 64-byte row (8-row core matrices 512 B apart, as the K-major A_K64 tile)
+              const uint64_t bd = BKM ? gmma_desc(b_hi, b_addr + k * 32, 16) : gmma_desc(b_hi, b_addr + k * C::B_KSTEP, C::B_LBO);
+              wgmma_n<RW, C::A_MN ? 1 : 0, BKM ? 0 : 1>(acc, ad, bd, (first && k == 0) ? 0 : 1);
             }
           };
           switch (R) {
@@ -424,6 +430,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 
 // Launch one contraction (implemented in tc_engine.cu).  ak/bk select the instantiation.
 int launch_contract(int ak, int bk, GemmParams& p, cudaStream_t stream);
+// the same with a K-major B operand (A_K64, BK = 32; no resident B)
+int launch_contract_bkm(GemmParams& p, cudaStream_t stream);
 
 }  // namespace tc
 }  // namespace mpgcn

@@ -1,6 +1,6 @@
 """Autograd-aware operators of the hot path, each a thin call into the C ABI.
 
-    bdgcn(X, G, W, b, activation)  <->  reference BDGCN.forward           (MPGCN.py:24-50)
+    bdgcn(X, G, W, b, activation)  <->  reference BDGCN.forward           (MPGCN.py:24-50), dL/dG too with support_grad=True
     lstm_last(x_seq, w_ih, w_hh, b_ih, b_hh)  <->  nn.LSTM(...)[:, -1, :]  (MPGCN.py:69,100-104)
     lstm_stack(x_seq, params, precision)      <->  the same with num_layers = L >= 2
     lstm_module_last(lstm, x_seq, precision)  <->  either of them, or the module itself where the engine has no kernel
@@ -135,7 +135,7 @@ def _prepared_supports(lib, G, Gc, planes: int, N: int):
 
 class _BDGCNFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, X, G_o, G_d, W, b, dynamic: bool, act: int, precision, grad_mode: bool):
+    def forward(ctx, X, G_o, G_d, W, b, dynamic: bool, act: int, precision, grad_mode: bool, support_grad: bool):
         import ctypes
         lib = _lib.load()
         B, N, N2, C = X.shape
@@ -174,14 +174,17 @@ class _BDGCNFn(torch.autograd.Function):
         ctx.meta = (bool(dynamic), act, prec, b is not None)
         ctx.x_producer = _producer_node(X) if need_grad else None
         ctx.preps = preps
-        ctx.save_for_backward(out, Goc, Gdc, Wc, saved if saved is not None else torch.empty(0, device=X.device))
+        # the support gradient reads X (dG_d = sum X Y_d): kept only when a support asks for its gradient
+        ctx.sgrad = need_grad and support_grad and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
+        empty = torch.empty(0, device=X.device)
+        ctx.save_for_backward(out, Goc, Gdc, Wc, saved if saved is not None else empty, Xc if ctx.sgrad else empty)
         return out
 
     @staticmethod
     def backward(ctx, d_out):
         import ctypes
         lib = _lib.load()
-        out, Goc, Gdc, Wc, saved = ctx.saved_tensors
+        out, Goc, Gdc, Wc, saved, Xc = ctx.saved_tensors
         B, N, K, C, H = ctx.shape
         dynamic, act, prec, has_bias = ctx.meta
         if saved.numel() == 0:
@@ -195,20 +198,40 @@ class _BDGCNFn(torch.autograd.Function):
         dx_absmax = torch.empty(1, dtype=torch.float32, device=dev) if (need_dx and tc) else None
         dW = torch.empty_like(Wc)
         db = torch.empty(H, dtype=torch.float32, device=dev) if has_bias else None
-        ws = _scratch(lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, K, C, H, int(dynamic), prec), dev)
         ex = _lib.BdgcnExtras()
         ex.go_prepared, ex.gd_prepared = _ptr(ctx.preps[0]), _ptr(ctx.preps[1])
         ex.d_out_absmax, ex.dX_absmax = _ptr(hint), _ptr(dx_absmax)
-        with torch.cuda.device(dev):
-            _lib.check(lib.mpgcn_bdgcn_backward_x(_ptr(d_out), _ptr(out), _ptr(Goc), _ptr(Gdc), int(dynamic),
-                                                  _ptr(Wc), act, _ptr(saved), _ptr(dX), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), B, N, K,
-                                                  C, H, prec, ctypes.addressof(ex), _stream()), "bdgcn_backward")
+        dGo = dGd = None
+        if ctx.sgrad:
+            # static: one gradient for the one stack (returned for G_o; G_d is the same tensor); dynamic: one per side, which
+            # autograd adds up when the caller passed one tensor as both
+            if not dynamic:
+                dGo = torch.empty((K, N, N), dtype=torch.float32, device=dev)
+            else:
+                dGo = torch.empty((B, K, N, N), dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+                dGd = torch.empty((B, K, N, N), dtype=torch.float32, device=dev) if ctx.needs_input_grad[2] else None
+            ws = _scratch(lib.mpgcn_bdgcn_support_grad_workspace_bytes(B, N, K, C, H, int(dynamic), prec), dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.mpgcn_bdgcn_backward_supports(_ptr(d_out), _ptr(out), _ptr(Goc), _ptr(Gdc), int(dynamic), _ptr(Wc), act,
+                                                             _ptr(saved), _ptr(dX), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), B, N, K, C,
+                                                             H, prec, ctypes.addressof(ex), _ptr(Xc), _ptr(dGo), _ptr(dGd), _stream()),
+                           "bdgcn_backward_supports")
+        else:
+            ws = _scratch(lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, K, C, H, int(dynamic), prec), dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.mpgcn_bdgcn_backward_x(_ptr(d_out), _ptr(out), _ptr(Goc), _ptr(Gdc), int(dynamic),
+                                                      _ptr(Wc), act, _ptr(saved), _ptr(dX), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), B, N, K,
+                                                      C, H, prec, ctypes.addressof(ex), _stream()), "bdgcn_backward")
         _put_hint(ctx.x_producer, dX, dx_absmax)
-        return dX, None, None, dW, db, None, None, None, None
+        return dX, dGo, dGd, dW, db, None, None, None, None, None
 
 
-def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None) -> torch.Tensor:
-    """out = act(cat_{o,d}(G_o^T X G_d) W + b); G is a [K,N,N] tensor or a pair of [B,K,N,N] tensors."""
+def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None, support_grad: bool = False) -> torch.Tensor:
+    """out = act(cat_{o,d}(G_o^T X G_d) W + b); G is a [K,N,N] tensor or a pair of [B,K,N,N] tensors.
+
+    support_grad=True: a G that requires grad receives dL/dG (static: one [K,N,N] gradient; dynamic: one per side of the pair).
+    It adds 2 K B N^3 (C + H) flops to the backward, as much as its N^3 work without it, so it is opt-in: by default a G that
+    requires grad is refused."""
     _require_cuda(X, "X")
     if isinstance(G, torch.Tensor):
         G_o = G_d = G
@@ -221,12 +244,13 @@ def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None) ->
         if g.device != X.device:
             raise RuntimeError("mpgcn_b200: X and G must be on the same device")
     grad_mode = torch.is_grad_enabled()
-    if grad_mode and (G_o.requires_grad or G_d.requires_grad):
+    if grad_mode and (G_o.requires_grad or G_d.requires_grad) and not support_grad:
         # the reference's einsums would deliver dL/dG through autograd; the trainer never asks for it (static G is a plain
-        # tensor, dynamic G comes from the data loader) and the engine has no dG kernels: refuse instead of returning None
+        # tensor, dynamic G comes from the data loader), and the dG stages double the layer's N^3 backward work: a support that
+        # requires grad by accident is refused instead of silently paying for it (or silently getting None)
         raise NotImplementedError("mpgcn_b200.bdgcn: gradients with respect to the supports G are not implemented "
-                                  "(pass G.detach(), or learnable supports through the reference's einsum path)")
-    return _BDGCNFn.apply(X, G_o, G_d, W, b, dynamic, 1 if relu else 0, precision, grad_mode)
+                                  "by default (pass G.detach(), or support_grad=True / BDGCN.support_grad = True to compute them)")
+    return _BDGCNFn.apply(X, G_o, G_d, W, b, dynamic, 1 if relu else 0, precision, grad_mode, bool(support_grad))
 
 
 def resolve_lstm_precision(name, T, C) -> int:
