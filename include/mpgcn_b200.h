@@ -208,6 +208,14 @@ MPGCN_API int mpgcn_adj_num_supports(int kernel_type, int K);
 MPGCN_API size_t mpgcn_adj_workspace_bytes(int B, int N, int kernel_type, int K);
 MPGCN_API int mpgcn_adj_process(const float* flow, float* supports, int B, int N, int kernel_type, int K, void* workspace, size_t workspace_bytes,
                       void* stream);
+/* Its adjoint: d_flow [B,N,N] = dL/dflow from d_supports [B,Ks,N,N] = dL/dsupports, given the forward's flow and its output
+ * supports (read, not recomputed).  All fp32 on CUDA cores: the Chebyshev recursion's adjoint is 2(K-1) N^3 SGEMMs per series per
+ * batch element.  Where the forward masked 1/sum to 0 (random walk, both series) that row's or column's contribution is exactly 0;
+ * the symmetric kernels give non-finite values where their forward does.  K = 0 (identity only): d_flow = 0.  No allocation, no
+ * synchronisation; arguments are checked before any CUDA call.  workspace: mpgcn_adj_backward_workspace_bytes (0: bad arguments). */
+MPGCN_API size_t mpgcn_adj_backward_workspace_bytes(int B, int N, int kernel_type, int K);
+MPGCN_API int mpgcn_adj_process_backward(const float* flow, const float* supports, const float* d_supports, float* d_flow, int B, int N,
+                               int kernel_type, int K, void* workspace, size_t workspace_bytes, void* stream);
 
 MPGCN_API int mpgcn_lstm_last_backward_ex(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                                 const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, void* workspace,

@@ -9,16 +9,64 @@ Differences, all deliberate: the result lives on the CUDA device (the trainer's 
 Chebyshev kernel always rescales with lambda_max = 2 -- the branch the reference takes on every torch >= 2 because `torch.eig`
 no longer exists and its bare `except` swallows the error (reference GCN.py:117-126).  The reference's unused 1-D `GCN` layer
 (GCN.py:6-45, never imported by name) is not provided.
+
+Gradients.  `process` is differentiable with respect to `flow`, as the reference's tensor algebra is: a flow that requires grad
+(a learnable adjacency, an `nn.Parameter` OD matrix) gets `dL/dflow` through the supports, from the adjoint of the builder on the
+GPU (`mpgcn_adj_process_backward`).  A CPU or float64 flow gets its `.grad` in its own place and type.  At K = 0 the chebyshev
+and random-walk kernels return the identity alone, which carries no gradient (as in the reference).  One deliberate difference:
+where the random-walk normalisation masks 1/sum to 0 (an empty row, or a column in the dual kernel's backward series; also a
+sum so small that its fp32 inverse overflows), that row's or column's contribution to `dL/dflow` is exactly 0.  The reference
+returns NaN there (its `pow(s, -1)` backward multiplies 0 by inf), so a learnable OD matrix with an empty station would turn NaN
+after one optimiser step.  The symmetric kernels have no such mask: a zero-sum row makes their forward non-finite, and their
+gradient then contains NaN, as the reference's does.
 """
 from __future__ import annotations
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .ops import _f32c, _ptr, _scratch, _stream
 
 _KERNELS = {"localpool": 0, "chebyshev": 1, "random_walk_diffusion": 2, "dual_random_walk_diffusion": 3}
 _INVALID = "Invalid kernel_type. Must be one of [chebyshev, localpool, random_walk_diffusion, dual_random_walk_diffusion]."
+
+
+def _adj_process(f: torch.Tensor, kt: int, K: int) -> torch.Tensor:
+    """f: float32, contiguous, on the CUDA device -> supports [B, Ks, N, N]."""
+    lib = _lib.load()
+    B, N = f.shape[0], f.shape[1]
+    Ks = lib.mpgcn_adj_num_supports(kt, K)
+    out = torch.empty((B, Ks, N, N), dtype=torch.float32, device=f.device)
+    ws = _scratch(lib.mpgcn_adj_workspace_bytes(B, N, kt, K), f.device)
+    with torch.cuda.device(f.device):
+        _lib.check(lib.mpgcn_adj_process(_ptr(f), _ptr(out), B, N, kt, K, _ptr(ws), ws.numel(), _stream()), "adj_process")
+    return out
+
+
+class _AdjProcessFn(torch.autograd.Function):
+    """supports = process(flow); the backward reads the saved flow and supports (the T_{k-1} of the recursion's adjoint)."""
+    @staticmethod
+    def forward(ctx, f, kt: int, K: int, grad_mode: bool):
+        out = _adj_process(_f32c(f), kt, K)
+        if grad_mode and ctx.needs_input_grad[0]:
+            ctx.save_for_backward(f, out)
+            ctx.kt, ctx.K = kt, K
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        f, out = ctx.saved_tensors
+        lib = _lib.load()
+        B, N = f.shape[0], f.shape[1]
+        g = _f32c(d_out)
+        d_flow = torch.empty_like(f)
+        ws = _scratch(lib.mpgcn_adj_backward_workspace_bytes(B, N, ctx.kt, ctx.K), f.device)
+        with torch.cuda.device(f.device):
+            _lib.check(lib.mpgcn_adj_process_backward(_ptr(f), _ptr(out), _ptr(g), _ptr(d_flow), B, N, ctx.kt, ctx.K, _ptr(ws), ws.numel(),
+                                                      _stream()), "adj_process_backward")
+        return d_flow, None, None, None
 
 
 class Adj_Processor():
@@ -59,16 +107,11 @@ class Adj_Processor():
             flow = flow.to(self._staging_device(), non_blocking=True)
         elif self._seen_device is None:
             self._seen_device = flow.device
-        lib = _lib.load()
         kt = _KERNELS[self.kernel_type]
-        B, N = flow.shape[0], flow.shape[1]
-        Ks = lib.mpgcn_adj_num_supports(kt, self.K)
-        f = _f32c(flow)
-        out = torch.empty((B, Ks, N, N), dtype=torch.float32, device=f.device)
-        ws = _scratch(lib.mpgcn_adj_workspace_bytes(B, N, kt, self.K), f.device)
-        with torch.cuda.device(f.device):
-            _lib.check(lib.mpgcn_adj_process(_ptr(f), _ptr(out), B, N, kt, self.K, _ptr(ws), ws.numel(), _stream()), "adj_process")
-        return out
+        f = flow.to(dtype=torch.float32).contiguous()       # autograd ops: a float64 flow gets a float64 .grad
+        if kt != _KERNELS["localpool"] and self.K == 0:
+            return _adj_process(f.detach(), kt, 0)            # the identity alone: no gradient, as in the reference
+        return _AdjProcessFn.apply(f, kt, self.K, torch.is_grad_enabled())
 
     # ---- the reference's static helpers, kept for API compatibility (plain tensor algebra on the caller's device) ----
     @staticmethod

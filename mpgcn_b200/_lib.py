@@ -94,6 +94,9 @@ _SIGS = {
     "mpgcn_bdgcn_support_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 7),
     "mpgcn_bdgcn_backward_supports": (ctypes.c_int, [_c_f, _c_f, _c_f, _c_f, ctypes.c_int, _c_f, ctypes.c_int, _c_f, _c_f, _c_f, _c_f, _c_f,
                                                      ctypes.c_size_t] + [ctypes.c_int] * 6 + [ctypes.c_void_p, _c_f, _c_f, _c_f, ctypes.c_void_p]),
+    "mpgcn_adj_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 4),
+    "mpgcn_adj_process_backward": (ctypes.c_int, [_c_f, _c_f, _c_f, _c_f, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_f,
+                                                  ctypes.c_size_t, ctypes.c_void_p]),
 }
 ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)

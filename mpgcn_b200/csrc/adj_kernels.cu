@@ -137,4 +137,190 @@ int adj_process(const float* flow, float* supports, int B, int N, int kernel_typ
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Backward: d_flow from d_supports (the adjoint of adj_process, per batch element A = flow[b], G_k = dL/dT_k).
+//
+//   series adjoint, k = K .. 2:   gx += 2 G_k T_{k-1}^T,   G_{k-1} += 2 x^T G_k,   G_{k-2} -= G_k;   then gx += G_1
+//     (gx is accumulated in G_1's plane, which no step reads as an operand; G_0 belongs to the identity and is discarded)
+//   random walk   x_ij = A_ji dinv_j:   dA_ji += gx_ij dinv_j,   dA_j. += -dinv_j^2 sum_i gx_ij A_ji
+//   dual, backward series x_ij = A_ij cinv_j:   dA_ij += gx_ij cinv_j,   dA_.j += -cinv_j^2 sum_i gx_ij A_ij
+//   symmetric     An = D A D, d = r^-1/2, gAn = -gx (chebyshev) or d_supports[0] (localpool):
+//                 dA_ij = d_i d_j gAn_ij + gr_i,   gr_i = -1/2 r_i^-3/2 (sum_j gAn_ij A_ij d_j + sum_j gAn_ji d_j A_ji)
+// dinv / cinv are masked to 0 exactly where the forward masked them (isinf(1/s)), so such a row or column contributes exactly 0.
+//
+// Workspace: [B][Ks][N][N] working copy of d_supports (only when K >= 2), then row sums, column sums and two per-row reductions.
+// ---------------------------------------------------------------------------------------------------------------------------
+static size_t adj_bwd_grads_bytes(int B, int N, int kernel_type, int K) {
+  if (kernel_type == ADJ_LOCALPOOL || K < 2) return 0;
+  return align_up((size_t)B * adj_num_supports(kernel_type, K) * N * N * sizeof(float), 256);
+}
+
+size_t adj_backward_workspace_bytes(int B, int N, int kernel_type, int K) {
+  return 256 + adj_bwd_grads_bytes(B, N, kernel_type, K) + 4 * align_up((size_t)B * N * sizeof(float), 256);
+}
+
+__device__ __forceinline__ float masked_inv(float s) {
+  const float v = 1.f / s;
+  return isinf(v) ? 0.f : v;
+}
+
+// out[b][i] (+)= sum_j P(i,j) Q(i,j) w(j), P(i,j) = P[b*pz + i*pi + j*pj] (Q likewise), w(j) = rowsum[b][j]^-1/2 (sym_w) or 1;
+// one warp per (b, i)
+__global__ void adj_wsum_kernel(const float* __restrict__ P, long long pz, long long pi, long long pj, const float* __restrict__ Q,
+                                long long qz, long long qi, long long qj, const float* __restrict__ rowsum, int sym_w,
+                                float* __restrict__ out, int accumulate, int B, int N) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= (long long)B * N) return;
+  const int b = (int)(w / N), i = (int)(w % N);
+  const float* Pb = P + b * pz + i * pi;
+  const float* Qb = Q + b * qz + i * qi;
+  float s = 0.f;
+  for (int j = lane; j < N; j += 32) {
+    float v = Pb[j * pj] * Qb[j * qj];
+    if (sym_w) v *= powf(rowsum[(size_t)b * N + j], -0.5f);
+    s += v;
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) out[w] = accumulate ? out[w] + s : s;
+}
+
+// d_flow[b][a][c] for one kernel type (every element written).  gx: G_1 plane of the forward series, gy: of the backward series
+// (dual only), both with batch stride gz; red0 / red1: the per-row reductions of adj_wsum_kernel.
+//   mode 0 / 1 (localpool / chebyshev, sg = +1 / -1):  sg (d_a d_c gx[a][c] - 1/2 r_a^-3/2 red0[a])
+//   mode 2 / 3 (random walk / dual):  gx[c][a] dinv_a - dinv_a^2 red0[a]   (+ gy[a][c] cinv_c - cinv_c^2 red1[c])
+__global__ void adj_norm_grad_kernel(const float* __restrict__ A, const float* __restrict__ gx, const float* __restrict__ gy, long long gz,
+                                     const float* __restrict__ rowsum, const float* __restrict__ colsum, const float* __restrict__ red0,
+                                     const float* __restrict__ red1, float* __restrict__ dA, int B, int N, int mode) {
+  const size_t total = (size_t)B * N * N;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += stride) {
+    const int c = (int)(t % N);
+    const int a = (int)((t / N) % N);
+    const int b = (int)(t / ((size_t)N * N));
+    const float* gxb = gx + b * gz;
+    const size_t ra = (size_t)b * N + a, rc = (size_t)b * N + c;
+    float v;
+    if (mode <= 1) {
+      const float r = rowsum[ra];
+      const float gan = gxb[(size_t)a * N + c];
+      v = powf(r, -0.5f) * powf(rowsum[rc], -0.5f) * gan - 0.5f * powf(r, -1.5f) * red0[ra];
+      if (mode == 1) v = -v;
+    } else {
+      const float di = masked_inv(rowsum[ra]);
+      v = gxb[(size_t)c * N + a] * di - di * di * red0[ra];
+      if (mode == 3) {
+        const float ci = masked_inv(colsum[rc]);
+        v += gy[b * gz + (size_t)a * N + c] * ci - ci * ci * red1[rc];
+      }
+    }
+    dA[t] = v;
+  }
+}
+
+// G_{k-2} -= G_k for every series (Z1 = nser, series stride sser) and batch element (stride bz)
+__global__ void adj_sub_plane_kernel(float* __restrict__ G, long long bz, long long sser, int nser, int dst, int src, int B, long long NN) {
+  const size_t total = (size_t)B * nser * NN;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += stride) {
+    const long long e = (long long)(t % NN);
+    const int s = (int)((t / NN) % nser);
+    const int b = (int)(t / ((size_t)NN * nser));
+    float* base = G + b * bz + s * sser;
+    base[(long long)dst * NN + e] -= base[(long long)src * NN + e];
+  }
+}
+
+// D = 2 op(X) op(Y) + D over B batch elements and nser series; planes are indices into [B][Ks][N][N] stacks, the series differ by
+// K planes.  tx / ty: take the operand transposed.
+static int adj_bwd_gemm(const float* X, int px, int tx, const float* Y, int py, int ty, float* D, int pd, int B, int N, int Ks, int K,
+                        int nser, cudaStream_t st) {
+  const long long NN = (long long)N * N;
+  SgemmParams p{};
+  p.A = X + px * NN; p.B = Y + py * NN; p.D = D + pd * NN; p.Cin = p.D;
+  p.M = N; p.N = N; p.K = N;
+  p.a_si = tx ? 1 : N; p.a_sk = tx ? N : 1;
+  p.b_sk = ty ? 1 : N; p.b_sj = ty ? N : 1;
+  p.d_si = N;
+  p.nseg = 1; p.Z0 = B; p.Z1 = nser; p.Z2 = 1;
+  for (int i = 0; i < 3; ++i) { p.a_sz[i] = 0; p.b_sz[i] = 0; p.d_sz[i] = 0; p.c_sz[i] = 0; }
+  p.a_sz[0] = p.b_sz[0] = p.d_sz[0] = p.c_sz[0] = (long long)Ks * NN;
+  p.a_sz[1] = p.b_sz[1] = p.d_sz[1] = p.c_sz[1] = (long long)K * NN;
+  p.ksplit = 1; p.alpha = 2.f; p.beta = 1.f;
+  return simt_sgemm(p, st);
+}
+
+int adj_process_backward(const float* flow, const float* supports, const float* d_supports, float* d_flow, int B, int N, int kernel_type,
+                         int K, void* ws, size_t ws_bytes, cudaStream_t st) {
+  MPGCN_CHECK(adj_num_supports(kernel_type, 1) >= 1,
+              "Invalid kernel_type. Must be one of [chebyshev, localpool, random_walk_diffusion, dual_random_walk_diffusion].");
+  MPGCN_CHECK(B >= 1 && N >= 1 && K >= 0, "adj_process_backward: bad shape B=%d N=%d K=%d", B, N, K);
+  const int Ks = adj_num_supports(kernel_type, K);
+  const size_t need = adj_backward_workspace_bytes(B, N, kernel_type, K);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "adj_process_backward: workspace too small (%zu < %zu bytes)", ws_bytes, need);
+  const size_t total = (size_t)B * N * N;
+  if (kernel_type != ADJ_LOCALPOOL && K == 0) {       // only the identity: its gradient is not the flow's
+    MPGCN_CUDA(cudaMemsetAsync(d_flow, 0, total * sizeof(float), st));
+    return 0;
+  }
+  const long long NN = (long long)N * N;
+  const size_t vec = align_up((size_t)B * N * sizeof(float), 256);
+  uint8_t* w8 = static_cast<uint8_t*>(ws);
+  float* grads = reinterpret_cast<float*>(w8);
+  float* rowsum = reinterpret_cast<float*>(w8 + adj_bwd_grads_bytes(B, N, kernel_type, K));
+  float* colsum = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + vec);
+  float* red0 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + 2 * vec);
+  float* red1 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + 3 * vec);
+  const unsigned warp_blocks = (unsigned)(((size_t)B * N * 32 + 255) / 256);
+  const bool dual = kernel_type == ADJ_DUAL_RANDOM_WALK;
+
+  prof_count(PROF_ELEMENTWISE);
+  adj_sums_kernel<<<warp_blocks, 256, 0, st>>>(flow, rowsum, B, N, 0);
+  if (dual) {
+    prof_count(PROF_ELEMENTWISE);
+    adj_sums_kernel<<<warp_blocks, 256, 0, st>>>(flow, colsum, B, N, 1);
+  }
+
+  // gx of each series in plane 1 (forward series) and K + 1 (backward series) of a [B][Ks][N][N] stack
+  const float* g = d_supports;
+  if (kernel_type != ADJ_LOCALPOOL && K >= 2) {
+    MPGCN_CUDA(cudaMemcpyAsync(grads, d_supports, (size_t)B * Ks * NN * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    const int nser = dual ? 2 : 1;
+    for (int k = K; k >= 2; --k) {
+      // gx += 2 G_k T_{k-1}^T;  G_{k-1} += 2 x^T G_k  (x = T_1);  G_{k-2} -= G_k
+      if (int e = adj_bwd_gemm(grads, k, 0, supports, k - 1, 1, grads, 1, B, N, Ks, K, nser, st)) return e;
+      if (int e = adj_bwd_gemm(supports, 1, 1, grads, k, 0, grads, k - 1, B, N, Ks, K, nser, st)) return e;
+      if (k - 2 >= 1) {
+        prof_count(PROF_ELEMENTWISE);
+        adj_sub_plane_kernel<<<adj_grid((size_t)B * nser * NN, 256), 256, 0, st>>>(grads, (long long)Ks * NN, (long long)K * NN, nser,
+                                                                                    k - 2, k, B, NN);
+        MPGCN_CUDA(cudaGetLastError());
+      }
+    }
+    g = grads;
+  }
+  const long long gz = (long long)Ks * NN;
+  const float* gx = kernel_type == ADJ_LOCALPOOL ? g : g + NN;
+  const float* gy = dual ? g + (long long)(K + 1) * NN : nullptr;
+
+  // per-row reductions
+  if (kernel_type <= ADJ_CHEBYSHEV) {           // red0[i] = sum_j g_ij A_ij d_j + sum_j g_ji A_ji d_j
+    prof_count(PROF_ELEMENTWISE);
+    adj_wsum_kernel<<<warp_blocks, 256, 0, st>>>(gx, gz, N, 1, flow, NN, N, 1, rowsum, 1, red0, 0, B, N);
+    prof_count(PROF_ELEMENTWISE);
+    adj_wsum_kernel<<<warp_blocks, 256, 0, st>>>(gx, gz, 1, N, flow, NN, 1, N, rowsum, 1, red0, 1, B, N);
+  } else {                                      // red0[j] = sum_i gx_ij A_ji
+    prof_count(PROF_ELEMENTWISE);
+    adj_wsum_kernel<<<warp_blocks, 256, 0, st>>>(gx, gz, 1, N, flow, NN, N, 1, rowsum, 0, red0, 0, B, N);
+    if (dual) {                                 // red1[j] = sum_i gy_ij A_ij
+      prof_count(PROF_ELEMENTWISE);
+      adj_wsum_kernel<<<warp_blocks, 256, 0, st>>>(gy, gz, 1, N, flow, NN, 1, N, rowsum, 0, red1, 0, B, N);
+    }
+  }
+  prof_count(PROF_ELEMENTWISE);
+  adj_norm_grad_kernel<<<adj_grid(total, 256), 256, 0, st>>>(flow, gx, gy, gz, rowsum, colsum, red0, red1, d_flow, B, N, kernel_type);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace mpgcn

@@ -268,6 +268,16 @@ int mpgcn_adj_process(const float* flow, float* supports, int B, int N, int kern
   MPGCN_CHECK(flow && supports, "mpgcn_adj_process: null pointer argument");
   return adj_process(flow, supports, B, N, kernel_type, K, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
+size_t mpgcn_adj_backward_workspace_bytes(int B, int N, int kernel_type, int K) {
+  if (adj_num_supports(kernel_type, K) < 1 || B < 1 || N < 1 || K < 0) return 0;
+  return adj_backward_workspace_bytes(B, N, kernel_type, K);
+}
+int mpgcn_adj_process_backward(const float* flow, const float* supports, const float* d_supports, float* d_flow, int B, int N, int kernel_type,
+                               int K, void* workspace, size_t workspace_bytes, void* stream) {
+  MPGCN_CHECK(flow && supports && d_supports && d_flow && workspace, "mpgcn_adj_process_backward: null pointer argument");
+  return adj_process_backward(flow, supports, d_supports, d_flow, B, N, kernel_type, K, workspace, workspace_bytes,
+                              static_cast<cudaStream_t>(stream));
+}
 
 int mpgcn_head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                        void* stream) {

@@ -101,6 +101,10 @@ enum AdjKernel { ADJ_LOCALPOOL = 0, ADJ_CHEBYSHEV = 1, ADJ_RANDOM_WALK = 2, ADJ_
 int adj_num_supports(int kernel_type, int K);
 size_t adj_workspace_bytes(int B, int N, int kernel_type, int K);
 int adj_process(const float* flow, float* supports, int B, int N, int kernel_type, int K, void* ws, size_t ws_bytes, cudaStream_t st);
+// its adjoint: d_flow [B,N,N] from d_supports [B,Ks,N,N], reading the forward's supports (no allocation, no synchronisation)
+size_t adj_backward_workspace_bytes(int B, int N, int kernel_type, int K);
+int adj_process_backward(const float* flow, const float* supports, const float* d_supports, float* d_flow, int B, int N, int kernel_type,
+                         int K, void* ws, size_t ws_bytes, cudaStream_t st);
 
 // dynamic O / D graphs from the OD history (dyn_graph_kernels.cu)
 size_t dyn_graph_workspace_bytes(int P, int N);
