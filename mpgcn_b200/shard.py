@@ -332,6 +332,15 @@ class _nullcontext:
         return False
 
 
+def _refuse_support_grad(ctx, grad_mode):
+    """The part kernels have no dG stages: a support (G_o, G_d: inputs 1 and 2 of both sharded layer Functions) that requires
+    grad would silently get none, whatever layer.support_grad says, so it is refused as ops.bdgcn refuses one without
+    support_grad.  Runs first in each Function's forward, which every sharded layer goes through."""
+    if grad_mode and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
+        raise NotImplementedError("mpgcn_b200.shard: gradients with respect to the supports G exist for whole layers only "
+                                  "(ops.bdgcn with support_grad=True); pass G.detach() to the sharded model")
+
+
 class _RowShardLayerFn(torch.autograd.Function):
     """Sample by sample, so that the exchange of sample b overlaps the contractions of sample b + 1 (forward: partial pre of b is
     reduce-scattered while b + 1 is computed; backward: every dPre slab is put on the wire up front and the gradient
@@ -339,6 +348,7 @@ class _RowShardLayerFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_mode):
+        _refuse_support_grad(ctx, grad_mode)
         B, rows, N, C = X.shape
         K, H = G_o.shape[-3], W.shape[1]
         prec = _ENGINE.resolve_precision(precision, 1, N, K, C, H)
@@ -429,6 +439,7 @@ class _RowShardLayerFn(torch.autograd.Function):
 class _KShardLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, X, G_o, G_d_local, W, b, dynamic, act, precision, plan, grad_mode):
+        _refuse_support_grad(ctx, grad_mode)
         B, N, _, C = X.shape
         K, H = G_o.shape[-3], W.shape[1]
         Kd = plan.Kd

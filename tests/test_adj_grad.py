@@ -3,8 +3,9 @@
 CPU: the float64 adjoint (tests/adj_grad_oracle.py) against the reference's autograd fixtures `agrad_*` and against central
 finite differences of the forward, the C-ABI surface and the entry point's argument checks.  GPU: the engine's d_flow against
 float64 for every kernel type across sizes, the fixtures, the zero-row rule, the unchanged forward, when a gradient is (not)
-tracked, CPU leaves, a flow feeding both sides of a dynamic pair, and Adam steps on a learnable adjacency against the reference
-model fed by the reference's Adj_Processor.
+tracked, CPU leaves, a flow feeding both sides of a dynamic pair, Adam steps on a learnable adjacency against the reference
+model fed by the reference's Adj_Processor, the whole chain flow -> supports -> model at the default (fp16) precision, and Adam on a
+learnable adjacency in fp16 against fp32.
 """
 import importlib.util
 import os
@@ -396,3 +397,104 @@ def test_adam_on_a_learnable_static_adjacency_tracks_the_reference(cuda_device):
 @pytest.mark.gpu
 def test_adam_on_a_learnable_dynamic_pair_tracks_the_reference(cuda_device):
     _adam_runs(False, cuda_device)
+
+
+def _chain(model, procs, flows, x, d_y, dev):
+    """flow -> Adj_Processor -> model, one forward / backward: procs / flows for the static adjacency [1,N,N] (branch 0) and the OD
+    pair [B,N,N] x 2 (branch 1).  -> (captured layers of both branches, the supports, their gradients captured by tensor hooks)."""
+    from test_support_grad import capture_layer_grads
+    sups, grads = [], {}
+    for i, f in enumerate(flows):
+        S = procs[0 if i == 0 else 1].process(f)
+        S.register_hook(lambda g, i=i: grads.__setitem__(i, g.detach().clone()))
+        sups.append(S)
+    caps = [capture_layer_grads(model, m) for m in range(2)]
+    model(x_seq=x, G_list=[sups[0][0], (sups[1], sups[2])]).backward(d_y)
+    torch.cuda.synchronize()
+    for _, handles in caps:
+        for h in handles:
+            h.remove()
+    return [c for c, _ in caps], sups, [grads[i] for i in range(len(flows))]
+
+
+@pytest.mark.gpu
+def test_learnable_adjacency_chain_at_the_default_precision(cuda_device):
+    """flow -> Adj_Processor (random walk: static adjacency; dual random walk: OD pair) -> model with every layer at the default
+    precision, which resolves to the fp16 tensor cores at hidden 32: each flow's gradient is the builder's adjoint of its supports'
+    own gradient (captured by a tensor hook) at TOL, and that support gradient passes the float64 model check at fp16's 2e-3
+    (on an H100 the largest errors were 3.8e-6 and 4.5e-4)."""
+    from test_support_grad import TOL as SG_TOL, _live_model, model_support_grad_float64
+    from mpgcn_b200 import ops
+    B, T, N, K, hid = 2, 4, 20, 3, 32
+    rng = np.random.default_rng(77)
+    model = _live_model(N, K, hid, None, cuda_device)
+    for mod in model.modules():
+        if isinstance(mod, shim.BDGCN):
+            assert mod.precision is None and ops.resolve_precision(mod.precision, B, N, K, hid, hid) == _lib.PREC_FP16_TC
+    t = lambda a: torch.from_numpy(a).to(cuda_device)
+    flows = [t(_flow(rng, 1, N)).requires_grad_(True)] + [t(_flow(rng, B, N)).requires_grad_(True) for _ in range(2)]
+    procs = (Adj_Processor("random_walk_diffusion", K - 1), Adj_Processor("dual_random_walk_diffusion", 1))
+    x = t((rng.random((B, T, N, N, 1)) * 4).astype(np.float32))
+    d_y = t(rng.standard_normal((B, 1, N, N, 1)).astype(np.float32))
+    caps, sups, d_sups = _chain(model, procs, flows, x, d_y, cuda_device)
+    for i, (f, d) in enumerate(zip(flows, d_sups)):
+        kind, order = ("random_walk_diffusion", K - 1) if i == 0 else ("dual_random_walk_diffusion", 1)
+        assert float(d.abs().max()) > 0
+        _check(f.grad, adj_process_grad(f.detach().cpu().numpy(), d.cpu().numpy(), kind, order), TOL, f"chain/auto: flow {i} grad")
+    ref_s = model_support_grad_float64(caps[0], sups[0][0], cuda_device)
+    _check(d_sups[0][0], ref_s, SG_TOL["fp16"], "chain/auto: static support grad vs float64 on the engine masks")
+    ref_o, ref_d = model_support_grad_float64(caps[1], (sups[1], sups[2]), cuda_device)
+    _check(d_sups[1], ref_o, SG_TOL["fp16"], "chain/auto: G_o support grad vs float64 on the engine masks")
+    _check(d_sups[2], ref_d, SG_TOL["fp16"], "chain/auto: G_d support grad vs float64 on the engine masks")
+
+
+# Adam divides each element's update by its own gradient's running magnitude, so flow elements whose gradient is near zero move
+# by a near-random sign in either precision: on an H100 (80GB HBM3, 700 W) the fp16 update differs from the fp32 one by rel_L2
+# 0.23; the bar is 4x that, so it mostly catches an update that stays at zero (rel_L2 1).  The elements whose gradient kept its
+# sign (the fp32 run moved them at least half its largest move) have a determined update: there the difference measured 0.092,
+# and the bar of 4x that rejects an update off by a factor of 2 or of the wrong sign.
+ADAM_FLOW_UPDATE_TOL = 0.95
+ADAM_STEADY_UPDATE_TOL = 0.4
+
+
+@pytest.mark.gpu
+def test_adam_on_a_learnable_adjacency_is_equivalent_in_fp16_and_fp32(cuda_device):
+    """20 Adam steps on the model plus a learnable static adjacency (random walk), every layer and the LSTM on the fp16 tensor
+    cores against the fp32 kernels, from one initial state: the loss curves within test_gpu_at_size's 2e-2 (max relative
+    difference; measured 2.1e-3), and the flow's update in rel_L2 within ADAM_FLOW_UPDATE_TOL over every element (measured 0.23)
+    and within ADAM_STEADY_UPDATE_TOL over the elements the fp32 run moved steadily (measured 0.092)."""
+    B, T, N, K, hid = 2, 4, 12, 3, 32
+    rng = np.random.default_rng(2026)
+    x = torch.from_numpy((rng.random((B, T, N, N, 1)) * 4).astype(np.float32)).to(cuda_device)
+    target = torch.from_numpy(rng.random((B, 1, N, N, 1)).astype(np.float32)).to(cuda_device)
+    adj0 = torch.from_numpy(_flow(rng, 1, N)).to(cuda_device)
+    od = tuple(torch.from_numpy(_flow(rng, B, N)).to(cuda_device) for _ in range(2))
+    from test_support_grad import _live_model
+    runs = {}
+    for prec in ("fp32", "fp16"):
+        model = _live_model(N, K, hid, prec, cuda_device, seed=2026)
+        adj = nn.Parameter(adj0.clone())
+        opt = torch.optim.Adam(list(model.parameters()) + [adj], lr=1e-3)
+        pair = tuple(Adj_Processor("dual_random_walk_diffusion", 1).process(t) for t in od)
+        proc = Adj_Processor("random_walk_diffusion", K - 1)
+        losses = []
+        for _ in range(20):
+            opt.zero_grad()
+            loss = torch.mean((model(x, [proc.process(adj)[0], pair]) - target) ** 2)
+            loss.backward()
+            opt.step()
+            losses.append(float(loss.detach()))
+        runs[prec] = (np.asarray(losses), (adj.detach() - adj0).cpu().numpy())
+    a, r = runs["fp16"][0], runs["fp32"][0]
+    assert np.all(np.isfinite(a)) and r[-1] < r[0], f"fp32 loss did not move: {r[0]:.4f} -> {r[-1]:.4f}"
+    rel = np.abs(a - r) / r
+    record_parity("adam-20 learnable adjacency: loss curve fp16 vs fp32 (max rel diff)", float(rel.max()),
+                  float(np.linalg.norm(a - r) / np.linalg.norm(r)), 2e-2)
+    assert rel.max() <= 2e-2, f"loss curves diverge: max rel diff {rel.max():.3e} at step {int(rel.argmax())}"
+    moved = runs["fp32"][1]
+    assert np.abs(moved).max() > 1e-4
+    _check(runs["fp16"][1], moved, ADAM_FLOW_UPDATE_TOL, "adam-20 learnable adjacency: flow update fp16 vs fp32", l2_only=True)
+    steady = np.abs(moved) >= 0.5 * np.abs(moved).max()          # elements whose gradient kept its sign over the steps
+    assert steady.sum() >= 10
+    _check(runs["fp16"][1][steady], moved[steady], ADAM_STEADY_UPDATE_TOL,
+           "adam-20 learnable adjacency: flow update fp16 vs fp32 where fp32 moved >= half its largest move", l2_only=True)

@@ -251,25 +251,14 @@ def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn, row0=None, prec=1, alloc=_nan
         r["bufs"].update(dX=dX_b, wsb=wsb)
     torch.cuda.synchronize()
 
-    def h16(buf, o, *shape):
-        return buf[o:o + 2 * math.prod(shape)].view(torch.float16).view(*shape)
-
-    def f32(buf, o, *shape):
-        return buf[o:o + 4 * math.prod(shape)].view(torch.float32).view(*shape)
-
     if prec != 1:
         r.update(z=saved.view(torch.float32).view(B, Kd, R, N, C), u=f32(ws, fo["u"], B, Ko, R, N, H))
         if backward:
-            r.update(v=f32(wsb, bo["v"], B, Ko, R, N, H), y=f32(wsb, bo["y"], B, Kd, R, N, C), wq=f32(wsb, bo["wq"], Kd, Ko, H, C))
-            if not part:
-                r["dpre"] = f32(wsb, bo["dpre"], B, N, N, H)
+            r.update(simt_backward_views(wsb, bo, B, R, N, C, H, Ko, Kd, part))
         return r
-    cC, cH = C // 32, H // 32
-    in_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, Kd, R, N, C)      # [B][d][lc][n][e][32] -> [B][d][n][e][C]
-    out_planes = lambda t: t.permute(0, 1, 3, 4, 2, 5).reshape(B, Ko, R, N, H)     # [B][o][hc][n][e][32] -> [B][o][n][e][H]
+    cC = C // 32
     r.update(x16=h16(ws, fo["x16"], B, R, N, C), gd16=h16(ws, fo["gd16"], nz, Kd, N, Np), dd=f32(ws, fo["dd"], nz, Kd, N),
-             w16=h16(ws, fo["w16"], 2, cH, Ko, Kd, cC, 32, 32).permute(0, 2, 3, 4, 5, 1, 6).reshape(2, Ko, Kd, C, H),
-             u=h16(ws, fo["u16"], B, cH, Ko, R, N, 32).permute(0, 2, 3, 4, 1, 5).reshape(B, Ko, R, N, H),
+             w16=w16_view(ws, fo["w16"], Ko, Kd, C, H), u=u16_view(ws, fo["u16"], B, Ko, R, N, H),
              z=in_planes(saved.view(torch.float16).view(B, Kd, cC, R, N, 32)))
     # G_o gets its own fp16 copy (and remainders) unless it is the G_d buffer with as many planes: nothing writes go16 / dgo then
     r["own_go"] = own_go = Go.data_ptr() != Gd.data_ptr() or Ko != Kd
@@ -277,12 +266,57 @@ def run_layer_wide(X, Go, Gd, W, bias, d_out, dyn, row0=None, prec=1, alloc=_nan
     if R < N:
         r["dgo_masked"] = f32(ws, fo["dgo_masked"], nz, Ko, N)
     if backward:
-        prepared = d_pre16 is not None
-        r.update(dp=d_pre16[0] if prepared else h16(wsb, bo["dp16"], B, N, N, H), scale=d_pre16[1] if prepared else f32(wsb, bo["scale"], 2),
-                 bgd16=h16(wsb, bo["gd16"], nz, Kd, N, Np), v=out_planes(h16(wsb, bo["v16"], B, Ko, cH, R, N, 32)),
-                 y=in_planes(h16(wsb, bo["y16"], B, Kd, cC, R, N, 32)),
-                 wq16=h16(wsb, bo["wq16"], Kd, cC, Ko, cH, 32, 32).permute(2, 0, 1, 5, 3, 4).reshape(Ko, Kd, C, H))
-        r["bgo16"] = h16(wsb, bo["go16"], nz, Ko, N, Np) if own_go else r["bgd16"]
+        r.update(tc_backward_views(wsb, bo, B, R, N, C, H, Ko, Kd, nz, own_go))
+        if d_pre16 is not None:
+            r.update(dp=d_pre16[0], scale=d_pre16[1])
+    return r
+
+
+def h16(buf, o, *shape):
+    return buf[o:o + 2 * math.prod(shape)].view(torch.float16).view(*shape)
+
+
+def f32(buf, o, *shape):
+    return buf[o:o + 4 * math.prod(shape)].view(torch.float32).view(*shape)
+
+
+def in_planes(t):
+    """[B][d][lc][n][e][32] -> [B][d][n][e][C]"""
+    B, Kd, cC, R, N = t.shape[:5]
+    return t.permute(0, 1, 3, 4, 2, 5).reshape(B, Kd, R, N, 32 * cC)
+
+
+def out_planes(t):
+    """[B][o][hc][n][e][32] -> [B][o][n][e][H]"""
+    B, Ko, cH, R, N = t.shape[:5]
+    return t.permute(0, 1, 3, 4, 2, 5).reshape(B, Ko, R, N, 32 * cH)
+
+
+def w16_view(buf, o, Ko, Kd, C, H):
+    """The mix's fp16 W split [2][hc][o][d][lc][32][32] -> [2][o][d][C][H]"""
+    return h16(buf, o, 2, H // 32, Ko, Kd, C // 32, 32, 32).permute(0, 2, 3, 4, 5, 1, 6).reshape(2, Ko, Kd, C, H)
+
+
+def u16_view(buf, o, B, Ko, R, N, H):
+    """U16 [B][hc][o][n][e][32] -> [B][o][n][e][H]"""
+    return h16(buf, o, B, H // 32, Ko, R, N, 32).permute(0, 2, 3, 4, 1, 5).reshape(B, Ko, R, N, H)
+
+
+def tc_backward_views(wsb, bo, B, R, N, C, H, Ko, Kd, nz, own_go):
+    """The tensor-core backward workspace in logical layouts: dP16, [S, 1/S], the fp16 supports, V16 / Y16 and Wq16 [o][d][C][H]."""
+    Np, cC, cH = (N + 7) // 8 * 8, C // 32, H // 32
+    r = dict(dp=h16(wsb, bo["dp16"], B, N, N, H), scale=f32(wsb, bo["scale"], 2), bgd16=h16(wsb, bo["gd16"], nz, Kd, N, Np),
+             v=out_planes(h16(wsb, bo["v16"], B, Ko, cH, R, N, 32)), y=in_planes(h16(wsb, bo["y16"], B, Kd, cC, R, N, 32)),
+             wq16=h16(wsb, bo["wq16"], Kd, cC, Ko, cH, 32, 32).permute(2, 0, 1, 5, 3, 4).reshape(Ko, Kd, C, H))
+    r["bgo16"] = h16(wsb, bo["go16"], nz, Ko, N, Np) if own_go else r["bgd16"]
+    return r
+
+
+def simt_backward_views(wsb, bo, B, R, N, C, H, Ko, Kd, part):
+    """The fp32 backward workspace: V, Y, Wq [d][o][H][C] as stored and (whole layer) dPre."""
+    r = dict(v=f32(wsb, bo["v"], B, Ko, R, N, H), y=f32(wsb, bo["y"], B, Kd, R, N, C), wq=f32(wsb, bo["wq"], Kd, Ko, H, C))
+    if not part:
+        r["dpre"] = f32(wsb, bo["dpre"], B, N, N, H)
     return r
 
 

@@ -1,7 +1,8 @@
 """world_size-2 gloo tests (CPU) of the model-parallel shards (mpgcn_b200/shard.py): the exchange logic -- reduce-scatter of the
 partial pre-activation / all-gather of dPre (origin-row shard), all-reduce of pre and dX + row-sharded LSTM (K shard), the
 plan-aware gradient reduction -- with the CUDA engine replaced by a torch stand-in (tests/shard_standin.py), against the numpy
-oracle of the WHOLE model (reference MPGCN.py:89-112)."""
+oracle of the WHOLE model (reference MPGCN.py:89-112).  One-rank runs check that a sharded layer, and the whole sharded model in
+both kinds, refuse supports that require grad (the part kernels have no support gradient)."""
 import os
 import socket
 import subprocess
@@ -92,3 +93,77 @@ def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
         assert set(r["grads"]) == set(grads_o)
         for k, g in r["grads"].items():
             assert max(orc.rel_errors(g.numpy(), grads_o[k])) <= 2e-5, (kind, k)
+
+
+@pytest.fixture
+def world1(monkeypatch):
+    """A one-rank gloo group in this process and the torch stand-in engine: a sharded layer runs end to end on the CPU."""
+    import torch.distributed as dist
+    from mpgcn_b200 import shard
+    from shard_standin import TorchEngine
+    assert not dist.is_initialized()
+    dist.init_process_group("gloo", store=dist.HashStore(), rank=0, world_size=1)
+    monkeypatch.setattr(shard, "_ENGINE", TorchEngine())
+    try:
+        yield shard
+    finally:
+        dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("kind", ["row", "k"])
+@pytest.mark.parametrize("support_grad", [False, True])
+def test_sharded_layer_refuses_a_support_that_requires_grad(kind, support_grad, world1):
+    """The part kernels have no dG stages, so a sharded layer given a support that requires grad raises instead of leaving
+    G.grad None, whether or not the layer opted into support gradients; without grad mode, or with G detached, it runs."""
+    import MPGCN as shim
+    shard = world1
+    B, N, K, C = 2, 6, 3, 4
+    torch.manual_seed(0)
+    layer = shim.BDGCN(K=K, input_dim=C, hidden_dim=C, use_bias=True, activation=nn.ReLU)
+    layer.support_grad = support_grad
+    plan = shard.ShardPlan(kind, 0, 1, N, K)
+    X = torch.rand(B, N, N, C)
+    G = (torch.rand(K, N, N) / N).requires_grad_(True)
+    dyn = lambda: torch.rand(B, K, N, N) / N
+    learnable_o = (dyn().requires_grad_(True), dyn())
+    learnable_d = (dyn(), dyn().requires_grad_(True))
+    for g in (G, learnable_o, learnable_d):
+        with pytest.raises(NotImplementedError, match="whole layers only"):
+            shard.sharded_bdgcn(layer, X, g, plan).sum().backward()
+    with torch.no_grad():
+        assert shard.sharded_bdgcn(layer, X, G, plan).shape == (B, N, N, C)
+    out = shard.sharded_bdgcn(layer, X, G.detach(), plan)
+    out.sum().backward()
+    assert G.grad is None and layer.W.grad is not None and float(layer.W.grad.abs().max()) > 0
+
+
+@pytest.mark.parametrize("kind", ["row", "k"])
+@pytest.mark.parametrize("learnable", ["static", "dynamic"])
+def test_sharded_model_refuses_learnable_supports(kind, learnable, world1):
+    """The whole sharded model (the trainer's M = 2 layout) with a learnable static stack or a learnable dynamic pair: every branch
+    refuses it, including the K shard's static branch, whose layers take the whole stack as G_o and the rank's slice as G_d."""
+    import MPGCN as shim
+    shard = world1
+    B, T, N, K, hid = 2, 3, 6, 3, 4
+    torch.manual_seed(0)
+    model = shim.MPGCN(M=2, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=3, num_nodes=N,
+                       user_bias=True, activation=nn.ReLU)
+    for mod in model.modules():
+        if isinstance(mod, shim.BDGCN):
+            mod.support_grad = True
+    plan = shard.ShardPlan(kind, 0, 1, N, K)
+    x, y = torch.rand(B, T, N, N, 1), torch.rand(B, 1, N, N, 1)
+    G = torch.rand(K, N, N) / N
+    go, gd = torch.rand(B, K, N, N) / N, torch.rand(B, K, N, N) / N
+    xs, ys, gos, gds = shard.shard_host_inputs(plan, x, y, go, gd)
+    if learnable == "static":
+        G = G.requires_grad_(True)
+    else:
+        gos, gds = gos.requires_grad_(True), gds.requires_grad_(True)
+    with pytest.raises(NotImplementedError, match="whole layers only"):
+        shard.sharded_mse_loss(plan, shard.sharded_forward(model, plan, xs, G, (gos, gds)), ys).backward()
+    with torch.no_grad():
+        shard.sharded_forward(model, plan, xs, G, (gos, gds))
+    detached = shard.sharded_forward(model, plan, xs, G.detach(), (gos.detach(), gds.detach()))
+    shard.sharded_mse_loss(plan, detached, ys).backward()
+    assert all(p.grad is not None for p in model.parameters())

@@ -3,7 +3,8 @@
 CPU: the float64 factored dG (tests/support_grad_oracle.py) against the reference's autograd fixtures `sgrad_*`, the C-ABI
 surface of the new entry point and its argument checks.  GPU: the engine's dG against float64 at ragged sizes, supports counts
 and channel widths, at size, against the fixtures (layer and whole model), unchanged dX / dW / db / out, the default refusal,
-re-staging of a learnable support after an optimiser step, and a few Adam steps against the reference model.
+re-staging of a learnable support after an optimiser step, a few Adam steps against the reference model, and the whole model's dG
+against float64 on the engine's own ReLU masks in both precisions.  The dG stages in isolation: test_gpu_support_grad_stages.py.
 """
 import ctypes
 import importlib.util
@@ -382,3 +383,67 @@ def test_adam_on_a_learnable_support_tracks_the_reference(cuda_device):
     moved = runs["ref"][1] - g0.cpu().numpy()
     assert np.abs(moved).max() > 1e-4
     _check(runs["ours"][1] - g0.cpu().numpy(), moved, 1e-3, "adam: G update", l2_only=True)
+
+
+def capture_layer_grads(model, m):
+    """Forward hooks on branch m's BDGCN layers -> [(layer, {"X", "out", "d_out"})] filled by the next forward / backward: each
+    layer's input and output, and by a tensor hook on the output its upstream gradient."""
+    caps = []
+
+    def hook(layer, inp, out):
+        rec = {"X": inp[0].detach(), "out": out.detach()}
+        out.register_hook(lambda g: rec.__setitem__("d_out", g.detach().clone()))
+        caps.append((layer, rec))
+    handles = [layer.register_forward_hook(hook) for layer in model.branch_models[m]['spatial']]
+    return caps, handles
+
+
+def model_support_grad_float64(caps, G, dev):
+    """sum over the captured layers of support_grads on each layer's own ReLU mask: the float64 dL/dG of the function the engine
+    computed (static: [K,N,N]; dynamic: (dG_o, dG_d))."""
+    total = None
+    G = tuple(g.detach() for g in G) if isinstance(G, tuple) else G.detach()
+    for layer, rec in caps:
+        r = support_grads(rec["X"], G, layer.W.detach(), layer.b.detach(), "relu", rec["d_out"], mask_from=rec["out"], device=dev)
+        total = r if total is None else (tuple(a + b for a, b in zip(total, r)) if isinstance(r, tuple) else total + r)
+    return total
+
+
+def _live_model(N, K, hid, prec, dev, seed=5):
+    """The trainer's model (M = 2, three layers) with support gradients on and live heads (a dead FC ReLU would leave the supports
+    without a gradient); prec None keeps every layer at the default precision."""
+    torch.manual_seed(seed)
+    model = _model(None, N, K, hid, prec, dev)
+    with torch.no_grad():
+        for branch in model.branch_models:
+            branch['fc'][0].bias.fill_(0.5)
+    return model
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("prec", ["fp32", "fp16"])
+@pytest.mark.parametrize("dyn", [False, True])
+def test_model_support_grad_against_float64_on_the_engine_masks(dyn, prec, cuda_device):
+    """A learnable static G (an nn.Parameter in branch 0), or a learnable dynamic pair (branch 1): G.grad, which the three layers'
+    gradients add into, against the float64 sum over the layers of support_grads on each layer's captured input, output (its ReLU
+    mask) and upstream gradient, on rel_L2 and rel_Linf at TOL (on an H100 the largest error was 3.4e-4 in fp16, 7.0e-7 in fp32)."""
+    B, T, N, K, hid = 2, 4, 20, 3, 32
+    rng = np.random.default_rng(31 + int(dyn))
+    t = lambda a: torch.from_numpy(a.astype(np.float32)).to(cuda_device)
+    model = _live_model(N, K, hid, prec, cuda_device)
+    G = nn.Parameter(t(rng.random((K, N, N)) / N))
+    pair = tuple(nn.Parameter(t(rng.random((B, K, N, N)) / N)) for _ in range(2))
+    G_list = [G, pair] if not dyn else [G.detach(), pair]
+    caps, handles = capture_layer_grads(model, 1 if dyn else 0)
+    model(x_seq=t(rng.random((B, T, N, N, 1)) * 4), G_list=G_list).backward(t(rng.standard_normal((B, 1, N, N, 1))))
+    torch.cuda.synchronize()
+    for h in handles:
+        h.remove()
+    assert len(caps) == 3
+    ref = model_support_grad_float64(caps, pair if dyn else G, cuda_device)
+    what = f"model {'dynamic pair' if dyn else 'static G'}/{prec}: dG vs float64 on the engine masks"
+    if dyn:
+        _check(pair[0].grad, ref[0], TOL[prec], what + "/dG_o")
+        _check(pair[1].grad, ref[1], TOL[prec], what + "/dG_d")
+    else:
+        _check(G.grad, ref, TOL[prec], what)
