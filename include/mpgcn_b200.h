@@ -282,7 +282,8 @@ MPGCN_API int mpgcn_dyn_graph_build(const float* od_history, int periods, float*
  *   g    HOST array of M device pointers, each [cells, C] (cells = B*N*N);  w [M,C], bias [M];  y [cells]
  *   pre  [M,cells] pre-activations kept for backward, or NULL (inference)
  * backward: dy [cells]; dg HOST array of M device pointers [cells, C] (or NULL / NULL entries), dw [M,C], db [M];
- * dg_absmax [M] (nullable) receives max|dg_m| per branch (see mpgcn_bdgcn_backward_ex). */
+ * dg_absmax [M] (nullable) receives max|dg_m| per branch (see mpgcn_bdgcn_backward_ex).
+ * 1 <= M <= 8, C a multiple of 4; w, every g[m] (never NULL) and every non-NULL dg[m] 16-byte aligned: checked before any CUDA call. */
 MPGCN_API int mpgcn_head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                        void* stream);
 MPGCN_API int mpgcn_head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,

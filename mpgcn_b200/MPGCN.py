@@ -134,13 +134,19 @@ class MPGCN(nn.Module):
                 cur.wait_stream(self._streams[m])
                 if not capturing:       # under CUDA-graph capture the join above is a graph dependency: later frees / re-uses are ordered by it
                     feats[m].record_stream(cur)
-        fcs = [self.branch_models[m]['fc'][0] for m in range(self.M)]
-        if all(fc.out_features == 1 for fc in fcs) and feats[0].shape[-1] % 4 == 0 and self.M <= 8:
-            # Linear(C -> 1) + ReLU per branch and the mean over branches in one fused pass (reference MPGCN.py:107,110)
-            w = torch.cat([fc.weight for fc in fcs], dim=0)            # [M, C]
-            b = torch.cat([fc.bias for fc in fcs], dim=0)              # [M]
-            ensemble_out = ops.fc_relu_mean(feats, w, b)               # [B, N, N, 1]
-        else:
-            branch_out = [self.branch_models[m]['fc'](feats[m]) for m in range(self.M)]
-            ensemble_out = torch.mean(torch.stack(branch_out, dim=-1), dim=-1)
+        ensemble_out = fc_head([self.branch_models[m]['fc'] for m in range(self.M)], feats)
         return ensemble_out.unsqueeze(dim=1)
+
+
+def fc_head(fcs, feats, fused=None):
+    """The FC head of every branch and the mean over branches (reference MPGCN.py:107,110): fcs[m] is branch m's
+    Sequential(Linear(C -> input_dim), ReLU), feats[m] its last BDGCN output [..., C] -> [..., input_dim].
+    Where the fused kernel applies (input_dim 1, C a multiple of 4, at most 8 branches) it computes all of it in one pass:
+    `fused(feats, w [M, C], b [M])`, by default ops.fc_relu_mean; otherwise each branch runs its own modules.  The whole model
+    and the sharded one (shard.sharded_forward) both decide here."""
+    lins = [fc[0] for fc in fcs]
+    if all(lin.out_features == 1 for lin in lins) and feats[0].shape[-1] % 4 == 0 and len(fcs) <= 8:
+        w = torch.cat([lin.weight for lin in lins], dim=0)             # [M, C]
+        b = torch.cat([lin.bias for lin in lins], dim=0)               # [M]
+        return (fused or ops.fc_relu_mean)(feats, w, b)                # [..., 1]
+    return torch.mean(torch.stack([fc(f) for fc, f in zip(fcs, feats)], dim=-1), dim=-1)

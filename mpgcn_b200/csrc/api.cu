@@ -282,6 +282,7 @@ int mpgcn_adj_process_backward(const float* flow, const float* supports, const f
 int mpgcn_head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                        void* stream) {
   MPGCN_CHECK(g && w && bias && y && cells >= 1, "mpgcn_head_forward: null pointer or empty input");
+  if (head_check("mpgcn_head_forward", g, w, nullptr, C, M)) return 1;
   ProfRegion region(PROF_HEAD, 2.0 * cells * C * M, static_cast<cudaStream_t>(stream));
   return head_forward(g, w, bias, y, pre, cells, C, M, static_cast<cudaStream_t>(stream));
 }
@@ -289,6 +290,7 @@ int mpgcn_head_forward(const float* const* g, const float* w, const float* bias,
 int mpgcn_head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
                         float* dg_absmax, long long cells, int C, int M, void* stream) {
   MPGCN_CHECK(g && w && pre && dy && dw && db && cells >= 1, "mpgcn_head_backward: null pointer or empty input");
+  if (head_check("mpgcn_head_backward", g, w, dg, C, M)) return 1;
   ProfRegion region(PROF_HEAD, 4.0 * cells * C * M, static_cast<cudaStream_t>(stream));
   return head_backward(g, w, pre, dy, dg, dw, db, dg_absmax, cells, C, M, static_cast<cudaStream_t>(stream));
 }

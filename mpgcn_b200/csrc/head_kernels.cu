@@ -149,15 +149,27 @@ static int head_grid(long long cells) {
   return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Everything the kernels dereference without a bounds check, refused on the host before any CUDA call: w and each g[m] are read
+// and each dg[m] written as float4, so all must be 16-byte aligned; every g[m] is read; a dg[m] may be null (no gradient).
+int head_check(const char* what, const float* const* g, const float* w, float* const* dg, int C, int M) {
+  MPGCN_CHECK(M >= 1 && M <= kMaxBranches, "%s: %d branches unsupported (1..%d)", what, M, kMaxBranches);
+  MPGCN_CHECK(C >= 4 && C % 4 == 0, "%s: C=%d must be a multiple of 4", what, C);
+  MPGCN_CHECK(aligned16(w), "%s: w must be 16-byte aligned", what);
+  for (int m = 0; m < M; ++m) {
+    MPGCN_CHECK(g[m] != nullptr, "%s: branch %d input is a null pointer", what, m);
+    MPGCN_CHECK(aligned16(g[m]), "%s: branch %d input must be 16-byte aligned", what, m);
+    MPGCN_CHECK(dg == nullptr || aligned16(dg[m]), "%s: branch %d gradient must be 16-byte aligned", what, m);
+  }
+  return 0;
+}
+
+// head_forward / head_backward: arguments already passed head_check (api.cu)
 int head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                  cudaStream_t st) {
-  MPGCN_CHECK(M >= 1 && M <= kMaxBranches, "head: %d branches unsupported (1..%d)", M, kMaxBranches);
-  MPGCN_CHECK(C >= 4 && C % 4 == 0, "head: C=%d must be a multiple of 4", C);
   HeadPtrs p{};
-  for (int m = 0; m < M; ++m) {
-    MPGCN_CHECK(g[m] != nullptr && (reinterpret_cast<uintptr_t>(g[m]) & 15) == 0, "head: branch %d input null or misaligned", m);
-    p.g[m] = g[m];
-  }
+  for (int m = 0; m < M; ++m) p.g[m] = g[m];
   prof_count(PROF_ELEMENTWISE);
   switch (M) {
     case 1: head_fwd_kernel<1><<<head_grid(cells), 256, 0, st>>>(p, w, bias, y, pre, cells, C, M); break;
@@ -172,8 +184,6 @@ int head_forward(const float* const* g, const float* w, const float* bias, float
 
 int head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
                   float* dg_absmax, long long cells, int C, int M, cudaStream_t st) {
-  MPGCN_CHECK(M >= 1 && M <= kMaxBranches, "head: %d branches unsupported (1..%d)", M, kMaxBranches);
-  MPGCN_CHECK(C >= 4 && C % 4 == 0, "head: C=%d must be a multiple of 4", C);
   HeadPtrs p{};
   for (int m = 0; m < M; ++m) {
     p.g[m] = g[m];

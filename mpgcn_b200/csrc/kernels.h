@@ -91,6 +91,7 @@ int lstm_bwd_cells_per_block(int T, int C);
 int lstm_copy_bias_grad(const float* d_b_ih, float* d_b_hh, int n, cudaStream_t st);
 
 // FC head + branch mean (head_kernels.cu); g / dg are HOST arrays of M device pointers
+int head_check(const char* what, const float* const* g, const float* w, float* const* dg, int C, int M);
 int head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                  cudaStream_t st);
 int head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,

@@ -492,7 +492,24 @@ class _HeadFn(torch.autograd.Function):
 
 
 def fc_relu_mean(gs, w, b) -> torch.Tensor:
-    """(1/M) * sum_m relu(g_m @ w[m] + b[m]) for M branch activations g_m [..., C]; w [M, C], b [M] -> [..., 1]."""
-    for g in gs:
-        _require_cuda(g, "branch activation")
+    """(1/M) * sum_m relu(g_m @ w[m] + b[m]) for M branch activations g_m [..., C]; w [M, C], b [M] -> [..., 1].
+    1 <= M <= 8 branches of one shape, C a multiple of 4 (the kernel reads float4s), all on one CUDA device."""
+    gs = list(gs)
+    M = len(gs)
+    if not 1 <= M <= 8:
+        raise ValueError(f"fc_relu_mean: 1 to 8 branches, got {M}")
+    shape = tuple(gs[0].shape)
+    if not shape or shape[-1] % 4 or shape[-1] == 0:
+        raise ValueError(f"fc_relu_mean: branch activations must be [..., C] with C a multiple of 4, got {shape}")
+    C = shape[-1]
+    for m, g in enumerate(gs):
+        if tuple(g.shape) != shape:
+            raise ValueError(f"fc_relu_mean: branch {m} has shape {tuple(g.shape)}, branch 0 {shape}")
+    if tuple(w.shape) != (M, C) or tuple(b.shape) != (M,):
+        raise ValueError(f"fc_relu_mean: w must be {(M, C)} and b {(M,)} for {M} branches of width {C}, got {tuple(w.shape)} and {tuple(b.shape)}")
+    dev = gs[0].device
+    for what, t in [("w", w), ("b", b)] + [(f"branch {m}", g) for m, g in enumerate(gs)]:
+        if t.device != dev:
+            raise ValueError(f"fc_relu_mean: {what} is on {t.device}, branch 0 on {dev}")
+    _require_cuda(gs[0], "branch activation")
     return _HeadFn.apply(torch.is_grad_enabled(), w, b, *gs)

@@ -29,6 +29,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib, ops
+from .MPGCN import fc_head
 from .dist import shard_range
 
 
@@ -554,10 +555,8 @@ def sharded_forward(model, plan: ShardPlan, x_slab, G_static, G_dyn):
         for m in range(model.M):
             cur.wait_stream(plan.streams[m])
             feats[m].record_stream(cur)
-    fcs = [model.branch_models[m]['fc'][0] for m in range(model.M)]
-    w = torch.cat([fc.weight for fc in fcs], dim=0)
-    b = torch.cat([fc.bias for fc in fcs], dim=0)
-    return _ENGINE.head(feats, w, b).unsqueeze(dim=1)
+    # the head is row-local: the same decision (fused kernel or each branch's own modules) as the whole model's
+    return fc_head([model.branch_models[m]['fc'] for m in range(model.M)], feats, fused=_ENGINE.head).unsqueeze(dim=1)
 
 
 def _static_k_layer(layer, X, G_pair, plan):

@@ -167,3 +167,43 @@ def test_sharded_model_refuses_learnable_supports(kind, learnable, world1):
     detached = shard.sharded_forward(model, plan, xs, G.detach(), (gos.detach(), gds.detach()))
     shard.sharded_mse_loss(plan, detached, ys).backward()
     assert all(p.grad is not None for p in model.parameters())
+
+
+@pytest.mark.parametrize("kind", ["row", "k"])
+def test_sharded_model_with_two_input_features_matches_whole_model_oracle(kind, world1):
+    """input_dim = 2: each branch's fc is Linear(C -> 2), which the fused head (one output per branch) cannot compute, so the
+    sharded model must take the per-branch modules, as the whole model does.  The prediction [B,1,N,N,2], the loss and every
+    gradient against the float64 oracle of the whole model."""
+    import MPGCN as shim
+    shard = world1
+    B, T, N, K, I, hid = 2, 3, 6, 3, 2, 8
+    torch.manual_seed(0)
+    model = shim.MPGCN(M=2, K=K, input_dim=I, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=2, num_nodes=N,
+                       user_bias=True, activation=nn.ReLU)
+    with torch.no_grad():
+        for p in model.parameters():
+            if p.dim() == 1:
+                p.add_(0.05)
+    rng = np.random.default_rng(3)
+    x = (rng.random((B, T, N, N, I)) * 4).astype(np.float32)
+    y = rng.random((B, 1, N, N, I)).astype(np.float32)
+    G = (rng.random((K, N, N)) / N).astype(np.float32)
+    go = (rng.random((B, K, N, N)) / N).astype(np.float32)
+    gd = (rng.random((B, K, N, N)) / N).astype(np.float32)
+    plan = shard.ShardPlan(kind, 0, 1, N, K)
+    xs, ys, gos, gds = shard.shard_host_inputs(plan, *(torch.from_numpy(a) for a in (x, y, go, gd)))
+    pred = shard.sharded_forward(model, plan, xs, torch.from_numpy(G), (gos, gds))
+    assert tuple(pred.shape) == (B, 1, N, N, I)
+    loss = shard.sharded_mse_loss(plan, pred, ys)
+    loss.backward()
+    params = {k: v.detach().numpy().astype(np.float64) for k, v in model.state_dict().items()}
+    GL = [G.astype(np.float64), (go.astype(np.float64), gd.astype(np.float64))]
+    y_o = orc.mpgcn_forward(params, x.astype(np.float64), GL, M=2, gcn_num_layers=2)
+    _, grads_o = orc.mpgcn_forward_backward(params, x.astype(np.float64), GL, M=2, gcn_num_layers=2, d_y=2.0 * (y_o - y) / y.size)
+    assert max(orc.rel_errors(pred.detach().numpy(), y_o)) <= 1e-5
+    loss_o = float(((y_o - y) ** 2).mean())
+    assert abs(float(loss.detach()) - loss_o) <= 1e-5 * loss_o
+    named = dict(model.named_parameters())
+    assert set(named) == set(grads_o)
+    for k, p in named.items():
+        assert max(orc.rel_errors(p.grad.numpy(), grads_o[k])) <= 2e-5, (kind, k)
