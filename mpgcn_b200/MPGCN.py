@@ -22,6 +22,7 @@ never materialises the `[B*N*N, T, C]` output sequence.
 from __future__ import annotations
 
 import contextlib
+from typing import Callable, NamedTuple
 
 import torch
 from torch import nn
@@ -53,6 +54,13 @@ class BDGCN(nn.Module):
     def extra_repr(self) -> str:
         return f"K={self.K}, {self.input_dim} -> {self.hidden_dim}, bias={self.use_bias}"
 
+    def fused_act(self):
+        """The activation the layer kernels fuse into their epilogue: 1 ReLU, 0 none.  None for any other activation, which
+        forward() applies after the kernel and the sharded layers (mpgcn_b200.shard.sharded_bdgcn) refuse."""
+        if self.activation is None:
+            return 0
+        return 1 if isinstance(self.activation, nn.ReLU) else None
+
     def forward(self, X: torch.Tensor, G):
         if isinstance(G, torch.Tensor):                     # static supports (K, N, N)
             assert self.K == G.shape[-3]
@@ -63,12 +71,21 @@ class BDGCN(nn.Module):
         else:
             raise NotImplementedError
         assert X.dim() == 4 and X.shape[1] == X.shape[2] == G[0].shape[-1] and X.shape[3] == self.input_dim
-        fused_relu = isinstance(self.activation, nn.ReLU)
-        out = ops.bdgcn(X, G, self.W, self.b if self.use_bias else None, relu=fused_relu, precision=self.precision,
+        act = self.fused_act()
+        out = ops.bdgcn(X, G, self.W, self.b if self.use_bias else None, relu=act == 1, precision=self.precision,
                         support_grad=self.support_grad)
-        if self.activation is not None and not fused_relu:  # any other activation: unfused epilogue
+        if act is None:                                     # any other activation: unfused epilogue
             out = self.activation(out)
         return out
+
+
+class BranchRunner(NamedTuple):
+    """How MPGCN._forward evaluates a branch: with the whole model's own parts (MPGCN.forward) or a shard's
+    (mpgcn_b200.shard.sharded_forward)."""
+    temporal: Callable      # (nn.LSTM, x_seq [B,T,rows,N,I]) -> the LSTM's last hidden state [B, rows, N, C] (the K shard: all N rows)
+    layer: Callable         # (BDGCN, X, G, branch index) -> the layer's output
+    head: Callable          # the fused head of fc_head: (feats, w [M, C], b [M]) -> [..., 1]
+    streams: bool           # evaluate the branches on one CUDA stream each
 
 
 class MPGCN(nn.Module):
@@ -107,14 +124,19 @@ class MPGCN(nn.Module):
         return [(weight.new_zeros(shape), weight.new_zeros(shape)) for _ in range(self.M)]
 
     def _temporal(self, lstm: nn.LSTM, x_seq: torch.Tensor) -> torch.Tensor:
-        return ops.lstm_module_last(lstm, x_seq, self.lstm_precision)
+        B, _, rows, N, _ = x_seq.shape
+        return ops.lstm_module_last(lstm, x_seq, self.lstm_precision).reshape(B, rows, N, self.lstm_hidden_dim)
 
     def forward(self, x_seq: torch.Tensor, G_list: list):
         """x_seq (B, T, N, N, 1); G_list: per branch a static (K,N,N) tensor or a dynamic tuple.  -> (B, 1, N, N, 1)"""
-        assert (len(x_seq.shape) == 5) & (self.num_nodes == x_seq.shape[2] == x_seq.shape[3])
+        run = BranchRunner(self._temporal, lambda layer, X, G, m: layer(X, G), ops.fc_relu_mean, bool(self.branch_streams))
+        return self._forward(x_seq, G_list, self.num_nodes, run)
+
+    def _forward(self, x_seq: torch.Tensor, G_list: list, rows: int, run: BranchRunner):
+        """The branches and the head on x_seq [B, T, rows, N, I]: every origin row (rows = N), or a shard's slab of them."""
+        assert (len(x_seq.shape) == 5) & (rows == x_seq.shape[2]) & (self.num_nodes == x_seq.shape[3])
         assert len(G_list) == self.M
-        B, N = x_seq.shape[0], self.num_nodes
-        use_streams = bool(self.branch_streams) and x_seq.is_cuda and self.M > 1
+        use_streams = run.streams and x_seq.is_cuda and self.M > 1
         capturing = use_streams and torch.cuda.is_current_stream_capturing()
         cur = torch.cuda.current_stream() if use_streams else None
         if use_streams and (self._streams is None or self._streams[0].device != x_seq.device):
@@ -125,28 +147,27 @@ class MPGCN(nn.Module):
             if use_streams:
                 self._streams[m].wait_stream(cur)
             with (torch.cuda.stream(self._streams[m]) if use_streams else contextlib.nullcontext()):
-                gcn_in = self._temporal(branch['temporal'], x_seq).reshape(B, N, N, self.lstm_hidden_dim)
+                gcn_in = run.temporal(branch['temporal'], x_seq)
                 for layer in branch['spatial']:
-                    gcn_in = layer(gcn_in, G_list[m])
+                    gcn_in = run.layer(layer, gcn_in, G_list[m], m)
             feats.append(gcn_in)
         if use_streams:
             for m in range(self.M):
                 cur.wait_stream(self._streams[m])
                 if not capturing:       # under CUDA-graph capture the join above is a graph dependency: later frees / re-uses are ordered by it
                     feats[m].record_stream(cur)
-        ensemble_out = fc_head([self.branch_models[m]['fc'] for m in range(self.M)], feats)
+        ensemble_out = fc_head([self.branch_models[m]['fc'] for m in range(self.M)], feats, run.head)
         return ensemble_out.unsqueeze(dim=1)
 
 
-def fc_head(fcs, feats, fused=None):
+def fc_head(fcs, feats, fused):
     """The FC head of every branch and the mean over branches (reference MPGCN.py:107,110): fcs[m] is branch m's
     Sequential(Linear(C -> input_dim), ReLU), feats[m] its last BDGCN output [..., C] -> [..., input_dim].
     Where the fused kernel applies (input_dim 1, C a multiple of 4, at most 8 branches) it computes all of it in one pass:
-    `fused(feats, w [M, C], b [M])`, by default ops.fc_relu_mean; otherwise each branch runs its own modules.  The whole model
-    and the sharded one (shard.sharded_forward) both decide here."""
+    `fused(feats, w [M, C], b [M])`; otherwise each branch runs its own modules."""
     lins = [fc[0] for fc in fcs]
     if all(lin.out_features == 1 for lin in lins) and feats[0].shape[-1] % 4 == 0 and len(fcs) <= 8:
         w = torch.cat([lin.weight for lin in lins], dim=0)             # [M, C]
         b = torch.cat([lin.bias for lin in lins], dim=0)               # [M]
-        return (fused or ops.fc_relu_mean)(feats, w, b)                # [..., 1]
+        return fused(feats, w, b)                                      # [..., 1]
     return torch.mean(torch.stack([fc(f) for fc, f in zip(fcs, feats)], dim=-1), dim=-1)

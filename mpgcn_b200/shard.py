@@ -29,7 +29,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib, ops
-from .MPGCN import fc_head
+from .MPGCN import BranchRunner
 from .dist import shard_range
 
 
@@ -48,8 +48,6 @@ class ShardPlan:
         self.d_lo, self.d_hi = shard_range(K, rank, world) if kind == "k" else (0, K)
         self.Kd = self.d_hi - self.d_lo
         self.peer = None          # PeerExchange once enable_peer_exchange() succeeded (row shard over NVLink peer memory)
-        self.branch = 0           # which model branch is being evaluated (selects that branch's pair of exchange buffers)
-        self.streams = None       # one CUDA stream per branch (sharded_forward): the branches are independent until the head
 
     def describe(self) -> dict:
         d = {"kind": self.kind, "world": self.world, "rows_per_rank": self.rows,
@@ -321,25 +319,31 @@ class _AllGatherRowsFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 # sharded BDGCN layers
 # ------------------------------------------------------------------------------------------------
-def _f32c(t):
-    return t.detach().to(dtype=torch.float32).contiguous()
-
-
-class _nullcontext:
-    def __enter__(self):
-        return None
-
-    def __exit__(self, *a):
-        return False
-
-
-def _refuse_support_grad(ctx, grad_mode):
-    """The part kernels have no dG stages: a support (G_o, G_d: inputs 1 and 2 of both sharded layer Functions) that requires
-    grad would silently get none, whatever layer.support_grad says, so it is refused as ops.bdgcn refuses one without
-    support_grad.  Runs first in each Function's forward, which every sharded layer goes through."""
+def _begin_forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_mode, samples):
+    """The start of both sharded layer Functions' forward (inputs X, G_o, G_d, W, b, ...): resolve the precision for part calls of
+    `samples` samples, make the operands fp32 and contiguous and note on ctx what backward needs.
+    -> (prec, Xc, Goc, Gdc, Wc, bias, keep); keep: the forward stashes what backward reads.
+    The part kernels have no dG stages: a support that requires grad would silently get none, whatever layer.support_grad says,
+    so it is refused as ops.bdgcn refuses one without support_grad."""
     if grad_mode and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
         raise NotImplementedError("mpgcn_b200.shard: gradients with respect to the supports G exist for whole layers only "
                                   "(ops.bdgcn with support_grad=True); pass G.detach() to the sharded model")
+    N, C = X.shape[2], X.shape[3]
+    K, H = G_o.shape[-3], W.shape[1]
+    prec = _ENGINE.resolve_precision(precision, samples, N, K, C, H)
+    Xc, Goc, Wc = ops._f32c(X), ops._f32c(G_o), ops._f32c(W)
+    Gdc = Goc if G_d is G_o else ops._f32c(G_d)
+    keep = grad_mode and any(ctx.needs_input_grad)
+    ctx.meta = (dynamic, act, prec, b is not None, N, K, C, H)
+    ctx.keep, ctx.plan = keep, plan
+    return prec, Xc, Goc, Gdc, Wc, None if b is None else ops._f32c(b), keep
+
+
+def _begin_backward(ctx, d_out):
+    """-> d_out as fp32 contiguous; refuses a backward through a forward that kept nothing"""
+    if not ctx.keep:
+        raise RuntimeError("mpgcn_b200.shard: backward called but forward ran without requires_grad inputs")
+    return ops._f32c(d_out)
 
 
 class _RowShardLayerFn(torch.autograd.Function):
@@ -348,29 +352,22 @@ class _RowShardLayerFn(torch.autograd.Function):
     contractions of sample b start as soon as ITS rows have arrived)."""
 
     @staticmethod
-    def forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_mode):
-        _refuse_support_grad(ctx, grad_mode)
-        B, rows, N, C = X.shape
-        K, H = G_o.shape[-3], W.shape[1]
-        prec = _ENGINE.resolve_precision(precision, 1, N, K, C, H)
-        Xc, Goc, Wc = _f32c(X), _f32c(G_o), _f32c(W)
-        Gdc = Goc if G_d is G_o else _f32c(G_d)
-        keep = grad_mode and any(ctx.needs_input_grad)
+    def forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, branch, grad_mode):
+        prec, Xc, Goc, Gdc, Wc, bias, keep = _begin_forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_mode, 1)
+        N, K, C, H = ctx.meta[4:]
+        B, rows = X.shape[:2]
         if plan.peer is not None:
             # peer-memory exchange: the whole batch in one part call, partial written straight into the symmetric buffer,
             # one barrier, then the reduce-scatter + bias + ReLU kernel reads this rank's rows from every rank's buffer
-            buf, hdl = plan.peer.next(("fwd", plan.branch), (B, N, N, H))
-            ctx.branch = plan.branch
+            buf, hdl = plan.peer.next(("fwd", branch), (B, N, N, H))
+            ctx.branch = branch
             planes = (B if dynamic else 1) * K
             go_p = _ENGINE.prepared(G_o, Goc, planes, N, prec)
             preps = (go_p, go_p if G_d is G_o else _ENGINE.prepared(G_d, Gdc, planes, N, prec))
             ctx.preps = preps
-            bias = None if b is None else _f32c(b)
             _, saved = _ENGINE.forward_part(Xc, Goc, Gdc, dynamic, Wc, N, plan.row_lo, K, K, prec, keep, out=buf, preps=preps)
             hdl.barrier()
             out = _ENGINE.rows_reduce_bias_act(list(hdl.buffer_ptrs), B, N, plan.row_lo, rows, H, bias, act, X.device)
-            ctx.meta = (dynamic, act, prec, b is not None, N, K, C, keep)
-            ctx.plan = plan
             ctx.stash = [saved]
             ctx.save_for_backward(out, Goc, Gdc, Wc)
             return out
@@ -384,23 +381,19 @@ class _RowShardLayerFn(torch.autograd.Function):
         for p, _ in pending:
             p.wait()
         del pending
-        _ENGINE.bias_act(out, None if b is None else _f32c(b), act)
-        ctx.meta = (dynamic, act, prec, b is not None, N, K, C, keep)
-        ctx.plan = plan
+        _ENGINE.bias_act(out, bias, act)
         ctx.stash = stash
         ctx.save_for_backward(out, Goc, Gdc, Wc)
         return out
 
     @staticmethod
     def backward(ctx, d_out):
+        d_out = _begin_backward(ctx, d_out)
         out, Goc, Gdc, Wc = ctx.saved_tensors
-        dynamic, act, prec, has_bias, N, K, C, keep = ctx.meta
+        dynamic, act, prec, has_bias, N, K, C, H = ctx.meta
         plan = ctx.plan
-        if not keep:
-            raise RuntimeError("mpgcn_b200.shard: backward called but forward ran without requires_grad inputs")
-        B, H = d_out.shape[0], d_out.shape[-1]
+        B = d_out.shape[0]
         if plan.peer is not None:
-            d_out = _f32c(d_out)
             if prec == _lib.PREC_FP16_TC:
                 # tensor-core path: the gathered dPre travels as fp16 (what the contraction reads anyway), scaled by ONE power of two
                 # derived from the global max|dOut| -- half the bytes, and no rank casts / scans the gathered tensor
@@ -419,8 +412,8 @@ class _RowShardLayerFn(torch.autograd.Function):
                                                ctx.needs_input_grad[0])
             ctx.stash = None
             ctx.preps = None
-            return dX, None, None, dW, db, None, None, None, None, None
-        d_pre_slab, db = _ENGINE.relu_backward(_f32c(d_out), out, act, has_bias)       # mask + bias gradient of the rank's own rows
+            return dX, None, None, dW, db, None, None, None, None, None, None
+        d_pre_slab, db = _ENGINE.relu_backward(d_out, out, act, has_bias)       # mask + bias gradient of the rank's own rows
         d_pre = d_pre_slab.new_empty((B, N, N, H))
         pending = [all_gather_rows_begin(d_pre_slab[s], d_pre[s], plan) for s in range(B)]     # the ONE exchange step of the layer backward
         need_dx = ctx.needs_input_grad[0]
@@ -434,43 +427,34 @@ class _RowShardLayerFn(torch.autograd.Function):
                 dX[s:s + 1] = dx_s
             dW = dw_s if dW is None else dW + dw_s
         ctx.stash = None
-        return dX, None, None, dW, db, None, None, None, None, None
+        return dX, None, None, dW, db, None, None, None, None, None, None
 
 
 class _KShardLayerFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, X, G_o, G_d_local, W, b, dynamic, act, precision, plan, grad_mode):
-        _refuse_support_grad(ctx, grad_mode)
-        B, N, _, C = X.shape
-        K, H = G_o.shape[-3], W.shape[1]
+    def forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, branch, grad_mode):
+        prec, Xc, Goc, Gdc, Wc, bias, keep = _begin_forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_mode, X.shape[0])
+        N, K, C, H = ctx.meta[4:]
         Kd = plan.Kd
-        prec = _ENGINE.resolve_precision(precision, B, N, K, C, H)
-        Xc, Goc = _f32c(X), _f32c(G_o)
-        keep = grad_mode and any(ctx.needs_input_grad)
-        saved = Wl = Gdc = None
+        saved = Wl = None
         if Kd > 0:
-            Gdc = _f32c(G_d_local)
-            Wl = W.detach().view(K, K, C, H)[:, plan.d_lo:plan.d_hi].reshape(K * Kd * C, H).to(torch.float32).contiguous()
+            Wl = Wc.view(K, K, C, H)[:, plan.d_lo:plan.d_hi].reshape(K * Kd * C, H).contiguous()
             pre, saved = _ENGINE.forward_part(Xc, Goc, Gdc, dynamic, Wl, N, 0, K, Kd, prec, keep)
         else:               # more ranks than supports: this rank only takes part in the exchange
-            pre = torch.zeros((B, N, N, H), dtype=torch.float32, device=X.device)
+            pre = torch.zeros((X.shape[0], N, N, H), dtype=torch.float32, device=X.device)
         dist.all_reduce(pre, group=plan.group)                   # the ONE exchange step of the layer forward
-        _ENGINE.bias_act(pre, None if b is None else _f32c(b), act)
-        ctx.meta = (dynamic, act, prec, b is not None, N, K, C, H, keep)
-        ctx.plan = plan
-        ctx.save_for_backward(pre, Goc, Gdc if Gdc is not None else torch.empty(0, device=X.device),
-                              Wl if Wl is not None else torch.empty(0, device=X.device),
-                              saved if saved is not None else torch.empty(0, device=X.device))
+        _ENGINE.bias_act(pre, bias, act)
+        empty = torch.empty(0, device=X.device)
+        ctx.save_for_backward(pre, Goc, Gdc, Wl if Wl is not None else empty, saved if saved is not None else empty)
         return pre
 
     @staticmethod
     def backward(ctx, d_out):
+        d_out = _begin_backward(ctx, d_out)
         out, Goc, Gdc, Wl, saved = ctx.saved_tensors
-        dynamic, act, prec, has_bias, N, K, C, H, keep = ctx.meta
+        dynamic, act, prec, has_bias, N, K, C, H = ctx.meta
         plan = ctx.plan
-        if not keep:
-            raise RuntimeError("mpgcn_b200.shard: backward called but forward ran without requires_grad inputs")
-        d_pre, db = _ENGINE.relu_backward(_f32c(d_out), out, act, has_bias)            # replicated: identical on every rank
+        d_pre, db = _ENGINE.relu_backward(d_out, out, act, has_bias)            # replicated: identical on every rank
         dW = torch.zeros((K, K, C, H), dtype=torch.float32, device=d_out.device)
         need_dx = ctx.needs_input_grad[0]
         if plan.Kd > 0:
@@ -482,20 +466,24 @@ class _KShardLayerFn(torch.autograd.Function):
             dist.all_reduce(dX, group=plan.group)                # the ONE exchange step of the layer backward
         if db is not None:
             db = db / plan.world          # replicated quantity: the parameter-gradient exchange SUMS over the ranks
-        return dX, None, None, dW.view(K * K * C, H), db, None, None, None, None, None
+        return dX, None, None, dW.view(K * K * C, H), db, None, None, None, None, None, None
 
 
-def sharded_bdgcn(layer, X, G, plan: ShardPlan):
+def sharded_bdgcn(layer, X, G, plan: ShardPlan, branch: int = 0):
     """One BDGCN layer (mpgcn_b200.MPGCN.BDGCN: parameters W, b; activation None or ReLU) on this rank's shard.
-    row: X [B,rows,N,C] -> [B,rows,N,H];  k: X [B,N,N,C] -> [B,N,N,H] (replicated), G_d already sliced to the rank's supports."""
-    from torch import nn
-    dynamic = not isinstance(G, torch.Tensor)
-    G_o, G_d = (G if dynamic else (G, G))
-    relu = isinstance(layer.activation, nn.ReLU)
-    if layer.activation is not None and not relu:
+    row: X [B,rows,N,C] -> [B,rows,N,H];  k: X [B,N,N,C] -> [B,N,N,H] (replicated).
+    G: the whole static [K,N,N] stack, or the dynamic pair (G_o [B,K,N,N], G_d) with G_d whole (row shard) or the rank's slice
+    [B,Kd,N,N] (K shard, shard_host_inputs).  `branch`: the model branch, whose pair of peer-exchange buffers the row shard uses."""
+    act = layer.fused_act()
+    if act is None:
         raise NotImplementedError("sharded layers fuse None / ReLU only")
+    dynamic = not isinstance(G, torch.Tensor)
+    if dynamic:
+        G_o, G_d = G
+    else:           # the K shard contracts the destination side over its own supports only
+        G_o, G_d = G, (G[plan.d_lo:plan.d_hi] if plan.kind == "k" else G)
     fn = _RowShardLayerFn if plan.kind == "row" else _KShardLayerFn
-    return fn.apply(X, G_o, G_d, layer.W, layer.b if layer.use_bias else None, dynamic, 1 if relu else 0, layer.precision, plan,
+    return fn.apply(X, G_o, G_d, layer.W, layer.b if layer.use_bias else None, dynamic, act, layer.precision, plan, branch,
                     torch.is_grad_enabled())
 
 
@@ -518,53 +506,22 @@ def shard_host_inputs(plan: ShardPlan, x_seq, y_true, g_o, g_d):
 
 
 def sharded_forward(model, plan: ShardPlan, x_slab, G_static, G_dyn):
-    """model: mpgcn_b200.MPGCN.MPGCN.  x_slab [B,T,rows,N,1] (shard_host_inputs).  G_static [K,N,N] (whole, on every rank);
+    """model: mpgcn_b200.MPGCN.MPGCN, run through its own forward with the LSTM and the layers on this rank's shard.
+    x_slab [B,T,rows,N,1] (shard_host_inputs).  G_static [K,N,N] (whole, on every rank);
     G_dyn = (G_o [B,K,N,N], G_d) with G_d whole (row shard) or the rank's slice [B,Kd,N,N] (K shard).
     -> row shard: y of the rank's rows [B,1,rows,N,1];  K shard: the whole y [B,1,N,N,1] on every rank."""
     assert len(model.branch_models) == 2 == model.M, "the trainer's M = 2 layout: static branch, dynamic branch"
-    B, T, rows, N, _ = x_slab.shape
-    C = model.lstm_hidden_dim
-    if plan.kind == "k":
-        G_list = [(G_static, G_static[plan.d_lo:plan.d_hi]), G_dyn]       # static supports: origin side whole, destination side sliced
-    else:
-        G_list = [G_static, G_dyn]
+
+    def temporal(lstm, x):
+        B, _, rows, N, _ = x.shape
+        h = _ENGINE.lstm_last(x, lstm, model.lstm_precision).reshape(B, rows, N, model.lstm_hidden_dim)
+        return h if plan.kind == "row" else _AllGatherRowsFn.apply(h, plan)
+
     # The branches are independent until the head: each runs on its own CUDA stream, so that the exchange steps of one branch
     # (NVLink-bound kernels that leave the SMs mostly idle) overlap the contractions of the other.  autograd replays every
-    # backward node on the stream of its forward, so the backward overlaps the same way.
-    use_streams = x_slab.is_cuda
-    cur = torch.cuda.current_stream() if use_streams else None
-    if use_streams and plan.streams is None:
-        plan.streams = [torch.cuda.Stream(device=x_slab.device) for _ in range(model.M)]
-    feats = []
-    for m in range(model.M):
-        branch = model.branch_models[m]
-        plan.branch = m
-        if use_streams:
-            plan.streams[m].wait_stream(cur)
-        with (torch.cuda.stream(plan.streams[m]) if use_streams else _nullcontext()):
-            h = _ENGINE.lstm_last(x_slab, branch['temporal'], model.lstm_precision).reshape(B, rows, N, C)
-            g = h if plan.kind == "row" else _AllGatherRowsFn.apply(h, plan)
-            Gm = G_list[m]
-            for layer in branch['spatial']:
-                if plan.kind == "k" and isinstance(Gm, tuple) and Gm[0].dim() == 3:
-                    g = _static_k_layer(layer, g, Gm, plan)
-                else:
-                    g = sharded_bdgcn(layer, g, Gm, plan)
-        feats.append(g)
-    if use_streams:
-        for m in range(model.M):
-            cur.wait_stream(plan.streams[m])
-            feats[m].record_stream(cur)
-    # the head is row-local: the same decision (fused kernel or each branch's own modules) as the whole model's
-    return fc_head([model.branch_models[m]['fc'] for m in range(model.M)], feats, fused=_ENGINE.head).unsqueeze(dim=1)
-
-
-def _static_k_layer(layer, X, G_pair, plan):
-    """K shard with STATIC supports: G_o = the whole [K,N,N] stack, G_d = the rank's [Kd,N,N] slice of the same stack."""
-    from torch import nn
-    relu = isinstance(layer.activation, nn.ReLU)
-    return _KShardLayerFn.apply(X, G_pair[0], G_pair[1], layer.W, layer.b if layer.use_bias else None, False, 1 if relu else 0, layer.precision,
-                                plan, torch.is_grad_enabled())
+    # backward node on the stream of its forward, so the backward overlaps the same way.  The head is row-local.
+    run = BranchRunner(temporal, lambda layer, X, G, m: sharded_bdgcn(layer, X, G, plan, m), _ENGINE.head, streams=True)
+    return model._forward(x_slab, [G_static, G_dyn], plan.rows, run)
 
 
 def sharded_mse_loss(plan: ShardPlan, y_pred, y_true):

@@ -1,5 +1,6 @@
 """Worker of tests/test_shard_gloo.py: one rank of a world-2 gloo run of the sharded model (CPU stand-in engine).
-Arguments: kind, output path[, lstm_hidden_dim, gcn_hidden_dim] (both 8 by default)."""
+Arguments: kind, output path[, lstm_hidden_dim, gcn_hidden_dim] (both 8 by default); kind "k-layer": one K-shard layer on a
+static support stack instead of the model."""
 import os
 import sys
 
@@ -59,5 +60,30 @@ def main(kind, out_path, lstm_hid=8, gcn_hid=8):
     dist.destroy_process_group()
 
 
+def k_layer(out_path):
+    """shard.sharded_bdgcn on a K shard with a static [K,N,N] stack (C != H), its parameter gradients summed over the ranks"""
+    rank, world = mdist.init_from_env("gloo")
+    shard._ENGINE = TorchEngine()
+    B, N, K, C, H = 2, 8, 3, 4, 6
+    torch.manual_seed(0)
+    layer = shim.BDGCN(K=K, input_dim=C, hidden_dim=H, use_bias=True, activation=nn.ReLU)
+    with torch.no_grad():
+        layer.b.add_(0.05)
+    rng = np.random.default_rng(2)
+    X = torch.from_numpy(rng.random((B, N, N, C)).astype(np.float32)).requires_grad_(True)
+    G = torch.from_numpy((rng.random((K, N, N)) / N).astype(np.float32))
+    d_out = torch.from_numpy(rng.standard_normal((B, N, N, H)).astype(np.float32))
+    plan = shard.ShardPlan("k", rank, world, N, K)
+    out = shard.sharded_bdgcn(layer, X, G, plan)
+    (out * d_out).sum().backward()
+    shard.allreduce_sum_gradients([layer.W, layer.b], plan)
+    torch.save({"X": X.detach(), "G": G, "W": layer.W.detach(), "b": layer.b.detach(), "d_out": d_out, "out": out.detach(),
+                "dX": X.grad, "dW": layer.W.grad, "db": layer.b.grad}, out_path)
+    dist.destroy_process_group()
+
+
 if __name__ == "__main__":
-    main(sys.argv[1], sys.argv[2], *(int(a) for a in sys.argv[3:5]))
+    if sys.argv[1] == "k-layer":
+        k_layer(sys.argv[2])
+    else:
+        main(sys.argv[1], sys.argv[2], *(int(a) for a in sys.argv[3:5]))

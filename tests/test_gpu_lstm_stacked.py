@@ -12,17 +12,12 @@ Hidden 128 and every other configuration keep nn.LSTM, in the model and in the s
 
 Bounds are those of the single-layer path: h_T 1e-3, gradients 2e-3.
 """
-import json
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 from torch import nn
 
+import _shard_nccl_worker as nccl_worker
 from conftest import golden_names, load_golden, record_parity
 from oracle import lstm_tc_oracle as emu
 from oracle import mpgcn_oracle as orc
@@ -33,7 +28,6 @@ from mpgcn_b200 import _lib, ops
 from tools.gen_golden_stacked_lstm import KEYS, stacked_lstm_params
 from tools.gen_golden_wide import params_checksum, wide_model_params
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 FIXTURE_TOL = 2e-5
 H_TOL, G_TOL = 1e-3, 2e-3
 FP16_MODEL_FWD_TOL = 3.5e-3     # whole model in fp16 against the reference (test_gpu_lstm_widths.py, DESIGN.md section 3)
@@ -415,19 +409,15 @@ def test_sharded_model_with_stacked_lstm_matches_the_whole_model(world, tmp_path
     test_gpu_shard.py; the sharded model runs the model's own dispatch, so hidden 64 at T = 16 falls back to nn.LSTM there too."""
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        port = s.getsockname()[1]
-    out = tmp_path / "res.json"
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr",
-                        "127.0.0.1", "--master-port", str(port), os.path.join(HERE, "_shard_nccl_worker_stacked.py"), str(out)],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    rows = json.load(open(out))["rows"]
+    # (hidden, T, LSTM precision, forward / gradient bars): the tensor-core stacks at 32 and 96, and hidden 64 at T = 16, which the
+    # model runs on nn.LSTM (the fp32 kernels' backward does not hold 16 steps at 64); the layers on the fp32 engine
+    models = [dict(N=40, T=T, hidden=hid, gcn_hidden=32, lstm_layers=2, seed=hid, yardstick="same", cases=[(prec, "fp32", tol_f, tol_g)])
+              for hid, T, prec, tol_f, tol_g in ((32, 5, "fp16", 1e-3, 8e-2), (96, 4, "fp16", 1e-3, 8e-2), (64, 16, "auto", 1e-5, 2e-3))]
+    rows = nccl_worker.run(world, tmp_path, models)["rows"]
     assert {row["hid"] for row in rows} == {32, 96, 64}
     for row in rows:
         record_parity(row["what"], row["linf"], row["l2"], row["tol"])
-        assert row["linf"] <= row["tol"] and row["l2"] <= row["tol"], row
+        assert row["err"] <= row["tol"], row
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

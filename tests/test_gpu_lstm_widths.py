@@ -11,17 +11,12 @@ tensor-core pass reduces to the weight gradients).  Hidden 64 stays on the fp32 
 
 Bounds are those of the hidden-32 path (test_gpu_parity.py): h_T 1e-3, gradients 2e-3.
 """
-import json
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 from torch import nn
 
+import _shard_nccl_worker as nccl_worker
 from conftest import golden_names, load_golden, record_parity
 from oracle import mpgcn_oracle as orc
 
@@ -30,7 +25,6 @@ from mpgcn_b200 import _lib, ops
 from tools.gen_golden_wide import params_checksum, wide_model_params
 from tools.gen_golden_wide_lstm import lstm_params
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 FIXTURE_TOL = 2e-5
 H_TOL, G_TOL = 1e-3, 2e-3
 # whole model in fp16 at hidden 128 against the reference, forward rel_L2: the fp16 BDGCN layers at C = H = 128 reach 2.18e-3 on
@@ -430,16 +424,11 @@ def test_row_sharded_model_at_wide_hidden(hid, world, tmp_path):
     World 1 runs the whole sharded path (plan, slabs, collectives, gradient reduction) on one GPU; world 2 needs two."""
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        port = s.getsockname()[1]
-    out = tmp_path / "res.json"
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr",
-                        "127.0.0.1", "--master-port", str(port), os.path.join(HERE, "_shard_nccl_worker_wide.py"), str(hid), str(out)],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.load(open(out))
+    # the LSTM on the tensor-core kernel at both layer precisions; the whole model at the same precisions is the yardstick:
+    # fp32 layers -> summation order only; fp16 layers -> the fp16 row partials against the fp16 whole layer
+    res = nccl_worker.run(world, tmp_path, [dict(N=66, hidden=hid, dynamic="diffusion", yardstick="same",
+                                                 cases=[("fp16", "fp32", 1e-5, 2e-3), ("fp16", "fp16", 1e-3, 8e-2)])])
     assert len(res["rows"]) == 2 * world * (1 + len(_model(5, 3, hid, 0, "cpu").state_dict()))
     for row in res["rows"]:
         record_parity(row["what"], row["linf"], row["l2"], row["tol"])
-        assert row["linf"] <= row["tol"] and row["l2"] <= row["tol"], row
+        assert row["err"] <= row["tol"], row

@@ -43,8 +43,8 @@ def test_sharded_model_with_lstm_hidden_unlike_gcn_hidden_matches_whole_model_or
     _run_and_check(kind, tmp_path, 8, 12)
 
 
-def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
-    nproc = 4 if kind == "rowhyb" else 2
+def _run_workers(nproc, tmp_path, kind, *args):
+    """tests/_shard_worker.py on `nproc` gloo ranks -> what each rank saved"""
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         port = s.getsockname()[1]
@@ -52,10 +52,15 @@ def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
     procs = []
     for r in range(nproc):
         env = dict(os.environ, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(r), WORLD_SIZE=str(nproc))
-        procs.append(subprocess.Popen([sys.executable, worker, kind, str(tmp_path / f"r{r}.pt"), str(lstm_hid), str(gcn_hid)], env=env))
+        procs.append(subprocess.Popen([sys.executable, worker, kind, str(tmp_path / f"r{r}.pt"), *map(str, args)], env=env))
     for p in procs:
         assert p.wait(timeout=300) == 0
-    res = [torch.load(tmp_path / f"r{r}.pt") for r in range(nproc)]
+    return [torch.load(tmp_path / f"r{r}.pt") for r in range(nproc)]
+
+
+def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
+    nproc = 4 if kind == "rowhyb" else 2
+    res = _run_workers(nproc, tmp_path, kind, lstm_hid, gcn_hid)
     # the same model / inputs as the worker builds, evaluated whole by the oracle
     sys.path.insert(0, os.path.dirname(HERE))
     import MPGCN as shim
@@ -93,6 +98,21 @@ def _run_and_check(kind, tmp_path, lstm_hid, gcn_hid):
         assert set(r["grads"]) == set(grads_o)
         for k, g in r["grads"].items():
             assert max(orc.rel_errors(g.numpy(), grads_o[k])) <= 2e-5, (kind, k)
+
+
+def test_k_sharded_layer_on_a_static_stack_world2_matches_the_whole_layer(tmp_path):
+    """sharded_bdgcn on a K shard over 2 ranks with a static [K,N,N] stack: each rank contracts the destination side over its own
+    supports only.  The replicated output, dX and the rank-summed W / b gradients against a float64 evaluation of the whole layer."""
+    res = _run_workers(2, tmp_path, "k-layer")
+    r = res[0]
+    f64 = lambda t: t.numpy().astype(np.float64)  # noqa: E731
+    X, G, W, b, d_out = (f64(r[k]) for k in ("X", "G", "W", "b", "d_out"))
+    out_o = orc.bdgcn_forward(X, G, W, b, "relu")
+    dX_o, dW_o, db_o = orc.bdgcn_backward(X, G, W, b, "relu", d_out)
+    for r in res:
+        assert max(orc.rel_errors(r["out"].numpy(), out_o)) <= 1e-5
+        for k, want in (("dX", dX_o), ("dW", dW_o), ("db", db_o)):
+            assert max(orc.rel_errors(r[k].numpy(), want)) <= 2e-5, k
 
 
 @pytest.fixture
@@ -207,3 +227,27 @@ def test_sharded_model_with_two_input_features_matches_whole_model_oracle(kind, 
     assert set(named) == set(grads_o)
     for k, p in named.items():
         assert max(orc.rel_errors(p.grad.numpy(), grads_o[k])) <= 2e-5, (kind, k)
+
+
+@pytest.mark.parametrize("kind", ["row", "k"])
+def test_sharded_model_refuses_what_the_whole_model_refuses(kind, world1):
+    """Inputs whose node count is not the model's num_nodes, and a model whose branch count does not match the supports given
+    (the sharded model always passes the trainer's two): the sharded model raises the whole model's AssertionError."""
+    import MPGCN as shim
+    shard = world1
+    B, T, N, K, hid = 2, 3, 6, 3, 4
+
+    def model(M, num_nodes):
+        return shim.MPGCN(M=M, K=K, input_dim=1, lstm_hidden_dim=hid, lstm_num_layers=1, gcn_hidden_dim=hid, gcn_num_layers=2,
+                          num_nodes=num_nodes, user_bias=True, activation=nn.ReLU)
+
+    x, y = torch.rand(B, T, N, N, 1), torch.rand(B, 1, N, N, 1)
+    G = torch.rand(K, N, N) / N
+    go, gd = torch.rand(B, K, N, N) / N, torch.rand(B, K, N, N) / N
+    plan = shard.ShardPlan(kind, 0, 1, N, K)
+    xs, _, gos, gds = shard.shard_host_inputs(plan, x, y, go, gd)
+    for wrong in (model(2, N + 1), model(3, N)):
+        with pytest.raises(AssertionError):
+            wrong(x_seq=x, G_list=[G, (go, gd)])
+        with pytest.raises(AssertionError):
+            shard.sharded_forward(wrong, plan, xs, G, (gos, gds))
