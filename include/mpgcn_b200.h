@@ -46,6 +46,18 @@ extern "C" {
 MPGCN_API int mpgcn_abi_version(void);
 MPGCN_API const char* mpgcn_last_error(void);
 
+/* Deterministic mode of the CALLING HOST THREAD (thread-local, off by default; DESIGN.md section 11).  With it on, every sum that
+ * the default kernels form across CTAs with floating-point atomics -- the LSTM weight and bias gradients, the BDGCN bias gradient,
+ * the fp32 BDGCN dW, the head's dw / db, the column norms of mpgcn_dyn_graph_build -- is formed from per-CTA partials ("slots") in
+ * the workspace, added by one kernel in a fixed order.  Results are then bitwise reproducible for a given shape on a given GPU model
+ * and SM count (the promise cuBLAS makes), whatever runs concurrently.  The workspace queries of the affected calls read the same
+ * mode (they grow by the slots; with the mode off they return what they always did), and every call checks before its first CUDA
+ * call that its workspace is large enough for the current mode.  mpgcn_head_backward has no workspace: with the mode on it refuses,
+ * and mpgcn_head_backward_ex takes one.  mpgcn_relu_backward and mpgcn_relu_backward_scatter[_f16] have no deterministic
+ * implementation: with the mode on they return an error.  set returns the previous value. */
+MPGCN_API int mpgcn_set_deterministic(int on);
+MPGCN_API int mpgcn_get_deterministic(void);
+
 /* 1 if `precision` can serve this layer shape, else 0 (replaces nothing in the reference; the
  * Python binding uses it to pick the kernel family). */
 MPGCN_API int mpgcn_bdgcn_precision_supported(int B, int N, int K, int C, int H, int precision);
@@ -288,6 +300,12 @@ MPGCN_API int mpgcn_head_forward(const float* const* g, const float* w, const fl
                        void* stream);
 MPGCN_API int mpgcn_head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
                         float* dg_absmax, long long cells, int C, int M, void* stream);
+/* The backward with a workspace (256-byte aligned) of mpgcn_head_backward_workspace_bytes: 0 with the deterministic mode off
+ * (then identical to mpgcn_head_backward), else one [M*C + M] float slot per block of the kernel's grid. */
+MPGCN_API size_t mpgcn_head_backward_workspace_bytes(long long cells, int C, int M);
+MPGCN_API int mpgcn_head_backward_ex(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw,
+                                     float* db, float* dg_absmax, long long cells, int C, int M, void* workspace, size_t workspace_bytes,
+                                     void* stream);
 
 /* Launch accounting (bench.py evidence).  Every launch of a kernel of this library is counted per tag
  * (0 FWD_A, 1 FWD_MIX, 2 FWD_B, 3 BWD_V, 4 BWD_DW, 5 BWD_MIX, 6 BWD_DX: wgmma contractions; 7 fp32 SIMT GEMM;

@@ -47,6 +47,7 @@ def _adj_process(f: torch.Tensor, kt: int, K: int) -> torch.Tensor:
 class _AdjProcessFn(torch.autograd.Function):
     """supports = process(flow); the backward reads the saved flow and supports (the T_{k-1} of the recursion's adjoint)."""
     @staticmethod
+    @_lib.engine_buffers()
     def forward(ctx, f, kt: int, K: int, grad_mode: bool):
         out = _adj_process(_f32c(f), kt, K)
         if grad_mode and ctx.needs_input_grad[0]:
@@ -56,9 +57,11 @@ class _AdjProcessFn(torch.autograd.Function):
 
     @staticmethod
     @once_differentiable
+    @_lib.engine_buffers()
     def backward(ctx, d_out):
         f, out = ctx.saved_tensors
         lib = _lib.load()
+        _lib.sync_deterministic()        # already fixed-order; set like every backward so the thread's mode is never stale
         B, N = f.shape[0], f.shape[1]
         g = _f32c(d_out)
         d_flow = torch.empty_like(f)

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes
 import os
 import subprocess
+import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmpgcn_b200.so")
@@ -97,6 +98,11 @@ _SIGS = {
     "mpgcn_adj_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 4),
     "mpgcn_adj_process_backward": (ctypes.c_int, [_c_f, _c_f, _c_f, _c_f, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_f,
                                                   ctypes.c_size_t, ctypes.c_void_p]),
+    "mpgcn_set_deterministic": (ctypes.c_int, [ctypes.c_int]),
+    "mpgcn_get_deterministic": (ctypes.c_int, []),
+    "mpgcn_head_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong, ctypes.c_int, ctypes.c_int]),
+    "mpgcn_head_backward_ex": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), _c_f, _c_f, _c_f, ctypes.POINTER(ctypes.c_void_p), _c_f, _c_f,
+                                              _c_f, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, _c_f, ctypes.c_size_t, ctypes.c_void_p]),
 }
 ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)
@@ -142,6 +148,59 @@ def load() -> ctypes.CDLL:
         raise RuntimeError("mpgcn_b200: ABI version mismatch between the Python binding and libmpgcn_b200.so")
     _lib = lib
     return lib
+
+
+# The library's deterministic mode is per host thread (mpgcn_set_deterministic); this is the value last set on each thread, so that a
+# thread whose mode already matches makes no call.  A thread starts at 0 in both.
+_DET = threading.local()
+
+
+def set_deterministic(on: bool) -> bool:
+    """Set the calling thread's library mode to `on` (one ctypes call only when it changes); -> `on`."""
+    on = bool(on)
+    if getattr(_DET, "on", False) != on:
+        load().mpgcn_set_deterministic(int(on))
+        _DET.on = on
+    return on
+
+
+def sync_deterministic() -> bool:
+    """Give the calling thread's library mode the value of torch.are_deterministic_algorithms_enabled(); -> that value.
+    Every autograd Function calls it in forward AND in backward: autograd runs CUDA backward on its own device thread, where a mode
+    set during forward does not hold."""
+    import torch
+    return set_deterministic(torch.are_deterministic_algorithms_enabled())
+
+
+class engine_buffers:
+    """Context (and decorator) for the engine's own allocations: under torch.use_deterministic_algorithms(True) torch fills every
+    torch.empty tensor with NaN (torch.utils.deterministic.fill_uninitialized_memory).  The engine's workspaces, stashes and outputs
+    are written in full by its kernels before anything reads them (the stage tests prefill them with NaN and check), so that fill
+    is pure memory traffic -- gigabytes per step at N = 1000.  Inside this context it is skipped.  The setting is process-wide:
+    another thread allocating meanwhile may skip its fill too, which changes no result."""
+
+    def __enter__(self):
+        import torch
+        import torch.utils.deterministic as det
+        self._prev = torch.are_deterministic_algorithms_enabled() and det.fill_uninitialized_memory
+        if self._prev:
+            det.fill_uninitialized_memory = False
+        return self
+
+    def __exit__(self, *exc):
+        if self._prev:
+            import torch.utils.deterministic as det
+            det.fill_uninitialized_memory = True
+        return False
+
+    def __call__(self, fn):
+        import functools
+
+        @functools.wraps(fn)
+        def wrapped(*args, **kwargs):
+            with engine_buffers():
+                return fn(*args, **kwargs)
+        return wrapped
 
 
 def check(code: int, what: str) -> None:

@@ -59,6 +59,9 @@ extern "C" {
 int mpgcn_abi_version(void) { return MPGCN_B200_ABI_VERSION; }
 const char* mpgcn_last_error(void) { return last_error(); }
 
+int mpgcn_set_deterministic(int on) { return det_set(on); }
+int mpgcn_get_deterministic(void) { return det_mode(); }
+
 int mpgcn_bdgcn_precision_supported(int B, int N, int K, int C, int H, int precision) {
   const BdgcnShape s = mk(B, N, K, C, H, 0, 0);
   if (precision == PREC_FP32_SIMT) return B >= 1 && N >= 1 && K >= 1 && C >= 1 && H >= 1;
@@ -240,12 +243,14 @@ int mpgcn_rows_reduce_bias_act(float* out, const float* const* partials, int g, 
 
 int mpgcn_relu_backward_scatter(const float* d_out, const float* out, int act, float* const* dsts, int g, float* db, int B, int N, int row0,
                                 int rows, int H, void* stream) {
+  MPGCN_CHECK(!det_mode(), "mpgcn_relu_backward_scatter: no deterministic implementation (the mode of mpgcn_set_deterministic is on)");
   MPGCN_CHECK(d_out && dsts && B >= 1 && (act == 0 || (act == 1 && out)), "mpgcn_relu_backward_scatter: bad argument");
   return relu_backward_scatter(d_out, out, act, dsts, g, db, B, N, row0, rows, H, static_cast<cudaStream_t>(stream));
 }
 
 int mpgcn_relu_backward_scatter_f16(const float* d_out, const float* out, int act, void* const* dsts, int g, float* db, const float* absmax,
                                     float* scale2, int B, int N, int row0, int rows, int H, void* stream) {
+  MPGCN_CHECK(!det_mode(), "mpgcn_relu_backward_scatter_f16: no deterministic implementation (the mode of mpgcn_set_deterministic is on)");
   MPGCN_CHECK(d_out && dsts && B >= 1 && (act == 0 || (act == 1 && out)), "mpgcn_relu_backward_scatter_f16: bad argument");
   return relu_backward_scatter_f16(d_out, out, act, reinterpret_cast<__half* const*>(dsts), g, db, absmax, scale2, B, N, row0, rows, H,
                                    static_cast<cudaStream_t>(stream));
@@ -257,6 +262,7 @@ int mpgcn_absmax(const float* x, long long n, float* out, void* stream) {
 }
 
 int mpgcn_relu_backward(const float* d_out, const float* out, int act, float* d_pre, float* db, long long n, int H, void* stream) {
+  MPGCN_CHECK(!det_mode(), "mpgcn_relu_backward: no deterministic implementation (the mode of mpgcn_set_deterministic is on)");
   MPGCN_CHECK(d_out && d_pre && n >= 1 && (act == 0 || (act == 1 && out)), "mpgcn_relu_backward: bad argument");
   return relu_bwd_prep(d_out, out, act, nullptr, d_pre, db, (size_t)n, H, nullptr, static_cast<cudaStream_t>(stream));
 }
@@ -289,10 +295,24 @@ int mpgcn_head_forward(const float* const* g, const float* w, const float* bias,
 
 int mpgcn_head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
                         float* dg_absmax, long long cells, int C, int M, void* stream) {
+  MPGCN_CHECK(!det_mode(), "mpgcn_head_backward: the deterministic mode needs a workspace: call mpgcn_head_backward_ex");
+  return mpgcn_head_backward_ex(g, w, pre, dy, dg, dw, db, dg_absmax, cells, C, M, nullptr, 0, stream);
+}
+
+size_t mpgcn_head_backward_workspace_bytes(long long cells, int C, int M) {
+  return det_mode() && cells >= 1 && C >= 1 && M >= 1 ? head_bwd_slot_bytes(cells, C, M) : 0;
+}
+
+int mpgcn_head_backward_ex(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
+                           float* dg_absmax, long long cells, int C, int M, void* workspace, size_t workspace_bytes, void* stream) {
   MPGCN_CHECK(g && w && pre && dy && dw && db && cells >= 1, "mpgcn_head_backward: null pointer or empty input");
   if (head_check("mpgcn_head_backward", g, w, dg, C, M)) return 1;
+  const size_t need = mpgcn_head_backward_workspace_bytes(cells, C, M);
+  MPGCN_CHECK(workspace_bytes >= need && (need == 0 || workspace != nullptr), "mpgcn_head_backward: workspace too small for the %s mode (%zu < %zu bytes)",
+              det_mode() ? "deterministic" : "default", workspace_bytes, need);
   ProfRegion region(PROF_HEAD, 4.0 * cells * C * M, static_cast<cudaStream_t>(stream));
-  return head_backward(g, w, pre, dy, dg, dw, db, dg_absmax, cells, C, M, static_cast<cudaStream_t>(stream));
+  return head_backward(g, w, pre, dy, dg, dw, db, dg_absmax, cells, C, M, static_cast<cudaStream_t>(stream),
+                       det_mode() ? static_cast<float*>(workspace) : nullptr);
 }
 
 void mpgcn_profile_enable(int on) { prof_enable(on); }
@@ -324,8 +344,10 @@ int mpgcn_lstm_precision_supported(int T, int C, int precision) {
 // sizes for the width of the tensor-core kernel; a width it does not run keeps the hidden-32 size these always returned
 static int lstm_tc_size_width(int C) { return lstm_tc_supported(1, C) ? C : 32; }
 
+// precision 0: 256 bytes, plus its slots in deterministic mode (a hidden size it does not run keeps the 256)
 size_t mpgcn_lstm_bwd_workspace_bytes(int B, int T, long long NN, int C, int precision) {
-  return precision == PREC_FP16_TC ? lstm_tc_bwd_workspace_bytes(B, T, NN, lstm_tc_size_width(C)) : 256;
+  if (precision == PREC_FP16_TC) return lstm_tc_bwd_workspace_bytes(B, T, NN, lstm_tc_size_width(C));
+  return 256 + (det_mode() && C >= 1 && C <= 64 ? lstm_bwd_slot_bytes(C) : 0);
 }
 
 size_t mpgcn_lstm_saved_bytes(int B, int T, long long NN, int C, int precision) {
@@ -386,7 +408,13 @@ int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const 
     return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, C, workspace,
                                  workspace_bytes, d_hT_absmax, st);
   }
-  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st);
+  if (!det_mode()) return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st);
+  const size_t need = mpgcn_lstm_bwd_workspace_bytes(B, T, NN, C, precision);
+  MPGCN_CHECK(workspace != nullptr && workspace_bytes >= need, "lstm backward: workspace too small for the deterministic mode (%zu < %zu)",
+              workspace_bytes, need);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
+  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st,
+                            reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + 256));
 }
 
 int mpgcn_lstm_stack_supported(int T, int C, int L, int precision) {

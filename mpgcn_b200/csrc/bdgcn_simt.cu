@@ -40,10 +40,23 @@ size_t simt_saved_bytes(const BdgcnShape& s) { return (size_t)s.B * s.Kd * rn(s)
 size_t simt_fwd_ws_bytes(const BdgcnShape& s) {
   return 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256) + align_up(simt_saved_bytes(s), 256);
 }
-size_t simt_bwd_ws_bytes(const BdgcnShape& s) {
+static size_t simt_bwd_base_bytes(const BdgcnShape& s) {
   return 1024 + align_up((size_t)s.B * s.N * s.N * s.H * 4, 256) + align_up((size_t)s.B * s.Ko * rn(s) * s.H * 4, 256) +
          align_up((size_t)s.B * s.Kd * rn(s) * s.C * 4, 256) + align_up((size_t)s.Ko * s.Kd * s.C * s.H * 4, 256);
 }
+// dW = sum over R*N rows: split-K into up to 256 slices of >= 2048 rows
+static int dw_ksplit(const BdgcnShape& s) {
+  long long ks = (long long)rn(s) / 2048;
+  return (int)(ks < 1 ? 1 : ks > 256 ? 256 : ks);
+}
+static int dw_mt(const BdgcnShape& s) { return (s.Kd * s.C + 127) / 128; }
+// Deterministic mode appends, after the mode-off workspace, the bias-gradient slots and (ksplit > 1) the dW slices in the layout of
+// reduce_dw_partials: [slice][MT * 128 rows d*C + c][Ko*H columns o*H + h], MT = ceil(Kd*C / 128).
+static size_t simt_det_bytes(const BdgcnShape& s) {
+  const int ks = dw_ksplit(s);
+  return bias_grad_slot_bytes(s.H) + (ks > 1 ? align_up((size_t)ks * dw_mt(s) * 128 * s.Ko * s.H * 4, 256) : 0);
+}
+size_t simt_bwd_ws_bytes(const BdgcnShape& s) { return simt_bwd_base_bytes(s) + (det_mode() ? simt_det_bytes(s) : 0); }
 
 static void zero3(long long (&a)[3]) { a[0] = a[1] = a[2] = 0; }
 
@@ -100,13 +113,15 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
   return 0;
 }
 
-size_t simt_sgrad_ws_bytes(const BdgcnShape& s) {
-  return simt_bwd_ws_bytes(s) + 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256);
+static size_t simt_sgrad_base_bytes(const BdgcnShape& s) {
+  return simt_bwd_base_bytes(s) + 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256);
 }
+size_t simt_sgrad_ws_bytes(const BdgcnShape& s) { return simt_sgrad_base_bytes(s) + (det_mode() ? simt_det_bytes(s) : 0); }
 
-// form_y: form Y even without dX (the support gradient reads it)
+// form_y: form Y even without dX (the support gradient reads it); det: the deterministic-mode region (simt_det_bytes) or null
 static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                              const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, bool form_y, cudaStream_t st) {
+                              const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, bool form_y, uint8_t* det,
+                              cudaStream_t st) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   MPGCN_CHECK(Z != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
@@ -120,7 +135,9 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
 
   const float* dP = d_out;         // a partial call receives dPre itself (every origin row m, already masked)
   if (!s.partial) {
-    if (int e = relu_bwd_prep(d_out, out, s.act, nullptr, dPre, db, (size_t)s.B * NN * H, (int)H, nullptr, st)) return e;
+    if (int e = relu_bwd_prep(d_out, out, s.act, nullptr, dPre, db, (size_t)s.B * NN * H, (int)H, nullptr, st,
+                              det ? reinterpret_cast<float*>(det) : nullptr))
+      return e;
     dP = dPre;
   }
 
@@ -138,7 +155,9 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
     if (int e = simt_sgemm(p, st)) return e;
   }
   {  // dW[o,d] (l x h) = sum_b Z[b,d]^T (l x rows) * V[b,o] (rows x h)
-    MPGCN_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * Ko * Kd * C * H, st));
+    const int ks = dw_ksplit(s);
+    const bool slices = det && ks > 1;      // deterministic: every slice stores its partial, reduce_dw_partials adds them in order
+    if (!slices) MPGCN_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * Ko * Kd * C * H, st));
     SgemmParams p{};
     p.A = Z; p.B = V; p.D = dW;
     p.M = (int)C; p.N = (int)H; p.K = (int)RN;
@@ -149,11 +168,15 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
     p.a_sz[1] = RN * C;
     p.b_sz[0] = RN * H;
     p.d_sz[0] = Kd * C * H; p.d_sz[1] = C * H;
-    long long ks = RN / 2048;
-    if (ks < 1) ks = 1;
-    if (ks > 256) ks = 256;
-    p.ksplit = (int)ks; p.alpha = 1.f;
+    p.ksplit = ks; p.alpha = 1.f;
+    float* P = slices ? reinterpret_cast<float*>(det + bias_grad_slot_bytes((int)H)) : nullptr;
+    if (slices) {
+      p.D = P; p.d_si = Ko * H; p.d_sz[0] = H; p.d_sz[1] = C * Ko * H;
+      p.d_sslice = (long long)dw_mt(s) * 128 * Ko * H;
+    }
     if (int e = simt_sgemm(p, st)) return e;
+    if (slices)
+      if (int e = reduce_dw_partials(P, dW, ks, dw_mt(s), (int)Ko, (int)Kd, (int)C, (int)H, nullptr, st)) return e;
   }
   if (dX || form_y) {
     if (int e = permute_w_bwd(W, Wq, (int)Ko, (int)Kd, (int)C, (int)H, st)) return e;
@@ -195,7 +218,10 @@ namespace mpgcn {
 
 int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                         const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st) {
-  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, false, st);
+  MPGCN_CHECK(!det_mode() || ws_bytes >= simt_bwd_ws_bytes(s), "bdgcn_backward: workspace too small for the deterministic mode (%zu < %zu bytes)",
+              ws_bytes, simt_bwd_ws_bytes(s));
+  uint8_t* det = det_mode() ? static_cast<uint8_t*>(ws) + simt_bwd_base_bytes(s) : nullptr;
+  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, false, det, st);
 }
 
 int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
@@ -205,7 +231,8 @@ int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const 
   MPGCN_CHECK(ws_bytes >= simt_sgrad_ws_bytes(s), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes,
               simt_sgrad_ws_bytes(s));
   const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
-  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, want_d, st)) return e;
+  uint8_t* det = det_mode() ? static_cast<uint8_t*>(ws) + simt_sgrad_base_bytes(s) : nullptr;
+  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, want_d, det, st)) return e;
   const long long N = s.N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   Carver cv(ws, ws_bytes);                          // the backward's regions, then U

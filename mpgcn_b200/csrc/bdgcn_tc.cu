@@ -174,7 +174,9 @@ static BwdLayout bwd_layout(const BdgcnShape& s) {
   L.total = align_up(off, 1024);
   return L;
 }
-size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s).total; }
+// deterministic mode appends the bias-gradient slots (relu_bwd_prep) to the mode-off workspace; dW and dG already reduce their
+// split-K partials in a fixed order
+size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s).total + (det_mode() ? bias_grad_slot_bytes(s.H) : 0); }
 
 // support-gradient workspace: the backward's, then X16, U16, the forward's fp16 W split and the dG partials
 struct SgradLayout { size_t x16, u16, w16, partials, total; };
@@ -195,7 +197,7 @@ static SgradLayout sgrad_layout(const BdgcnShape& s) {
   L.total = align_up(off, 1024);
   return L;
 }
-size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return sgrad_layout(s).total; }
+size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return sgrad_layout(s).total + (det_mode() ? bias_grad_slot_bytes(s.H) : 0); }
 
 // which: 0 x16, 1 gd16, 2 go16, 3 w16, 4 u16 (forward); 10 dp16, 11 gd16, 12 go16, 13 v16, 14 y16, 15 wq16, 16 partials,
 // 17 number of dW slices (not an offset)
@@ -511,10 +513,10 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
   return 0;
 }
 
-// form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it)
+// form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it); db_slots: deterministic mode's bias-gradient slots
 static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                             const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
-                            bool form_y, cudaStream_t st) {
+                            bool form_y, float* db_slots, cudaStream_t st) {
   MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
               s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
@@ -547,9 +549,11 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
     float* scale2_ws = reinterpret_cast<float*>(wb + L.scale);
     if (int e = grad_scale_prepare(d_out, (size_t)s.B * NNfull * s.H, scale2_ws, ex.d_out_absmax, st)) return e;
     if (ex.out_f16 != nullptr && act) {
-      if (int e = relu_bwd_prep_f16mask(d_out, static_cast<const __half*>(ex.out_f16), act, dp16_ws, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st)) return e;
+      if (int e = relu_bwd_prep_f16mask(d_out, static_cast<const __half*>(ex.out_f16), act, dp16_ws, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st,
+                                        db_slots))
+        return e;
     } else {
-      if (int e = relu_bwd_prep(d_out, out, act, dp16_ws, nullptr, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st)) return e;
+      if (int e = relu_bwd_prep(d_out, out, act, dp16_ws, nullptr, db, (size_t)s.B * NNfull * s.H, s.H, scale2_ws, st, db_slots)) return e;
     }
   }
   SideG gd{}, go{};
@@ -575,7 +579,11 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
                       cudaStream_t st) {
-  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, false, st);
+  const size_t base = bwd_layout(s).total;
+  MPGCN_CHECK(!det_mode() || ws_bytes >= tc_bwd_ws_bytes(s), "bdgcn_backward: workspace too small for the deterministic mode (%zu < %zu bytes)",
+              ws_bytes, tc_bwd_ws_bytes(s));
+  float* db_slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + base) : nullptr;
+  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, false, db_slots, st);
 }
 
 // One support-gradient contraction into the partials [slice][N][ldp] (ldp = 32 ceil(N/32): a 32-column chunk never runs into
@@ -665,7 +673,9 @@ int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const fl
   MPGCN_CHECK(ws_bytes >= S.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, S.total);
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(X) & 15) == 0, "bdgcn_backward_supports: X must be 16-byte aligned");
   const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
-  if (int e = backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, want_d, st)) return e;
+  MPGCN_CHECK(ws_bytes >= tc_sgrad_ws_bytes(s), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, tc_sgrad_ws_bytes(s));
+  float* db_slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + S.total) : nullptr;
+  if (int e = backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, want_d, db_slots, st)) return e;
   const BwdLayout L = bwd_layout(s);
   uint8_t* wb = static_cast<uint8_t*>(ws);
   const __half* z16 = static_cast<const __half*>(saved);

@@ -208,6 +208,11 @@ int make_tmap_f16(CUtensorMap* out, const void* gptr, int rank, const uint64_t* 
 
 int device_sm_count();
 
+// Deterministic mode of the calling host thread (mpgcn_set_deterministic, DESIGN.md section 11): every cross-CTA floating-point
+// sum writes per-CTA partials ("slots") to the workspace and one fixed-order kernel adds them, instead of atomics.
+int det_mode();
+int det_set(int on);
+
 // Function attributes (the > 48 KB dynamic shared-memory opt-in) belong to a device / context, not to the process: a
 // kernel that already ran on cuda:0 still needs the opt-in on cuda:1.  One cache per kernel, indexed by device ordinal.
 struct DynSmemAttr { int bytes[64]; };

@@ -24,8 +24,9 @@ __global__ void period_mean_kernel(const float* __restrict__ od, float* __restri
   }
 }
 
-// one warp per (t, i): rn2 = |A_t[i, :]|^2 (coalesced);  cn2 = |A_t[:, i]|^2 is accumulated by the same pass with atomics
-// on a pre-zeroed buffer (each lane owns column j of the row it reads)
+// one warp per (t, i): rn2 = |A_t[i, :]|^2 (coalesced);  COLS: cn2 = |A_t[:, i]|^2 is accumulated by the same pass with atomics
+// on a pre-zeroed buffer (each lane owns column j of the row it reads).  Deterministic mode runs COLS = false and col_norms_kernel.
+template <bool COLS = true>
 __global__ void norms_kernel(const float* __restrict__ avg, float* __restrict__ rn2, float* __restrict__ cn2, int P, int N) {
   const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -36,10 +37,24 @@ __global__ void norms_kernel(const float* __restrict__ avg, float* __restrict__ 
   for (int j = lane; j < N; j += 32) {
     const float v = row[j];
     s = fmaf(v, v, s);
-    atomicAdd(&cn2[t * N + j], v * v);
+    if (COLS) atomicAdd(&cn2[t * N + j], v * v);
   }
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) rn2[warp] = s;
+}
+
+// cn2[t][j] = |A_t[:, j]|^2 in row order: one thread per (t, j), consecutive threads read consecutive columns of a row
+__global__ void col_norms_kernel(const float* __restrict__ avg, float* __restrict__ cn2, int P, int N) {
+  const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= (size_t)P * N) return;
+  const size_t t = k / N, j = k % N;
+  const float* col = avg + t * (size_t)N * N + j;
+  float s = 0.f;
+  for (int i = 0; i < N; ++i) {
+    const float v = col[(size_t)i * N];
+    s += v * v;
+  }
+  cn2[k] = s;
 }
 
 // R[t][i][k] = A[i][k] / |A[i,:]| ;  C[t][i][k] = A[k][i] / |A[:,i]|   (32 x 32 smem tile transpose for C)
@@ -106,9 +121,16 @@ int dyn_graph_build(const float* od_hist, int periods, float* o_g, float* d_g, i
 
   prof_count(PROF_ELEMENTWISE);
   period_mean_kernel<<<dg_grid((size_t)P * NN, 256), 256, 0, st>>>(od_hist, avg, P, periods, NN);
-  MPGCN_CUDA(cudaMemsetAsync(cn2, 0, (size_t)P * N * sizeof(float), st));
-  prof_count(PROF_ELEMENTWISE);
-  norms_kernel<<<(unsigned)(((size_t)P * N * 32 + 255) / 256), 256, 0, st>>>(avg, rn2, cn2, P, N);
+  if (det_mode()) {      // column norms in a fixed order: no atomics (DESIGN.md section 11), no extra workspace
+    prof_count(PROF_ELEMENTWISE);
+    norms_kernel<false><<<(unsigned)(((size_t)P * N * 32 + 255) / 256), 256, 0, st>>>(avg, rn2, cn2, P, N);
+    prof_count(PROF_ELEMENTWISE);
+    col_norms_kernel<<<(unsigned)(((size_t)P * N + 255) / 256), 256, 0, st>>>(avg, cn2, P, N);
+  } else {
+    MPGCN_CUDA(cudaMemsetAsync(cn2, 0, (size_t)P * N * sizeof(float), st));
+    prof_count(PROF_ELEMENTWISE);
+    norms_kernel<true><<<(unsigned)(((size_t)P * N * 32 + 255) / 256), 256, 0, st>>>(avg, rn2, cn2, P, N);
+  }
   prof_count(PROF_ELEMENTWISE);
   normalize_kernel<<<dim3((N + 31) / 32, (N + 31) / 32, P), dim3(32, 8), 0, st>>>(avg, rn2, cn2, R, Cm, N);
   fill_kernel<<<(N + 255) / 256, 256, 0, st>>>(ones, 1.f, N);

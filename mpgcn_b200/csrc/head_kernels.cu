@@ -143,6 +143,66 @@ __global__ void head_bwd_kernel(HeadPtrs p, const float* __restrict__ w, const f
   }
 }
 
+// The same gradients in a fixed order (deterministic mode): a block's cells and the cells of each thread are those of
+// head_bwd_kernel, but the weight sums never meet an atomic.  Channels go in chunks of 32: in chunk l0 thread (cell lane
+// c = threadIdx.x / 8, sub) keeps channels l0 + 4 sub .. + 3 of its cells in registers, then thread t < 32 adds channel l0 + t over the
+// 32 cell lanes in lane order; the bias sum is formed the same way in chunk 0.  The block stores [dw M x C | db M] to its slot,
+// which reduce_slots adds over the blocks in block order.
+template <int MT>
+__global__ void head_bwd_det_kernel(HeadPtrs p, const float* __restrict__ w, const float* __restrict__ pre, const float* __restrict__ dy,
+                                    float* __restrict__ slots, float* __restrict__ dg_absmax, long long cells, int C, int Mrt) {
+  const int M = MT ? MT : Mrt;
+  __shared__ float s_red[5][257];      // [4 channels | bias][thread]
+  const int sub = threadIdx.x & 7, lane = threadIdx.x >> 3;
+  const long long stride = (long long)gridDim.x * (blockDim.x >> 3);
+  const float inv_m = 1.f / (float)M;
+  float* slot = slots + (size_t)blockIdx.x * M * (C + 1);
+#pragma unroll
+  for (int m = 0; m < (MT ? MT : kMaxBranches); ++m) {
+    if (!MT && m >= M) break;
+    float amax = 0.f;
+    for (int l0 = 0; l0 < C; l0 += 32) {
+      const int l = l0 + sub * 4;
+      const bool mine = l < C;
+      const float4 ww = mine ? *reinterpret_cast<const float4*>(w + m * C + l) : make_float4(0.f, 0.f, 0.f, 0.f);
+      float wacc[4] = {0.f, 0.f, 0.f, 0.f}, bacc = 0.f;
+      for (long long cell = (long long)blockIdx.x * (blockDim.x >> 3) + lane; cell < cells; cell += stride) {
+        const float d = pre[(long long)m * cells + cell] > 0.f ? dy[cell] * inv_m : 0.f;
+        if (mine) {
+          const float4 vv = *reinterpret_cast<const float4*>(p.g[m] + cell * C + l);
+          wacc[0] += d * vv.x; wacc[1] += d * vv.y; wacc[2] += d * vv.z; wacc[3] += d * vv.w;
+          if (p.dg[m]) {
+            const float4 o = make_float4(d * ww.x, d * ww.y, d * ww.z, d * ww.w);
+            *reinterpret_cast<float4*>(p.dg[m] + cell * C + l) = o;
+            amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
+          }
+        }
+        bacc += d;
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) s_red[e][threadIdx.x] = wacc[e];
+      s_red[4][threadIdx.x] = bacc;
+      __syncthreads();
+      if (threadIdx.x < 32 && l0 + (int)threadIdx.x < C) {
+        const int sb = threadIdx.x >> 2, e = threadIdx.x & 3;
+        float sum = 0.f;
+        for (int c = 0; c < 32; ++c) sum += s_red[e][c * 8 + sb];
+        slot[m * C + l0 + threadIdx.x] = sum;
+      }
+      if (l0 == 0 && threadIdx.x == 32) {
+        float sum = 0.f;
+        for (int c = 0; c < 32; ++c) sum += s_red[4][c * 8];
+        slot[M * C + m] = sum;
+      }
+      __syncthreads();
+    }
+    if (dg_absmax) {
+      for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(dg_absmax + m), __float_as_uint(amax));
+    }
+  }
+}
+
 static int head_grid(long long cells) {
   long long b = (cells + 31) / 32;
   const long long cap = (long long)device_sm_count() * 8;
@@ -182,12 +242,28 @@ int head_forward(const float* const* g, const float* w, const float* bias, float
   return 0;
 }
 
+size_t head_bwd_slot_bytes(long long cells, int C, int M) { return align_up((size_t)head_grid(cells) * M * (C + 1) * sizeof(float), 256); }
+
 int head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
-                  float* dg_absmax, long long cells, int C, int M, cudaStream_t st) {
+                  float* dg_absmax, long long cells, int C, int M, cudaStream_t st, float* slots) {
   HeadPtrs p{};
   for (int m = 0; m < M; ++m) {
     p.g[m] = g[m];
     p.dg[m] = dg ? dg[m] : nullptr;
+  }
+  if (slots) {
+    if (dg_absmax) MPGCN_CUDA(cudaMemsetAsync(dg_absmax, 0, sizeof(float) * M, st));
+    const int grid = head_grid(cells);
+    prof_count(PROF_ELEMENTWISE);
+    switch (M) {
+      case 1: head_bwd_det_kernel<1><<<grid, 256, 0, st>>>(p, w, pre, dy, slots, dg_absmax, cells, C, M); break;
+      case 2: head_bwd_det_kernel<2><<<grid, 256, 0, st>>>(p, w, pre, dy, slots, dg_absmax, cells, C, M); break;
+      case 3: head_bwd_det_kernel<3><<<grid, 256, 0, st>>>(p, w, pre, dy, slots, dg_absmax, cells, C, M); break;
+      case 4: head_bwd_det_kernel<4><<<grid, 256, 0, st>>>(p, w, pre, dy, slots, dg_absmax, cells, C, M); break;
+      default: head_bwd_det_kernel<0><<<grid, 256, 0, st>>>(p, w, pre, dy, slots, dg_absmax, cells, C, M); break;
+    }
+    MPGCN_CUDA(cudaGetLastError());
+    return reduce_slots(slots, grid, (long long)M * (C + 1), 1, 0, slot_image(dw, (long long)M * C, db, M), st);
   }
   MPGCN_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * M * C, st));
   MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * M, st));

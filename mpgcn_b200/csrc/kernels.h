@@ -24,7 +24,8 @@ struct SgemmParams {
   long long a_sseg, b_sseg;
   int Z0, Z1, Z2;              // batch z = (z0*Z1 + z1)*Z2 + z2
   long long a_sz[3], b_sz[3], d_sz[3];
-  int ksplit;                  // > 1: split each segment's K into slices, atomically add into D (D pre-zeroed)
+  int ksplit;                  // > 1: split each segment's K into slices, atomically add into D (D pre-zeroed) ...
+  long long d_sslice;          // ... or, when non-zero, slice s stores its partial at D + s * d_sslice (deterministic mode)
   float alpha;
   const float* bias;
   int bias_mod;
@@ -35,6 +36,20 @@ struct SgemmParams {
 };
 int simt_sgemm(const SgemmParams& p, cudaStream_t stream);
 
+// ---- fixed-order reduction of per-CTA partials (deterministic mode; simt_kernels.cu) ------------------------------------
+// A slot is one CTA's contribution laid out as an "image" of up to three outputs back to back: image[i] for i < end[0] goes to
+// dst[0][i], end[0] <= i < end[1] to dst[1][i - end[0]], then dst[2].  For each row a < rows:
+//     dst_k[a * width_k + j] = sum_{s < slots} P[a * a_stride + s * s_stride + start_k + j]
+// summed in the same order on every run: 32 interleaved groups of slots, each in slot order, then the groups in order.
+struct SlotImage {
+  float* dst[3];
+  long long end[3];
+};
+SlotImage slot_image(float* d0, long long n0, float* d1 = nullptr, long long n1 = 0, float* d2 = nullptr, long long n2 = 0);
+int reduce_slots(const float* P, int slots, long long s_stride, int rows, long long a_stride, const SlotImage& img, cudaStream_t s);
+// the slots of the bias gradient of relu_bwd_prep*: one [H] partial per block of its grid (at most 16 blocks per SM)
+size_t bias_grad_slot_bytes(int H);
+
 // ---- elementwise / layout helpers (simt_kernels.cu) ---------------------------------------
 int cvt_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t s);
 // delta[p*N + i] = G[p][i][i] - float(fp16(G[p][i][i])) for `planes` N x N matrices
@@ -42,12 +57,12 @@ int support_diag_delta(const float* G, float* delta, size_t planes, int N, cudaS
 // [rows][cols] fp32 -> [rows][ld] fp16 (ld >= cols, padding zeroed)
 int cvt_f32_to_f16_padded(const float* src, __half* dst, size_t rows, int cols, int ld, cudaStream_t s);
 // d_pre = d_out * (out > 0) (relu) or d_out, 1 <= H <= 1024; exactly one output: fp32, or fp16(scale[0] * d_pre) (scale: device
-// scalar); db[h] = sum d_pre (nullable)
+// scalar); db[h] = sum d_pre (nullable); db_slots (bias_grad_slot_bytes, nullable): db from per-block partials in a fixed order
 int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d_pre16, float* d_pre32, float* db, size_t n, int H,
-                  const float* scale, cudaStream_t s);
+                  const float* scale, cudaStream_t s, float* db_slots = nullptr);
 // the same with the ReLU mask taken from an fp16 copy of the forward output (tensor-core path: fp16 d_pre only)
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d_pre16, float* db, size_t n, int H,
-                          const float* scale, cudaStream_t s);
+                          const float* scale, cudaStream_t s, float* db_slots = nullptr);
 // scale2[0] = S = 2^k with S*max|d_out| in [16,32), scale2[1] = 1/S (S = 1 for an all-zero or non-finite input).
 // fp16 has 5 exponent bits: realistic gradients (MSE mean over B*N*N cells ~ 1e-7) must be rescaled before the cast.
 // absmax_hint: optional device scalar already holding max|d_out| (produced by the epilogue that wrote d_out): skips the pass
@@ -83,7 +98,9 @@ int lstm_last_forward(const float* x_seq, const float* w_ih, const float* w_hh, 
                       int B, int T, long long NN, int C, cudaStream_t s);
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
-                       long long NN, int C, cudaStream_t s);
+                       long long NN, int C, cudaStream_t s, float* slots = nullptr);
+// slots of that backward in deterministic mode: one [4C x C | 4C | 4C] partial per block (<= SMs blocks)
+size_t lstm_bwd_slot_bytes(int C);
 // cells per block of the backward, which keeps every recomputed step of its cells in shared memory; 0 where not even one cell
 // fits (T above 15 at hidden 64, 95 at 48, 224 at 32) or C is outside 1..64
 int lstm_bwd_cells_per_block(int T, int C);
@@ -95,7 +112,9 @@ int head_check(const char* what, const float* const* g, const float* w, float* c
 int head_forward(const float* const* g, const float* w, const float* bias, float* y, float* pre, long long cells, int C, int M,
                  cudaStream_t st);
 int head_backward(const float* const* g, const float* w, const float* pre, const float* dy, float* const* dg, float* dw, float* db,
-                  float* dg_absmax /*[M] or null*/, long long cells, int C, int M, cudaStream_t st);
+                  float* dg_absmax /*[M] or null*/, long long cells, int C, int M, cudaStream_t st, float* slots = nullptr);
+// slots of head_backward in deterministic mode: one [M x C | M] partial per block of its grid
+size_t head_bwd_slot_bytes(long long cells, int C, int M);
 
 // support-matrix builder (adj_kernels.cu): reference GCN.Adj_Processor.process
 enum AdjKernel { ADJ_LOCALPOOL = 0, ADJ_CHEBYSHEV = 1, ADJ_RANDOM_WALK = 2, ADJ_DUAL_RANDOM_WALK = 3 };

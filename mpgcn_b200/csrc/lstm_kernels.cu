@@ -114,6 +114,9 @@ int lstm_last_forward(const float* x_seq, const float* w_ih, const float* w_hh, 
 // ---------------------------------------------------------------------------------------
 // backward (BPTT with in-kernel recomputation)
 // ---------------------------------------------------------------------------------------
+// DET (deterministic mode): instead of adding its accumulators to the gradients with atomics, a block stores them, in their shared-
+// memory order [4C x C w_hh | 4C w_ih | 4C b], to its slot d_w_hh + blockIdx.x * (4C x C + 8C); reduce_slots adds the blocks in order.
+template <bool DET>
 __global__ void lstm_bwd_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                                 const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                                 float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, float* __restrict__ d_x,
@@ -240,10 +243,16 @@ __global__ void lstm_bwd_kernel(const float* __restrict__ x_seq, const float* __
       __syncthreads();
     }
   }
-  for (int e = tid; e < G * C; e += nthr) atomicAdd(&d_w_hh[e], acc_whh[e]);
-  for (int j = tid; j < G; j += nthr) {
-    atomicAdd(&d_w_ih[j], acc_wih[j]);
-    atomicAdd(&d_b[j], acc_b[j]);
+  if constexpr (DET) {
+    __syncthreads();
+    float* slot = d_w_hh + (size_t)blockIdx.x * (G * C + 2 * G);
+    for (int e = tid; e < G * C + 2 * G; e += nthr) slot[e] = acc_whh[e];
+  } else {
+    for (int e = tid; e < G * C; e += nthr) atomicAdd(&d_w_hh[e], acc_whh[e]);
+    for (int j = tid; j < G; j += nthr) {
+      atomicAdd(&d_w_ih[j], acc_wih[j]);
+      atomicAdd(&d_b[j], acc_b[j]);
+    }
   }
 }
 
@@ -275,7 +284,7 @@ int lstm_bwd_cells_per_block(int T, int C) {
 
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
-                       long long NN, int C, cudaStream_t st) {
+                       long long NN, int C, cudaStream_t st, float* slots) {
   MPGCN_CHECK(B > 0 && T > 0 && NN > 0, "lstm: empty input");
   MPGCN_CHECK(C >= 1 && C <= 64, "lstm backward: hidden size %d unsupported (1..64)", C);
   const long long cells = (long long)B * NN;
@@ -284,20 +293,33 @@ int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh,
   MPGCN_CHECK(CELLS >= 1, "lstm backward: sequence length %d too long for the shared-memory stash", T);
   const int threads = CELLS * C;
   const size_t smem = lstm_bwd_fixed_bytes(C) + (size_t)CELLS * lstm_bwd_per_cell_bytes(T, C);
-  static DynSmemAttr attr = {};
-  if (int e = ensure_dyn_smem(lstm_bwd_kernel, (int)(kBwdSmemBudget + 4096), attr)) return e;
-  MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G, st));
-  MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G * C, st));
-  MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G, st));
+  static DynSmemAttr attr = {}, attr_det = {};
+  if (slots) {
+    if (int e = ensure_dyn_smem(lstm_bwd_kernel<true>, (int)(kBwdSmemBudget + 4096), attr_det)) return e;
+  } else {
+    if (int e = ensure_dyn_smem(lstm_bwd_kernel<false>, (int)(kBwdSmemBudget + 4096), attr)) return e;
+    MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G * C, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G, st));
+  }
   const long long tiles = (cells + CELLS - 1) / CELLS;
   long long grid = device_sm_count();
   if (grid > tiles) grid = tiles;
   prof_begin(PROF_LSTM_BWD, 16.0 * C * (C + 1) * (double)cells * T, st);
-  lstm_bwd_kernel<<<(unsigned)grid, threads, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, cells, T,
-                                                           NN, C, CELLS);
+  if (slots)
+    lstm_bwd_kernel<true><<<(unsigned)grid, threads, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, nullptr, slots, nullptr, d_x, cells, T,
+                                                                 NN, C, CELLS);
+  else
+    lstm_bwd_kernel<false><<<(unsigned)grid, threads, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, cells, T,
+                                                                  NN, C, CELLS);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
+  if (slots)
+    if (int e = reduce_slots(slots, (int)grid, (long long)G * C + 2 * G, 1, 0, slot_image(d_w_hh, (long long)G * C, d_w_ih, G, d_b_ih, G), st))
+      return e;
   return lstm_copy_bias_grad(d_b_ih, d_b_hh, G, st);
 }
+
+size_t lstm_bwd_slot_bytes(int C) { return align_up((size_t)device_sm_count() * (4 * C * C + 8 * C) * sizeof(float), 256); }
 
 }  // namespace mpgcn

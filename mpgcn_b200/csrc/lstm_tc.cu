@@ -356,7 +356,9 @@ constexpr size_t kBwdSavedSmem =
     (size_t)kBwdRing * Dims<1>::THREADS * 2 * sizeof(float) +    // x ring: [slot][thread][row h]
     Dims<1>::G4 * sizeof(float) + 2 * kBwdRing * sizeof(uint64_t);
 
-template <bool DX>
+// DET (deterministic mode): the flush stores the CTA's dWext to its slot d_w_hh + blockIdx.x * 4352, laid out as the outputs
+// [128 x 32 w_hh | 128 w_ih | 128 b] (the two x columns of w_ih added in the CTA first), instead of adding it with atomics.
+template <bool DX, bool DET = false>
 __global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::BWD_CTAS_PER_SM)
 lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
@@ -552,16 +554,31 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
   }
   if (have_prev) dwext(prev_slot, prev_phase);
   // ---- flush the weight-gradient accumulator ----
+  if constexpr (DET) {
+    float* slot = d_w_hh + (size_t)blockIdx.x * (D::G4 * C + 2 * D::G4);
 #pragma unroll
-  for (int nt = 0; nt < 5; ++nt)
+    for (int nt = 0; nt < 5; ++nt)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int j = 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1);
-      const float v = dw[nt][i] * invS;
-      if (col < C) atomicAdd(&d_w_hh[j * C + col], v);
-      else if (col == 32 || col == 34) atomicAdd(&d_w_ih[j], v);
-      else if (col == 33) atomicAdd(&d_b[j], v);
-    }
+      for (int i = 0; i < 4; ++i) {
+        const int j = 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1);
+        const float v = dw[nt][i] * invS;
+        const float next = __shfl_down_sync(0xffffffffu, v, 1);     // lane q + 1: column col + 2
+        if (col < C) slot[j * C + col] = v;
+        else if (col == 32) slot[D::G4 * C + j] = v + next;          // columns 32 and 34: the x hi / lo pair of w_ih
+        else if (col == 33) slot[D::G4 * C + D::G4 + j] = v;
+      }
+  } else {
+#pragma unroll
+    for (int nt = 0; nt < 5; ++nt)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int j = 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1);
+        const float v = dw[nt][i] * invS;
+        if (col < C) atomicAdd(&d_w_hh[j * C + col], v);
+        else if (col == 32 || col == 34) atomicAdd(&d_w_ih[j], v);
+        else if (col == 33) atomicAdd(&d_b[j], v);
+      }
+  }
 }
 
 // =======================================================================================
@@ -890,7 +907,9 @@ constexpr int DW_DA_LD = 136;
 template <int CH, bool UP = false>
 constexpr size_t kDwSmem = (size_t)Dims<CH>::CELLS * (DW_DA_LD + Dims<CH, UP>::HX_LD) * sizeof(__half);
 
-template <int CH, bool UP = false>
+// DET (deterministic mode): CTA (js, split) stores its rows to the split's slot d_w_hh + split * (4H x H + 4H x KI + 4H), laid out as
+// the outputs [4H x H w_hh | 4H x KI w_ih | 4H b] (KI = H for UP, else 1 with the x hi / lo columns added first), without atomics.
+template <int CH, bool UP = false, bool DET = false>
 __global__ void __launch_bounds__(DW_THREADS)
 lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ saved, const __half* __restrict__ da_rec,
                    float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, const float* __restrict__ scale2,
@@ -974,20 +993,42 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     }
   }
   const float invS = scale2[1];
+  if constexpr (DET) {
+    constexpr int KI = UP ? D::H : 1;
+    float* slot = d_w_hh + (size_t)blockIdx.y * (D::G4 * D::H + D::G4 * KI + D::G4);
+    float* s_ih = slot + D::G4 * D::H;
+    float* s_b = s_ih + D::G4 * KI;
 #pragma unroll
-  for (int nt = 0; nt < NX; ++nt)
+    for (int nt = 0; nt < NX; ++nt)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
-      const float v = dw[nt][i] * row_scale(r) * invS;
-      if (col < D::H) atomicAdd(&d_w_hh[(size_t)j * D::H + col], v);
-      else if (UP) {
-        if (col < 2 * D::H) atomicAdd(&d_w_ih[(size_t)j * D::H + col - D::H], v);
-        else if (col == 2 * D::H) atomicAdd(&d_b[j], v);     // (column 2 H + 1, against b_lo, is the same sum)
+      for (int i = 0; i < 4; ++i) {
+        const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
+        const float v = dw[nt][i] * row_scale(r) * invS;
+        const float next = __shfl_down_sync(0xffffffffu, v, 1);     // lane q + 1: column col + 2
+        if (col < D::H) slot[(size_t)j * D::H + col] = v;
+        else if (UP) {
+          if (col < 2 * D::H) s_ih[(size_t)j * D::H + col - D::H] = v;
+          else if (col == 2 * D::H) s_b[j] = v;
+        }
+        else if (col == D::H) s_ih[j] = v + next;
+        else if (col == D::H + 1) s_b[j] = v;
       }
-      else if (col == D::H || col == D::H + 2) atomicAdd(&d_w_ih[j], v);
-      else if (col == D::H + 1) atomicAdd(&d_b[j], v);
-    }
+  } else {
+#pragma unroll
+    for (int nt = 0; nt < NX; ++nt)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
+        const float v = dw[nt][i] * row_scale(r) * invS;
+        if (col < D::H) atomicAdd(&d_w_hh[(size_t)j * D::H + col], v);
+        else if (UP) {
+          if (col < 2 * D::H) atomicAdd(&d_w_ih[(size_t)j * D::H + col - D::H], v);
+          else if (col == 2 * D::H) atomicAdd(&d_b[j], v);     // (column 2 H + 1, against b_lo, is the same sum)
+        }
+        else if (col == D::H || col == D::H + 2) atomicAdd(&d_w_ih[j], v);
+        else if (col == D::H + 1) atomicAdd(&d_b[j], v);
+      }
+  }
 }
 
 }  // namespace lstm_tc
@@ -1022,9 +1063,18 @@ static size_t lstm_tcw_da_bytes(int B, int T, long long NN, int C) {
   return (size_t)lstm_tc_padded_cells(B, NN, C) * T * 4 * C * sizeof(__half);
 }
 
-// workspace of a backward that is handed the forward's saved state: the grad scale (1 KB) and, at the wide widths, the da records
+// Deterministic mode: the slots of the weight-gradient flush, one image [4C x C w_hh | 4C x KI w_ih | 4C b] (KI = C in an upper
+// stack layer, else 1) per CTA of the single-layer hidden-32 walk, or per split of the wide dW pass (every stack layer included)
+static size_t lstm_tc_slot_bytes(int C, bool up) {
+  const size_t G4 = 4 * (size_t)C, image = G4 * C + G4 * (up ? C : 1) + G4;
+  const size_t n = C == 32 && !up ? (size_t)Dims<1>::BWD_CTAS_PER_SM * device_sm_count() : (size_t)4 * device_sm_count() / (C / 32);
+  return align_up(n * image * sizeof(float), 256);
+}
+
+// workspace of a backward that is handed the forward's saved state: the grad scale (1 KB), at the wide widths the da records, and
+// in deterministic mode the slots
 static size_t lstm_tc_bwd_saved_workspace_bytes(int B, int T, long long NN, int C) {
-  return 1024 + (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256));
+  return 1024 + (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256)) + (det_mode() ? lstm_tc_slot_bytes(C, false) : 0);
 }
 
 // without a saved buffer from the forward, the backward first re-runs the (training) forward into its workspace
@@ -1050,26 +1100,58 @@ static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* 
 
 // lstm_backward_h32 and lstm_backward_tcw<CH>: the kernels of one width's backward, run once the grad scale and the zeroed
 // weight gradients are in place.  da_rec: the gate-gradient records of the wide walk (the hidden-32 walk keeps them on chip).
+// slots: deterministic mode's flush slots (lstm_tc_slot_bytes), null for the atomic flush
 static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved,
-                             void* /*da_rec*/, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                             void* /*da_rec*/, float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
   using D = Dims<1>;
   if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  auto kern = d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true> : lstm_tc::lstm_bwd_saved_tc_kernel<false>;
-  static DynSmemAttr attr_x = {}, attr_n = {};
-  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, d_x ? attr_x : attr_n)) return e;
+  auto kern = slots ? (d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true, true> : lstm_tc::lstm_bwd_saved_tc_kernel<false, true>)
+                    : (d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true> : lstm_tc::lstm_bwd_saved_tc_kernel<false>);
+  static DynSmemAttr attr_x = {}, attr_n = {}, attr_xd = {}, attr_nd = {};
+  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, slots ? (d_x ? attr_xd : attr_nd) : (d_x ? attr_x : attr_n))) return e;
+  const int grid = lstm_grid<1>(cells, D::BWD_CTAS_PER_SM);
   prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  kern<<<lstm_grid<1>(cells, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells, T, NN);
+  kern<<<grid, D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, slots ? slots : d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells, T, NN);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
+  if (slots)
+    return reduce_slots(slots, grid, (long long)D::G4 * D::H + 2 * D::G4, 1, 0,
+                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, D::G4, d_b, D::G4), st);
+  return 0;
+}
+
+// the wide dW pass of one layer (KI = H for an upper stack layer, else 1), then in deterministic mode the reduction of its slots
+template <int CH, bool UP>
+static int lstm_dw_pass(const float* x_seq, const void* saved, const void* da_rec, float* d_w_ih, float* d_w_hh, float* d_b, float* slots,
+                        const float* scale2, long long cells, int T, long long NN, const void* h_in, double flops, cudaStream_t st) {
+  using D = Dims<CH>;
+  constexpr int KI = UP ? D::H : 1;
+  auto dw = slots ? lstm_tc::lstm_dw_tcw_kernel<CH, UP, true> : lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
+  constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
+  static DynSmemAttr attr_d = {}, attr_dd = {};
+  if (dw_smem)
+    if (int e = ensure_dyn_smem(dw, (int)dw_smem, slots ? attr_dd : attr_d)) return e;
+  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
+  long long splits = 4LL * device_sm_count() / CH;
+  if (splits > records) splits = records;
+  prof_begin(PROF_LSTM_BWD, flops, st);
+  dw<<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, dw_smem, st>>>(x_seq, static_cast<const __half*>(saved),
+                                                                      static_cast<const __half*>(da_rec), d_w_ih, slots ? slots : d_w_hh,
+                                                                      d_b, scale2, cells, T, NN, static_cast<const __half*>(h_in));
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  if (slots)
+    return reduce_slots(slots, (int)splits, (long long)D::G4 * (D::H + KI + 1), 1, 0,
+                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, (long long)D::G4 * KI, d_b, D::G4), st);
   return 0;
 }
 
 template <int CH>
 static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, void* da_rec,
-                             const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                             float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
   constexpr size_t smem = lstm_tc::kWalkSmem<CH>;
   static DynSmemAttr attr_b = {};
@@ -1082,15 +1164,8 @@ static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float*
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   // ... and the weight gradient (8 H (H + 1) / 2 more: 12 H (H + 1) in all)
-  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
-  long long splits = 4LL * device_sm_count() / CH;
-  if (splits > records) splits = records;
-  prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  lstm_tc::lstm_dw_tcw_kernel<CH><<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, 0, st>>>(
-      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2, cells, T, NN, nullptr);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  return lstm_dw_pass<CH, false>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, slots, scale2, cells, T, NN, nullptr,
+                                 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
 }
 
 int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
@@ -1120,7 +1195,10 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
   MPGCN_CHECK(C == 32 || C == 96 || C == 128, "lstm backward: no tensor-core kernel for hidden=%d", C);
   float* scale2 = static_cast<float*>(ws);
-  void* da_rec = static_cast<uint8_t*>(ws) + 1024;   // wide widths: the da records follow the grad scale
+  void* da_rec = static_cast<uint8_t*>(ws) + 1024;   // wide widths: the da records follow the grad scale, then the slots
+  float* slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024 +
+                                                       (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256)))
+                            : nullptr;
   if (saved == nullptr) {          // the caller kept no forward state: rebuild it (same kernel, same bits as the training forward)
     void* tmp = static_cast<uint8_t*>(ws) + lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C);
     if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C, st)) return e;
@@ -1132,7 +1210,7 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4 * C, st));
   MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4, st));
   auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
-  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, scale2, cells, T, NN, st))
+  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, slots, scale2, cells, T, NN, st))
     return e;
   return lstm_copy_bias_grad(d_b_ih, d_b_hh, G4, st);
 }
@@ -1163,8 +1241,10 @@ size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int 
 static size_t lstm_tc_stack_dseq_bytes(int B, int T, long long NN, int C) {
   return align_up((size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(float), 256);
 }
+// deterministic mode: the slots of the dW passes (lstm_tc_slot_bytes of an upper layer, the largest) sit before the da records
+static size_t lstm_tc_stack_slot_bytes(int C) { return det_mode() ? lstm_tc_slot_bytes(C, true) : 0; }
 size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int /*L*/) {
-  return 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
+  return 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + lstm_tc_stack_slot_bytes(C) + align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
 }
 
 template <int CH, bool SAVE, bool UP, bool HSEQ>
@@ -1218,7 +1298,7 @@ static int stack_forward(const float* x_seq, int L, const float* const* w_ih, co
 template <int CH, bool UP, bool DHIN>
 static int stack_bwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* d_hT,
                            float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, const void* h_in, void* da_rec,
-                           float* d_seq, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                           float* d_seq, float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
   constexpr int KH = UP ? 2 * D::H : D::H;     // the input and recurrent columns of the gate GEMM
   auto walk = lstm_tc::lstm_bwd_walk_tcw_kernel<CH, UP, DHIN>;
@@ -1232,29 +1312,16 @@ static int stack_bwd_layer(const float* x_seq, const float* w_ih, const float* w
                                                                            scale2, cells, T, NN, static_cast<const __half*>(h_in), d_seq);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
-  // ... and the weight gradient
-  auto dw = lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
-  constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
-  static DynSmemAttr attr_d = {};
-  if (dw_smem)
-    if (int e = ensure_dyn_smem(dw, (int)dw_smem, attr_d)) return e;
-  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
-  long long splits = 4LL * device_sm_count() / CH;
-  if (splits > records) splits = records;
-  prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (KH + 1) * (double)cells * T, st);      // ... and 4 H (KH + 1)
-  dw<<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, dw_smem, st>>>(x_seq, static_cast<const __half*>(saved),
-                                                                       static_cast<const __half*>(da_rec), d_w_ih, d_w_hh, d_b, scale2,
-                                                                       cells, T, NN, static_cast<const __half*>(h_in));
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  // ... and the weight gradient, 4 H (KH + 1)
+  return lstm_dw_pass<CH, UP>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, slots, scale2, cells, T, NN, h_in,
+                              4.0 * D::H * (KH + 1) * (double)cells * T, st);
 }
 
 template <int CH>
 static int stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b,
-                          float* d_x, const void* saved, uint8_t* da_rec, size_t da_stride, float* d_seq, const float* scale2, int B,
-                          int T, long long NN, cudaStream_t st) {
+                          float* d_x, const void* saved, uint8_t* da_rec, size_t da_stride, float* d_seq, float* slots, const float* scale2,
+                          int B, int T, long long NN, cudaStream_t st) {
   const long long cells = (long long)B * NN;
   const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, 32 * CH);
   auto lsaved = [&](int l) { return static_cast<const uint8_t*>(saved) + (size_t)l * layer_bytes; };
@@ -1264,13 +1331,13 @@ static int stack_backward(const float* x_seq, int L, const float* const* w_ih, c
     int e;
     if (l == 0)
       e = stack_bwd_layer<CH, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, d_w_ih[0], d_w_hh[0], d_b[0], d_x, lsaved(0),
-                                           nullptr, rec, d_seq, scale2, cells, T, NN, st);
+                                           nullptr, rec, d_seq, slots, scale2, cells, T, NN, st);
     else if (top)
       e = stack_bwd_layer<CH, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], d_hT, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, scale2, cells, T, NN, st);
+                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, slots, scale2, cells, T, NN, st);
     else
       e = stack_bwd_layer<CH, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, scale2, cells, T, NN, st);
+                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, slots, scale2, cells, T, NN, st);
     if (e) return e;
   }
   return 0;
@@ -1302,7 +1369,8 @@ int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, 
   const long long cells = (long long)B * NN;
   float* scale2 = static_cast<float*>(ws);
   float* d_seq = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024);
-  uint8_t* da_rec = static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C);
+  float* slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C)) : nullptr;
+  uint8_t* da_rec = static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + lstm_tc_stack_slot_bytes(C);
   const size_t da_region = align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
   const size_t da_stride = ws_bytes >= need + (size_t)(L - 1) * da_region ? da_region : 0;     // every layer's records, or one region
   // one gradient scale S for the whole stack, from max|d_hT|: every walk keeps dh, dc and d_seq in units of S
@@ -1314,9 +1382,9 @@ int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, 
     MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
   }
   const int e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
-                                            scale2, B, T, NN, st)
+                                            slots, scale2, B, T, NN, st)
                         : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
-                                            scale2, B, T, NN, st);
+                                            slots, scale2, B, T, NN, st);
   if (e) return e;
   for (int l = 0; l < L; ++l)
     if (int e2 = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e2;

@@ -31,7 +31,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const SgemmParams p, int til
 
   const float* A = p.A + z0 * p.a_sz[0] + z1 * p.a_sz[1] + z2 * p.a_sz[2];
   const float* B = p.B + z0 * p.b_sz[0] + z1 * p.b_sz[1] + z2 * p.b_sz[2];
-  float* D = p.D + z0 * p.d_sz[0] + z1 * p.d_sz[1] + z2 * p.d_sz[2];
+  float* D = p.D + z0 * p.d_sz[0] + z1 * p.d_sz[1] + z2 * p.d_sz[2] + slice * p.d_sslice;
   const float* Cin = p.Cin ? p.Cin + z0 * p.c_sz[0] + z1 * p.c_sz[1] + z2 * p.c_sz[2] : nullptr;
 
   const int tid = threadIdx.x;
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const SgemmParams p, int til
       if (gj >= p.N) continue;
       float v = acc[x][y] * p.alpha;
       float* dst = D + gi * p.d_si + gj;
-      if (p.ksplit > 1) {
+      if (p.ksplit > 1 && p.d_sslice == 0) {
         atomicAdd(dst, v);
       } else {
         if (Cin) v = fmaf(p.beta, Cin[gi * p.d_si + gj], v);
@@ -112,6 +112,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const SgemmParams p, int til
 int simt_sgemm(const SgemmParams& p, cudaStream_t stream) {
   MPGCN_CHECK(p.M > 0 && p.N > 0 && p.K > 0 && p.nseg > 0 && p.ksplit > 0, "simt_sgemm: empty problem");
   MPGCN_CHECK(p.Cin == nullptr || p.ksplit == 1, "simt_sgemm: Cin needs ksplit == 1");
+  MPGCN_CHECK(p.d_sslice == 0 || (p.bias == nullptr && !p.relu), "simt_sgemm: slice partials take no epilogue");
   const int bn = (p.N <= 32) ? 32 : 64;
   const int tiles_m = (p.M + 63) / 64;
   const int tiles_n = (p.N + bn - 1) / bn;
@@ -254,8 +255,9 @@ __device__ __forceinline__ void st_v(__half* p, const float (&v)[4], float S) {
 
 // db[c] += the block's partial sums of channel c.  The block is a multiple of H / V threads with at least H of them, so thread t
 // owns channels V * (t % (H / V)) .. + V - 1 for its whole grid-stride loop; thread c < H adds the partials of channel c in thread order.
+// With slots (deterministic mode) the block stores that sum in its own [H] slot instead, for reduce_slots to add in block order.
 template <int V>
-__device__ __forceinline__ void block_bias_grad(const float (&local)[V], float* db, int H) {
+__device__ __forceinline__ void block_bias_grad(const float (&local)[V], float* db, float* slots, int H) {
   extern __shared__ float s_db[];   // [V][blockDim.x]
   const int nt = blockDim.x;
 #pragma unroll
@@ -265,7 +267,8 @@ __device__ __forceinline__ void block_bias_grad(const float (&local)[V], float* 
     const int q = threadIdx.x / V, e = threadIdx.x % V;
     float sum = 0.f;
     for (int t = q; t < nt; t += H / V) sum += s_db[e * nt + t];
-    atomicAdd(&db[threadIdx.x], sum);
+    if (slots) slots[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * H + threadIdx.x] = sum;
+    else atomicAdd(&db[threadIdx.x], sum);
   }
 }
 
@@ -273,7 +276,7 @@ __device__ __forceinline__ void block_bias_grad(const float (&local)[V], float* 
 // 32 registers, so that 2048 threads fit on an SM: a streaming kernel needs every load in flight it can get.
 template <int V, Mask M, class T>
 __global__ void __launch_bounds__(1024, 2) relu_bwd_kernel(const float* __restrict__ d_out, const void* __restrict__ mask, PeerPtrs<T> dst, int g, float* __restrict__ db,
-                                const float* __restrict__ scale, size_t n, size_t full, size_t off, int H) {
+                                float* __restrict__ db_slots, const float* __restrict__ scale, size_t n, size_t full, size_t off, int H) {
   using MaskT = std::conditional_t<M == Mask::F16, __half, float>;
   const float S = std::is_same<T, __half>::value ? __ldg(scale) : 1.f;
   const size_t b = blockIdx.y;
@@ -293,7 +296,7 @@ __global__ void __launch_bounds__(1024, 2) relu_bwd_kernel(const float* __restri
 #pragma unroll
     for (int e = 0; e < V; ++e) local[e] += v[e];
   }
-  if (db) block_bias_grad<V>(local, db, H);
+  if (db) block_bias_grad<V>(local, db, db_slots, H);
 }
 
 static bool aligned(const void* p, size_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
@@ -309,7 +312,7 @@ static int channel_block(int H, int V) {
 // for the vector access, else V = 1.  The exchange steps (PROF_EXCHANGE) are timed, the local pass is counted.
 template <Mask M, class T>
 static int relu_bwd_launch(const float* d_out, const void* mask, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
-                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s) {
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr) {
   MPGCN_CHECK(H >= 1 && H <= 1024, "relu backward: H=%d unsupported (1..1024)", H);
   MPGCN_CHECK(g >= 1 && g <= 8, "relu backward: %d ranks unsupported (1..8)", g);
   constexpr bool f16 = std::is_same<T, __half>::value;
@@ -321,40 +324,45 @@ static int relu_bwd_launch(const float* d_out, const void* mask, T* const* dsts,
     pp.p[j] = dsts[j];
     vec = vec && aligned(dsts[j], 4 * sizeof(T));
   }
-  if (db) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, s));
+  MPGCN_CHECK(!db_slots || B == 1, "relu backward: fixed-order bias gradient of one sample only");
+  if (db && !db_slots) MPGCN_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * H, s));
+  if (!db) db_slots = nullptr;
   const int V = vec ? 4 : 1, threads = channel_block(H, V);
   const dim3 grid(grid_for(n / V, threads), (unsigned)B);
   const size_t smem = (size_t)V * threads * sizeof(float);
   if (tag == PROF_EXCHANGE) prof_begin(tag, 0.0, s);
   else prof_count(tag);
-  if (vec) relu_bwd_kernel<4, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, scale, n, full, off, H);
-  else relu_bwd_kernel<1, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, scale, n, full, off, H);
+  if (vec) relu_bwd_kernel<4, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, db_slots, scale, n, full, off, H);
+  else relu_bwd_kernel<1, M, T><<<grid, threads, smem, s>>>(d_out, mask, pp, g, db, db_slots, scale, n, full, off, H);
   prof_end(s);
   MPGCN_CUDA(cudaGetLastError());
+  if (db_slots) return reduce_slots(db_slots, (int)grid.x, H, 1, 0, slot_image(db, H), s);
   return 0;
 }
 // the same with the ReLU mask taken from the fp32 forward output (act 1) or no mask (act 0)
 template <class T>
 static int relu_bwd_launch(const float* d_out, const float* out, int act, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
-                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s) {
-  return act ? relu_bwd_launch<Mask::F32>(d_out, out, dsts, g, db, scale, B, n, full, off, H, tag, s)
-             : relu_bwd_launch<Mask::None>(d_out, nullptr, dsts, g, db, scale, B, n, full, off, H, tag, s);
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr) {
+  return act ? relu_bwd_launch<Mask::F32>(d_out, out, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots)
+             : relu_bwd_launch<Mask::None>(d_out, nullptr, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots);
 }
 
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d16, float* db, size_t n, int H, const float* scale,
-                          cudaStream_t s) {
+                          cudaStream_t s, float* db_slots) {
   if (n == 0) return 0;
-  if (!relu) return relu_bwd_launch<Mask::None>(d_out, nullptr, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
-  return relu_bwd_launch<Mask::F16>(d_out, out16, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
+  if (!relu) return relu_bwd_launch<Mask::None>(d_out, nullptr, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
+  return relu_bwd_launch<Mask::F16>(d_out, out16, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
 }
 
 int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d16, float* d32, float* db, size_t n, int H,
-                  const float* scale, cudaStream_t s) {
+                  const float* scale, cudaStream_t s, float* db_slots) {
   if (n == 0) return 0;
   MPGCN_CHECK((d16 == nullptr) != (d32 == nullptr), "relu_bwd_prep: exactly one of the fp16 and fp32 outputs");
-  if (d16) return relu_bwd_launch(d_out, out, relu, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
-  return relu_bwd_launch(d_out, out, relu, &d32, 1, db, nullptr, 1, n, n, 0, H, PROF_ELEMENTWISE, s);
+  if (d16) return relu_bwd_launch(d_out, out, relu, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
+  return relu_bwd_launch(d_out, out, relu, &d32, 1, db, nullptr, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
 }
+
+size_t bias_grad_slot_bytes(int H) { return align_up((size_t)device_sm_count() * 16 * H * sizeof(float), 256); }
 
 // max |x| over a tensor as the bit pattern of a non-negative float (monotone as unsigned int)
 __global__ void absmax_kernel(const float* __restrict__ x, size_t n, unsigned int* __restrict__ amax_bits) {
@@ -480,6 +488,43 @@ __global__ void reduce_dg_kernel(const float* __restrict__ P, float* __restrict_
 int reduce_dg_partials(const float* P, float* dG, int slices, int N, int ldp, const float* inv_scale, int accumulate, cudaStream_t s) {
   prof_count(PROF_BWD_DG);
   reduce_dg_kernel<<<grid_for((size_t)N * N, 256), 256, 0, s>>>(P, dG, slices, N, ldp, inv_scale, accumulate);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Block (32, 32): lane x owns image element blockIdx.x * 32 + x (coalesced across the slot), warp y adds slots y, y + 32, ... in
+// slot order, and warp 0 adds the 32 group sums in group order.  The order depends on the slot count only, never on timing.
+__global__ void __launch_bounds__(1024) reduce_slots_kernel(const float* __restrict__ P, int slots, long long s_stride,
+                                                            long long a_stride, SlotImage img) {
+  __shared__ float part[32][33];
+  const long long i = (long long)blockIdx.x * 32 + threadIdx.x;
+  const float* src = P + (long long)blockIdx.y * a_stride + i;
+  float acc = 0.f;
+  if (i < img.end[2])
+    for (int t = threadIdx.y; t < slots; t += 32) acc += src[(long long)t * s_stride];
+  part[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y == 0 && i < img.end[2]) {
+    float sum = 0.f;
+#pragma unroll
+    for (int w = 0; w < 32; ++w) sum += part[w][threadIdx.x];
+    const int k = i < img.end[0] ? 0 : i < img.end[1] ? 1 : 2;
+    const long long start = k == 0 ? 0 : img.end[k - 1];
+    img.dst[k][(long long)blockIdx.y * (img.end[k] - start) + (i - start)] = sum;
+  }
+}
+
+SlotImage slot_image(float* d0, long long n0, float* d1, long long n1, float* d2, long long n2) {
+  SlotImage m;
+  m.dst[0] = d0; m.dst[1] = d1; m.dst[2] = d2;
+  m.end[0] = n0; m.end[1] = n0 + n1; m.end[2] = n0 + n1 + n2;
+  return m;
+}
+
+int reduce_slots(const float* P, int slots, long long s_stride, int rows, long long a_stride, const SlotImage& img, cudaStream_t s) {
+  MPGCN_CHECK(slots >= 1 && rows >= 1 && img.end[2] >= 1, "reduce_slots: empty reduction");
+  prof_count(PROF_ELEMENTWISE);
+  reduce_slots_kernel<<<dim3((unsigned)((img.end[2] + 31) / 32), (unsigned)rows), dim3(32, 32), 0, s>>>(P, slots, s_stride, a_stride, img);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }

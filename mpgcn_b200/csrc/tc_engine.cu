@@ -21,6 +21,15 @@ void set_error(const char* fmt, ...) {
 }
 const char* last_error() { return g_err; }
 
+// deterministic mode, per host thread like the error string: one thread's setting never changes another's launches
+static thread_local int g_det = 0;
+int det_mode() { return g_det; }
+int det_set(int on) {
+  const int prev = g_det;
+  g_det = on ? 1 : 0;
+  return prev;
+}
+
 int ensure_dyn_smem_impl(const void* kernel, int bytes, DynSmemAttr& cache) {
   static std::mutex mu;
   int dev = 0;

@@ -20,6 +20,7 @@ def _history_len(num_days: int, split_ratio, perceived_period: int) -> int:
     return (train_len // perceived_period) * perceived_period               # :41-42 (the remainder is dropped)
 
 
+@_lib.engine_buffers()
 def construct_dyn_G(OD_data, split_ratio, perceived_period: int = 7, device=None):
     """OD_data [days, N, N, 1] (numpy or torch, un-normalised) -> (O_dyn_G, D_dyn_G), numpy float64 [N, N, perceived_period]."""
     od = torch.as_tensor(np.asarray(OD_data) if not isinstance(OD_data, torch.Tensor) else OD_data)
@@ -35,6 +36,7 @@ def construct_dyn_G(OD_data, split_ratio, perceived_period: int = 7, device=None
     if dev.type != "cuda":
         raise RuntimeError("mpgcn_b200.dyn_graph runs on a CUDA device only (there is no CPU path)")
     lib = _lib.load()
+    _lib.sync_deterministic()            # fixed-order column norms under torch.use_deterministic_algorithms(True)
     N = od.shape[1]
     hist = od[:used].to(device=dev, dtype=torch.float32).contiguous()
     o_g = torch.empty((P, N, N), dtype=torch.float32, device=dev)

@@ -12,7 +12,8 @@ What is captured is exactly `Model_Trainer.py:107-115`: `y_pred = model(x_seq=..
 `loss = criterion(y_pred, y_true)`, `optimizer.zero_grad()`, `loss.backward()`, `optimizer.step()`.  The optimizer must be
 capture-safe (`torch.optim.Adam(..., capturable=True)`; the trainer's `Model_Trainer.py:74-77` Adam takes that flag unchanged).
 The support staging cache of `mpgcn_b200.ops` is cleared before the capture so that the fp16 conversion of the (per-batch)
-dynamic supports is part of the graph.
+dynamic supports is part of the graph.  The graph keeps the kernels of the torch.use_deterministic_algorithms setting in force at
+capture (the fixed-order reductions or the atomic ones, DESIGN.md section 11): changing the flag later does not change a replay.
 """
 from __future__ import annotations
 

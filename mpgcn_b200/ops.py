@@ -135,6 +135,7 @@ def _prepared_supports(lib, G, Gc, planes: int, N: int):
 
 class _BDGCNFn(torch.autograd.Function):
     @staticmethod
+    @_lib.engine_buffers()
     def forward(ctx, X, G_o, G_d, W, b, dynamic: bool, act: int, precision, grad_mode: bool, support_grad: bool):
         import ctypes
         lib = _lib.load()
@@ -181,9 +182,11 @@ class _BDGCNFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_lib.engine_buffers()
     def backward(ctx, d_out):
         import ctypes
         lib = _lib.load()
+        _lib.sync_deterministic()       # this thread's mode, before the workspace query (autograd's device thread: set it here)
         out, Goc, Gdc, Wc, saved, Xc = ctx.saved_tensors
         B, N, K, C, H = ctx.shape
         dynamic, act, prec, has_bias = ctx.meta
@@ -280,6 +283,7 @@ def lstm_engine_supports(name, T, C) -> bool:
 
 class _LSTMLastFn(torch.autograd.Function):
     @staticmethod
+    @_lib.engine_buffers()
     def forward(ctx, x_seq, w_ih, w_hh, b_ih, b_hh, precision, grad_mode: bool):
         lib = _lib.load()
         B, T = x_seq.shape[0], x_seq.shape[1]
@@ -303,8 +307,10 @@ class _LSTMLastFn(torch.autograd.Function):
         return hT
 
     @staticmethod
+    @_lib.engine_buffers()
     def backward(ctx, d_hT):
         lib = _lib.load()
+        _lib.sync_deterministic()
         xc, w_ih, w_hh, b_ih, b_hh = ctx.saved_tensors
         B, T, NN, C, prec = ctx.dims
         hint = _take_hint(ctx, d_hT) if (prec == _lib.PREC_FP16_TC and d_hT.dtype == torch.float32 and d_hT.is_contiguous()) else None
@@ -383,6 +389,7 @@ def _ptr_array(ts):
 
 class _LSTMStackFn(torch.autograd.Function):
     @staticmethod
+    @_lib.engine_buffers()
     def forward(ctx, grad_mode: bool, x_seq, *params):
         lib = _lib.load()
         B, T = x_seq.shape[0], x_seq.shape[1]
@@ -407,8 +414,10 @@ class _LSTMStackFn(torch.autograd.Function):
         return hT
 
     @staticmethod
+    @_lib.engine_buffers()
     def backward(ctx, d_hT):
         lib = _lib.load()
+        _lib.sync_deterministic()
         xc, *ps = ctx.saved_tensors
         B, T, NN, C, L, prec = ctx.dims
         if ctx.lstm_saved is None:
@@ -448,6 +457,7 @@ def lstm_stack(x_seq: torch.Tensor, params) -> torch.Tensor:
 
 class _HeadFn(torch.autograd.Function):
     @staticmethod
+    @_lib.engine_buffers()
     def forward(ctx, grad_mode, w, b, *gs):
         import ctypes
         lib = _lib.load()
@@ -469,6 +479,7 @@ class _HeadFn(torch.autograd.Function):
         return y
 
     @staticmethod
+    @_lib.engine_buffers()
     def backward(ctx, dy):
         import ctypes
         lib = _lib.load()
@@ -484,8 +495,13 @@ class _HeadFn(torch.autograd.Function):
         dptrs = (ctypes.c_void_p * M)(*[(d.data_ptr() if d is not None else None) for d in dgs])
         amax = torch.empty(M, dtype=torch.float32, device=dy.device)
         with torch.cuda.device(dy.device):
-            _lib.check(lib.mpgcn_head_backward(ptrs, _ptr(wc), _ptr(pre), _ptr(dy), dptrs, _ptr(dw), _ptr(db), _ptr(amax), cells, C, M,
-                                               _stream()), "head_backward")
+            if _lib.sync_deterministic():      # fixed-order dw / db: the per-block partials need a workspace
+                ws = _scratch(lib.mpgcn_head_backward_workspace_bytes(cells, C, M), dy.device)
+                _lib.check(lib.mpgcn_head_backward_ex(ptrs, _ptr(wc), _ptr(pre), _ptr(dy), dptrs, _ptr(dw), _ptr(db), _ptr(amax), cells, C, M,
+                                                      _ptr(ws), ws.numel(), _stream()), "head_backward_ex")
+            else:
+                _lib.check(lib.mpgcn_head_backward(ptrs, _ptr(wc), _ptr(pre), _ptr(dy), dptrs, _ptr(dw), _ptr(db), _ptr(amax), cells, C, M,
+                                                   _stream()), "head_backward")
         for m, d in enumerate(dgs):
             _put_hint(ctx.g_producers[m], d, amax[m:m + 1])
         return (None, dw, db) + tuple(dgs)

@@ -24,6 +24,7 @@ back end; tests swap in a CPU stand-in to run the exchange logic under gloo (tes
 from __future__ import annotations
 
 import ctypes
+import warnings
 
 import torch
 import torch.distributed as dist
@@ -63,6 +64,20 @@ class ShardPlan:
 # ------------------------------------------------------------------------------------------------
 # compute back end (the C ABI); tests replace it by a CPU stand-in to exercise the exchange logic under gloo
 # ------------------------------------------------------------------------------------------------
+def _no_deterministic(op: str) -> None:
+    """The sharded layers' exchange kernels (mpgcn_relu_backward[_scatter[_f16]]) and NCCL have no fixed-order implementation.
+    Under torch.use_deterministic_algorithms(True) this raises, as torch's own ops without one do; with warn_only=True it warns and
+    the op runs as it does without the flag (this thread's library mode is set off for it)."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"mpgcn_b200.shard: {op} has no deterministic implementation (its exchange steps sum with atomics and NCCL), but "
+           "torch.use_deterministic_algorithms(True) is set")
+    if not torch.is_deterministic_algorithms_warn_only_enabled():
+        raise RuntimeError(msg)
+    warnings.warn(msg)
+    _lib.set_deterministic(False)
+
+
 class CudaEngine:
     def _part(self, row0, rows, Ko, Kd):
         return _lib.BdgcnPart(row0, rows, Ko, Kd)
@@ -125,6 +140,7 @@ class CudaEngine:
 
     def relu_backward(self, d_out, out, act, want_db):
         lib = _lib.load()
+        _no_deterministic("relu_backward")
         d_pre = torch.empty_like(d_out)
         db = torch.empty(d_out.shape[-1], dtype=torch.float32, device=d_out.device) if want_db else None
         with torch.cuda.device(d_out.device):
@@ -146,6 +162,7 @@ class CudaEngine:
     def relu_backward_scatter(self, d_out, out, act, ptrs, N, row0, want_db):
         """mask the rank's rows of d_out and store them into rows [row0, ..) of every buffer at `ptrs`; -> db or None"""
         lib = _lib.load()
+        _no_deterministic("relu_backward_scatter")
         B, rows, _, H = d_out.shape
         db = torch.empty(H, dtype=torch.float32, device=d_out.device) if want_db else None
         arr = (ctypes.c_void_p * len(ptrs))(*ptrs)
@@ -164,6 +181,7 @@ class CudaEngine:
     def relu_backward_scatter_f16(self, d_out, out, act, ptrs, N, row0, want_db, absmax):
         """fp16 flavour: -> (db or None, scale2 [S, 1/S]); every buffer at `ptrs` (fp16 [B,N,N,H]) receives fp16(S * masked d_out rows)"""
         lib = _lib.load()
+        _no_deterministic("relu_backward_scatter_f16")
         B, rows, _, H = d_out.shape
         db = torch.empty(H, dtype=torch.float32, device=d_out.device) if want_db else None
         scale2 = torch.empty(2, dtype=torch.float32, device=d_out.device)
@@ -477,6 +495,7 @@ def sharded_bdgcn(layer, X, G, plan: ShardPlan, branch: int = 0):
     act = layer.fused_act()
     if act is None:
         raise NotImplementedError("sharded layers fuse None / ReLU only")
+    _no_deterministic("sharded_bdgcn")
     dynamic = not isinstance(G, torch.Tensor)
     if dynamic:
         G_o, G_d = G
