@@ -23,10 +23,17 @@ int adj_num_supports(int kernel_type, int K) {
   }
 }
 
-size_t adj_workspace_bytes(int B, int N, int kernel_type, int K) {
-  (void)kernel_type; (void)K;
-  return 256 + 2 * align_up((size_t)B * N * sizeof(float), 256);      // row sums and column sums
+// forward workspace: row sums and column sums
+struct AdjLayout { size_t rowsum, colsum, total; };
+static AdjLayout adj_layout(int B, int N) {
+  AdjLayout L;
+  size_t off = 0;
+  L.rowsum = take(off, (size_t)B * N * sizeof(float), 256);
+  L.colsum = take(off, (size_t)B * N * sizeof(float), 256);
+  L.total = align_up(off, 256) + 256;    // unused padding: the size this workspace has always had
+  return L;
 }
+size_t adj_workspace_bytes(int B, int N) { return adj_layout(B, N).total; }
 
 // sums[b][i] = sum_j A[b][i][j] (by_col = 0) or sum_j A[b][j][i] (by_col = 1); one warp per (b, i)
 __global__ void adj_sums_kernel(const float* __restrict__ A, float* __restrict__ sums, int B, int N, int by_col) {
@@ -100,9 +107,10 @@ int adj_process(const float* flow, float* supports, int B, int N, int kernel_typ
   const int Ks = adj_num_supports(kernel_type, K);
   MPGCN_CHECK(Ks >= 1, "Invalid kernel_type. Must be one of [chebyshev, localpool, random_walk_diffusion, dual_random_walk_diffusion].");
   MPGCN_CHECK(B >= 1 && N >= 1 && K >= 0, "adj_process: bad shape B=%d N=%d K=%d", B, N, K);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= adj_workspace_bytes(B, N, kernel_type, K), "adj_process: workspace too small");
-  float* rowsum = static_cast<float*>(ws);
-  float* colsum = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + align_up((size_t)B * N * sizeof(float), 256));
+  const AdjLayout L = adj_layout(B, N);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "adj_process: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
+  float* rowsum = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + L.rowsum);
+  float* colsum = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + L.colsum);
   const size_t warps = (size_t)B * N;
   prof_count(PROF_ELEMENTWISE);
   adj_sums_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(flow, rowsum, B, N, 0);
@@ -150,14 +158,21 @@ int adj_process(const float* flow, float* supports, int B, int N, int kernel_typ
 //
 // Workspace: [B][Ks][N][N] working copy of d_supports (only when K >= 2), then row sums, column sums and two per-row reductions.
 // ---------------------------------------------------------------------------------------------------------------------------
-static size_t adj_bwd_grads_bytes(int B, int N, int kernel_type, int K) {
-  if (kernel_type == ADJ_LOCALPOOL || K < 2) return 0;
-  return align_up((size_t)B * adj_num_supports(kernel_type, K) * N * N * sizeof(float), 256);
+struct AdjBwdLayout { size_t grads, rowsum, colsum, red0, red1, total; };
+static AdjBwdLayout adj_bwd_layout(int B, int N, int kernel_type, int K) {
+  AdjBwdLayout L;
+  size_t off = 0;
+  const size_t vec = (size_t)B * N * sizeof(float);
+  L.grads = take(off, kernel_type == ADJ_LOCALPOOL || K < 2 ? 0 : (size_t)B * adj_num_supports(kernel_type, K) * N * N * sizeof(float), 256);
+  L.rowsum = take(off, vec, 256);
+  L.colsum = take(off, vec, 256);
+  L.red0 = take(off, vec, 256);
+  L.red1 = take(off, vec, 256);
+  L.total = align_up(off, 256) + 256;    // unused padding: the size this workspace has always had
+  return L;
 }
 
-size_t adj_backward_workspace_bytes(int B, int N, int kernel_type, int K) {
-  return 256 + adj_bwd_grads_bytes(B, N, kernel_type, K) + 4 * align_up((size_t)B * N * sizeof(float), 256);
-}
+size_t adj_backward_workspace_bytes(int B, int N, int kernel_type, int K) { return adj_bwd_layout(B, N, kernel_type, K).total; }
 
 __device__ __forceinline__ float masked_inv(float s) {
   const float v = 1.f / s;
@@ -256,21 +271,20 @@ int adj_process_backward(const float* flow, const float* supports, const float* 
               "Invalid kernel_type. Must be one of [chebyshev, localpool, random_walk_diffusion, dual_random_walk_diffusion].");
   MPGCN_CHECK(B >= 1 && N >= 1 && K >= 0, "adj_process_backward: bad shape B=%d N=%d K=%d", B, N, K);
   const int Ks = adj_num_supports(kernel_type, K);
-  const size_t need = adj_backward_workspace_bytes(B, N, kernel_type, K);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "adj_process_backward: workspace too small (%zu < %zu bytes)", ws_bytes, need);
+  const AdjBwdLayout L = adj_bwd_layout(B, N, kernel_type, K);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "adj_process_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   const size_t total = (size_t)B * N * N;
   if (kernel_type != ADJ_LOCALPOOL && K == 0) {       // only the identity: its gradient is not the flow's
     MPGCN_CUDA(cudaMemsetAsync(d_flow, 0, total * sizeof(float), st));
     return 0;
   }
   const long long NN = (long long)N * N;
-  const size_t vec = align_up((size_t)B * N * sizeof(float), 256);
   uint8_t* w8 = static_cast<uint8_t*>(ws);
-  float* grads = reinterpret_cast<float*>(w8);
-  float* rowsum = reinterpret_cast<float*>(w8 + adj_bwd_grads_bytes(B, N, kernel_type, K));
-  float* colsum = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + vec);
-  float* red0 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + 2 * vec);
-  float* red1 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(rowsum) + 3 * vec);
+  float* grads = reinterpret_cast<float*>(w8 + L.grads);
+  float* rowsum = reinterpret_cast<float*>(w8 + L.rowsum);
+  float* colsum = reinterpret_cast<float*>(w8 + L.colsum);
+  float* red0 = reinterpret_cast<float*>(w8 + L.red0);
+  float* red1 = reinterpret_cast<float*>(w8 + L.red1);
   const unsigned warp_blocks = (unsigned)(((size_t)B * N * 32 + 255) / 256);
   const bool dual = kernel_type == ADJ_DUAL_RANDOM_WALK;
 

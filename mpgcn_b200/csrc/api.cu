@@ -4,13 +4,10 @@
 #include "kernels.h"
 
 namespace mpgcn {
-size_t simt_saved_bytes(const BdgcnShape& s);
-size_t simt_fwd_ws_bytes(const BdgcnShape& s);
-size_t simt_bwd_ws_bytes(const BdgcnShape& s);
-size_t tc_saved_bytes(const BdgcnShape& s);
-size_t tc_fwd_ws_bytes(const BdgcnShape& s);
-size_t tc_bwd_ws_bytes(const BdgcnShape& s);
-long long tc_debug_offset(const BdgcnShape& s, int which);
+size_t bdgcn_saved_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_saved_bytes(s) : simt_saved_bytes(s); }
+size_t bdgcn_fwd_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_fwd_ws_bytes(s) : simt_fwd_ws_bytes(s); }
+size_t bdgcn_bwd_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_bwd_ws_bytes(s) : simt_bwd_ws_bytes(s); }
+size_t bdgcn_sgrad_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s); }
 }  // namespace mpgcn
 
 using namespace mpgcn;
@@ -69,17 +66,12 @@ int mpgcn_bdgcn_precision_supported(int B, int N, int K, int C, int H, int preci
   return 0;
 }
 
-size_t mpgcn_bdgcn_saved_bytes(int B, int N, int K, int C, int H, int precision) {
-  const BdgcnShape s = mk(B, N, K, C, H, 0, 0);
-  return precision == PREC_FP16_TC ? tc_saved_bytes(s) : simt_saved_bytes(s);
-}
+size_t mpgcn_bdgcn_saved_bytes(int B, int N, int K, int C, int H, int precision) { return bdgcn_saved_bytes(mk(B, N, K, C, H, 0, 0), precision); }
 size_t mpgcn_bdgcn_fwd_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision) {
-  const BdgcnShape s = mk(B, N, K, C, H, dynamic, 0);
-  return precision == PREC_FP16_TC ? tc_fwd_ws_bytes(s) : simt_fwd_ws_bytes(s);
+  return bdgcn_fwd_workspace_bytes(mk(B, N, K, C, H, dynamic, 0), precision);
 }
 size_t mpgcn_bdgcn_bwd_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision) {
-  const BdgcnShape s = mk(B, N, K, C, H, dynamic, 0);
-  return precision == PREC_FP16_TC ? tc_bwd_ws_bytes(s) : simt_bwd_ws_bytes(s);
+  return bdgcn_bwd_workspace_bytes(mk(B, N, K, C, H, dynamic, 0), precision);
 }
 
 static BdgcnExtras to_extras(const mpgcn_bdgcn_extras* x) {
@@ -138,7 +130,7 @@ int mpgcn_bdgcn_backward_x(const float* d_out, const float* out, const float* G_
 size_t mpgcn_bdgcn_support_grad_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision) {
   const BdgcnShape s = mk(B, N, K, C, H, dynamic, 0);
   if (check_shape(s, precision)) return 0;
-  return precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s);
+  return bdgcn_sgrad_workspace_bytes(s, precision);
 }
 
 int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const float* G_o, const float* G_d, int dynamic, const float* W, int act,
@@ -152,8 +144,6 @@ int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const fl
               "mpgcn_bdgcn_backward_supports: null pointer argument");
   MPGCN_CHECK(dynamic || (dG_o && !dG_d), "mpgcn_bdgcn_backward_supports: static supports take their gradient in dG_o; dG_d must be NULL");
   MPGCN_CHECK(!extras || !extras->d_pre_f16, "mpgcn_bdgcn_backward_supports: a prepared fp16 dPre belongs to a layer part");
-  const size_t need = precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s);
-  MPGCN_CHECK(workspace_bytes >= need, "mpgcn_bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
   // the supports' own gradient adds 2 K B N^3 (C + H) to the backward's flops
   const double dg_flops = 2.0 * s.K * s.B * (double)s.N * s.N * s.N * (s.C + s.H);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -182,16 +172,13 @@ int mpgcn_bdgcn_backward(const float* d_out, const float* out, const float* G_o,
 }
 
 size_t mpgcn_bdgcn_part_saved_bytes(int B, int N, int C, int H, int precision, const mpgcn_bdgcn_part* part) {
-  const BdgcnShape s = mk_part(B, N, C, H, 0, part);
-  return precision == PREC_FP16_TC ? tc_saved_bytes(s) : simt_saved_bytes(s);
+  return bdgcn_saved_bytes(mk_part(B, N, C, H, 0, part), precision);
 }
 size_t mpgcn_bdgcn_part_fwd_workspace_bytes(int B, int N, int C, int H, int dynamic, int precision, const mpgcn_bdgcn_part* part) {
-  const BdgcnShape s = mk_part(B, N, C, H, dynamic, part);
-  return precision == PREC_FP16_TC ? tc_fwd_ws_bytes(s) : simt_fwd_ws_bytes(s);
+  return bdgcn_fwd_workspace_bytes(mk_part(B, N, C, H, dynamic, part), precision);
 }
 size_t mpgcn_bdgcn_part_bwd_workspace_bytes(int B, int N, int C, int H, int dynamic, int precision, const mpgcn_bdgcn_part* part) {
-  const BdgcnShape s = mk_part(B, N, C, H, dynamic, part);
-  return precision == PREC_FP16_TC ? tc_bwd_ws_bytes(s) : simt_bwd_ws_bytes(s);
+  return bdgcn_bwd_workspace_bytes(mk_part(B, N, C, H, dynamic, part), precision);
 }
 
 int mpgcn_bdgcn_forward_part(const float* X, const float* G_o, const float* G_d, int dynamic, const float* W, float* pre_partial, void* saved,
@@ -268,7 +255,7 @@ int mpgcn_relu_backward(const float* d_out, const float* out, int act, float* d_
 }
 
 int mpgcn_adj_num_supports(int kernel_type, int K) { return adj_num_supports(kernel_type, K); }
-size_t mpgcn_adj_workspace_bytes(int B, int N, int kernel_type, int K) { return adj_workspace_bytes(B, N, kernel_type, K); }
+size_t mpgcn_adj_workspace_bytes(int B, int N, int kernel_type, int K) { return adj_workspace_bytes(B, N); }
 int mpgcn_adj_process(const float* flow, float* supports, int B, int N, int kernel_type, int K, void* workspace, size_t workspace_bytes,
                       void* stream) {
   MPGCN_CHECK(flow && supports, "mpgcn_adj_process: null pointer argument");
@@ -344,10 +331,9 @@ int mpgcn_lstm_precision_supported(int T, int C, int precision) {
 // sizes for the width of the tensor-core kernel; a width it does not run keeps the hidden-32 size these always returned
 static int lstm_tc_size_width(int C) { return lstm_tc_supported(1, C) ? C : 32; }
 
-// precision 0: 256 bytes, plus its slots in deterministic mode (a hidden size it does not run keeps the 256)
 size_t mpgcn_lstm_bwd_workspace_bytes(int B, int T, long long NN, int C, int precision) {
   if (precision == PREC_FP16_TC) return lstm_tc_bwd_workspace_bytes(B, T, NN, lstm_tc_size_width(C));
-  return 256 + (det_mode() && C >= 1 && C <= 64 ? lstm_bwd_slot_bytes(C) : 0);
+  return lstm_bwd_workspace_bytes(C);
 }
 
 size_t mpgcn_lstm_saved_bytes(int B, int T, long long NN, int C, int precision) {
@@ -408,13 +394,8 @@ int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const 
     return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, C, workspace,
                                  workspace_bytes, d_hT_absmax, st);
   }
-  if (!det_mode()) return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st);
-  const size_t need = mpgcn_lstm_bwd_workspace_bytes(B, T, NN, C, precision);
-  MPGCN_CHECK(workspace != nullptr && workspace_bytes >= need, "lstm backward: workspace too small for the deterministic mode (%zu < %zu)",
-              workspace_bytes, need);
-  MPGCN_CHECK((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
-  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, st,
-                            reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + 256));
+  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, workspace,
+                            workspace_bytes, st);
 }
 
 int mpgcn_lstm_stack_supported(int T, int C, int L, int precision) {

@@ -17,46 +17,51 @@
 
 namespace mpgcn {
 
-namespace {
-struct Carver {
-  uint8_t* base;
-  size_t off, cap;
-  Carver(void* p, size_t bytes) : base(static_cast<uint8_t*>(p)), off(0), cap(bytes) {}
-  template <class T>
-  T* take(size_t count) {
-    off = align_up(off, 256);
-    T* r = reinterpret_cast<T*>(base + off);
-    off += count * sizeof(T);
-    return r;
-  }
-  bool ok() const { return off <= cap; }
-};
-}  // namespace
-
 // cells of an activation slab: R origin rows x N destinations (R = N for a whole layer)
 static size_t rn(const BdgcnShape& s) { return (size_t)s.R * s.N; }
 
 size_t simt_saved_bytes(const BdgcnShape& s) { return (size_t)s.B * s.Kd * rn(s) * s.C * sizeof(float); }
-size_t simt_fwd_ws_bytes(const BdgcnShape& s) {
-  return 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256) + align_up(simt_saved_bytes(s), 256);
+
+// forward workspace: U, then Z (used only when the caller passes no `saved` buffer)
+struct SimtFwdLayout { size_t u, z, total; };
+static SimtFwdLayout simt_fwd_layout(const BdgcnShape& s) {
+  SimtFwdLayout L;
+  size_t off = 0;
+  L.u = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 4, 256);
+  L.z = take(off, simt_saved_bytes(s), 256);
+  L.total = align_up(off, 256) + 256;    // unused padding: the size this workspace has always had
+  return L;
 }
-static size_t simt_bwd_base_bytes(const BdgcnShape& s) {
-  return 1024 + align_up((size_t)s.B * s.N * s.N * s.H * 4, 256) + align_up((size_t)s.B * s.Ko * rn(s) * s.H * 4, 256) +
-         align_up((size_t)s.B * s.Kd * rn(s) * s.C * 4, 256) + align_up((size_t)s.Ko * s.Kd * s.C * s.H * 4, 256);
-}
+size_t simt_fwd_ws_bytes(const BdgcnShape& s) { return simt_fwd_layout(s).total; }
+
 // dW = sum over R*N rows: split-K into up to 256 slices of >= 2048 rows
 static int dw_ksplit(const BdgcnShape& s) {
   long long ks = (long long)rn(s) / 2048;
   return (int)(ks < 1 ? 1 : ks > 256 ? 256 : ks);
 }
 static int dw_mt(const BdgcnShape& s) { return (s.Kd * s.C + 127) / 128; }
-// Deterministic mode appends, after the mode-off workspace, the bias-gradient slots and (ksplit > 1) the dW slices in the layout of
-// reduce_dw_partials: [slice][MT * 128 rows d*C + c][Ko*H columns o*H + h], MT = ceil(Kd*C / 128).
-static size_t simt_det_bytes(const BdgcnShape& s) {
+
+// backward workspace: dPre (every origin row m, always), V, Y, Wq; `sgrad` (the support gradient) adds U, recomputed from the Z
+// stash.  Deterministic mode's region follows: the bias-gradient slots and (ksplit > 1) the dW slices in the layout of
+// reduce_dw_partials, [slice][MT * 128 rows d*C + c][Ko*H columns o*H + h], MT = ceil(Kd*C / 128); both empty with the mode off.
+struct SimtBwdLayout { size_t dpre, v, y, wq, u, db_slots, dw_slices, total; };
+static SimtBwdLayout simt_bwd_layout(const BdgcnShape& s, bool sgrad) {
+  SimtBwdLayout L{};
+  size_t off = 0;
+  L.dpre = take(off, (size_t)s.B * s.N * s.N * s.H * 4, 256);
+  L.v = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 4, 256);
+  L.y = take(off, (size_t)s.B * s.Kd * rn(s) * s.C * 4, 256);
+  L.wq = take(off, (size_t)s.Ko * s.Kd * s.C * s.H * 4, 256);
+  if (sgrad) L.u = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 4, 256);
+  off = align_up(off, 256) + (sgrad ? 1024 + 256 : 1024);     // unused padding: the sizes these workspaces have always had
   const int ks = dw_ksplit(s);
-  return bias_grad_slot_bytes(s.H) + (ks > 1 ? align_up((size_t)ks * dw_mt(s) * 128 * s.Ko * s.H * 4, 256) : 0);
+  L.db_slots = take(off, det_mode() ? bias_grad_slot_bytes(s.H) : 0, 256);
+  L.dw_slices = take(off, det_mode() && ks > 1 ? (size_t)ks * dw_mt(s) * 128 * s.Ko * s.H * 4 : 0, 256);
+  L.total = align_up(off, 256);
+  return L;
 }
-size_t simt_bwd_ws_bytes(const BdgcnShape& s) { return simt_bwd_base_bytes(s) + (det_mode() ? simt_det_bytes(s) : 0); }
+size_t simt_bwd_ws_bytes(const BdgcnShape& s) { return simt_bwd_layout(s, false).total; }
+size_t simt_sgrad_ws_bytes(const BdgcnShape& s) { return simt_bwd_layout(s, true).total; }
 
 static void zero3(long long (&a)[3]) { a[0] = a[1] = a[2] = 0; }
 
@@ -65,10 +70,11 @@ static void zero3(long long (&a)[3]) { a[0] = a[1] = a[2] = 0; }
 int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
                        float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
-  Carver cv(ws, ws_bytes);
-  float* U = cv.take<float>((size_t)s.B * Ko * RN * H);
-  float* Z = saved ? static_cast<float*>(saved) : cv.take<float>((size_t)s.B * Kd * RN * C);
-  MPGCN_CHECK(cv.ok(), "bdgcn_forward: workspace too small (%zu < %zu bytes)", ws_bytes, cv.off);
+  const SimtFwdLayout L = simt_fwd_layout(s);
+  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_forward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* U = reinterpret_cast<float*>(wb + L.u);
+  float* Z = saved ? static_cast<float*>(saved) : reinterpret_cast<float*>(wb + L.z);
   const long long go_sb = s.dynamic ? Ko * NN : 0, gd_sb = s.dynamic ? Kd * NN : 0;   // support batch strides
 
   {  // Z[b,d,n] (e x l) = G_d^T (e x c) * X[b,n] (c x l)
@@ -113,30 +119,25 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
   return 0;
 }
 
-static size_t simt_sgrad_base_bytes(const BdgcnShape& s) {
-  return simt_bwd_base_bytes(s) + 256 + align_up((size_t)s.B * s.Ko * rn(s) * s.H * sizeof(float), 256);
-}
-size_t simt_sgrad_ws_bytes(const BdgcnShape& s) { return simt_sgrad_base_bytes(s) + (det_mode() ? simt_det_bytes(s) : 0); }
-
-// form_y: form Y even without dX (the support gradient reads it); det: the deterministic-mode region (simt_det_bytes) or null
+// L: the layout, checked against the workspace; form_y: form Y even without dX (the support gradient reads it)
 static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                              const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, bool form_y, uint8_t* det,
+                              const void* saved, float* dX, float* dW, float* db, void* ws, const SimtBwdLayout& L, bool form_y,
                               cudaStream_t st) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   MPGCN_CHECK(Z != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
-  Carver cv(ws, ws_bytes);
-  float* dPre = cv.take<float>((size_t)s.B * NN * H);
-  float* V = cv.take<float>((size_t)s.B * Ko * RN * H);
-  float* Y = cv.take<float>((size_t)s.B * Kd * RN * C);
-  float* Wq = cv.take<float>((size_t)Ko * Kd * H * C);
-  MPGCN_CHECK(cv.ok(), "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, cv.off);
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* dPre = reinterpret_cast<float*>(wb + L.dpre);
+  float* V = reinterpret_cast<float*>(wb + L.v);
+  float* Y = reinterpret_cast<float*>(wb + L.y);
+  float* Wq = reinterpret_cast<float*>(wb + L.wq);
+  const bool det = det_mode();     // fixed-order sums from the slots instead of atomics
   const long long go_sb = s.dynamic ? Ko * NN : 0, gd_sb = s.dynamic ? Kd * NN : 0;
 
   const float* dP = d_out;         // a partial call receives dPre itself (every origin row m, already masked)
   if (!s.partial) {
     if (int e = relu_bwd_prep(d_out, out, s.act, nullptr, dPre, db, (size_t)s.B * NN * H, (int)H, nullptr, st,
-                              det ? reinterpret_cast<float*>(det) : nullptr))
+                              det ? reinterpret_cast<float*>(wb + L.db_slots) : nullptr))
       return e;
     dP = dPre;
   }
@@ -169,7 +170,7 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
     p.b_sz[0] = RN * H;
     p.d_sz[0] = Kd * C * H; p.d_sz[1] = C * H;
     p.ksplit = ks; p.alpha = 1.f;
-    float* P = slices ? reinterpret_cast<float*>(det + bias_grad_slot_bytes((int)H)) : nullptr;
+    float* P = slices ? reinterpret_cast<float*>(wb + L.dw_slices) : nullptr;
     if (slices) {
       p.D = P; p.d_si = Ko * H; p.d_sz[0] = H; p.d_sz[1] = C * Ko * H;
       p.d_sslice = (long long)dw_mt(s) * 128 * Ko * H;
@@ -218,30 +219,25 @@ namespace mpgcn {
 
 int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                         const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st) {
-  MPGCN_CHECK(!det_mode() || ws_bytes >= simt_bwd_ws_bytes(s), "bdgcn_backward: workspace too small for the deterministic mode (%zu < %zu bytes)",
-              ws_bytes, simt_bwd_ws_bytes(s));
-  uint8_t* det = det_mode() ? static_cast<uint8_t*>(ws) + simt_bwd_base_bytes(s) : nullptr;
-  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, false, det, st);
+  const SimtBwdLayout L = simt_bwd_layout(s, false);
+  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
+  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, false, st);
 }
 
 int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
                                  const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
                                  size_t ws_bytes, cudaStream_t st) {
   MPGCN_CHECK(s.whole(), "support gradients: whole layers only");
-  MPGCN_CHECK(ws_bytes >= simt_sgrad_ws_bytes(s), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes,
-              simt_sgrad_ws_bytes(s));
+  const SimtBwdLayout L = simt_bwd_layout(s, true);
+  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
-  uint8_t* det = det_mode() ? static_cast<uint8_t*>(ws) + simt_sgrad_base_bytes(s) : nullptr;
-  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, want_d, det, st)) return e;
+  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, want_d, st)) return e;
   const long long N = s.N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
-  Carver cv(ws, ws_bytes);                          // the backward's regions, then U
-  const float* dPre = cv.take<float>((size_t)s.B * NN * H);
-  cv.take<float>((size_t)s.B * Ko * NN * H);
-  const float* Y = cv.take<float>((size_t)s.B * Kd * NN * C);
-  cv.take<float>((size_t)Ko * Kd * C * H);
-  float* U = cv.take<float>((size_t)s.B * Ko * NN * H);
-  MPGCN_CHECK(cv.ok(), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, cv.off);
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  const float* dPre = reinterpret_cast<const float*>(wb + L.dpre);
+  const float* Y = reinterpret_cast<const float*>(wb + L.y);
+  float* U = reinterpret_cast<float*>(wb + L.u);
   if (dGo) {
     {  // U[b,o] (rows x h) = sum_d Z[b,d] (rows x l) * W[o,d] (l x h), as the forward
       SgemmParams p{};

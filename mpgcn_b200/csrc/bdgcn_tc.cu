@@ -116,25 +116,18 @@ size_t tc_saved_bytes(const BdgcnShape& s) { return (size_t)s.B * s.Kd * rn(s) *
 
 // workspace layouts (byte offsets); also served to tests by mpgcn_debug_tc_workspace_offset()
 struct FwdLayout { size_t x16, gd16, go16, w16, u16, z16, dd, dgo, dgo_masked, total; };
-struct BwdLayout { size_t dp16, gd16, go16, v16, y16, wq16, partials, scale, total; };
-static size_t take(size_t& off, size_t bytes) {
-  off = align_up(off, 1024);
-  const size_t r = off;
-  off += bytes;
-  return r;
-}
 static FwdLayout fwd_layout(const BdgcnShape& s) {
   FwdLayout L;
   size_t off = 0;
-  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2);
-  L.gd16 = take(off, g16_elems(s, s.Kd) * 2);
-  L.go16 = take(off, g16_elems(s, s.Ko) * 2);
-  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2);    // [hi | lo]
-  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
-  L.dd = take(off, g_planes(s, s.Kd) * s.N * 4);   // support-diagonal fp16 remainders (destination / origin)
-  L.dgo = take(off, g_planes(s, s.Ko) * s.N * 4);
-  L.dgo_masked = take(off, g_planes(s, s.Ko) * s.N * 4);   // origin remainders restricted to the row slab
-  L.z16 = take(off, tc_saved_bytes(s));            // used only when the caller passes no `saved` buffer
+  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2, 1024);
+  L.gd16 = take(off, g16_elems(s, s.Kd) * 2, 1024);
+  L.go16 = take(off, g16_elems(s, s.Ko) * 2, 1024);
+  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2, 1024);    // [hi | lo]
+  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2, 1024);
+  L.dd = take(off, g_planes(s, s.Kd) * s.N * 4, 1024);   // support-diagonal fp16 remainders (destination / origin)
+  L.dgo = take(off, g_planes(s, s.Ko) * s.N * 4, 1024);
+  L.dgo_masked = take(off, g_planes(s, s.Ko) * s.N * 4, 1024);   // origin remainders restricted to the row slab
+  L.z16 = take(off, tc_saved_bytes(s), 1024);            // used only when the caller passes no `saved` buffer
   L.total = align_up(off, 1024);
   return L;
 }
@@ -158,28 +151,7 @@ static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total) {
   *kb_total = total;
   return ceil_div(total, per);
 }
-static BwdLayout bwd_layout(const BdgcnShape& s) {
-  BwdLayout L;
-  size_t off = 0;
-  L.dp16 = take(off, (size_t)s.B * s.N * s.N * s.H * 2);       // dPre: every origin row m, always
-  L.gd16 = take(off, g16_elems(s, s.Kd) * 2);
-  L.go16 = take(off, g16_elems(s, s.Ko) * 2);
-  L.v16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
-  L.y16 = take(off, (size_t)s.B * s.Kd * rn(s) * s.C * 2);
-  L.wq16 = take(off, (size_t)s.Ko * s.Kd * s.C * s.H * 2);
-  int per = 1, total = 1;
-  const int slices = dw_slices(s, &per, &total);
-  L.partials = take(off, (size_t)slices * ceil_div(dw_row_chunks(s), 4) * 128 * s.Ko * s.H * 4);
-  L.scale = take(off, 64);
-  L.total = align_up(off, 1024);
-  return L;
-}
-// deterministic mode appends the bias-gradient slots (relu_bwd_prep) to the mode-off workspace; dW and dG already reduce their
-// split-K partials in a fixed order
-size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s).total + (det_mode() ? bias_grad_slot_bytes(s.H) : 0); }
-
-// support-gradient workspace: the backward's, then X16, U16, the forward's fp16 W split and the dG partials
-struct SgradLayout { size_t x16, u16, w16, partials, total; };
+// support gradients: the dG partials
 static int dg_chunks(const BdgcnShape& s) { return ceil_div(s.N, 32); }                 // 32-column chunks of a dG row
 static int dg_r(const BdgcnShape& s) { return dg_chunks(s) < 8 ? dg_chunks(s) : 8; }   // chunks per tile
 static int dg_max_slices(const BdgcnShape& s) {
@@ -187,23 +159,41 @@ static int dg_max_slices(const BdgcnShape& s) {
   const int want = device_sm_count() / tiles;
   return want < 1 ? 1 : want;
 }
-static SgradLayout sgrad_layout(const BdgcnShape& s) {
-  SgradLayout L;
-  size_t off = bwd_layout(s).total;
-  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2);
-  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2);
-  L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2);
-  L.partials = take(off, (size_t)dg_max_slices(s) * s.N * 32 * dg_chunks(s) * 4);
-  L.total = align_up(off, 1024);
+// backward workspace; `sgrad` (the support gradient) appends X16, U16, the forward's fp16 W split and the dG partials.  Last,
+// deterministic mode's bias-gradient slots (relu_bwd_prep), empty with the mode off; dW and dG already reduce their split-K
+// partials in a fixed order.
+struct BwdLayout { size_t dp16, gd16, go16, v16, y16, wq16, partials, scale, x16, u16, w16, dg_partials, db_slots, total; };
+static BwdLayout bwd_layout(const BdgcnShape& s, bool sgrad) {
+  BwdLayout L{};
+  size_t off = 0;
+  L.dp16 = take(off, (size_t)s.B * s.N * s.N * s.H * 2, 1024);       // dPre: every origin row m, always
+  L.gd16 = take(off, g16_elems(s, s.Kd) * 2, 1024);
+  L.go16 = take(off, g16_elems(s, s.Ko) * 2, 1024);
+  L.v16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2, 1024);
+  L.y16 = take(off, (size_t)s.B * s.Kd * rn(s) * s.C * 2, 1024);
+  L.wq16 = take(off, (size_t)s.Ko * s.Kd * s.C * s.H * 2, 1024);
+  int per = 1, total = 1;
+  const int slices = dw_slices(s, &per, &total);
+  L.partials = take(off, (size_t)slices * ceil_div(dw_row_chunks(s), 4) * 128 * s.Ko * s.H * 4, 1024);
+  L.scale = take(off, 64, 1024);
+  if (sgrad) {
+    L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2, 1024);
+    L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2, 1024);
+    L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2, 1024);
+    L.dg_partials = take(off, (size_t)dg_max_slices(s) * s.N * 32 * dg_chunks(s) * 4, 1024);
+  }
+  L.db_slots = take(off, det_mode() ? bias_grad_slot_bytes(s.H) : 0, 1024);
+  L.total = off;     // the slots end the workspace unpadded
   return L;
 }
-size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return sgrad_layout(s).total + (det_mode() ? bias_grad_slot_bytes(s.H) : 0); }
+size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s, false).total; }
+size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return bwd_layout(s, true).total; }
 
 // which: 0 x16, 1 gd16, 2 go16, 3 w16, 4 u16 (forward); 10 dp16, 11 gd16, 12 go16, 13 v16, 14 y16, 15 wq16, 16 partials,
 // 17 number of dW slices (not an offset)
 long long tc_debug_offset(const BdgcnShape& s, int which) {
   const FwdLayout F = fwd_layout(s);
-  const BwdLayout Bw = bwd_layout(s);
+  const BwdLayout Bw = bwd_layout(s, false);
   int per = 1, total = 1;
   switch (which) {
     case 0: return (long long)F.x16;
@@ -513,10 +503,10 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
   return 0;
 }
 
-// form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it); db_slots: deterministic mode's bias-gradient slots
+// L: the layout, checked against the workspace; form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it)
 static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                            const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
-                            bool form_y, float* db_slots, cudaStream_t st) {
+                            const void* saved, float* dX, float* dW, float* db, void* ws, const BwdLayout& L, const BdgcnExtras& ex,
+                            bool form_y, cudaStream_t st) {
   MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
               s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
@@ -527,10 +517,9 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
   MPGCN_CHECK(((reinterpret_cast<uintptr_t>(d_out) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, "bdgcn_backward: d_out / out must be 16-byte aligned");
   const size_t NNfull = (size_t)s.N * s.N;
   const __half* z16 = static_cast<const __half*>(saved);
-  const BwdLayout L = bwd_layout(s);
-  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "workspace must be 256-byte aligned");
   uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* db_slots = det_mode() ? reinterpret_cast<float*>(wb + L.db_slots) : nullptr;    // fixed-order bias gradient
   const __half* dp16 = reinterpret_cast<__half*>(wb + L.dp16);
   __half* v16 = reinterpret_cast<__half*>(wb + L.v16);
   __half* y16 = reinterpret_cast<__half*>(wb + L.y16);
@@ -579,11 +568,9 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
                       cudaStream_t st) {
-  const size_t base = bwd_layout(s).total;
-  MPGCN_CHECK(!det_mode() || ws_bytes >= tc_bwd_ws_bytes(s), "bdgcn_backward: workspace too small for the deterministic mode (%zu < %zu bytes)",
-              ws_bytes, tc_bwd_ws_bytes(s));
-  float* db_slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + base) : nullptr;
-  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, false, db_slots, st);
+  const BwdLayout L = bwd_layout(s, false);
+  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
+  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, ex, false, st);
 }
 
 // One support-gradient contraction into the partials [slice][N][ldp] (ldp = 32 ceil(N/32): a 32-column chunk never runs into
@@ -669,23 +656,20 @@ int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const fl
                                size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st) {
   MPGCN_CHECK(s.whole(), "support gradients: whole layers only");
   MPGCN_CHECK(ex.d_pre_f16 == nullptr, "support gradients: a prepared fp16 dPre belongs to a layer part");
-  const SgradLayout S = sgrad_layout(s);
-  MPGCN_CHECK(ws_bytes >= S.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, S.total);
+  const BwdLayout L = bwd_layout(s, true);
+  MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(X) & 15) == 0, "bdgcn_backward_supports: X must be 16-byte aligned");
   const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
-  MPGCN_CHECK(ws_bytes >= tc_sgrad_ws_bytes(s), "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, tc_sgrad_ws_bytes(s));
-  float* db_slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + S.total) : nullptr;
-  if (int e = backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, ws_bytes, ex, want_d, db_slots, st)) return e;
-  const BwdLayout L = bwd_layout(s);
+  if (int e = backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, ex, want_d, st)) return e;
   uint8_t* wb = static_cast<uint8_t*>(ws);
   const __half* z16 = static_cast<const __half*>(saved);
   const __half* dp16 = reinterpret_cast<const __half*>(wb + L.dp16);
   const __half* y16 = reinterpret_cast<const __half*>(wb + L.y16);
   const float* inv_scale = reinterpret_cast<const float*>(wb + L.scale) + 1;
-  __half* x16 = reinterpret_cast<__half*>(wb + S.x16);
-  __half* u16 = reinterpret_cast<__half*>(wb + S.u16);
-  __half* w16 = reinterpret_cast<__half*>(wb + S.w16);
-  float* partials = reinterpret_cast<float*>(wb + S.partials);
+  __half* x16 = reinterpret_cast<__half*>(wb + L.x16);
+  __half* u16 = reinterpret_cast<__half*>(wb + L.u16);
+  __half* w16 = reinterpret_cast<__half*>(wb + L.w16);
+  float* partials = reinterpret_cast<float*>(wb + L.dg_partials);
   const size_t NN = (size_t)s.N * s.N;
   if (dGo) {   // U16 again, as the forward formed it (FWD_MIX of the saved Z16)
     if (int e = permute_w_mix(W, w16, w16 + (size_t)s.Ko * s.Kd * s.C * s.H, s.Ko, s.Kd, s.C, s.H, st)) return e;

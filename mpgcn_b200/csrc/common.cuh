@@ -39,6 +39,15 @@ void set_error(const char* fmt, ...);
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Each workspace has one layout function: a struct of region offsets plus `total`, read by its size query and by its call.
+// take() places a region of `bytes` at the first multiple of `align` at or after `off` and moves `off` to its end.
+static inline size_t take(size_t& off, size_t bytes, size_t align) {
+  off = align_up(off, align);
+  const size_t r = off;
+  off += bytes;
+  return r;
+}
+
 // ----------------------------------------------------------------------------------------
 // device: shared-memory addresses, mbarrier
 // ----------------------------------------------------------------------------------------

@@ -93,11 +93,22 @@ __global__ void fill_kernel(float* x, float v, int n) {
   if (i < n) x[i] = v;
 }
 
-size_t dyn_graph_workspace_bytes(int P, int N) {
-  const size_t plane = align_up((size_t)P * N * N * sizeof(float), 256);
-  const size_t vec = align_up((size_t)P * N * sizeof(float), 256);
-  return 3 * plane + 2 * vec + align_up((size_t)N * sizeof(float), 256);
+// workspace: the period mean, the row- and column-normalised planes, the squared row and column norms, and a vector of ones
+struct DynGraphLayout { size_t avg, R, Cm, rn2, cn2, ones, total; };
+static DynGraphLayout dyn_graph_layout(int P, int N) {
+  DynGraphLayout L;
+  size_t off = 0;
+  const size_t plane = (size_t)P * N * N * sizeof(float), vec = (size_t)P * N * sizeof(float);
+  L.avg = take(off, plane, 256);
+  L.R = take(off, plane, 256);
+  L.Cm = take(off, plane, 256);
+  L.rn2 = take(off, vec, 256);
+  L.cn2 = take(off, vec, 256);
+  L.ones = take(off, (size_t)N * sizeof(float), 256);
+  L.total = align_up(off, 256);
+  return L;
 }
+size_t dyn_graph_workspace_bytes(int P, int N) { return dyn_graph_layout(P, N).total; }
 
 static unsigned dg_grid(size_t work, int threads) {
   size_t b = (work + threads - 1) / threads;
@@ -107,17 +118,16 @@ static unsigned dg_grid(size_t work, int threads) {
 
 int dyn_graph_build(const float* od_hist, int periods, float* o_g, float* d_g, int P, int N, void* ws, size_t ws_bytes, cudaStream_t st) {
   MPGCN_CHECK(P >= 1 && N >= 1 && periods >= 1, "dyn_graph: bad shape P=%d N=%d periods=%d", P, N, periods);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= dyn_graph_workspace_bytes(P, N), "dyn_graph: workspace too small");
+  const DynGraphLayout L = dyn_graph_layout(P, N);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "dyn_graph: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   const size_t NN = (size_t)N * N;
-  const size_t plane = align_up((size_t)P * NN * sizeof(float), 256);
-  const size_t vec = align_up((size_t)P * N * sizeof(float), 256);
   uint8_t* w = static_cast<uint8_t*>(ws);
-  float* avg = reinterpret_cast<float*>(w);
-  float* R = reinterpret_cast<float*>(w + plane);
-  float* Cm = reinterpret_cast<float*>(w + 2 * plane);
-  float* rn2 = reinterpret_cast<float*>(w + 3 * plane);
-  float* cn2 = reinterpret_cast<float*>(w + 3 * plane + vec);
-  float* ones = reinterpret_cast<float*>(w + 3 * plane + 2 * vec);
+  float* avg = reinterpret_cast<float*>(w + L.avg);
+  float* R = reinterpret_cast<float*>(w + L.R);
+  float* Cm = reinterpret_cast<float*>(w + L.Cm);
+  float* rn2 = reinterpret_cast<float*>(w + L.rn2);
+  float* cn2 = reinterpret_cast<float*>(w + L.cn2);
+  float* ones = reinterpret_cast<float*>(w + L.ones);
 
   prof_count(PROF_ELEMENTWISE);
   period_mean_kernel<<<dg_grid((size_t)P * NN, 256), 256, 0, st>>>(od_hist, avg, P, periods, NN);

@@ -98,9 +98,8 @@ int lstm_last_forward(const float* x_seq, const float* w_ih, const float* w_hh, 
                       int B, int T, long long NN, int C, cudaStream_t s);
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
-                       long long NN, int C, cudaStream_t s, float* slots = nullptr);
-// slots of that backward in deterministic mode: one [4C x C | 4C | 4C] partial per block (<= SMs blocks)
-size_t lstm_bwd_slot_bytes(int C);
+                       long long NN, int C, void* ws, size_t ws_bytes, cudaStream_t s);
+size_t lstm_bwd_workspace_bytes(int C);
 // cells per block of the backward, which keeps every recomputed step of its cells in shared memory; 0 where not even one cell
 // fits (T above 15 at hidden 64, 95 at 48, 224 at 32) or C is outside 1..64
 int lstm_bwd_cells_per_block(int T, int C);
@@ -119,7 +118,7 @@ size_t head_bwd_slot_bytes(long long cells, int C, int M);
 // support-matrix builder (adj_kernels.cu): reference GCN.Adj_Processor.process
 enum AdjKernel { ADJ_LOCALPOOL = 0, ADJ_CHEBYSHEV = 1, ADJ_RANDOM_WALK = 2, ADJ_DUAL_RANDOM_WALK = 3 };
 int adj_num_supports(int kernel_type, int K);
-size_t adj_workspace_bytes(int B, int N, int kernel_type, int K);
+size_t adj_workspace_bytes(int B, int N);
 int adj_process(const float* flow, float* supports, int B, int N, int kernel_type, int K, void* ws, size_t ws_bytes, cudaStream_t st);
 // its adjoint: d_flow [B,N,N] from d_supports [B,Ks,N,N], reading the forward's supports (no allocation, no synchronisation)
 size_t adj_backward_workspace_bytes(int B, int N, int kernel_type, int K);
@@ -169,9 +168,20 @@ struct BdgcnShape {
 enum Precision { PREC_FP32_SIMT = 0, PREC_FP16_TC = 1 };
 
 bool tc_supported(const BdgcnShape& s);
+// buffer sizes of a layer call in either precision (api.cu), from those of each kernel family
 size_t bdgcn_saved_bytes(const BdgcnShape& s, int precision);
 size_t bdgcn_fwd_workspace_bytes(const BdgcnShape& s, int precision);
 size_t bdgcn_bwd_workspace_bytes(const BdgcnShape& s, int precision);
+size_t bdgcn_sgrad_workspace_bytes(const BdgcnShape& s, int precision);
+size_t simt_saved_bytes(const BdgcnShape& s);
+size_t simt_fwd_ws_bytes(const BdgcnShape& s);
+size_t simt_bwd_ws_bytes(const BdgcnShape& s);
+size_t simt_sgrad_ws_bytes(const BdgcnShape& s);
+size_t tc_saved_bytes(const BdgcnShape& s);
+size_t tc_fwd_ws_bytes(const BdgcnShape& s);
+size_t tc_bwd_ws_bytes(const BdgcnShape& s);
+size_t tc_sgrad_ws_bytes(const BdgcnShape& s);
+long long tc_debug_offset(const BdgcnShape& s, int which);
 
 int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
                        float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st);
@@ -197,8 +207,6 @@ int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out,
                       cudaStream_t st);
 // the backward plus the support gradients (whole layer): static supports get dGo [K][N][N] = dG_o + dG_d summed over the batch
 // (dGd unused), dynamic ones dGo [B][K][N][N] and dGd [B][K][N][N] (either nullable).  dX / dW / db are those of the backward.
-size_t tc_sgrad_ws_bytes(const BdgcnShape& s);
-size_t simt_sgrad_ws_bytes(const BdgcnShape& s);
 int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
                                const float* W, const void* saved, float* dX, float* dW, float* db, float* dGo, float* dGd, void* ws,
                                size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st);

@@ -282,11 +282,27 @@ int lstm_bwd_cells_per_block(int T, int C) {
   return (int)(cells < cap ? cells : cap);
 }
 
+// workspace of the backward: 256 bytes it does not use (the size it has always had), then deterministic mode's slots: one
+// [4C x C | 4C | 4C] partial per block (<= SMs blocks), empty with the mode off or at a hidden size the backward does not run
+struct LstmBwdLayout { size_t slots, total; };
+static LstmBwdLayout lstm_bwd_layout(int C) {
+  LstmBwdLayout L;
+  size_t off = 256;
+  L.slots = take(off, det_mode() && C >= 1 && C <= 64 ? (size_t)device_sm_count() * (4 * C * C + 8 * C) * sizeof(float) : 0, 256);
+  L.total = align_up(off, 256);
+  return L;
+}
+size_t lstm_bwd_workspace_bytes(int C) { return lstm_bwd_layout(C).total; }
+
 int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                        const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, int B, int T,
-                       long long NN, int C, cudaStream_t st, float* slots) {
+                       long long NN, int C, void* ws, size_t ws_bytes, cudaStream_t st) {
   MPGCN_CHECK(B > 0 && T > 0 && NN > 0, "lstm: empty input");
   MPGCN_CHECK(C >= 1 && C <= 64, "lstm backward: hidden size %d unsupported (1..64)", C);
+  const LstmBwdLayout L = lstm_bwd_layout(C);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, L.total);
+  float* slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + L.slots) : nullptr;   // fixed-order flush
+  MPGCN_CHECK(!slots || (reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
   const long long cells = (long long)B * NN;
   const int G = 4 * C;
   const int CELLS = lstm_bwd_cells_per_block(T, C);
@@ -319,7 +335,5 @@ int lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh,
       return e;
   return lstm_copy_bias_grad(d_b_ih, d_b_hh, G, st);
 }
-
-size_t lstm_bwd_slot_bytes(int C) { return align_up((size_t)device_sm_count() * (4 * C * C + 8 * C) * sizeof(float), 256); }
 
 }  // namespace mpgcn

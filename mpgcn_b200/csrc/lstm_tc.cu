@@ -1071,16 +1071,20 @@ static size_t lstm_tc_slot_bytes(int C, bool up) {
   return align_up(n * image * sizeof(float), 256);
 }
 
-// workspace of a backward that is handed the forward's saved state: the grad scale (1 KB), at the wide widths the da records, and
-// in deterministic mode the slots
-static size_t lstm_tc_bwd_saved_workspace_bytes(int B, int T, long long NN, int C) {
-  return 1024 + (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256)) + (det_mode() ? lstm_tc_slot_bytes(C, false) : 0);
+// workspace of the backward: the grad scale (1 KB), at the wide widths the da records, deterministic mode's slots (empty with the
+// mode off) and, for a call without a saved buffer from the forward (`rebuild`), room to re-run the (training) forward into
+struct LstmTcBwdLayout { size_t scale, da, slots, saved, total; };
+static LstmTcBwdLayout lstm_tc_bwd_layout(int B, int T, long long NN, int C, bool rebuild) {
+  LstmTcBwdLayout L;
+  size_t off = 0;
+  L.scale = take(off, 1024, 256);
+  L.da = take(off, C == 32 ? 0 : lstm_tcw_da_bytes(B, T, NN, C), 256);
+  L.slots = take(off, det_mode() ? lstm_tc_slot_bytes(C, false) : 0, 256);
+  L.saved = take(off, rebuild ? lstm_tc_saved_bytes(B, T, NN, C) : 0, 256);
+  L.total = align_up(off, 256);
+  return L;
 }
-
-// without a saved buffer from the forward, the backward first re-runs the (training) forward into its workspace
-size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) {
-  return lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C) + align_up(lstm_tc_saved_bytes(B, T, NN, C), 256);
-}
+size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) { return lstm_tc_bwd_layout(B, T, NN, C, true).total; }
 
 template <int CH>
 static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
@@ -1189,18 +1193,17 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
                           const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
                           int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
   const long long cells = (long long)B * NN;
-  const size_t need = saved ? lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C) : lstm_tc_bwd_workspace_bytes(B, T, NN, C);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, need);
+  const LstmTcBwdLayout L = lstm_tc_bwd_layout(B, T, NN, C, saved == nullptr);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, L.total);
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm backward: saved buffer must be 16-byte aligned");
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
   MPGCN_CHECK(C == 32 || C == 96 || C == 128, "lstm backward: no tensor-core kernel for hidden=%d", C);
-  float* scale2 = static_cast<float*>(ws);
-  void* da_rec = static_cast<uint8_t*>(ws) + 1024;   // wide widths: the da records follow the grad scale, then the slots
-  float* slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024 +
-                                                       (C == 32 ? 0 : align_up(lstm_tcw_da_bytes(B, T, NN, C), 256)))
-                            : nullptr;
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* scale2 = reinterpret_cast<float*>(wb + L.scale);
+  void* da_rec = wb + L.da;
+  float* slots = det_mode() ? reinterpret_cast<float*>(wb + L.slots) : nullptr;     // fixed-order flush instead of atomics
   if (saved == nullptr) {          // the caller kept no forward state: rebuild it (same kernel, same bits as the training forward)
-    void* tmp = static_cast<uint8_t*>(ws) + lstm_tc_bwd_saved_workspace_bytes(B, T, NN, C);
+    void* tmp = wb + L.saved;
     if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C, st)) return e;
     saved = tmp;
   }
@@ -1225,27 +1228,38 @@ bool lstm_tc_stack_supported(int T, int C, int L) { return L >= 2 && (C == 32 ||
 // training state of the stack: one lstm_tc_saved_bytes block per layer (multiples of 256 bytes)
 size_t lstm_tc_stack_saved_bytes(int B, int T, long long NN, int C, int L) { return (size_t)L * lstm_tc_saved_bytes(B, T, NN, C); }
 
-// the h-only sequence (C halves per cell and step) an inference layer hands to the layer above
-static size_t lstm_tc_hseq_bytes(int B, int T, long long NN, int C) {
-  return align_up((size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(__half), 256);
+// inference forward: the h-only sequences (C halves per cell and step) that an inference layer hands to the layer above, of two
+// consecutive layers (layer l writes h[l & 1]; one sequence for L = 2)
+struct StackFwdLayout { size_t h[2], total; };
+static StackFwdLayout stack_fwd_layout(int B, int T, long long NN, int C, int L) {
+  StackFwdLayout Y;
+  size_t off = 0;
+  const size_t hseq = (size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(__half);
+  Y.h[0] = take(off, hseq, 256);
+  Y.h[1] = L >= 3 ? take(off, hseq, 256) : Y.h[0];
+  Y.total = align_up(off, 256);
+  return Y;
 }
+size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L) { return stack_fwd_layout(B, T, NN, C, L).total; }
 
-// inference forward: the h sequences of two consecutive layers (one for L = 2)
-size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L) {
-  return (L >= 3 ? 2 : 1) * lstm_tc_hseq_bytes(B, T, NN, C);
+// backward: the grad scale (1 KB), the fp32 gradient sequence d(h^{l-1}_t) between consecutive walks (lstm_tc::dseq_off),
+// deterministic mode's slots of the dW passes (lstm_tc_slot_bytes of an upper layer, the largest; empty with the mode off) and
+// the da records of one layer (the layers run one after another).  A workspace of `every_layer` bytes keeps every layer's
+// records (layer l at da + l * da_stride) instead of reusing one region, so that they can be read back after the call.
+struct StackBwdLayout { size_t scale, d_seq, slots, da, da_stride, total, every_layer; };
+static StackBwdLayout stack_bwd_layout(int B, int T, long long NN, int C, int L) {
+  StackBwdLayout Y;
+  size_t off = 0;
+  Y.scale = take(off, 1024, 256);
+  Y.d_seq = take(off, (size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(float), 256);
+  Y.slots = take(off, det_mode() ? lstm_tc_slot_bytes(C, true) : 0, 256);
+  Y.da_stride = align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
+  Y.da = take(off, Y.da_stride, 256);
+  Y.total = off;
+  Y.every_layer = off + (size_t)(L - 1) * Y.da_stride;
+  return Y;
 }
-
-// backward: the grad scale (1 KB), the fp32 gradient sequence d(h^{l-1}_t) between consecutive walks (lstm_tc::dseq_off) and
-// the da records of one layer (the layers run one after another).  A workspace with room for L da regions keeps every
-// layer's records (layer l in region l) instead of reusing one, so that they can be read back after the call.
-static size_t lstm_tc_stack_dseq_bytes(int B, int T, long long NN, int C) {
-  return align_up((size_t)lstm_tc_padded_cells(B, NN, C) * T * C * sizeof(float), 256);
-}
-// deterministic mode: the slots of the dW passes (lstm_tc_slot_bytes of an upper layer, the largest) sit before the da records
-static size_t lstm_tc_stack_slot_bytes(int C) { return det_mode() ? lstm_tc_slot_bytes(C, true) : 0; }
-size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int /*L*/) {
-  return 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + lstm_tc_stack_slot_bytes(C) + align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
-}
+size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L) { return stack_bwd_layout(B, T, NN, C, L).total; }
 
 template <int CH, bool SAVE, bool UP, bool HSEQ>
 static int stack_fwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
@@ -1266,12 +1280,13 @@ static int stack_fwd_layer(const float* x_seq, const float* w_ih, const float* w
 
 template <int CH>
 static int stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                         const float* const* b_hh, float* hT, void* saved, void* ws, int B, int T, long long NN, cudaStream_t st) {
+                         const float* const* b_hh, float* hT, void* saved, void* ws, const StackFwdLayout& Y, int B, int T, long long NN,
+                         cudaStream_t st) {
   const int C = 32 * CH;
   const long long cells = (long long)B * NN;
-  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C), hseq_bytes = lstm_tc_hseq_bytes(B, T, NN, C);
+  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
   auto lsaved = [&](int l) { return static_cast<uint8_t*>(saved) + (size_t)l * layer_bytes; };
-  auto hbuf = [&](int l) { return static_cast<uint8_t*>(ws) + (size_t)(l & 1) * hseq_bytes; };   // inference: h of layer l
+  auto hbuf = [&](int l) { return static_cast<uint8_t*>(ws) + Y.h[l & 1]; };   // inference: h of layer l
   for (int l = 0; l < L; ++l) {
     const bool top = l == L - 1;
     float* out = top ? hT : nullptr;
@@ -1348,13 +1363,13 @@ int lstm_stack_forward_tc(const float* x_seq, int L, const float* const* w_ih, c
                           cudaStream_t st) {
   MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack forward: saved buffer must be 256-byte aligned");
-  if (saved == nullptr) {
-    const size_t need = lstm_tc_stack_fwd_workspace_bytes(B, T, NN, C, L);
-    MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm stack forward: workspace too small (%zu < %zu)", ws_bytes, need);
+  const StackFwdLayout Y = stack_fwd_layout(B, T, NN, C, L);
+  if (saved == nullptr) {      // inference: the h sequences live in the workspace
+    MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack forward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
     MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack forward: workspace must be 256-byte aligned");
   }
-  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, B, T, NN, st)
-                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, B, T, NN, st);
+  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, Y, B, T, NN, st)
+                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, Y, B, T, NN, st);
 }
 
 int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
@@ -1362,17 +1377,17 @@ int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, 
                            float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,
                            int C, const float* d_hT_absmax, cudaStream_t st) {
   MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
-  const size_t need = lstm_tc_stack_bwd_workspace_bytes(B, T, NN, C, L);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= need, "lstm stack backward: workspace too small (%zu < %zu)", ws_bytes, need);
+  const StackBwdLayout Y = stack_bwd_layout(B, T, NN, C, L);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack backward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack backward: saved buffer must be 256-byte aligned");
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack backward: workspace must be 256-byte aligned");
   const long long cells = (long long)B * NN;
-  float* scale2 = static_cast<float*>(ws);
-  float* d_seq = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024);
-  float* slots = det_mode() ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C)) : nullptr;
-  uint8_t* da_rec = static_cast<uint8_t*>(ws) + 1024 + lstm_tc_stack_dseq_bytes(B, T, NN, C) + lstm_tc_stack_slot_bytes(C);
-  const size_t da_region = align_up(lstm_tcw_da_bytes(B, T, NN, C), 256);
-  const size_t da_stride = ws_bytes >= need + (size_t)(L - 1) * da_region ? da_region : 0;     // every layer's records, or one region
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* scale2 = reinterpret_cast<float*>(wb + Y.scale);
+  float* d_seq = reinterpret_cast<float*>(wb + Y.d_seq);
+  float* slots = det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr;     // fixed-order flush instead of atomics
+  uint8_t* da_rec = wb + Y.da;
+  const size_t da_stride = ws_bytes >= Y.every_layer ? Y.da_stride : 0;     // every layer's records, or one region
   // one gradient scale S for the whole stack, from max|d_hT|: every walk keeps dh, dc and d_seq in units of S
   if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
   const int G4 = 4 * C;

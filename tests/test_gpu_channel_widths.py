@@ -132,8 +132,8 @@ def test_lstm_keeps_its_fp32_kernels_at_hidden_64():
 # one layer through the C ABI at any width, the chunk layouts read back from the workspaces
 # ------------------------------------------------------------------------------------------------------------------------------
 class Layout(dict):
-    """name -> byte offset of consecutive regions, each starting at a multiple of `align` (bdgcn_tc.cu `take`: 1024; bdgcn_simt.cu
-    `Carver`: 256); .size[name] = its bytes, .total = the workspace size the library asks for (`slack` bytes added)."""
+    """name -> byte offset of consecutive regions, each starting at a multiple of `align` (bdgcn_tc.cu layouts: 1024; bdgcn_simt.cu
+    layouts: 256); .size[name] = its bytes, .total = the workspace size the library asks for (`slack` bytes added)."""
 
     def __init__(self, parts, align=1024, slack=0):
         super().__init__()
@@ -173,7 +173,7 @@ def ws_layout(B, N, K, C, H, dyn, sms):
 
 
 def simt_ws_layout(B, N, C, H, R, Ko, Kd):
-    """The fp32 family's workspaces (bdgcn_simt.cu `Carver`): forward U (Z lives in `saved`; its region serves only a call without
+    """The fp32 family's workspaces (bdgcn_simt.cu simt_fwd_layout / simt_bwd_layout): forward U (Z lives in `saved`; its region serves only a call without
     one); backward dPre (whole layer: a part reads the caller's), V, Y, Wq [d][o][h][l].  The size functions add 256 / 1024 bytes."""
     RN = R * N
     fwd = Layout([("u", B * Ko * RN * H * 4), ("z", B * Kd * RN * C * 4)], 256, 256)

@@ -128,7 +128,7 @@ def test_part_cases_cover_slabs_subsets_widths_kinds_and_scales():
 
 
 def test_fp32_workspace_layouts_match_the_library_sizes():
-    """the Carver layouts of bdgcn_simt.cu (and the tensor-core forward layout, which does not depend on the SM count) against the
+    """the fp32 layouts of bdgcn_simt.cu (and the tensor-core forward layout, which does not depend on the SM count) against the
     sizes the library reports; the backward tensor-core layout is checked on the GPU, inside run_layer_wide"""
     lib = _lib.load()
     for C, H, N, K, Ko, Kd, R, row0, B, dyn, _ in FP32_CASES:

@@ -72,9 +72,9 @@ def dg_max_slices(N, sms):
 
 
 def sgrad_ws_layout(B, N, K, C, H, dyn, prec, sms):
-    """The support-gradient workspace (tensor cores: bdgcn_tc.cu sgrad_layout; fp32: bdgcn_simt.cu) -> (its Layout, the backward's
-    Layout it begins with).  Tensor cores: the backward's regions, X16, U16, the fp16 W split and the fp32 partials
-    [slice][N][32 ceil(N/32)], 1024-aligned; fp32: the backward's Carver regions, then U, 256-aligned (the size adds 1024 + 256)."""
+    """The support-gradient workspace (tensor cores: bdgcn_tc.cu bwd_layout(s, true); fp32: bdgcn_simt.cu simt_bwd_layout(s, true))
+    -> (its Layout, the backward's Layout it begins with).  Tensor cores: the backward's regions, X16, U16, the fp16 W split and the fp32 partials
+    [slice][N][32 ceil(N/32)], 1024-aligned; fp32: the backward's regions, then U, 256-aligned (the size adds 1024 + 256)."""
     if prec == 1:
         _, bo = ws_layout(B, N, K, C, H, dyn, sms)
         chunks = -(-N // 32)
