@@ -138,6 +138,30 @@ MPGCN_API int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out
                                   int B, int N, int K, int C, int H, int precision, const mpgcn_bdgcn_extras* extras, const float* X,
                                   float* dG_o, float* dG_d, void* stream);
 
+/* ---- Sparse static supports (DESIGN.md section 12) --------------------------------------------------------------------------------
+ * A static [K,N,N] stack given by its nonzeros runs the precision-0 layer with its four N^3 contractions (Z = X x_2 G_d,
+ * out = sum_o G_o^T x_1 U_o, V = G_o x_1 dPre, dX = sum_d Y_d x_2 G_d^T) replaced by gathers over the stored entries: 2 B N nnz ch
+ * flops each instead of 2 B K N^3 ch.  Results are fp32, each output element summed in a fixed order (support, then ascending index),
+ * so they do not depend on mpgcn_set_deterministic.  Only stored entries are multiplied: a non-finite X does not reach an output
+ * through a zero of G (the dense layer's 0 * inf = NaN).
+ *   mpgcn_sparse_supports_build: indices [3][nnz] int64 (support k, row, column; torch's COO `indices()`), values [nnz] fp32, in any
+ *   order; duplicates are kept and add up; entries outside [0,K) x [0,N) x [0,N) are ignored.  Builds the CSR and CSC of every support
+ *   (int32 indices) into `supports` (mpgcn_sparse_supports_bytes, 256-byte aligned; 0 for K < 1, N < 1, nnz < 0 or nnz >= 2^31)
+ *   with a counting sort on the device, without synchronising.  The buffer must stay unmodified while layer calls use it.
+ *   mpgcn_bdgcn_forward_sparse / _backward_sparse: mpgcn_bdgcn_forward / _backward (precision 0, static supports) with G_o, G_d and
+ *   `dynamic` replaced by that buffer, its size and nnz.  saved, workspaces: the precision-0 queries (mpgcn_bdgcn_saved_bytes,
+ *   mpgcn_bdgcn_fwd / _bwd_workspace_bytes with dynamic 0, precision 0).  Every argument is checked before the first CUDA call.
+ *   Their gathers count as tag 7 (fp32 SIMT) launches with flops 2 B N nnz ch; they open no layer region (tags 11, 12). */
+MPGCN_API size_t mpgcn_sparse_supports_bytes(int K, int N, long long nnz);
+MPGCN_API int mpgcn_sparse_supports_build(const long long* indices, const float* values, long long nnz, int K, int N, void* supports,
+                                          size_t supports_bytes, void* stream);
+MPGCN_API int mpgcn_bdgcn_forward_sparse(const float* X, const void* supports, size_t supports_bytes, long long nnz, const float* W,
+                                         const float* bias, int act, float* out, void* saved, void* workspace, size_t workspace_bytes,
+                                         int B, int N, int K, int C, int H, void* stream);
+MPGCN_API int mpgcn_bdgcn_backward_sparse(const float* d_out, const float* out, const void* supports, size_t supports_bytes, long long nnz,
+                                          const float* W, int act, const void* saved, float* dX, float* dW, float* db, void* workspace,
+                                          size_t workspace_bytes, int B, int N, int K, int C, int H, void* stream);
+
 /* ---- PARTS of a layer: what one GPU evaluates when a layer is sharded (SURVEY.md section 8(e)) -----------------------------------
  * The reference has no multi-GPU code; these entry points are the engine's own addition behind the same BDGCN.forward math
  * (MPGCN.py:24-50).  A part is described by

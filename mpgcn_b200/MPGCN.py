@@ -15,7 +15,7 @@ and the trainer runs unchanged on our kernels.  What is kept identical to the re
     (reference MPGCN.py:26-42, 95-96).
 
 What differs: the arithmetic.  No einsum / cat / cuDNN -- `BDGCN.forward` is one call of
-`ops.bdgcn` (factored 2K-contraction engine) and the per-cell LSTM is `ops.lstm_module_last`, which reads
+`ops.bdgcn` (factored 2K-contraction engine; a static G may be a sparse COO tensor, DESIGN.md section 12) and the per-cell LSTM is `ops.lstm_module_last`, which reads
 `x_seq` in place, assumes the zero initial state the reference always passes (MPGCN.py:80-87,98) and
 never materialises the `[B*N*N, T, C]` output sequence.
 """
@@ -70,7 +70,8 @@ class BDGCN(nn.Module):
             assert G[0].dim() == 4 and G[1].dim() == 4 and G[0].shape[0] == X.shape[0] == G[1].shape[0]
         else:
             raise NotImplementedError
-        assert X.dim() == 4 and X.shape[1] == X.shape[2] == G[0].shape[-1] and X.shape[3] == self.input_dim
+        N = (G if isinstance(G, torch.Tensor) else G[0]).shape[-1]      # (no select on a sparse stack)
+        assert X.dim() == 4 and X.shape[1] == X.shape[2] == N and X.shape[3] == self.input_dim
         act = self.fused_act()
         out = ops.bdgcn(X, G, self.W, self.b if self.use_bias else None, relu=act == 1, precision=self.precision,
                         support_grad=self.support_grad)

@@ -217,6 +217,47 @@ int mpgcn_bdgcn_backward_part(const float* d_pre, const float* G_o, const float*
   return bdgcn_backward_simt(s, d_pre, nullptr, G_o, G_d, W, saved, dX, dW, nullptr, workspace, workspace_bytes, st);
 }
 
+size_t mpgcn_sparse_supports_bytes(int K, int N, long long nnz) { return sparse_supports_bytes(K, N, nnz); }
+
+int mpgcn_sparse_supports_build(const long long* indices, const float* values, long long nnz, int K, int N, void* supports,
+                                size_t supports_bytes, void* stream) {
+  MPGCN_CHECK(sparse_shape_ok(K, N, nnz), "mpgcn_sparse_supports_build: bad stack K=%d N=%d nnz=%lld (int32 indices: nnz < 2^31)", K, N, nnz);
+  MPGCN_CHECK(supports && (nnz == 0 || (indices && values)), "mpgcn_sparse_supports_build: null pointer argument");
+  MPGCN_CHECK(supports_bytes >= sparse_supports_bytes(K, N, nnz), "mpgcn_sparse_supports_build: buffer too small (%zu < %zu bytes)",
+              supports_bytes, sparse_supports_bytes(K, N, nnz));
+  return sparse_supports_build(indices, values, nnz, K, N, supports, static_cast<cudaStream_t>(stream));
+}
+
+static int check_sparse(const char* what, const BdgcnShape& s, const void* supports, size_t supports_bytes, long long nnz) {
+  if (int e = check_shape(s, PREC_FP32_SIMT)) return e;
+  MPGCN_CHECK(sparse_shape_ok(s.K, s.N, nnz), "%s: bad support stack K=%d N=%d nnz=%lld", what, s.K, s.N, nnz);
+  MPGCN_CHECK(supports != nullptr, "%s: null pointer argument", what);
+  MPGCN_CHECK(supports_bytes >= sparse_supports_bytes(s.K, s.N, nnz), "%s: support buffer too small (%zu < %zu bytes)", what,
+              supports_bytes, sparse_supports_bytes(s.K, s.N, nnz));
+  return 0;
+}
+
+int mpgcn_bdgcn_forward_sparse(const float* X, const void* supports, size_t supports_bytes, long long nnz, const float* W, const float* bias,
+                               int act, float* out, void* saved, void* workspace, size_t workspace_bytes, int B, int N, int K, int C, int H,
+                               void* stream) {
+  const BdgcnShape s = mk(B, N, K, C, H, 0, act);
+  if (int e = check_sparse("mpgcn_bdgcn_forward_sparse", s, supports, supports_bytes, nnz)) return e;
+  MPGCN_CHECK(X && W && out && workspace, "mpgcn_bdgcn_forward_sparse: null pointer argument");
+  const SparseSupports sp = sparse_supports_view(supports, K, N, nnz);
+  return bdgcn_forward_simt(s, X, nullptr, nullptr, W, bias, out, saved, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), &sp);
+}
+
+int mpgcn_bdgcn_backward_sparse(const float* d_out, const float* out, const void* supports, size_t supports_bytes, long long nnz,
+                                const float* W, int act, const void* saved, float* dX, float* dW, float* db, void* workspace,
+                                size_t workspace_bytes, int B, int N, int K, int C, int H, void* stream) {
+  const BdgcnShape s = mk(B, N, K, C, H, 0, act);
+  if (int e = check_sparse("mpgcn_bdgcn_backward_sparse", s, supports, supports_bytes, nnz)) return e;
+  MPGCN_CHECK(d_out && out && W && saved && dW && workspace, "mpgcn_bdgcn_backward_sparse: null pointer argument");
+  const SparseSupports sp = sparse_supports_view(supports, K, N, nnz);
+  return bdgcn_backward_simt(s, d_out, out, nullptr, nullptr, W, saved, dX, dW, db, workspace, workspace_bytes,
+                             static_cast<cudaStream_t>(stream), &sp);
+}
+
 int mpgcn_bias_act(float* x, const float* bias, int act, long long n, int H, void* stream) {
   MPGCN_CHECK(x && n >= 1 && (act == 0 || act == 1), "mpgcn_bias_act: bad argument");
   return bias_act_inplace(x, bias, act, (size_t)n, H, static_cast<cudaStream_t>(stream));

@@ -13,6 +13,8 @@
 //     dX[b,n,c,l]  = sum_{d,e} Y[b,d,n,e,l] G_d[c,e]
 //   support gradients (opt-in; U recomputed from the Z stash)
 //     dG_o[n,m] = sum_{b,e,h} U_o[b,n,e,h] dPre[b,m,e,h]     dG_d[c,e] = sum_{b,n,l} X[b,n,c,l] Y_d[b,n,e,l]
+// Sparse static supports (bdgcn_sparse.cu) replace the four N^3 stages (Z, out, V, dX) by gathers over their nonzeros; the mix
+// stages, dW, Y, the layouts and the stash stay these.
 #include "kernels.h"
 
 namespace mpgcn {
@@ -68,7 +70,7 @@ static void zero3(long long (&a)[3]) { a[0] = a[1] = a[2] = 0; }
 // Activations are [B][*][R rows n][N][ch] slabs (rows [row0, row0 + R) of the N origins), G_d has Kd planes, G_o has Ko,
 // W is the [Ko][Kd][C][H] slice; `partial`: the forward stops at the raw partial pre-activation, the backward starts from dPre.
 int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
-                       float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st) {
+                       float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st, const SparseSupports* sp) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const SimtFwdLayout L = simt_fwd_layout(s);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_forward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
@@ -77,7 +79,9 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
   float* Z = saved ? static_cast<float*>(saved) : reinterpret_cast<float*>(wb + L.z);
   const long long go_sb = s.dynamic ? Ko * NN : 0, gd_sb = s.dynamic ? Kd * NN : 0;   // support batch strides
 
-  {  // Z[b,d,n] (e x l) = G_d^T (e x c) * X[b,n] (c x l)
+  if (sp) {
+    if (int e = sparse_stage(SPARSE_FWD_A, s, *sp, X, Z, nullptr, st)) return e;
+  } else {  // Z[b,d,n] (e x l) = G_d^T (e x c) * X[b,n] (c x l)
     SgemmParams p{};
     p.A = Gd; p.B = X; p.D = Z;
     p.M = (int)N; p.N = (int)C; p.K = (int)N;
@@ -103,7 +107,9 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
     p.ksplit = 1; p.alpha = 1.f;
     if (int e = simt_sgemm(p, st)) return e;
   }
-  {  // out[b] (m x (e,h)) = act( sum_o G_o[row0.., :]^T (m x n) * U[b,o] (n x (e,h)) + bias[h] ): one k-segment per support
+  if (sp) {
+    if (int e = sparse_stage(SPARSE_FWD_B, s, *sp, U, out, bias, st)) return e;
+  } else {  // out[b] (m x (e,h)) = act( sum_o G_o[row0.., :]^T (m x n) * U[b,o] (n x (e,h)) + bias[h] ): one k-segment per support
     SgemmParams p{};
     p.A = Go + (long long)s.row0 * N; p.B = U; p.D = out;
     p.M = (int)N; p.N = (int)(N * H); p.K = (int)R;
@@ -122,7 +128,7 @@ int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, con
 // L: the layout, checked against the workspace; form_y: form Y even without dX (the support gradient reads it)
 static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                               const void* saved, float* dX, float* dW, float* db, void* ws, const SimtBwdLayout& L, bool form_y,
-                              cudaStream_t st) {
+                              cudaStream_t st, const SparseSupports* sp) {
   const long long N = s.N, R = s.R, RN = R * N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   MPGCN_CHECK(Z != nullptr, "bdgcn_backward: forward was run without a `saved` buffer");
@@ -142,7 +148,9 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
     dP = dPre;
   }
 
-  {  // V[b,o] (n x (e,h)) = G_o[row0.., :] (n x m) * dPre[b] (m x (e,h))
+  if (sp) {
+    if (int e = sparse_stage(SPARSE_BWD_V, s, *sp, dP, V, nullptr, st)) return e;
+  } else {  // V[b,o] (n x (e,h)) = G_o[row0.., :] (n x m) * dPre[b] (m x (e,h))
     SgemmParams p{};
     p.A = Go + (long long)s.row0 * N; p.B = dP; p.D = V;
     p.M = (int)R; p.N = (int)(N * H); p.K = (int)N;
@@ -195,7 +203,9 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
       p.ksplit = 1; p.alpha = 1.f;
       if (int e = simt_sgemm(p, st)) return e;
     }
-    if (dX) {  // dX[b,n] (c x l) = sum_d G_d (c x e) * Y[b,d,n] (e x l)
+    if (dX && sp) {
+      if (int e = sparse_stage(SPARSE_BWD_DX, s, *sp, Y, dX, nullptr, st)) return e;
+    } else if (dX) {  // dX[b,n] (c x l) = sum_d G_d (c x e) * Y[b,d,n] (e x l)
       SgemmParams p{};
       p.A = Gd; p.B = Y; p.D = dX;
       p.M = (int)N; p.N = (int)C; p.K = (int)N;
@@ -218,10 +228,11 @@ static int backward_simt_impl(const BdgcnShape& s, const float* d_out, const flo
 namespace mpgcn {
 
 int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st) {
+                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st,
+                        const SparseSupports* sp) {
   const SimtBwdLayout L = simt_bwd_layout(s, false);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
-  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, false, st);
+  return backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, false, st, sp);
 }
 
 int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,
@@ -231,7 +242,7 @@ int bdgcn_backward_supports_simt(const BdgcnShape& s, const float* d_out, const 
   const SimtBwdLayout L = simt_bwd_layout(s, true);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward_supports: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   const bool want_d = dGd != nullptr || (!s.dynamic && dGo != nullptr);
-  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, want_d, st)) return e;
+  if (int e = backward_simt_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, want_d, st, nullptr)) return e;
   const long long N = s.N, NN = N * N, C = s.C, H = s.H, Ko = s.Ko, Kd = s.Kd;
   const float* Z = static_cast<const float*>(saved);
   uint8_t* wb = static_cast<uint8_t*>(ws);

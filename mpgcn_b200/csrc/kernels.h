@@ -183,10 +183,35 @@ size_t tc_bwd_ws_bytes(const BdgcnShape& s);
 size_t tc_sgrad_ws_bytes(const BdgcnShape& s);
 long long tc_debug_offset(const BdgcnShape& s, int which);
 
+// ---- sparse static supports (bdgcn_sparse.cu): CSR and CSC of a [K,N,N] stack in one device buffer ----------------------
+struct SparseSupports {
+  int K, N;
+  long long nnz;
+  const int* csr_ptr;          // [K][N + 1] offsets into csr_idx / csr_val (row r of support k: [ptr[k][r], ptr[k][r + 1]))
+  const int* csr_idx;          // column of each nonzero, ascending within a row
+  const float* csr_val;
+  const int* csc_ptr;          // the same for G^T: column c of support k, its rows ascending
+  const int* csc_idx;
+  const float* csc_val;
+};
+// K >= 1, N >= 1, 0 <= nnz < 2^31 (int32 indices)
+bool sparse_shape_ok(int K, int N, long long nnz);
+size_t sparse_supports_bytes(int K, int N, long long nnz);
+// indices [3][nnz] int64 (support, row, column), values [nnz]: any order, duplicates kept (they add up); entries outside the stack
+// are ignored.  No host synchronisation.
+int sparse_supports_build(const long long* indices, const float* values, long long nnz, int K, int N, void* buf, cudaStream_t st);
+SparseSupports sparse_supports_view(const void* buf, int K, int N, long long nnz);
+// the four N^3 stages of the fp32 layer as gathers over the nonzeros (whole static layers); bias / act: FWD_B's epilogue
+enum SparseStage { SPARSE_FWD_A, SPARSE_FWD_B, SPARSE_BWD_V, SPARSE_BWD_DX };
+int sparse_stage(SparseStage stage, const BdgcnShape& s, const SparseSupports& sp, const float* in, float* out, const float* bias,
+                 cudaStream_t st);
+
+// sp (nullable): sparse static supports, whose gathers replace the four N^3 SGEMMs (Go / Gd unused)
 int bdgcn_forward_simt(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
-                       float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st);
+                       float* out, void* saved, void* ws, size_t ws_bytes, cudaStream_t st, const SparseSupports* sp = nullptr);
 int bdgcn_backward_simt(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
-                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st);
+                        const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, cudaStream_t st,
+                        const SparseSupports* sp = nullptr);
 // optional side inputs / outputs of the tensor-core layer (mirror of mpgcn_bdgcn_extras in include/mpgcn_b200.h); all nullable
 struct BdgcnExtras {
   const void* go_prepared = nullptr;    // supports already converted by bdgcn_prepare_supports (fp16 padded + diagonal remainders)

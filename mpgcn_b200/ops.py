@@ -1,6 +1,7 @@
 """Autograd-aware operators of the hot path, each a thin call into the C ABI.
 
-    bdgcn(X, G, W, b, activation)  <->  reference BDGCN.forward           (MPGCN.py:24-50), dL/dG too with support_grad=True
+    bdgcn(X, G, W, b, activation)  <->  reference BDGCN.forward           (MPGCN.py:24-50), dL/dG too with support_grad=True;
+                                        a sparse COO static G runs the gathers over its nonzeros (DESIGN.md section 12)
     lstm_last(x_seq, w_ih, w_hh, b_ih, b_hh)  <->  nn.LSTM(...)[:, -1, :]  (MPGCN.py:69,100-104)
     lstm_stack(x_seq, params, precision)      <->  the same with num_layers = L >= 2
     lstm_module_last(lstm, x_seq, precision)  <->  either of them, or the module itself where the engine has no kernel
@@ -102,35 +103,64 @@ def _take_hint(node, grad):
 
 
 # Supports staged once: the same G_o / G_d serve every layer of a branch, forward and backward (6 calls per training step),
-# so their fp16 conversion (+ diagonal remainders) is cached per support TENSOR OBJECT.  An entry is valid only while that
-# very object is alive (weak reference), unmodified (version counter), at the same address and used on the same stream.
+# so their fp16 conversion (+ diagonal remainders) -- or, for a sparse stack, its CSR / CSC structure -- is cached per support
+# TENSOR OBJECT.  An entry is valid only while that very object is alive (weak reference), unmodified (version counter), at the
+# same address (a sparse stack: of its values) and used on the same stream.
 _SUPPORT_CACHE = {}
+_SPARSE_CACHE = {}
 _SUPPORT_CACHE_MAX = 8
 
 
-def _prepared_supports(lib, G, Gc, planes: int, N: int):
+def _cached(cache, G, ptr: int, make):
     import weakref
     key = id(G)
     stream = _stream()
-    e = _SUPPORT_CACHE.get(key)
+    e = cache.get(key)
     if e is not None:
-        ref, ver, ptr, st, blob = e
-        if ref() is G and ver == G._version and ptr == Gc.data_ptr() and st == stream and blob.device == Gc.device:
-            return blob
-        del _SUPPORT_CACHE[key]
-    for k in [k for k, v in _SUPPORT_CACHE.items() if v[0]() is None]:      # supports that no longer exist: free their staging now
-        del _SUPPORT_CACHE[k]
-    while len(_SUPPORT_CACHE) >= _SUPPORT_CACHE_MAX:
-        _SUPPORT_CACHE.pop(next(iter(_SUPPORT_CACHE)))
-    nbytes = lib.mpgcn_bdgcn_supports_prepared_bytes(planes, N)
-    blob = torch.empty(nbytes, dtype=torch.uint8, device=Gc.device)
-    with torch.cuda.device(Gc.device):
-        _lib.check(lib.mpgcn_bdgcn_prepare_supports(_ptr(Gc), _ptr(blob), nbytes, planes, N, stream), "bdgcn_prepare_supports")
+        ref, ver, p, st, dev, val = e
+        if ref() is G and ver == G._version and p == ptr and st == stream and dev == G.device:
+            return val
+        del cache[key]
+    for k in [k for k, v in cache.items() if v[0]() is None]:      # supports that no longer exist: free their staging now
+        del cache[k]
+    while len(cache) >= _SUPPORT_CACHE_MAX:
+        cache.pop(next(iter(cache)))
+    val = make(stream)
     try:
-        _SUPPORT_CACHE[key] = (weakref.ref(G), G._version, Gc.data_ptr(), stream, blob)
+        cache[key] = (weakref.ref(G), G._version, ptr, stream, G.device, val)
     except TypeError:        # not weak-referenceable: do not cache
         pass
-    return blob
+    return val
+
+
+def _prepared_supports(lib, G, Gc, planes: int, N: int):
+    def make(stream):
+        nbytes = lib.mpgcn_bdgcn_supports_prepared_bytes(planes, N)
+        blob = torch.empty(nbytes, dtype=torch.uint8, device=Gc.device)
+        with torch.cuda.device(Gc.device):
+            _lib.check(lib.mpgcn_bdgcn_prepare_supports(_ptr(Gc), _ptr(blob), nbytes, planes, N, stream), "bdgcn_prepare_supports")
+        return blob
+    return _cached(_SUPPORT_CACHE, G, Gc.data_ptr(), make)
+
+
+def _sparse_supports(lib, G, K: int, N: int):
+    """(structure, nnz) of a sparse COO stack [K,N,N]: CSR and CSC of every support, built on the device (mpgcn_sparse_supports_build)
+    from the coalesced tensor, so that duplicate entries add up as in the dense sum."""
+    def make(stream):
+        Gc = G.detach()
+        if not Gc.is_coalesced():
+            Gc = Gc.coalesce()
+        idx = Gc._indices().contiguous()
+        val = Gc._values().to(torch.float32).contiguous()
+        nnz = val.numel()
+        nbytes = lib.mpgcn_sparse_supports_bytes(K, N, nnz)
+        if nbytes == 0:
+            raise RuntimeError(f"mpgcn_b200.bdgcn: a sparse support stack holds {nnz} nonzeros; its int32 indices take fewer than 2^31")
+        blob = torch.empty(nbytes, dtype=torch.uint8, device=G.device)
+        with torch.cuda.device(G.device):
+            _lib.check(lib.mpgcn_sparse_supports_build(_ptr(idx), _ptr(val), nnz, K, N, _ptr(blob), nbytes, stream), "sparse_supports_build")
+        return blob, nnz
+    return _cached(_SPARSE_CACHE, G, G._values().data_ptr(), make)
 
 
 class _BDGCNFn(torch.autograd.Function):
@@ -142,9 +172,11 @@ class _BDGCNFn(torch.autograd.Function):
         B, N, N2, C = X.shape
         K = G_o.shape[-3]
         H = W.shape[1]
-        prec = resolve_precision(precision, B, N, K, C, H)
+        sparse = G_o.layout == torch.sparse_coo          # bdgcn() checked it: static, fp32 family, no gradient
+        prec = _lib.PREC_FP32 if sparse else resolve_precision(precision, B, N, K, C, H)
         tc = prec == _lib.PREC_FP16_TC
-        Xc, Goc, Wc = _f32c(X), _f32c(G_o), _f32c(W)
+        Xc, Wc = _f32c(X), _f32c(W)
+        Goc = torch.empty(0, device=X.device) if sparse else _f32c(G_o)
         Gdc = Goc if G_d is G_o else _f32c(G_d)
         bc = None if b is None else _f32c(b)
         out = torch.empty((B, N, N, H), dtype=torch.float32, device=X.device)
@@ -167,10 +199,17 @@ class _BDGCNFn(torch.autograd.Function):
                 gd_p = go_p if G_d is G_o else _prepared_supports(lib, G_d, Gdc, planes, N)
             preps = (go_p, gd_p)
             ex.go_prepared, ex.gd_prepared = _ptr(go_p), _ptr(gd_p)
+        ctx.sparse_nnz = None
         with torch.cuda.device(X.device):
-            _lib.check(lib.mpgcn_bdgcn_forward_x(_ptr(Xc), _ptr(Goc), _ptr(Gdc), int(dynamic), _ptr(Wc), _ptr(bc), act, _ptr(out),
-                                                 _ptr(saved), _ptr(ws), ws.numel(), B, N, K, C, H, prec, ctypes.addressof(ex), _stream()),
-                       "bdgcn_forward")
+            if sparse:      # the stack's CSR / CSC (built once per tensor) travel as the first prepared-supports entry
+                sp, ctx.sparse_nnz = _sparse_supports(lib, G_o, K, N)
+                preps = (sp, None)
+                _lib.check(lib.mpgcn_bdgcn_forward_sparse(_ptr(Xc), _ptr(sp), sp.numel(), ctx.sparse_nnz, _ptr(Wc), _ptr(bc), act, _ptr(out),
+                                                          _ptr(saved), _ptr(ws), ws.numel(), B, N, K, C, H, _stream()), "bdgcn_forward_sparse")
+            else:
+                _lib.check(lib.mpgcn_bdgcn_forward_x(_ptr(Xc), _ptr(Goc), _ptr(Gdc), int(dynamic), _ptr(Wc), _ptr(bc), act, _ptr(out),
+                                                     _ptr(saved), _ptr(ws), ws.numel(), B, N, K, C, H, prec, ctypes.addressof(ex), _stream()),
+                           "bdgcn_forward")
         ctx.shape = (B, N, K, C, H)
         ctx.meta = (bool(dynamic), act, prec, b is not None)
         ctx.x_producer = _producer_node(X) if need_grad else None
@@ -205,7 +244,14 @@ class _BDGCNFn(torch.autograd.Function):
         ex.go_prepared, ex.gd_prepared = _ptr(ctx.preps[0]), _ptr(ctx.preps[1])
         ex.d_out_absmax, ex.dX_absmax = _ptr(hint), _ptr(dx_absmax)
         dGo = dGd = None
-        if ctx.sgrad:
+        if ctx.sparse_nnz is not None:
+            sp = ctx.preps[0]
+            ws = _scratch(lib.mpgcn_bdgcn_bwd_workspace_bytes(B, N, K, C, H, 0, prec), dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.mpgcn_bdgcn_backward_sparse(_ptr(d_out), _ptr(out), _ptr(sp), sp.numel(), ctx.sparse_nnz, _ptr(Wc), act,
+                                                           _ptr(saved), _ptr(dX), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), B, N, K, C, H,
+                                                           _stream()), "bdgcn_backward_sparse")
+        elif ctx.sgrad:
             # static: one gradient for the one stack (returned for G_o; G_d is the same tensor); dynamic: one per side, which
             # autograd adds up when the caller passed one tensor as both
             if not dynamic:
@@ -229,19 +275,46 @@ class _BDGCNFn(torch.autograd.Function):
         return dX, dGo, dGd, dW, db, None, None, None, None, None
 
 
+def _check_sparse_supports(G, precision, grad_mode: bool) -> None:
+    """A sparse static stack runs the sparse fp32 kernels: a COO tensor [K,N,N] of a floating type, with no dense dimensions and no
+    gradient, under precision "auto" or "fp32"."""
+    if G.layout != torch.sparse_coo:
+        raise NotImplementedError(f"mpgcn_b200.bdgcn: sparse supports must be a sparse COO tensor (G.to_sparse()), got layout {G.layout}")
+    if G.dense_dim() != 0 or G.sparse_dim() != 3:
+        raise ValueError(f"mpgcn_b200.bdgcn: a sparse support stack must be [K,N,N] with 3 sparse dimensions and no dense ones, got "
+                         f"{G.sparse_dim()} sparse and {G.dense_dim()} dense")
+    if not G.is_floating_point():
+        raise ValueError(f"mpgcn_b200.bdgcn: sparse supports must hold floating-point values, got {G.dtype}")
+    if grad_mode and G.requires_grad:
+        raise NotImplementedError("mpgcn_b200.bdgcn: sparse supports have no gradient (support_grad needs a dense G); pass G.detach()")
+    name = default_precision() if precision is None else precision
+    if name not in _PREC_NAMES:
+        raise ValueError(f"unknown precision {name!r}; expected one of {sorted(_PREC_NAMES)}")
+    if name == "fp16":
+        raise RuntimeError("mpgcn_b200.bdgcn: there are no fp16 sparse kernels; sparse supports run in fp32 (precision 'auto' or 'fp32')")
+
+
 def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None, support_grad: bool = False) -> torch.Tensor:
     """out = act(cat_{o,d}(G_o^T X G_d) W + b); G is a [K,N,N] tensor or a pair of [B,K,N,N] tensors.
 
     support_grad=True: a G that requires grad receives dL/dG (static: one [K,N,N] gradient; dynamic: one per side of the pair).
     It adds 2 K B N^3 (C + H) flops to the backward, as much as its N^3 work without it, so it is opt-in: by default a G that
-    requires grad is refused."""
-    _require_cuda(X, "X")
+    requires grad is refused.
+
+    A static G given as a sparse COO tensor [K,N,N] runs the fp32 layer with its four N^3 contractions replaced by gathers over
+    the stored entries (precision "auto" or "fp32"; its CSR / CSC structure is built once per tensor and cached).  Only stored
+    entries are multiplied, so a non-finite X does not leak through a zero of G as it does in the dense layer."""
     if isinstance(G, torch.Tensor):
         G_o = G_d = G
         dynamic = False
+        if G.layout != torch.strided:
+            _check_sparse_supports(G, precision, torch.is_grad_enabled())
     else:
         G_o, G_d = G
         dynamic = True
+        if G_o.layout != torch.strided or G_d.layout != torch.strided:
+            raise NotImplementedError("mpgcn_b200.bdgcn: sparse supports are static only; both members of a dynamic pair must be dense")
+    _require_cuda(X, "X")
     for g in (G_o, G_d):
         _require_cuda(g, "G")
         if g.device != X.device:

@@ -73,7 +73,7 @@ class _GraphedInference:
         if torch.is_grad_enabled() or self.model.training or not x_seq.is_cuda:
             return self.eager(x_seq=x_seq, G_list=G_list)
         gs = self._flat(G_list)
-        key = (tuple(x_seq.shape), x_seq.device, tuple((id(g), g._version, g.data_ptr()) for g in gs))
+        key = (tuple(x_seq.shape), x_seq.device, tuple((id(g), g._version, (g._values() if g.is_sparse else g).data_ptr()) for g in gs))
         if key != self.key:
             self.key = None
             self.graph = self.static_x = self.static_y = None

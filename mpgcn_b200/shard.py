@@ -496,6 +496,8 @@ def sharded_bdgcn(layer, X, G, plan: ShardPlan, branch: int = 0):
     if act is None:
         raise NotImplementedError("sharded layers fuse None / ReLU only")
     _no_deterministic("sharded_bdgcn")
+    if any(g.layout != torch.strided for g in ((G,) if isinstance(G, torch.Tensor) else G)):
+        raise NotImplementedError("sharded layers take dense supports; a sparse stack runs on one GPU (mpgcn_b200.ops.bdgcn)")
     dynamic = not isinstance(G, torch.Tensor)
     if dynamic:
         G_o, G_d = G

@@ -12,7 +12,10 @@ What it does, and nothing more:
   * `--gpu-dyn-graphs`: `mpgcn_b200.dyn_graph.install(Data_Container_OD.DataInput)` -- `construct_dyn_G` on the GPU
     (Data_Container_OD.py:39-59: 2*7*N^2 scipy calls otherwise);
   * `--graph-rollout`: `mpgcn_b200.rollout.install(model)` on the trainer's model -- the `pred_len` forward passes of
-    `ModelTrainer.test` (Model_Trainer.py:157-165) replay one captured CUDA graph per batch.
+    `ModelTrainer.test` (Model_Trainer.py:157-165) replay one captured CUDA graph per batch;
+  * `--sparse-static-supports`: the static support stack of `ModelTrainer.preprocess_adj` (Model_Trainer.py:38-42) becomes a
+    sparse COO tensor (`.to_sparse()`), so the static branch's layers run the gathers over its nonzeros (fp32; DESIGN.md
+    section 12) instead of dense N^3 contractions.
 Everything after `--` is Main.py's own command line (Main.py:11-37).
 """
 import argparse
@@ -28,6 +31,7 @@ def main():
     ap.add_argument("--reference-dir", default=os.path.join(ROOT, "oracle", "_ref"))
     ap.add_argument("--graph-rollout", action="store_true")
     ap.add_argument("--gpu-dyn-graphs", action="store_true")
+    ap.add_argument("--sparse-static-supports", action="store_true")
     ap.add_argument("--seed", type=int, default=None, help="torch.manual_seed / numpy seed before Main.py runs (the reference sets none)")
     ap.add_argument("--stock", action="store_true", help="do NOT shadow MPGCN / GCN: run the reference as it is (CPU plumbing check)")
     ap.add_argument("main_args", nargs=argparse.REMAINDER)
@@ -54,6 +58,10 @@ def main():
             from mpgcn_b200 import rollout
             get_model = Model_Trainer.ModelTrainer.get_model
             Model_Trainer.ModelTrainer.get_model = lambda self: rollout.install(get_model(self))
+        if a.sparse_static_supports:
+            import Model_Trainer
+            preprocess_adj = Model_Trainer.ModelTrainer.preprocess_adj
+            Model_Trainer.ModelTrainer.preprocess_adj = lambda self, *args, **kw: preprocess_adj(self, *args, **kw).to_sparse()
     if a.seed is not None:
         import numpy as np
         import torch
