@@ -301,6 +301,22 @@ MPGCN_API int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* 
                                         size_t saved_bytes, void* workspace, size_t workspace_bytes, int B, int T, long long NN, int C,
                                         int precision, const float* d_hT_absmax, void* stream);
 
+/* Recomputing LSTM backward (L = 1 or a stack; precision 1 wherever mpgcn_lstm_stack_supported(T, C, L, 1) holds), for a
+ * forward that kept no training state: mpgcn_lstm_last_forward, or mpgcn_lstm_stack_forward with saved == NULL.  The state
+ * is rebuilt and walked back one chunk of cells at a time, so the workspace is O(chunk_cells), not O(B NN T C), at the cost of
+ * one more forward.  A chunk is chunk_cells (>= 1) rounded up to whole tiles, at least one wave of the backward grid, at most
+ * every cell.  d_x and the per-cell gradients are bitwise those of mpgcn_lstm_last_backward_saved / mpgcn_lstm_stack_backward;
+ * the weight gradients differ in fp32 summation order only.  Parameters as mpgcn_lstm_stack_backward's (HOST arrays of L
+ * device pointers).  Workspace (256-byte aligned) from mpgcn_lstm_recompute_bwd_workspace_bytes (0: arguments it does not
+ * support): [S, 1/S] (1024 B), a stack's fp32 d(h^{l-1}_t) sequence of one chunk, deterministic mode's slots (one region per
+ * layer), the chunk's saved state of every layer, and at C = 96, 128 or in a stack the chunk's gate-gradient records. */
+MPGCN_API size_t mpgcn_lstm_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells, int precision);
+MPGCN_API int mpgcn_lstm_backward_recompute(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh,
+                                            const float* const* b_ih, const float* const* b_hh, const float* d_hT, float* const* d_w_ih,
+                                            float* const* d_w_hh, float* const* d_b_ih, float* const* d_b_hh, float* d_x,
+                                            long long chunk_cells, void* workspace, size_t workspace_bytes, int B, int T, long long NN,
+                                            int C, int precision, const float* d_hT_absmax, void* stream);
+
 /* Dynamic origin / destination graphs from the OD history = DataInput.construct_dyn_G (reference Data_Container_OD.py:39-59).
  *   od_history [periods * P, N, N]  the first periods*P days of the (un-normalised) OD tensor, P = perceived period (7)
  *   o_graph, d_graph [P, N, N]      slot t: A_t = mean_k od_history[t + k P];

@@ -103,6 +103,9 @@ class MPGCN(nn.Module):
         self.lstm_num_layers = lstm_num_layers
         self.gcn_num_layers = gcn_num_layers
         self.lstm_precision = None      # None -> ops.default_precision(); or "auto" / "fp16" / "fp32"
+        # True (or a number of cells per chunk): the tensor-core LSTM keeps no training state in the forward and its backward
+        # rebuilds it a chunk at a time (ops.lstm_last), for models whose state does not fit; None -> off
+        self.lstm_recompute = None
         # True: evaluate the M branches on M CUDA streams (they are independent until the head, reference MPGCN.py:101-110), so that
         # the HBM-bound elementwise kernels of one branch run beside the tensor-bound contractions of the other; None -> off
         self.branch_streams = None
@@ -126,7 +129,7 @@ class MPGCN(nn.Module):
 
     def _temporal(self, lstm: nn.LSTM, x_seq: torch.Tensor) -> torch.Tensor:
         B, _, rows, N, _ = x_seq.shape
-        return ops.lstm_module_last(lstm, x_seq, self.lstm_precision).reshape(B, rows, N, self.lstm_hidden_dim)
+        return ops.lstm_module_last(lstm, x_seq, self.lstm_precision, self.lstm_recompute).reshape(B, rows, N, self.lstm_hidden_dim)
 
     def forward(self, x_seq: torch.Tensor, G_list: list):
         """x_seq (B, T, N, N, 1); G_list: per branch a static (K,N,N) tensor or a dynamic tuple.  -> (B, 1, N, N, 1)"""

@@ -110,6 +110,11 @@ _SIGS = {
                                                   ctypes.c_size_t] + [ctypes.c_int] * 5 + [ctypes.c_void_p]),
     "mpgcn_bdgcn_backward_sparse": (ctypes.c_int, [_c_f, _c_f, _c_f, ctypes.c_size_t, ctypes.c_longlong, _c_f, ctypes.c_int, _c_f, _c_f, _c_f,
                                                    _c_f, _c_f, ctypes.c_size_t] + [ctypes.c_int] * 5 + [ctypes.c_void_p]),
+    "mpgcn_lstm_recompute_bwd_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int,
+                                                                    ctypes.c_longlong, ctypes.c_int]),
+    "mpgcn_lstm_backward_recompute": (ctypes.c_int, [_c_f, ctypes.c_int] + [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f] +
+                                      [ctypes.POINTER(ctypes.c_void_p)] * 4 + [_c_f, ctypes.c_longlong, _c_f, ctypes.c_size_t, ctypes.c_int,
+                                      ctypes.c_int, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, _c_f, ctypes.c_void_p]),
 }
 ABI_VERSION = 4          # MPGCN_B200_ABI_VERSION of include/mpgcn_b200.h this binding was written against
 EXPORTED_SYMBOLS = tuple(_SIGS)

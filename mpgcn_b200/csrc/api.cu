@@ -491,4 +491,29 @@ int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* const* w_i
                                 B, T, NN, C, d_hT_absmax, static_cast<cudaStream_t>(stream));
 }
 
+size_t mpgcn_lstm_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells, int precision) {
+  if (precision != PREC_FP16_TC || L < 1 || !mpgcn_lstm_stack_supported(T, C, L, precision) || B < 1 || NN < 1 || chunk_cells < 1) return 0;
+  return lstm_tc_recompute_bwd_workspace_bytes(B, T, NN, C, L, chunk_cells);
+}
+
+int mpgcn_lstm_backward_recompute(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                                  const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh,
+                                  float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* workspace,
+                                  size_t workspace_bytes, int B, int T, long long NN, int C, int precision, const float* d_hT_absmax,
+                                  void* stream) {
+  const char* what = "mpgcn_lstm_backward_recompute";
+  MPGCN_CHECK(L >= 1, "%s: L=%d", what, L);
+  MPGCN_CHECK(x_seq && w_ih && w_hh && b_ih && b_hh && d_hT && d_w_ih && d_w_hh && d_b_ih && d_b_hh, "%s: null pointer argument", what);
+  for (int l = 0; l < L; ++l)
+    MPGCN_CHECK(w_ih[l] && w_hh[l] && b_ih[l] && b_hh[l] && d_w_ih[l] && d_w_hh[l] && d_b_ih[l] && d_b_hh[l],
+                "%s: null pointer argument (layer %d)", what, l);
+  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "%s: empty input", what);
+  // precision 0 keeps no training state in the first place: its backward always recomputes
+  MPGCN_CHECK(precision == PREC_FP16_TC && mpgcn_lstm_stack_supported(T, C, L, precision),
+              "%s: precision %d does not support T=%d, hidden=%d, L=%d (tensor-core kernels only)", what, precision, T, C, L);
+  MPGCN_CHECK(chunk_cells >= 1, "%s: chunk_cells=%lld (at least 1)", what, chunk_cells);
+  return lstm_recompute_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, chunk_cells, workspace,
+                                    workspace_bytes, B, T, NN, C, d_hT_absmax, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -151,6 +151,12 @@ int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, 
                            const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
                            float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,
                            int C, const float* d_hT_absmax, cudaStream_t s);
+// backward without training state (L = 1 or a stack): the state is rebuilt and walked back one chunk of chunk_cells cells at a time
+size_t lstm_tc_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells);
+int lstm_recompute_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                               const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh,
+                               float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* ws, size_t ws_bytes,
+                               int B, int T, long long NN, int C, const float* d_hT_absmax, cudaStream_t s);
 
 // ---- BDGCN layer orchestration ---------------------------------------------------------------
 struct BdgcnShape {

@@ -235,6 +235,9 @@ __device__ __forceinline__ float cell_grad(const float (&acc)[16][4], int h, con
   return dx;
 }
 
+// Every kernel runs the tiles tile0 .. tile0 + tiles - 1 of the `cells` cells.  x_seq, h_T, d_hT and d_x are addressed by the
+// global cell, (tile0 + tile) CELLS + ..; the training state, the da records, h_seq and d_seq by the tile within the range, so a
+// range's region of them has the layout the full-size buffer has for those tiles (tile0 = 0 and all tiles: the whole call).
 // Training state written by the forward kernels and read by the backward ones: per (tile, step) NW x 1024 halves,
 // [warp][c | h][lane][16 halves], the 16 halves of a thread in slot order h * 8 + s (its register fragment, stored as is);
 // warp = cg CH + js.
@@ -268,27 +271,29 @@ __device__ __forceinline__ size_t dseq_off(long long tile, int T, int t, int war
 // =======================================================================================
 // H = 32
 // =======================================================================================
-// forward: the thread's h_t, packed to fp16 pairs, is its A fragment of the next step's h k-blocks
-template <bool SAVE>
+// forward: the thread's h_t, packed to fp16 pairs, is its A fragment of the next step's h k-blocks.
+// RANGE: runs the tiles tile0 .. tile0 + tiles - 1; without, every tile of `cells` (tile0 and tiles are not read), which keeps the
+// code of the headline's whole-call launches as it was before tile ranges (the same holds for lstm_bwd_saved_tc_kernel)
+template <bool SAVE, bool RANGE = false>
 __global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::FWD_CTAS_PER_SM)
 lstm_fwd_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                    const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
-                   long long cells, int T, long long NN) {
+                   long long cells, long long tile0, long long tiles, int T, long long NN) {
   using D = Dims<1>;
   __shared__ __align__(16) __half sWx[D::G4 * D::WX_LD];
   load_wx<1>(sWx, w_ih, w_hh, b_ih, b_hh);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
   const uint32_t wx_addr = smem_u32(sWx);
-  const long long tiles = (cells + D::CELLS - 1) / D::CELLS;
-  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+  const long long t0 = RANGE ? tile0 : 0, ntiles = RANGE ? tiles : (cells + D::CELLS - 1) / D::CELLS;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     long long cell[2];
     bool live[2];
     size_t xb[2];
     float xv[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      cell[h] = tile * D::CELLS + warp * 16 + g + 8 * h;
+      cell[h] = (t0 + tile) * D::CELLS + warp * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
       xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
       xv[h] = live[h] ? x_seq[xb[h]] : 0.f;
@@ -357,13 +362,15 @@ constexpr size_t kBwdSavedSmem =
     Dims<1>::G4 * sizeof(float) + 2 * kBwdRing * sizeof(uint64_t);
 
 // DET (deterministic mode): the flush stores the CTA's dWext to its slot d_w_hh + blockIdx.x * 4352, laid out as the outputs
-// [128 x 32 w_hh | 128 w_ih | 128 b] (the two x columns of w_ih added in the CTA first), instead of adding it with atomics.
-template <bool DX, bool DET = false>
+// [128 x 32 w_hh | 128 w_ih | 128 b] (the two x columns of w_ih added in the CTA first), instead of adding it with atomics; with
+// acc it adds to the slot instead (a later chunk of lstm_recompute_backward_tc: the CTA owns the slot, the stream orders the chunks).
+template <bool DX, bool DET = false, bool RANGE = false>
 __global__ void __launch_bounds__(Dims<1>::THREADS, Dims<1>::BWD_CTAS_PER_SM)
 lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                          float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, float* __restrict__ d_x,
-                         const __half* __restrict__ saved, const float* __restrict__ scale2, long long cells, int T, long long NN) {
+                         const __half* __restrict__ saved, const float* __restrict__ scale2, long long cells, long long tile0, long long tiles,
+                         int T, long long NN, bool acc) {
   using D = Dims<1>;
   constexpr int C = D::H, CELLS = D::CELLS;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -389,7 +396,7 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
   const uint32_t wx_addr = smem_u32(sWx), wt_addr = smem_u32(sWT), da_addr = smem_u32(sDA), hx_addr = smem_u32(sHX);
-  const long long tiles = (cells + CELLS - 1) / CELLS;
+  const long long t0 = RANGE ? tile0 : 0, ntiles = RANGE ? tiles : (cells + CELLS - 1) / CELLS;
   const float S = scale2[0], invS = scale2[1];
   float dw[5][4];                     // dWext: gate 16 warp + g + 8 (i >> 1), column 8 nt + 2 q + (i & 1); columns 40..47 are 0
 #pragma unroll
@@ -402,12 +409,12 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
   auto pf_cells = [&]() {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const long long cell = pf_tile * CELLS + warp * 16 + g + 8 * h;
-      pf_xb[h] = pf_tile < tiles && cell < cells ? x_base(cell, T, NN) : ~(size_t)0;
+      const long long cell = (t0 + pf_tile) * CELLS + warp * 16 + g + 8 * h;
+      pf_xb[h] = pf_tile < ntiles && cell < cells ? x_base(cell, T, NN) : ~(size_t)0;
     }
   };
   auto fetch = [&](int slot) {
-    if (pf_tile < tiles) {
+    if (pf_tile < ntiles) {
       const uint4* pc = reinterpret_cast<const uint4*>(saved + save_off<1>(pf_tile, T, pf_t, warp, 0, lane));
       const uint4* ph = reinterpret_cast<const uint4*>(saved + save_off<1>(pf_tile, T, pf_t, warp, 1, lane));
       uint4* dst = sST + (slot * D::NW + warp) * 128 + lane;
@@ -449,14 +456,14 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
   uint32_t phase = 0, prev_phase = 0; // (k / kBwdRing) & 1: the barrier phase of the slot's current use
   bool have_prev = false;
 
-  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     long long cell[2];
     bool live[2];
     size_t xb[2];
     float dh[2][8], dc[2][8];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      cell[h] = tile * CELLS + warp * 16 + g + 8 * h;
+      cell[h] = (t0 + tile) * CELLS + warp * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
       xb[h] = DX && live[h] ? x_base(cell[h], T, NN) : 0;
 #pragma unroll
@@ -556,6 +563,7 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
   // ---- flush the weight-gradient accumulator ----
   if constexpr (DET) {
     float* slot = d_w_hh + (size_t)blockIdx.x * (D::G4 * C + 2 * D::G4);
+    auto put = [&](int i, float v) { slot[i] = acc ? slot[i] + v : v; };
 #pragma unroll
     for (int nt = 0; nt < 5; ++nt)
 #pragma unroll
@@ -563,9 +571,9 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
         const int j = 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1);
         const float v = dw[nt][i] * invS;
         const float next = __shfl_down_sync(0xffffffffu, v, 1);     // lane q + 1: column col + 2
-        if (col < C) slot[j * C + col] = v;
-        else if (col == 32) slot[D::G4 * C + j] = v + next;          // columns 32 and 34: the x hi / lo pair of w_ih
-        else if (col == 33) slot[D::G4 * C + D::G4 + j] = v;
+        if (col < C) put(j * C + col, v);
+        else if (col == 32) put(D::G4 * C + j, v + next);            // columns 32 and 34: the x hi / lo pair of w_ih
+        else if (col == 33) put(D::G4 * C + D::G4 + j, v);
       }
   } else {
 #pragma unroll
@@ -608,7 +616,8 @@ template <int CH, bool SAVE, bool UP = false, bool HSEQ = false>
 __global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::FWD_CTAS_PER_SM)
 lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                     const float* __restrict__ b_ih, const float* __restrict__ b_hh, float* __restrict__ hT, __half* __restrict__ saved,
-                    long long cells, int T, long long NN, const __half* __restrict__ h_in, __half* __restrict__ h_seq) {
+                    long long cells, long long tile0, long long tiles, int T, long long NN, const __half* __restrict__ h_in,
+                    __half* __restrict__ h_seq) {
   using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
   constexpr int IN_LD = SAVE ? 1024 : 512;
@@ -622,7 +631,6 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
   const uint32_t wx_addr = smem_u32(sWx + js * 128 * D::WX_LD);
   // this lane's ldmatrix row address in the h tile: row 16 cg + (lane & 15), column 8 (lane >> 4)
   const uint32_t h_addr = smem_u32(sH + (cg * 16 + (lane & 15)) * D::H_LD + 8 * (lane >> 4));
-  const long long tiles = (cells + CELLS - 1) / CELLS;
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     long long cell[2];
     bool live[2];
@@ -630,7 +638,7 @@ lstm_fwd_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w
     float xv[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      cell[h] = tile * CELLS + cg * 16 + g + 8 * h;
+      cell[h] = (tile0 + tile) * CELLS + cg * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
       xb[h] = !UP && live[h] ? x_base(cell[h], T, NN) : 0;
       xv[h] = !UP && live[h] ? x_seq[xb[h]] : 0.f;
@@ -740,8 +748,8 @@ __global__ void __launch_bounds__(Dims<CH>::THREADS, Dims<CH>::BWD_CTAS_PER_SM)
 lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                          const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ d_hT,
                          float* __restrict__ d_x, const __half* __restrict__ saved, __half* __restrict__ da_rec,
-                         const float* __restrict__ scale2, long long cells, int T, long long NN, const __half* __restrict__ h_in,
-                         float* __restrict__ d_seq) {
+                         const float* __restrict__ scale2, long long cells, long long tile0, long long tiles, int T, long long NN,
+                         const __half* __restrict__ h_in, float* __restrict__ d_seq) {
   using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -758,7 +766,6 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
   const int cg = warp / CH, js = warp % CH;
   const uint32_t wx_all = smem_u32(sWx), wx_addr = wx_all + (uint32_t)(js * 128 * D::WX_LD * 2);
   const uint32_t da_addr = smem_u32(sDA + (cg * 16 + (lane & 15)) * D::DA_LD + 8 * (lane >> 4));
-  const long long tiles = (cells + CELLS - 1) / CELLS;
   const float S = scale2[0], invS = scale2[1];
 
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
@@ -768,7 +775,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
     float dh[2][8], dc[2][8];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      cell[h] = tile * CELLS + cg * 16 + g + 8 * h;
+      cell[h] = (tile0 + tile) * CELLS + cg * 16 + g + 8 * h;
       live[h] = cell[h] < cells;
       xb[h] = live[h] ? x_base(cell[h], T, NN) : 0;
 #pragma unroll
@@ -779,7 +786,7 @@ lstm_bwd_walk_tcw_kernel(const float* __restrict__ x_seq, const float* __restric
       }
     }
     // the dx writer of the group (lanes 0..15 of slice 0) owns row 16 cg + lane
-    const long long dx_cell = tile * CELLS + cg * 16 + (lane & 15);
+    const long long dx_cell = (tile0 + tile) * CELLS + cg * 16 + (lane & 15);
     const bool dx_live = !UP && d_x != nullptr && js == 0 && lane < 16 && dx_cell < cells;
     const size_t dx_base = dx_live ? x_base(dx_cell, T, NN) : 0;
 
@@ -908,12 +915,13 @@ template <int CH, bool UP = false>
 constexpr size_t kDwSmem = (size_t)Dims<CH>::CELLS * (DW_DA_LD + Dims<CH, UP>::HX_LD) * sizeof(__half);
 
 // DET (deterministic mode): CTA (js, split) stores its rows to the split's slot d_w_hh + split * (4H x H + 4H x KI + 4H), laid out as
-// the outputs [4H x H w_hh | 4H x KI w_ih | 4H b] (KI = H for UP, else 1 with the x hi / lo columns added first), without atomics.
+// the outputs [4H x H w_hh | 4H x KI w_ih | 4H b] (KI = H for UP, else 1 with the x hi / lo columns added first), without atomics;
+// with acc it adds them to the slot (a later chunk of lstm_recompute_backward_tc).
 template <int CH, bool UP = false, bool DET = false>
 __global__ void __launch_bounds__(DW_THREADS)
 lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ saved, const __half* __restrict__ da_rec,
                    float* __restrict__ d_w_ih, float* __restrict__ d_w_hh, float* __restrict__ d_b, const float* __restrict__ scale2,
-                   long long cells, int T, long long NN, const __half* __restrict__ h_in) {
+                   long long cells, long long tile0, long long tiles, int T, long long NN, const __half* __restrict__ h_in, bool acc) {
   using D = Dims<CH, UP>;
   constexpr int CELLS = D::CELLS;
   constexpr int HX_LD = D::HX_LD;
@@ -932,7 +940,7 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
   }
   const int js = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3, mi = lane >> 3;
-  const long long tiles = (cells + CELLS - 1) / CELLS, records = tiles * T;
+  const long long records = tiles * T;
   const long long per = (records + gridDim.y - 1) / gridDim.y;
   const long long r0 = blockIdx.y * per, r1 = r0 + per < records ? r0 + per : records;
   for (int e = threadIdx.x; e < CELLS; e += blockDim.x)          // constant zero columns KX - 8 .. KX - 1
@@ -973,7 +981,7 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     } else {
       for (int e = threadIdx.x; e < CELLS * 4; e += blockDim.x) {     // x columns H .. H + 7
         const int row = e >> 2, qq = e & 3;
-        const long long cell = tile * CELLS + row;
+        const long long cell = (tile0 + tile) * CELLS + row;
         const float x = cell < cells ? x_seq[x_base(cell, T, NN) + (size_t)t * NN] : 0.f;
         *reinterpret_cast<uint32_t*>(sHX + row * HX_LD + D::H + 2 * qq) = x_cols(x, qq);
       }
@@ -998,6 +1006,7 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
     float* slot = d_w_hh + (size_t)blockIdx.y * (D::G4 * D::H + D::G4 * KI + D::G4);
     float* s_ih = slot + D::G4 * D::H;
     float* s_b = s_ih + D::G4 * KI;
+    auto put = [&](float* p, float v) { *p = acc ? *p + v : v; };
 #pragma unroll
     for (int nt = 0; nt < NX; ++nt)
 #pragma unroll
@@ -1005,13 +1014,13 @@ lstm_dw_tcw_kernel(const float* __restrict__ x_seq, const __half* __restrict__ s
         const int r = 128 * js + 16 * warp + g + 8 * (i >> 1), col = 8 * nt + 2 * q + (i & 1), j = gate_row<CH>(r);
         const float v = dw[nt][i] * row_scale(r) * invS;
         const float next = __shfl_down_sync(0xffffffffu, v, 1);     // lane q + 1: column col + 2
-        if (col < D::H) slot[(size_t)j * D::H + col] = v;
+        if (col < D::H) put(slot + (size_t)j * D::H + col, v);
         else if (UP) {
-          if (col < 2 * D::H) s_ih[(size_t)j * D::H + col - D::H] = v;
-          else if (col == 2 * D::H) s_b[j] = v;
+          if (col < 2 * D::H) put(s_ih + (size_t)j * D::H + col - D::H, v);
+          else if (col == 2 * D::H) put(s_b + j, v);
         }
-        else if (col == D::H) s_ih[j] = v + next;
-        else if (col == D::H + 1) s_b[j] = v;
+        else if (col == D::H) put(s_ih + j, v + next);
+        else if (col == D::H + 1) put(s_b + j, v);
       }
   } else {
 #pragma unroll
@@ -1040,18 +1049,39 @@ using lstm_tc::Dims;
 
 bool lstm_tc_supported(int T, int C) { return (C == 32 || C == 96 || C == 128) && T >= 1 && T <= 256; }
 
-template <int CH>
-static int lstm_grid(long long cells, int ctas_per_sm) {
-  const long long tiles = (cells + Dims<CH>::CELLS - 1) / Dims<CH>::CELLS;
-  long long g = (long long)ctas_per_sm * device_sm_count();
-  return (int)(g < tiles ? g : tiles);
-}
+static long long lstm_tc_tile_cells(int C) { return C == 32 ? Dims<1>::CELLS : C == 96 ? Dims<3>::CELLS : Dims<4>::CELLS; }
 
 // cells of B NN rounded up to whole tiles of the width's kernels
 static long long lstm_tc_padded_cells(int B, long long NN, int C) {
-  const long long tc = C == 32 ? Dims<1>::CELLS : C == 96 ? Dims<3>::CELLS : Dims<4>::CELLS;
+  const long long tc = lstm_tc_tile_cells(C);
   return ((long long)B * NN + tc - 1) / tc * tc;
 }
+
+// the tiles [tile0, tile0 + n) of a launch (see lstm_tc::save_off): every tile of a call, or one chunk of the recomputing backward
+struct TileRange { long long tile0, n; };
+static TileRange all_tiles(long long cells, int C) { return {0, (cells + lstm_tc_tile_cells(C) - 1) / lstm_tc_tile_cells(C)}; }
+// the cells of a range that exist (the last tile of a call may be part padding)
+static long long range_cells(long long cells, TileRange r, int C) {
+  const long long end = (r.tile0 + r.n) * lstm_tc_tile_cells(C);
+  return (end < cells ? end : cells) - r.tile0 * lstm_tc_tile_cells(C);
+}
+
+static int lstm_grid(long long tiles, int ctas_per_sm) {
+  long long g = (long long)ctas_per_sm * device_sm_count();
+  return (int)(g < tiles ? g : tiles);
+}
+// CTAs per slice of the wide dW pass over `tiles` tiles: up to 4 per SM in all, each a contiguous range of (tile, step) records
+template <int CH>
+static int lstm_dw_splits(long long tiles, int T) {
+  const long long records = tiles * T, s = 4LL * device_sm_count() / CH;
+  return (int)(s < records ? s : records);
+}
+
+// Deterministic mode's weight-gradient flush (DESIGN.md section 11); slots == nullptr: atomics.  Each CTA of the hidden-32 walk,
+// or each split of a dW pass, writes its own slot image (acc: adds to it, a later chunk of the recomputing backward), and with
+// reduce_tiles > 0 the slots that a launch over that many tiles writes are then reduced into the outputs in a fixed order (0: a
+// chunk before the last; the recomputing backward reduces after its last chunk the slots its first, largest, chunk wrote).
+struct DetFlush { float* slots; bool acc; long long reduce_tiles; };
 
 // c_t | h_t of every cell (tiles padded) and step: 2 C halves, see lstm_tc::save_off
 size_t lstm_tc_saved_bytes(int B, int T, long long NN, int C) {
@@ -1088,66 +1118,71 @@ size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) { return l
 
 template <int CH>
 static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                            void* saved, long long cells, int T, long long NN, cudaStream_t st) {
+                            void* saved, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
   auto kern = saved ? lstm_tc::lstm_fwd_tcw_kernel<CH, true> : lstm_tc::lstm_fwd_tcw_kernel<CH, false>;
   constexpr size_t smem = lstm_tc::kFwdWideSmem<CH>;
   static DynSmemAttr attr_t = {}, attr_f = {};
   if (int e = ensure_dyn_smem(kern, (int)smem, saved ? attr_t : attr_f)) return e;
-  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  kern<<<lstm_grid<CH>(cells, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT,
-                                                                           static_cast<__half*>(saved), cells, T, NN, nullptr, nullptr);
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
+                                                                     r.tile0, r.n, T, NN, nullptr, nullptr);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }
 
-// lstm_backward_h32 and lstm_backward_tcw<CH>: the kernels of one width's backward, run once the grad scale and the zeroed
-// weight gradients are in place.  da_rec: the gate-gradient records of the wide walk (the hidden-32 walk keeps them on chip).
-// slots: deterministic mode's flush slots (lstm_tc_slot_bytes), null for the atomic flush
+// lstm_backward_h32 and lstm_backward_tcw<CH>: the kernels of one width's backward over the tiles r, run once the grad scale and
+// the zeroed weight gradients are in place.  da_rec: the gate-gradient records of the wide walk (the hidden-32 walk keeps them on
+// chip).  f.slots: deterministic mode's flush slots (lstm_tc_slot_bytes), null for the atomic flush
 static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved,
-                             void* /*da_rec*/, float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                             void* /*da_rec*/, DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN,
+                             cudaStream_t st) {
   using D = Dims<1>;
-  if (d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  auto kern = slots ? (d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true, true> : lstm_tc::lstm_bwd_saved_tc_kernel<false, true>)
-                    : (d_x ? lstm_tc::lstm_bwd_saved_tc_kernel<true> : lstm_tc::lstm_bwd_saved_tc_kernel<false>);
-  static DynSmemAttr attr_x = {}, attr_n = {}, attr_xd = {}, attr_nd = {};
-  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, slots ? (d_x ? attr_xd : attr_nd) : (d_x ? attr_x : attr_n))) return e;
-  const int grid = lstm_grid<1>(cells, D::BWD_CTAS_PER_SM);
-  prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  kern<<<grid, D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, slots ? slots : d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells, T, NN);
+  float* slots = f.slots;
+  using K = decltype(&lstm_tc::lstm_bwd_saved_tc_kernel<false>);
+  static const K kerns[2][2][2] = {     // [RANGE][DET][DX]
+      {{lstm_tc::lstm_bwd_saved_tc_kernel<false>, lstm_tc::lstm_bwd_saved_tc_kernel<true>},
+       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true>}},
+      {{lstm_tc::lstm_bwd_saved_tc_kernel<false, false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, false, true>},
+       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true, true>}}};
+  static DynSmemAttr attrs[2][2][2] = {};
+  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, D::H).n;
+  const K kern = kerns[range][slots != nullptr][d_x != nullptr];
+  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, attrs[range][slots != nullptr][d_x != nullptr])) return e;
+  prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, slots ? slots : d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells,
+      r.tile0, r.n, T, NN, f.acc);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
-  if (slots)
-    return reduce_slots(slots, grid, (long long)D::G4 * D::H + 2 * D::G4, 1, 0,
+  if (slots && f.reduce_tiles)
+    return reduce_slots(slots, lstm_grid(f.reduce_tiles, D::BWD_CTAS_PER_SM), (long long)D::G4 * D::H + 2 * D::G4, 1, 0,
                         slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, D::G4, d_b, D::G4), st);
   return 0;
 }
 
 // the wide dW pass of one layer (KI = H for an upper stack layer, else 1), then in deterministic mode the reduction of its slots
 template <int CH, bool UP>
-static int lstm_dw_pass(const float* x_seq, const void* saved, const void* da_rec, float* d_w_ih, float* d_w_hh, float* d_b, float* slots,
-                        const float* scale2, long long cells, int T, long long NN, const void* h_in, double flops, cudaStream_t st) {
+static int lstm_dw_pass(const float* x_seq, const void* saved, const void* da_rec, float* d_w_ih, float* d_w_hh, float* d_b, DetFlush f,
+                        const float* scale2, long long cells, TileRange r, int T, long long NN, const void* h_in, double flops, cudaStream_t st) {
   using D = Dims<CH>;
   constexpr int KI = UP ? D::H : 1;
+  float* slots = f.slots;
   auto dw = slots ? lstm_tc::lstm_dw_tcw_kernel<CH, UP, true> : lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
   constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
   static DynSmemAttr attr_d = {}, attr_dd = {};
   if (dw_smem)
     if (int e = ensure_dyn_smem(dw, (int)dw_smem, slots ? attr_dd : attr_d)) return e;
-  const long long records = (cells + D::CELLS - 1) / D::CELLS * T;
-  long long splits = 4LL * device_sm_count() / CH;
-  if (splits > records) splits = records;
   prof_begin(PROF_LSTM_BWD, flops, st);
-  dw<<<dim3(CH, (unsigned)splits), lstm_tc::DW_THREADS, dw_smem, st>>>(x_seq, static_cast<const __half*>(saved),
-                                                                      static_cast<const __half*>(da_rec), d_w_ih, slots ? slots : d_w_hh,
-                                                                      d_b, scale2, cells, T, NN, static_cast<const __half*>(h_in));
+  dw<<<dim3(CH, (unsigned)lstm_dw_splits<CH>(r.n, T)), lstm_tc::DW_THREADS, dw_smem, st>>>(
+      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, slots ? slots : d_w_hh, d_b, scale2, cells,
+      r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), f.acc);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
-  if (slots)
-    return reduce_slots(slots, (int)splits, (long long)D::G4 * (D::H + KI + 1), 1, 0,
+  if (slots && f.reduce_tiles)
+    return reduce_slots(slots, lstm_dw_splits<CH>(f.reduce_tiles, T), (long long)D::G4 * (D::H + KI + 1), 1, 0,
                         slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, (long long)D::G4 * KI, d_b, D::G4), st);
   return 0;
 }
@@ -1155,38 +1190,47 @@ static int lstm_dw_pass(const float* x_seq, const void* saved, const void* da_re
 template <int CH>
 static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, void* da_rec,
-                             float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                             DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
   constexpr size_t smem = lstm_tc::kWalkSmem<CH>;
+  const double rc = (double)range_cells(cells, r, D::H);
   static DynSmemAttr attr_b = {};
   if (int e = ensure_dyn_smem(lstm_tc::lstm_bwd_walk_tcw_kernel<CH>, (int)smem, attr_b)) return e;
   // walk: the gate recompute and dh_{t-1} (2 x 8 H (H + 1) per cell and step, as the hidden-32 count splits it) ...
-  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * (double)cells * T, st);
-  lstm_tc::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid<CH>(cells, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, T, NN,
-      nullptr, nullptr);
+  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * rc * T, st);
+  lstm_tc::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, r.tile0,
+      r.n, T, NN, nullptr, nullptr);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   // ... and the weight gradient (8 H (H + 1) / 2 more: 12 H (H + 1) in all)
-  return lstm_dw_pass<CH, false>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, slots, scale2, cells, T, NN, nullptr,
-                                 4.0 * D::H * (D::H + 1) * (double)cells * T, st);
+  return lstm_dw_pass<CH, false>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, f, scale2, cells, r, T, NN, nullptr,
+                                 4.0 * D::H * (D::H + 1) * rc * T, st);
+}
+
+// the single-layer forward over the tiles r (saved: their training state, or null)
+static int lstm_forward_range(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
+                              void* saved, long long cells, TileRange r, int T, long long NN, int C, cudaStream_t st) {
+  using D = Dims<1>;
+  if (C == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, r, T, NN, st);
+  if (C == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, r, T, NN, st);
+  MPGCN_CHECK(C == D::H, "lstm forward: no tensor-core kernel for hidden=%d", C);
+  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, C).n;
+  auto kern = range ? (saved ? lstm_tc::lstm_fwd_tc_kernel<true, true> : lstm_tc::lstm_fwd_tc_kernel<false, true>)
+                    : (saved ? lstm_tc::lstm_fwd_tc_kernel<true> : lstm_tc::lstm_fwd_tc_kernel<false>);
+  prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)range_cells(cells, r, C) * T, st);
+  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
+                                                                  r.tile0, r.n, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
                          void* saved, int B, int T, long long NN, int C, cudaStream_t st) {
-  using D = Dims<1>;
   const long long cells = (long long)B * NN;
   MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm forward: saved buffer must be 16-byte aligned");
-  if (C == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
-  if (C == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, T, NN, st);
-  MPGCN_CHECK(C == D::H, "lstm forward: no tensor-core kernel for hidden=%d", C);
-  auto kern = saved ? lstm_tc::lstm_fwd_tc_kernel<true> : lstm_tc::lstm_fwd_tc_kernel<false>;
-  prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)cells * T, st);
-  kern<<<lstm_grid<1>(cells, D::FWD_CTAS_PER_SM), D::THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
-                                                                       cells, T, NN);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
+  return lstm_forward_range(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, all_tiles(cells, C), T, NN, C, st);
 }
 
 int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
@@ -1212,8 +1256,11 @@ int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_
   MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4, st));
   MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4 * C, st));
   MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4, st));
+  if (C == 32 && d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
+  const TileRange r = all_tiles(cells, C);
   auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
-  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, slots, scale2, cells, T, NN, st))
+  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, DetFlush{slots, false, r.n}, scale2,
+                       cells, r, T, NN, st))
     return e;
   return lstm_copy_bias_grad(d_b_ih, d_b_hh, G4, st);
 }
@@ -1263,28 +1310,26 @@ size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int 
 
 template <int CH, bool SAVE, bool UP, bool HSEQ>
 static int stack_fwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                           void* saved, const void* h_in, void* h_seq, long long cells, int T, long long NN, cudaStream_t st) {
+                           void* saved, const void* h_in, void* h_seq, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
   auto kern = lstm_tc::lstm_fwd_tcw_kernel<CH, SAVE, UP, HSEQ>;
   constexpr size_t smem = lstm_tc::kFwdWideSmem<CH, UP>;
   static DynSmemAttr attr = {};
   if (int e = ensure_dyn_smem(kern, (int)smem, attr)) return e;
-  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * ((UP ? 2 : 1) * D::H + 1) * (double)cells * T, st);
-  kern<<<lstm_grid<CH>(cells, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved),
-                                                                           cells, T, NN, static_cast<const __half*>(h_in),
-                                                                           static_cast<__half*>(h_seq));
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * ((UP ? 2 : 1) * D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
+                                                                     r.tile0, r.n, T, NN, static_cast<const __half*>(h_in),
+                                                                     static_cast<__half*>(h_seq));
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
 }
 
+// the stack over the tiles r; training (saved != null): layer l's state at saved + l * layer_bytes
 template <int CH>
 static int stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                         const float* const* b_hh, float* hT, void* saved, void* ws, const StackFwdLayout& Y, int B, int T, long long NN,
-                         cudaStream_t st) {
-  const int C = 32 * CH;
-  const long long cells = (long long)B * NN;
-  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
+                         const float* const* b_hh, float* hT, void* saved, size_t layer_bytes, void* ws, const StackFwdLayout& Y,
+                         long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   auto lsaved = [&](int l) { return static_cast<uint8_t*>(saved) + (size_t)l * layer_bytes; };
   auto hbuf = [&](int l) { return static_cast<uint8_t*>(ws) + Y.h[l & 1]; };   // inference: h of layer l
   for (int l = 0; l < L; ++l) {
@@ -1293,17 +1338,17 @@ static int stack_forward(const float* x_seq, int L, const float* const* w_ih, co
     int e;
     if (saved) {       // training: every layer keeps c_t | h_t; the layer above reads the h half
       if (l == 0) e = stack_fwd_layer<CH, true, false, false>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], out, lsaved(0), nullptr, nullptr,
-                                                           cells, T, NN, st);
-      else e = stack_fwd_layer<CH, true, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], out, lsaved(l), lsaved(l - 1) + 1024, nullptr, cells, T, NN, st);
+                                                           cells, r, T, NN, st);
+      else e = stack_fwd_layer<CH, true, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], out, lsaved(l), lsaved(l - 1) + 1024, nullptr, cells, r, T, NN, st);
     } else if (l == 0) {
-      e = stack_fwd_layer<CH, false, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, nullptr, nullptr, hbuf(0), cells, T,
+      e = stack_fwd_layer<CH, false, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, nullptr, nullptr, hbuf(0), cells, r, T,
                                                   NN, st);
     } else if (!top) {
       e = stack_fwd_layer<CH, false, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, nullptr, hbuf(l - 1), hbuf(l),
-                                                 cells, T, NN, st);
+                                                 cells, r, T, NN, st);
     } else {
       e = stack_fwd_layer<CH, false, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], hT, nullptr, hbuf(l - 1), nullptr, cells,
-                                                  T, NN, st);
+                                                  r, T, NN, st);
     }
     if (e) return e;
   }
@@ -1313,46 +1358,46 @@ static int stack_forward(const float* x_seq, int L, const float* const* w_ih, co
 template <int CH, bool UP, bool DHIN>
 static int stack_bwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* d_hT,
                            float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, const void* h_in, void* da_rec,
-                           float* d_seq, float* slots, const float* scale2, long long cells, int T, long long NN, cudaStream_t st) {
+                           float* d_seq, DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   using D = Dims<CH>;
+  const double rc = (double)range_cells(cells, r, D::H);
   constexpr int KH = UP ? 2 * D::H : D::H;     // the input and recurrent columns of the gate GEMM
   auto walk = lstm_tc::lstm_bwd_walk_tcw_kernel<CH, UP, DHIN>;
   constexpr size_t smem = lstm_tc::kWalkSmem<CH, UP>;
   static DynSmemAttr attr_w = {};
   if (int e = ensure_dyn_smem(walk, (int)smem, attr_w)) return e;
   // the walk and the weight gradient, counted as the single layer's are, with the gate GEMM KH + 1 deep: 8 H (KH + 1) ...
-  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (KH + 1) * (double)cells * T, st);
-  walk<<<lstm_grid<CH>(cells, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x,
-                                                                           static_cast<const __half*>(saved), static_cast<__half*>(da_rec),
-                                                                           scale2, cells, T, NN, static_cast<const __half*>(h_in), d_seq);
+  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (KH + 1) * rc * T, st);
+  walk<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x,
+                                                                     static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2,
+                                                                     cells, r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), d_seq);
   prof_end(st);
   MPGCN_CUDA(cudaGetLastError());
   // ... and the weight gradient, 4 H (KH + 1)
-  return lstm_dw_pass<CH, UP>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, slots, scale2, cells, T, NN, h_in,
-                              4.0 * D::H * (KH + 1) * (double)cells * T, st);
+  return lstm_dw_pass<CH, UP>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, f, scale2, cells, r, T, NN, h_in, 4.0 * D::H * (KH + 1) * rc * T, st);
 }
 
 template <int CH>
 static int stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b,
-                          float* d_x, const void* saved, uint8_t* da_rec, size_t da_stride, float* d_seq, float* slots, const float* scale2,
-                          int B, int T, long long NN, cudaStream_t st) {
-  const long long cells = (long long)B * NN;
-  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, 32 * CH);
+                          float* d_x, const void* saved, size_t layer_bytes, uint8_t* da_rec, size_t da_stride, float* d_seq, DetFlush f,
+                          size_t slot_stride, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
   auto lsaved = [&](int l) { return static_cast<const uint8_t*>(saved) + (size_t)l * layer_bytes; };
   for (int l = L - 1; l >= 0; --l) {    // top-down: the walk of layer l leaves d(h^{l-1}_t) in d_seq for layer l - 1
     const bool top = l == L - 1;
     uint8_t* rec = da_rec + (size_t)l * da_stride;
+    // slot_stride floats apart, each layer's slots (0: the layers share one region, each reducing its own before the next)
+    const DetFlush fl = {f.slots ? f.slots + (size_t)l * slot_stride : nullptr, f.acc, f.reduce_tiles};
     int e;
     if (l == 0)
       e = stack_bwd_layer<CH, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, d_w_ih[0], d_w_hh[0], d_b[0], d_x, lsaved(0),
-                                           nullptr, rec, d_seq, slots, scale2, cells, T, NN, st);
+                                           nullptr, rec, d_seq, fl, scale2, cells, r, T, NN, st);
     else if (top)
       e = stack_bwd_layer<CH, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], d_hT, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, slots, scale2, cells, T, NN, st);
+                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, fl, scale2, cells, r, T, NN, st);
     else
       e = stack_bwd_layer<CH, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, slots, scale2, cells, T, NN, st);
+                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, fl, scale2, cells, r, T, NN, st);
     if (e) return e;
   }
   return 0;
@@ -1368,8 +1413,10 @@ int lstm_stack_forward_tc(const float* x_seq, int L, const float* const* w_ih, c
     MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack forward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
     MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack forward: workspace must be 256-byte aligned");
   }
-  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, Y, B, T, NN, st)
-                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, ws, Y, B, T, NN, st);
+  const long long cells = (long long)B * NN;
+  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
+  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, layer_bytes, ws, Y, cells, all_tiles(cells, C), T, NN, st)
+                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, layer_bytes, ws, Y, cells, all_tiles(cells, C), T, NN, st);
 }
 
 int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
@@ -1396,13 +1443,113 @@ int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, 
     MPGCN_CUDA(cudaMemsetAsync(d_w_hh[l], 0, sizeof(float) * G4 * C, st));
     MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
   }
-  const int e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
-                                            slots, scale2, B, T, NN, st)
-                        : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, da_stride, d_seq,
-                                            slots, scale2, B, T, NN, st);
+  const TileRange r = all_tiles(cells, C);
+  const DetFlush f = {slots, false, r.n};
+  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
+  const int e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, layer_bytes, da_rec,
+                                            da_stride, d_seq, f, 0, scale2, cells, r, T, NN, st)
+                        : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, layer_bytes, da_rec,
+                                            da_stride, d_seq, f, 0, scale2, cells, r, T, NN, st);
   if (e) return e;
   for (int l = 0; l < L; ++l)
     if (int e2 = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e2;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
+// recomputing backward: the forward kept no state; it is rebuilt and walked back one chunk of tiles at a time
+// ---------------------------------------------------------------------------------------
+// Per chunk: the SAVE forward of every layer over the chunk into the chunk's state region (layer l reads layer l - 1's, as in
+// the training forward), the walks top-down, the dW passes over the chunk's records.  The kernels are those of the stored-state
+// path, so every cell sees the same state bits and the same S (one grad scale over all cells): h_T, dx and the per-cell gate
+// gradients are bitwise those of mpgcn_lstm_last_backward_saved / mpgcn_lstm_stack_backward; the weight gradients differ only
+// in fp32 summation order.  Memory: O(chunk) instead of O(B NN T C); cost: one more forward.
+
+// tiles of a chunk: chunk_cells rounded up to whole tiles, raised to one wave of the backward grid (one CTA per SM at every
+// width) so that no chunk leaves SMs idle, and capped at every tile
+static long long recompute_chunk_tiles(long long cells, int C, long long chunk_cells) {
+  const long long tc = lstm_tc_tile_cells(C), all = all_tiles(cells, C).n;
+  const long long wave = (long long)Dims<1>::BWD_CTAS_PER_SM * device_sm_count();
+  long long n = chunk_cells / tc + (chunk_cells % tc != 0);
+  if (n < wave) n = wave;
+  return n < all ? n : all;
+}
+
+// workspace: the grad scale (1 KB); a stack's fp32 sequence d(h^{l-1}_t) of one chunk; deterministic mode's slots, one
+// lstm_tc_slot_bytes region per layer that accumulates across chunks (empty with the mode off); the chunk's training state of
+// every layer (lstm_tc_saved_bytes of the chunk's cells); the chunk's da records at the wide widths and in stacks, one region
+// reused by every layer
+struct RecomputeLayout { long long chunk_tiles; size_t scale, d_seq, slots, slot_stride, saved, saved_stride, da, total; };
+static RecomputeLayout recompute_layout(int B, int T, long long NN, int C, int L, long long chunk_cells) {
+  RecomputeLayout Y;
+  Y.chunk_tiles = recompute_chunk_tiles((long long)B * NN, C, chunk_cells);
+  const long long cc = Y.chunk_tiles * lstm_tc_tile_cells(C);
+  size_t off = 0;
+  Y.scale = take(off, 1024, 256);
+  Y.d_seq = take(off, L >= 2 ? (size_t)cc * T * C * sizeof(float) : 0, 256);
+  Y.slot_stride = det_mode() ? lstm_tc_slot_bytes(C, L >= 2) : 0;
+  Y.slots = take(off, (size_t)L * Y.slot_stride, 256);
+  Y.saved_stride = align_up(lstm_tc_saved_bytes(1, T, cc, C), 256);
+  Y.saved = take(off, (size_t)L * Y.saved_stride, 256);
+  Y.da = take(off, C == 32 && L == 1 ? 0 : lstm_tcw_da_bytes(1, T, cc, C), 256);
+  Y.total = align_up(off, 256);
+  return Y;
+}
+size_t lstm_tc_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells) {
+  return recompute_layout(B, T, NN, C, L, chunk_cells).total;
+}
+
+int lstm_recompute_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                               const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh,
+                               float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* ws, size_t ws_bytes,
+                               int B, int T, long long NN, int C, const float* d_hT_absmax, cudaStream_t st) {
+  MPGCN_CHECK(L == 1 ? lstm_tc_supported(T, C) : lstm_tc_stack_supported(T, C, L), "lstm recompute: no tensor-core kernels for L=%d, hidden=%d, T=%d",
+              L, C, T);
+  MPGCN_CHECK(chunk_cells >= 1, "lstm recompute: chunk_cells=%lld (at least 1)", chunk_cells);
+  const RecomputeLayout Y = recompute_layout(B, T, NN, C, L, chunk_cells);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm recompute: workspace too small (%zu < %zu)", ws_bytes, Y.total);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm recompute: workspace must be 256-byte aligned");
+  const long long cells = (long long)B * NN, all = all_tiles(cells, C).n;
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  float* scale2 = reinterpret_cast<float*>(wb + Y.scale);
+  float* d_seq = reinterpret_cast<float*>(wb + Y.d_seq);
+  float* slots = det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr;
+  void* saved = wb + Y.saved;
+  uint8_t* da_rec = wb + Y.da;
+  if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
+  const int G4 = 4 * C;
+  for (int l = 0; l < L; ++l) {
+    MPGCN_CUDA(cudaMemsetAsync(d_w_ih[l], 0, sizeof(float) * G4 * (l == 0 ? 1 : C), st));
+    MPGCN_CUDA(cudaMemsetAsync(d_w_hh[l], 0, sizeof(float) * G4 * C, st));
+    MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
+  }
+  // every launch below writes d_x of its chunk's cells in full, so d_x needs no clearing
+  for (long long t0 = 0; t0 < all; t0 += Y.chunk_tiles) {
+    const TileRange r = {t0, Y.chunk_tiles < all - t0 ? Y.chunk_tiles : all - t0};
+    const DetFlush f = {slots, t0 > 0, t0 + r.n == all ? Y.chunk_tiles : 0};
+    int e;
+    if (L == 1) {
+      e = lstm_forward_range(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, saved, cells, r, T, NN, C, st);
+      if (e == 0) {
+        auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
+        e = backward(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], d_hT, d_w_ih[0], d_w_hh[0], d_b_ih[0], d_x, saved, da_rec, f, scale2, cells,
+                     r, T, NN, st);
+      }
+    } else {
+      const StackFwdLayout none = {};      // (a training forward keeps no h sequence in a workspace)
+      const size_t slot_floats = Y.slot_stride / sizeof(float);
+      e = C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, nullptr, saved, Y.saved_stride, nullptr, none, cells, r, T, NN, st)
+                  : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, nullptr, saved, Y.saved_stride, nullptr, none, cells, r, T, NN, st);
+      if (e == 0)
+        e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, Y.saved_stride, da_rec, 0,
+                                        d_seq, f, slot_floats, scale2, cells, r, T, NN, st)
+                    : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, Y.saved_stride, da_rec, 0,
+                                        d_seq, f, slot_floats, scale2, cells, r, T, NN, st);
+    }
+    if (e) return e;
+  }
+  for (int l = 0; l < L; ++l)
+    if (int e = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e;
   return 0;
 }
 

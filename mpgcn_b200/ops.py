@@ -5,6 +5,7 @@
     lstm_last(x_seq, w_ih, w_hh, b_ih, b_hh)  <->  nn.LSTM(...)[:, -1, :]  (MPGCN.py:69,100-104)
     lstm_stack(x_seq, params, precision)      <->  the same with num_layers = L >= 2
     lstm_module_last(lstm, x_seq, precision)  <->  either of them, or the module itself where the engine has no kernel
+                                                  (each takes `recompute`: keep no LSTM training state, rebuild it in the backward)
 
 PyTorch supplies device memory, the current stream and the autograd tape; all arithmetic is in
 libmpgcn_b200.so.
@@ -329,6 +330,31 @@ def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None, su
     return _BDGCNFn.apply(X, G_o, G_d, W, b, dynamic, 1 if relu else 0, precision, grad_mode, bool(support_grad))
 
 
+# State budget of the recomputing LSTM backward with recompute=True: the chunk of cells whose rebuilt training state (and gate-
+# gradient records, and a stack's gradient sequence) takes about this much.  A choice, not a tuned value: chunks of this size
+# already fill every SM many times over, and it is small beside the state it replaces (tens of GB at N = 1000).
+LSTM_RECOMPUTE_BUDGET_BYTES = 1 << 30
+
+
+def _check_recompute(recompute) -> None:
+    if not (recompute is None or isinstance(recompute, bool) or (isinstance(recompute, int) and recompute >= 1)):
+        raise ValueError(f"recompute must be None, a bool or a positive number of cells per chunk, got {recompute!r}")
+
+
+def lstm_recompute_chunk_cells(recompute, T, C, L) -> int:
+    """Cells per chunk of the recomputing backward for `recompute` (None / False: 0, off; True: LSTM_RECOMPUTE_BUDGET_BYTES of
+    workspace; an int: that many cells)."""
+    if recompute is None or recompute is False:
+        return 0
+    if recompute is not True:
+        return int(recompute)
+    probe = 1 << 20        # the workspace is about linear in the chunk: size it from the query at one large chunk
+    per = _lib.load().mpgcn_lstm_recompute_bwd_workspace_bytes(1, T, probe, C, L, probe, _lib.PREC_FP16_TC)
+    if not per:
+        raise RuntimeError(f"LSTM recompute: no tensor-core kernels for T={T}, hidden={C}, L={L}")
+    return max(1, LSTM_RECOMPUTE_BUDGET_BYTES * probe // per)
+
+
 def resolve_lstm_precision(name, T, C) -> int:
     name = default_precision() if name is None else name
     if name not in _PREC_NAMES:
@@ -357,7 +383,7 @@ def lstm_engine_supports(name, T, C) -> bool:
 class _LSTMLastFn(torch.autograd.Function):
     @staticmethod
     @_lib.engine_buffers()
-    def forward(ctx, x_seq, w_ih, w_hh, b_ih, b_hh, precision, grad_mode: bool):
+    def forward(ctx, x_seq, w_ih, w_hh, b_ih, b_hh, precision, grad_mode: bool, recompute):
         lib = _lib.load()
         B, T = x_seq.shape[0], x_seq.shape[1]
         NN = x_seq[0, 0].numel()
@@ -366,16 +392,20 @@ class _LSTMLastFn(torch.autograd.Function):
         xc = _f32c(x_seq)
         ws = [_f32c(t) for t in (w_ih, w_hh, b_ih, b_hh)]
         hT = torch.empty((B * NN, C), dtype=torch.float32, device=x_seq.device)
-        # training: the forward keeps c_t / h_t of every step (fp16) so that the backward is one reverse walk
-        nsave = lib.mpgcn_lstm_saved_bytes(B, T, NN, C, prec) if (grad_mode and any(ctx.needs_input_grad[:5])) else 0
+        # training: the forward keeps c_t / h_t of every step (fp16) so that the backward is one reverse walk -- unless the
+        # backward is to rebuild them a chunk at a time (recompute; precision 0 keeps none anyway)
+        train = grad_mode and any(ctx.needs_input_grad[:5])
+        chunk = lstm_recompute_chunk_cells(recompute, T, C, 1) if (train and prec == _lib.PREC_FP16_TC) else 0
+        nsave = lib.mpgcn_lstm_saved_bytes(B, T, NN, C, prec) if (train and not chunk) else 0
         saved = torch.empty(nsave, dtype=torch.uint8, device=x_seq.device) if nsave else None
-        # (precision 0 keeps no state -- its backward recomputes -- so count the request, not the buffer)
-        STASH_BYTES["lstm"] += nsave if nsave else (1 if (grad_mode and any(ctx.needs_input_grad[:5])) else 0)
+        # (precision 0 and recompute keep no state, so count the request, not the buffer)
+        STASH_BYTES["lstm"] += nsave if nsave else (1 if train else 0)
         with torch.cuda.device(x_seq.device):
             _lib.check(lib.mpgcn_lstm_last_forward_train(_ptr(xc), *[_ptr(t) for t in ws], _ptr(hT), _ptr(saved), nsave, B, T, NN, C, prec,
                                                          _stream()), "lstm_last_forward")
         ctx.dims = (B, T, NN, C, prec)
         ctx.lstm_saved = saved
+        ctx.chunk = chunk
         ctx.save_for_backward(xc, *ws)
         return hT
 
@@ -392,6 +422,14 @@ class _LSTMLastFn(torch.autograd.Function):
         g_wih, g_whh = torch.empty_like(w_ih), torch.empty_like(w_hh)
         g_bih, g_bhh = torch.empty_like(b_ih), torch.empty_like(b_hh)
         d_x = torch.empty_like(xc) if ctx.needs_input_grad[0] else None
+        if ctx.chunk:
+            ws = _scratch(lib.mpgcn_lstm_recompute_bwd_workspace_bytes(B, T, NN, C, 1, ctx.chunk, prec), dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.mpgcn_lstm_backward_recompute(_ptr(xc), 1, *[_ptr_array([t]) for t in (w_ih, w_hh, b_ih, b_hh)], _ptr(d_hT),
+                                                             *[_ptr_array([t]) for t in (g_wih, g_whh, g_bih, g_bhh)], _ptr(d_x), ctx.chunk,
+                                                             _ptr(ws), ws.numel(), B, T, NN, C, prec, _ptr(hint), _stream()),
+                           "lstm_backward_recompute")
+            return d_x, g_wih, g_whh, g_bih, g_bhh, None, None, None
         saved = ctx.lstm_saved
         # with the forward's state in hand the backward needs its workspace minus the room for rebuilding that state
         ws_bytes = lib.mpgcn_lstm_bwd_workspace_bytes(B, T, NN, C, prec)
@@ -402,13 +440,16 @@ class _LSTMLastFn(torch.autograd.Function):
                                                           saved.numel() if saved is not None else 0, _ptr(ws), ws.numel(), B, T, NN, C,
                                                           prec, _ptr(hint), _stream()), "lstm_last_backward")
         ctx.lstm_saved = None
-        return d_x, g_wih, g_whh, g_bih, g_bhh, None, None
+        return d_x, g_wih, g_whh, g_bih, g_bhh, None, None, None
 
 
-def lstm_last(x_seq: torch.Tensor, w_ih, w_hh, b_ih, b_hh, precision=None) -> torch.Tensor:
-    """h_T of a 1-layer, input-size-1 LSTM run over every OD cell of x_seq [B,T,N,N,1] -> [B*N*N, C]."""
+def lstm_last(x_seq: torch.Tensor, w_ih, w_hh, b_ih, b_hh, precision=None, recompute=None) -> torch.Tensor:
+    """h_T of a 1-layer, input-size-1 LSTM run over every OD cell of x_seq [B,T,N,N,1] -> [B*N*N, C].
+    recompute (tensor cores): True or a number of cells per chunk -> the training forward keeps no c_t / h_t and the backward
+    rebuilds them a chunk at a time (lstm_recompute_chunk_cells); same h_T and dx, weight gradients up to fp32 summation order."""
     _require_cuda(x_seq, "x_seq")
-    return _LSTMLastFn.apply(x_seq, w_ih, w_hh, b_ih, b_hh, precision, torch.is_grad_enabled())
+    _check_recompute(recompute)
+    return _LSTMLastFn.apply(x_seq, w_ih, w_hh, b_ih, b_hh, precision, torch.is_grad_enabled(), recompute)
 
 
 def lstm_stack_supports(name, T, C, L) -> bool:
@@ -439,15 +480,17 @@ def lstm_runs_on_engine(lstm: torch.nn.LSTM, T: int, precision) -> bool:
     return lstm_stack_supports(precision, T, C, L)
 
 
-def lstm_module_last(lstm: torch.nn.LSTM, x_seq: torch.Tensor, precision=None) -> torch.Tensor:
-    """h_T of the top layer of `lstm` (batch_first, zero initial state) over every OD cell of x_seq [B,T,N,N,I] -> [B*N*N, C]."""
+def lstm_module_last(lstm: torch.nn.LSTM, x_seq: torch.Tensor, precision=None, recompute=None) -> torch.Tensor:
+    """h_T of the top layer of `lstm` (batch_first, zero initial state) over every OD cell of x_seq [B,T,N,N,I] -> [B*N*N, C].
+    recompute: as `lstm_last`; the module itself, where it runs, is unaffected."""
     B, T, N, N2, I = x_seq.shape
     L = lstm.num_layers
     if lstm_runs_on_engine(lstm, T, precision):
         if L == 1:
-            return lstm_last(x_seq, lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0, precision=precision)
+            return lstm_last(x_seq, lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0, precision=precision,
+                             recompute=recompute)
         params = [getattr(lstm, f"{k}_l{l}") for l in range(L) for k in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]
-        return lstm_stack(x_seq, params)
+        return lstm_stack(x_seq, params, recompute=recompute)
     # configurations without an engine kernel: input_dim > 1 (Model_Trainer.py:49-51 hard-codes input_dim=1), hidden sizes
     # above 64 other than 96 / 128, sequences longer than 256 steps above hidden 64, sequences whose fp32 backward does not fit
     # in shared memory (T > 15 at hidden 64, DESIGN.md 6.4), fp32 above 64, and stacks other than those above
@@ -463,7 +506,7 @@ def _ptr_array(ts):
 class _LSTMStackFn(torch.autograd.Function):
     @staticmethod
     @_lib.engine_buffers()
-    def forward(ctx, grad_mode: bool, x_seq, *params):
+    def forward(ctx, grad_mode: bool, recompute, x_seq, *params):
         lib = _lib.load()
         B, T = x_seq.shape[0], x_seq.shape[1]
         NN = x_seq[0, 0].numel()
@@ -472,10 +515,13 @@ class _LSTMStackFn(torch.autograd.Function):
         xc = _f32c(x_seq)
         ps = [_f32c(t) for t in params]
         hT = torch.empty((B * NN, C), dtype=torch.float32, device=x_seq.device)
-        # training: every layer keeps c_t / h_t of every step; inference keeps only the h sequence of the layer below (workspace)
-        need = grad_mode and any(ctx.needs_input_grad[1:])
+        # training: every layer keeps c_t / h_t of every step; inference keeps only the h sequence of the layer below (workspace),
+        # and so does training with recompute (its backward rebuilds the state a chunk at a time)
+        train = grad_mode and any(ctx.needs_input_grad[2:])
+        chunk = lstm_recompute_chunk_cells(recompute, T, C, L) if train else 0
+        need = train and not chunk
         saved = torch.empty(lib.mpgcn_lstm_stack_saved_bytes(B, T, NN, C, L, prec), dtype=torch.uint8, device=x_seq.device) if need else None
-        STASH_BYTES["lstm"] += saved.numel() if saved is not None else 0
+        STASH_BYTES["lstm"] += saved.numel() if saved is not None else (1 if chunk else 0)
         ws = None if need else _scratch(lib.mpgcn_lstm_stack_fwd_workspace_bytes(B, T, NN, C, L, prec), x_seq.device)
         with torch.cuda.device(x_seq.device):
             _lib.check(lib.mpgcn_lstm_stack_forward(_ptr(xc), L, *[_ptr_array(ps[k::4]) for k in range(4)], _ptr(hT), _ptr(saved),
@@ -483,6 +529,7 @@ class _LSTMStackFn(torch.autograd.Function):
                                                     B, T, NN, C, prec, _stream()), "lstm_stack_forward")
         ctx.dims = (B, T, NN, C, L, prec)
         ctx.lstm_saved = saved
+        ctx.chunk = chunk
         ctx.save_for_backward(xc, *ps)
         return hT
 
@@ -493,13 +540,21 @@ class _LSTMStackFn(torch.autograd.Function):
         _lib.sync_deterministic()
         xc, *ps = ctx.saved_tensors
         B, T, NN, C, L, prec = ctx.dims
-        if ctx.lstm_saved is None:
+        if ctx.lstm_saved is None and not ctx.chunk:
             raise RuntimeError("mpgcn_b200.lstm_stack: backward called but forward ran without requires_grad inputs")
         hint = _take_hint(ctx, d_hT) if (d_hT.dtype == torch.float32 and d_hT.is_contiguous()) else None
         d_hT = _f32c(d_hT)
         dev = xc.device
         grads = [torch.empty_like(p) for p in ps]
-        d_x = torch.empty_like(xc) if ctx.needs_input_grad[1] else None
+        d_x = torch.empty_like(xc) if ctx.needs_input_grad[2] else None
+        if ctx.chunk:
+            ws = _scratch(lib.mpgcn_lstm_recompute_bwd_workspace_bytes(B, T, NN, C, L, ctx.chunk, prec), dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.mpgcn_lstm_backward_recompute(_ptr(xc), L, *[_ptr_array(ps[k::4]) for k in range(4)], _ptr(d_hT),
+                                                             *[_ptr_array(grads[k::4]) for k in range(4)], _ptr(d_x), ctx.chunk,
+                                                             _ptr(ws), ws.numel(), B, T, NN, C, prec, _ptr(hint), _stream()),
+                           "lstm_backward_recompute")
+            return (None, None, d_x, *grads)
         saved = ctx.lstm_saved
         ws = _scratch(lib.mpgcn_lstm_stack_bwd_workspace_bytes(B, T, NN, C, L, prec), dev)
         with torch.cuda.device(dev):
@@ -507,12 +562,13 @@ class _LSTMStackFn(torch.autograd.Function):
                                                      *[_ptr_array(grads[k::4]) for k in range(4)], _ptr(d_x), _ptr(saved), saved.numel(),
                                                      _ptr(ws), ws.numel(), B, T, NN, C, prec, _ptr(hint), _stream()), "lstm_stack_backward")
         ctx.lstm_saved = None
-        return (None, d_x, *grads)
+        return (None, None, d_x, *grads)
 
 
-def lstm_stack(x_seq: torch.Tensor, params) -> torch.Tensor:
+def lstm_stack(x_seq: torch.Tensor, params, recompute=None) -> torch.Tensor:
     """h_T of the top layer of an L-layer, input-size-1 LSTM run over every OD cell of x_seq [B,T,N,N,1] -> [B*N*N, C];
-    params: [w_ih, w_hh, b_ih, b_hh] of layer 0, then of layer 1, ... (nn.LSTM's *_l0, *_l1, ...).  Tensor cores only."""
+    params: [w_ih, w_hh, b_ih, b_hh] of layer 0, then of layer 1, ... (nn.LSTM's *_l0, *_l1, ...).  Tensor cores only.
+    recompute: as `lstm_last`."""
     _require_cuda(x_seq, "x_seq")
     if len(params) < 8 or len(params) % 4:
         raise ValueError(f"lstm_stack: expected 4 parameters per layer and at least 2 layers, got {len(params)}")
@@ -525,7 +581,8 @@ def lstm_stack(x_seq: torch.Tensor, params) -> torch.Tensor:
         if tuple(p.shape) != want or not p.is_floating_point() or p.device != x_seq.device:
             raise ValueError(f"lstm_stack: parameter {i} (layer {l}) must be a float tensor of shape {want} on {x_seq.device}, "
                              f"got {tuple(p.shape)} {p.dtype} on {p.device}")
-    return _LSTMStackFn.apply(torch.is_grad_enabled(), x_seq, *params)
+    _check_recompute(recompute)
+    return _LSTMStackFn.apply(torch.is_grad_enabled(), recompute, x_seq, *params)
 
 
 class _HeadFn(torch.autograd.Function):

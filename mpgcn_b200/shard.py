@@ -191,8 +191,8 @@ class CudaEngine:
                                                            scale2.data_ptr(), B, N, row0, rows, H, ops._stream()), "relu_backward_scatter_f16")
         return db, scale2
 
-    def lstm_last(self, x_seq, lstm, precision):
-        return ops.lstm_module_last(lstm, x_seq, precision)
+    def lstm_last(self, x_seq, lstm, precision, recompute=None):
+        return ops.lstm_module_last(lstm, x_seq, precision, recompute)
 
     def head(self, feats, w, b):
         return ops.fc_relu_mean(feats, w, b)
@@ -535,7 +535,9 @@ def sharded_forward(model, plan: ShardPlan, x_slab, G_static, G_dyn):
 
     def temporal(lstm, x):
         B, _, rows, N, _ = x.shape
-        h = _ENGINE.lstm_last(x, lstm, model.lstm_precision).reshape(B, rows, N, model.lstm_hidden_dim)
+        # (the option is passed only when set, so an engine without it -- the CPU stand-ins of the tests -- is called as before)
+        extra = {"recompute": model.lstm_recompute} if getattr(model, "lstm_recompute", None) else {}
+        h = _ENGINE.lstm_last(x, lstm, model.lstm_precision, **extra).reshape(B, rows, N, model.lstm_hidden_dim)
         return h if plan.kind == "row" else _AllGatherRowsFn.apply(h, plan)
 
     # The branches are independent until the head: each runs on its own CUDA stream, so that the exchange steps of one branch

@@ -15,7 +15,10 @@ What it does, and nothing more:
     `ModelTrainer.test` (Model_Trainer.py:157-165) replay one captured CUDA graph per batch;
   * `--sparse-static-supports`: the static support stack of `ModelTrainer.preprocess_adj` (Model_Trainer.py:38-42) becomes a
     sparse COO tensor (`.to_sparse()`), so the static branch's layers run the gathers over its nonzeros (fp32; DESIGN.md
-    section 12) instead of dense N^3 contractions.
+    section 12) instead of dense N^3 contractions;
+  * `--lstm-recompute`: `model.lstm_recompute = True` on the trainer's model -- the tensor-core LSTM keeps no training state in
+    the forward and its backward rebuilds it a chunk of cells at a time (DESIGN.md section 6.5), so that hidden 96 and 128
+    fit at N = 1000.
 Everything after `--` is Main.py's own command line (Main.py:11-37).
 """
 import argparse
@@ -32,6 +35,7 @@ def main():
     ap.add_argument("--graph-rollout", action="store_true")
     ap.add_argument("--gpu-dyn-graphs", action="store_true")
     ap.add_argument("--sparse-static-supports", action="store_true")
+    ap.add_argument("--lstm-recompute", action="store_true")
     ap.add_argument("--seed", type=int, default=None, help="torch.manual_seed / numpy seed before Main.py runs (the reference sets none)")
     ap.add_argument("--stock", action="store_true", help="do NOT shadow MPGCN / GCN: run the reference as it is (CPU plumbing check)")
     ap.add_argument("main_args", nargs=argparse.REMAINDER)
@@ -62,6 +66,15 @@ def main():
             import Model_Trainer
             preprocess_adj = Model_Trainer.ModelTrainer.preprocess_adj
             Model_Trainer.ModelTrainer.preprocess_adj = lambda self, *args, **kw: preprocess_adj(self, *args, **kw).to_sparse()
+        if a.lstm_recompute:
+            import Model_Trainer
+            get_model_r = Model_Trainer.ModelTrainer.get_model
+
+            def get_model_recompute(self):
+                model = get_model_r(self)
+                model.lstm_recompute = True
+                return model
+            Model_Trainer.ModelTrainer.get_model = get_model_recompute
     if a.seed is not None:
         import numpy as np
         import torch
