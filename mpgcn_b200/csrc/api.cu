@@ -381,16 +381,54 @@ size_t mpgcn_lstm_saved_bytes(int B, int T, long long NN, int C, int precision) 
   return precision == PREC_FP16_TC ? lstm_tc_saved_bytes(B, T, NN, lstm_tc_size_width(C)) : 0;
 }
 
+int mpgcn_lstm_stack_supported(int T, int C, int L, int precision) {
+  if (L == 1) return mpgcn_lstm_precision_supported(T, C, precision);
+  return precision == PREC_FP16_TC && lstm_tc_stack_supported(T, C, L) ? 1 : 0;
+}
+
+size_t mpgcn_lstm_stack_saved_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_saved_bytes(B, T, NN, C, L) : 0;
+}
+size_t mpgcn_lstm_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_fwd_workspace_bytes(B, T, NN, C, L) : 0;
+}
+size_t mpgcn_lstm_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
+  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_bwd_workspace_bytes(B, T, NN, C, L) : 0;
+}
+
+size_t mpgcn_lstm_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells, int precision) {
+  if (precision != PREC_FP16_TC || L < 1 || !mpgcn_lstm_stack_supported(T, C, L, precision) || B < 1 || NN < 1 || chunk_cells < 1) return 0;
+  return lstm_tc_recompute_bwd_workspace_bytes(B, T, NN, C, L, chunk_cells);
+}
+
+// The argument checks of every LSTM entry, all before its first CUDA call: L layers (the stack entries take L >= 2), x_seq and
+// h (h_T or d_hT), the L device pointers of each weight array w = {w_ih, w_hh, b_ih, b_hh} and, in a backward, of each gradient
+// array g, a non-empty input, and kernels for (T, C, L) at the precision.  Precision 0 keeps no training state in the first
+// place, so the recomputing backward runs the tensor-core kernels only.
+enum LstmCall { LSTM_LAST, LSTM_STACK, LSTM_RECOMPUTE };
+static int check_lstm(const char* what, LstmCall call, int L, const float* x_seq, const float* h, const float* const* const* w,
+                      float* const* const* g, int B, int T, long long NN, int C, int precision) {
+  MPGCN_CHECK(L >= (call == LSTM_STACK ? 2 : 1), "%s: L=%d%s", what, L, call == LSTM_STACK ? " (a single layer is mpgcn_lstm_last_*)" : "");
+  MPGCN_CHECK(x_seq && h, "%s: null pointer argument", what);
+  for (int k = 0; k < 4; ++k) {
+    MPGCN_CHECK(w[k] && (!g || g[k]), "%s: null pointer argument", what);
+    for (int l = 0; l < L; ++l) MPGCN_CHECK(w[k][l] && (!g || g[k][l]), "%s: null pointer argument (layer %d)", what, l);
+  }
+  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "%s: empty input", what);
+  MPGCN_CHECK((call != LSTM_RECOMPUTE || precision == PREC_FP16_TC) && mpgcn_lstm_stack_supported(T, C, L, precision),
+              "%s: precision %d does not support T=%d, hidden=%d, L=%d", what, precision, T, C, L);
+  return 0;
+}
+
 int mpgcn_lstm_last_forward_train(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
                                   void* saved, size_t saved_bytes, int B, int T, long long NN, int C, int precision, void* stream) {
-  MPGCN_CHECK(x_seq && w_ih && w_hh && b_ih && b_hh && hT, "mpgcn_lstm_last_forward: null pointer argument");
-  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "mpgcn_lstm_last_forward: empty input");
-  MPGCN_CHECK(mpgcn_lstm_precision_supported(T, C, precision), "lstm: precision %d does not support T=%d, hidden=%d", precision, T, C);
+  const float* const* w[4] = {&w_ih, &w_hh, &b_ih, &b_hh};
+  if (int e = check_lstm("mpgcn_lstm_last_forward", LSTM_LAST, 1, x_seq, hT, w, nullptr, B, T, NN, C, precision)) return e;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (precision == PREC_FP16_TC) {
     MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN, C), "lstm forward: saved buffer too small (%zu < %zu)",
                 saved_bytes, lstm_tc_saved_bytes(B, T, NN, C));
-    return lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, B, T, NN, C, st);
+    return lstm_forward_tc(x_seq, 1, w[0], w[1], w[2], w[3], hT, saved, nullptr, 0, B, T, NN, C, st);
   }
   return lstm_last_forward(x_seq, w_ih, w_hh, b_ih, b_hh, hT, B, T, NN, C, st);
 }
@@ -403,7 +441,20 @@ int mpgcn_lstm_last_forward(const float* x_seq, const float* w_ih, const float* 
 int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                                    const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x,
                                    const void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes, int B, int T,
-                                   long long NN, int C, int precision, const float* d_hT_absmax, void* stream);
+                                   long long NN, int C, int precision, const float* d_hT_absmax, void* stream) {
+  const float* const* w[4] = {&w_ih, &w_hh, &b_ih, &b_hh};
+  float* const* g[4] = {&d_w_ih, &d_w_hh, &d_b_ih, &d_b_hh};
+  if (int e = check_lstm("mpgcn_lstm_last_backward", LSTM_LAST, 1, x_seq, d_hT, w, g, B, T, NN, C, precision)) return e;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (precision == PREC_FP16_TC) {
+    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN, C), "lstm backward: saved buffer too small (%zu < %zu)",
+                saved_bytes, lstm_tc_saved_bytes(B, T, NN, C));
+    return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, C, workspace,
+                                 workspace_bytes, d_hT_absmax, st);
+  }
+  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, workspace,
+                            workspace_bytes, st);
+}
 
 int mpgcn_lstm_last_backward(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                              const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, void* workspace,
@@ -420,60 +471,15 @@ int mpgcn_lstm_last_backward_ex(const float* x_seq, const float* w_ih, const flo
                                         workspace_bytes, B, T, NN, C, precision, d_hT_absmax, stream);
 }
 
-int mpgcn_lstm_last_backward_saved(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
-                                   const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x,
-                                   const void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes, int B, int T,
-                                   long long NN, int C, int precision, const float* d_hT_absmax, void* stream) {
-  MPGCN_CHECK(x_seq && w_ih && w_hh && b_ih && b_hh && d_hT && d_w_ih && d_w_hh && d_b_ih && d_b_hh,
-              "mpgcn_lstm_last_backward: null pointer argument");
-  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "mpgcn_lstm_last_backward: empty input");
-  MPGCN_CHECK(mpgcn_lstm_precision_supported(T, C, precision), "lstm: precision %d does not support T=%d, hidden=%d", precision, T, C);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (precision == PREC_FP16_TC) {
-    MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_saved_bytes(B, T, NN, C), "lstm backward: saved buffer too small (%zu < %zu)",
-                saved_bytes, lstm_tc_saved_bytes(B, T, NN, C));
-    return lstm_last_backward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, B, T, NN, C, workspace,
-                                 workspace_bytes, d_hT_absmax, st);
-  }
-  return lstm_last_backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, B, T, NN, C, workspace,
-                            workspace_bytes, st);
-}
-
-int mpgcn_lstm_stack_supported(int T, int C, int L, int precision) {
-  if (L == 1) return mpgcn_lstm_precision_supported(T, C, precision);
-  return precision == PREC_FP16_TC && lstm_tc_stack_supported(T, C, L) ? 1 : 0;
-}
-
-size_t mpgcn_lstm_stack_saved_bytes(int B, int T, long long NN, int C, int L, int precision) {
-  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_saved_bytes(B, T, NN, C, L) : 0;
-}
-size_t mpgcn_lstm_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
-  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_fwd_workspace_bytes(B, T, NN, C, L) : 0;
-}
-size_t mpgcn_lstm_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, int precision) {
-  return mpgcn_lstm_stack_supported(T, C, L, precision) && L >= 2 ? lstm_tc_stack_bwd_workspace_bytes(B, T, NN, C, L) : 0;
-}
-
-static int check_stack(const char* what, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                       const float* const* b_hh, int B, int T, long long NN, int C, int precision) {
-  MPGCN_CHECK(L >= 2, "%s: L=%d (a single layer is mpgcn_lstm_last_*)", what, L);
-  MPGCN_CHECK(w_ih && w_hh && b_ih && b_hh, "%s: null pointer argument", what);
-  for (int l = 0; l < L; ++l) MPGCN_CHECK(w_ih[l] && w_hh[l] && b_ih[l] && b_hh[l], "%s: null pointer argument (layer %d)", what, l);
-  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "%s: empty input", what);
-  MPGCN_CHECK(mpgcn_lstm_stack_supported(T, C, L, precision), "%s: precision %d does not support T=%d, hidden=%d, L=%d", what, precision, T,
-              C, L);
-  return 0;
-}
-
 int mpgcn_lstm_stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
                              const float* const* b_hh, float* hT, void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes,
                              int B, int T, long long NN, int C, int precision, void* stream) {
-  if (int e = check_stack("mpgcn_lstm_stack_forward", L, w_ih, w_hh, b_ih, b_hh, B, T, NN, C, precision)) return e;
-  MPGCN_CHECK(x_seq && hT, "mpgcn_lstm_stack_forward: null pointer argument");
+  const float* const* w[4] = {w_ih, w_hh, b_ih, b_hh};
+  if (int e = check_lstm("mpgcn_lstm_stack_forward", LSTM_STACK, L, x_seq, hT, w, nullptr, B, T, NN, C, precision)) return e;
   MPGCN_CHECK(saved == nullptr || saved_bytes >= lstm_tc_stack_saved_bytes(B, T, NN, C, L),
               "lstm stack forward: saved buffer too small (%zu < %zu)", saved_bytes, lstm_tc_stack_saved_bytes(B, T, NN, C, L));
-  return lstm_stack_forward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, workspace, workspace_bytes, B, T, NN, C,
-                               static_cast<cudaStream_t>(stream));
+  return lstm_forward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, workspace, workspace_bytes, B, T, NN, C,
+                         static_cast<cudaStream_t>(stream));
 }
 
 int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
@@ -481,19 +487,14 @@ int mpgcn_lstm_stack_backward(const float* x_seq, int L, const float* const* w_i
                               float* const* d_b_hh, float* d_x, const void* saved, size_t saved_bytes, void* workspace,
                               size_t workspace_bytes, int B, int T, long long NN, int C, int precision, const float* d_hT_absmax,
                               void* stream) {
-  if (int e = check_stack("mpgcn_lstm_stack_backward", L, w_ih, w_hh, b_ih, b_hh, B, T, NN, C, precision)) return e;
-  MPGCN_CHECK(x_seq && d_hT && d_w_ih && d_w_hh && d_b_ih && d_b_hh && saved, "mpgcn_lstm_stack_backward: null pointer argument");
-  for (int l = 0; l < L; ++l)
-    MPGCN_CHECK(d_w_ih[l] && d_w_hh[l] && d_b_ih[l] && d_b_hh[l], "mpgcn_lstm_stack_backward: null pointer argument (layer %d)", l);
+  const float* const* w[4] = {w_ih, w_hh, b_ih, b_hh};
+  float* const* g[4] = {d_w_ih, d_w_hh, d_b_ih, d_b_hh};
+  if (int e = check_lstm("mpgcn_lstm_stack_backward", LSTM_STACK, L, x_seq, d_hT, w, g, B, T, NN, C, precision)) return e;
+  MPGCN_CHECK(saved != nullptr, "mpgcn_lstm_stack_backward: null pointer argument");
   MPGCN_CHECK(saved_bytes >= lstm_tc_stack_saved_bytes(B, T, NN, C, L), "lstm stack backward: saved buffer too small (%zu < %zu)",
               saved_bytes, lstm_tc_stack_saved_bytes(B, T, NN, C, L));
   return lstm_stack_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, workspace, workspace_bytes,
                                 B, T, NN, C, d_hT_absmax, static_cast<cudaStream_t>(stream));
-}
-
-size_t mpgcn_lstm_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, int L, long long chunk_cells, int precision) {
-  if (precision != PREC_FP16_TC || L < 1 || !mpgcn_lstm_stack_supported(T, C, L, precision) || B < 1 || NN < 1 || chunk_cells < 1) return 0;
-  return lstm_tc_recompute_bwd_workspace_bytes(B, T, NN, C, L, chunk_cells);
 }
 
 int mpgcn_lstm_backward_recompute(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
@@ -501,17 +502,10 @@ int mpgcn_lstm_backward_recompute(const float* x_seq, int L, const float* const*
                                   float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* workspace,
                                   size_t workspace_bytes, int B, int T, long long NN, int C, int precision, const float* d_hT_absmax,
                                   void* stream) {
-  const char* what = "mpgcn_lstm_backward_recompute";
-  MPGCN_CHECK(L >= 1, "%s: L=%d", what, L);
-  MPGCN_CHECK(x_seq && w_ih && w_hh && b_ih && b_hh && d_hT && d_w_ih && d_w_hh && d_b_ih && d_b_hh, "%s: null pointer argument", what);
-  for (int l = 0; l < L; ++l)
-    MPGCN_CHECK(w_ih[l] && w_hh[l] && b_ih[l] && b_hh[l] && d_w_ih[l] && d_w_hh[l] && d_b_ih[l] && d_b_hh[l],
-                "%s: null pointer argument (layer %d)", what, l);
-  MPGCN_CHECK(B >= 1 && T >= 1 && NN >= 1, "%s: empty input", what);
-  // precision 0 keeps no training state in the first place: its backward always recomputes
-  MPGCN_CHECK(precision == PREC_FP16_TC && mpgcn_lstm_stack_supported(T, C, L, precision),
-              "%s: precision %d does not support T=%d, hidden=%d, L=%d (tensor-core kernels only)", what, precision, T, C, L);
-  MPGCN_CHECK(chunk_cells >= 1, "%s: chunk_cells=%lld (at least 1)", what, chunk_cells);
+  const float* const* w[4] = {w_ih, w_hh, b_ih, b_hh};
+  float* const* g[4] = {d_w_ih, d_w_hh, d_b_ih, d_b_hh};
+  if (int e = check_lstm("mpgcn_lstm_backward_recompute", LSTM_RECOMPUTE, L, x_seq, d_hT, w, g, B, T, NN, C, precision)) return e;
+  MPGCN_CHECK(chunk_cells >= 1, "mpgcn_lstm_backward_recompute: chunk_cells=%lld (at least 1)", chunk_cells);
   return lstm_recompute_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, chunk_cells, workspace,
                                     workspace_bytes, B, T, NN, C, d_hT_absmax, static_cast<cudaStream_t>(stream));
 }

@@ -129,24 +129,23 @@ int adj_process_backward(const float* flow, const float* supports, const float* 
 size_t dyn_graph_workspace_bytes(int P, int N);
 int dyn_graph_build(const float* od_hist, int periods, float* o_g, float* d_g, int P, int N, void* ws, size_t ws_bytes, cudaStream_t st);
 
-// tensor-core LSTM (lstm_tc.cu): hidden size C = 32, 96, 128
+// tensor-core LSTM (lstm_tc.cu): hidden size C = 32, 96, 128; per-layer weights as HOST arrays of L device pointers
 bool lstm_tc_supported(int T, int C);
 size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C);
 size_t lstm_tc_saved_bytes(int B, int T, long long NN, int C);
-// saved (nullable): training state c_t, h_t written by the forward; the backward walks it instead of recomputing the forward
-int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                         void* saved, int B, int T, long long NN, int C, cudaStream_t s);
+// L = 1 or a stack.  saved (nullable): training state c_t, h_t of every layer written by the forward; the backward walks it
+// instead of recomputing the forward.  ws: a stack's inference workspace (lstm_tc_stack_fwd_workspace_bytes), unused otherwise
+int lstm_forward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                    const float* const* b_hh, float* hT, void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN, int C,
+                    cudaStream_t s);
 int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                           const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
                           int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t s);
-// stacked (L >= 2 layers) at hidden 32 and 96; per-layer weights as HOST arrays of L device pointers
+// stacked (L >= 2 layers) at hidden 32 and 96
 bool lstm_tc_stack_supported(int T, int C, int L);
 size_t lstm_tc_stack_saved_bytes(int B, int T, long long NN, int C, int L);
 size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L);
 size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L);
-int lstm_stack_forward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                          const float* const* b_hh, float* hT, void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN, int C,
-                          cudaStream_t s);
 int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
                            const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
                            float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,

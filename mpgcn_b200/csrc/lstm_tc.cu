@@ -608,7 +608,7 @@ lstm_bwd_saved_tc_kernel(const float* __restrict__ x_seq, const float* __restric
 template <int CH, bool UP = false>
 constexpr size_t kFwdWideSmem = (size_t)(Dims<CH, UP>::G4 * Dims<CH, UP>::WX_LD + 2 * Dims<CH>::CELLS * Dims<CH>::H_LD) * sizeof(__half);
 
-// Layers of a stack (lstm_stack_forward_tc) run this kernel at every width, hidden 32 as CH = 1:
+// Layers of a stack (lstm_forward_tc) run this kernel at every width, hidden 32 as CH = 1:
 //   UP     the input is h^{l-1}_t of the layer below from h_in (see h_off) instead of x_seq: in training its saved state + 512
 //          (ld 1024), in inference its h-only sequence (ld 512);
 //   HSEQ   an inference layer below the top also writes h_t of every step to h_seq (h_off, ld 512) for the layer above.
@@ -1049,6 +1049,24 @@ using lstm_tc::Dims;
 
 bool lstm_tc_supported(int T, int C) { return (C == 32 || C == 96 || C == 128) && T >= 1 && T <= 256; }
 
+// Hidden 32 and 96 only: an upper layer's gate weights, 4H x (2H + 24) halves, take 22 KB and 162 KB of shared memory; at 128
+// they would take 280 KB, more than a CTA has.
+bool lstm_tc_stack_supported(int T, int C, int L) { return L >= 2 && (C == 32 || C == 96) && T >= 1 && T <= 256; }
+
+static bool lstm_tc_layers_supported(int T, int C, int L) { return L == 1 ? lstm_tc_supported(T, C) : lstm_tc_stack_supported(T, C, L); }
+
+// The one map from the hidden width C to the kernels' CH = C / 32: body(std::integral_constant<int, CH>{})
+template <class Body>
+static int with_width(int C, Body&& body) {
+  switch (C) {
+    case 32: return body(std::integral_constant<int, 1>{});
+    case 96: return body(std::integral_constant<int, 3>{});
+    case 128: return body(std::integral_constant<int, 4>{});
+  }
+  set_error("lstm: no tensor-core kernel for hidden=%d", C);
+  return 1;
+}
+
 static long long lstm_tc_tile_cells(int C) { return C == 32 ? Dims<1>::CELLS : C == 96 ? Dims<3>::CELLS : Dims<4>::CELLS; }
 
 // cells of B NN rounded up to whole tiles of the width's kernels
@@ -1101,7 +1119,10 @@ static size_t lstm_tc_slot_bytes(int C, bool up) {
   return align_up(n * image * sizeof(float), 256);
 }
 
-// workspace of the backward: the grad scale (1 KB), at the wide widths the da records, deterministic mode's slots (empty with the
+// ---------------------------------------------------------------------------------------
+// workspace layouts
+// ---------------------------------------------------------------------------------------
+// single-layer backward: the grad scale (1 KB), at the wide widths the da records, deterministic mode's slots (empty with the
 // mode off) and, for a call without a saved buffer from the forward (`rebuild`), room to re-run the (training) forward into
 struct LstmTcBwdLayout { size_t scale, da, slots, saved, total; };
 static LstmTcBwdLayout lstm_tc_bwd_layout(int B, int T, long long NN, int C, bool rebuild) {
@@ -1116,167 +1137,11 @@ static LstmTcBwdLayout lstm_tc_bwd_layout(int B, int T, long long NN, int C, boo
 }
 size_t lstm_tc_bwd_workspace_bytes(int B, int T, long long NN, int C) { return lstm_tc_bwd_layout(B, T, NN, C, true).total; }
 
-template <int CH>
-static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                            void* saved, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  using D = Dims<CH>;
-  auto kern = saved ? lstm_tc::lstm_fwd_tcw_kernel<CH, true> : lstm_tc::lstm_fwd_tcw_kernel<CH, false>;
-  constexpr size_t smem = lstm_tc::kFwdWideSmem<CH>;
-  static DynSmemAttr attr_t = {}, attr_f = {};
-  if (int e = ensure_dyn_smem(kern, (int)smem, saved ? attr_t : attr_f)) return e;
-  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
-  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
-                                                                     r.tile0, r.n, T, NN, nullptr, nullptr);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// lstm_backward_h32 and lstm_backward_tcw<CH>: the kernels of one width's backward over the tiles r, run once the grad scale and
-// the zeroed weight gradients are in place.  da_rec: the gate-gradient records of the wide walk (the hidden-32 walk keeps them on
-// chip).  f.slots: deterministic mode's flush slots (lstm_tc_slot_bytes), null for the atomic flush
-static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
-                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved,
-                             void* /*da_rec*/, DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN,
-                             cudaStream_t st) {
-  using D = Dims<1>;
-  float* slots = f.slots;
-  using K = decltype(&lstm_tc::lstm_bwd_saved_tc_kernel<false>);
-  static const K kerns[2][2][2] = {     // [RANGE][DET][DX]
-      {{lstm_tc::lstm_bwd_saved_tc_kernel<false>, lstm_tc::lstm_bwd_saved_tc_kernel<true>},
-       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true>}},
-      {{lstm_tc::lstm_bwd_saved_tc_kernel<false, false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, false, true>},
-       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true, true>}}};
-  static DynSmemAttr attrs[2][2][2] = {};
-  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, D::H).n;
-  const K kern = kerns[range][slots != nullptr][d_x != nullptr];
-  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, attrs[range][slots != nullptr][d_x != nullptr])) return e;
-  prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
-  kern<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, slots ? slots : d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells,
-      r.tile0, r.n, T, NN, f.acc);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  if (slots && f.reduce_tiles)
-    return reduce_slots(slots, lstm_grid(f.reduce_tiles, D::BWD_CTAS_PER_SM), (long long)D::G4 * D::H + 2 * D::G4, 1, 0,
-                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, D::G4, d_b, D::G4), st);
-  return 0;
-}
-
-// the wide dW pass of one layer (KI = H for an upper stack layer, else 1), then in deterministic mode the reduction of its slots
-template <int CH, bool UP>
-static int lstm_dw_pass(const float* x_seq, const void* saved, const void* da_rec, float* d_w_ih, float* d_w_hh, float* d_b, DetFlush f,
-                        const float* scale2, long long cells, TileRange r, int T, long long NN, const void* h_in, double flops, cudaStream_t st) {
-  using D = Dims<CH>;
-  constexpr int KI = UP ? D::H : 1;
-  float* slots = f.slots;
-  auto dw = slots ? lstm_tc::lstm_dw_tcw_kernel<CH, UP, true> : lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
-  constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
-  static DynSmemAttr attr_d = {}, attr_dd = {};
-  if (dw_smem)
-    if (int e = ensure_dyn_smem(dw, (int)dw_smem, slots ? attr_dd : attr_d)) return e;
-  prof_begin(PROF_LSTM_BWD, flops, st);
-  dw<<<dim3(CH, (unsigned)lstm_dw_splits<CH>(r.n, T)), lstm_tc::DW_THREADS, dw_smem, st>>>(
-      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, slots ? slots : d_w_hh, d_b, scale2, cells,
-      r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), f.acc);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  if (slots && f.reduce_tiles)
-    return reduce_slots(slots, lstm_dw_splits<CH>(f.reduce_tiles, T), (long long)D::G4 * (D::H + KI + 1), 1, 0,
-                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, (long long)D::G4 * KI, d_b, D::G4), st);
-  return 0;
-}
-
-template <int CH>
-static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
-                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, void* da_rec,
-                             DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  using D = Dims<CH>;
-  constexpr size_t smem = lstm_tc::kWalkSmem<CH>;
-  const double rc = (double)range_cells(cells, r, D::H);
-  static DynSmemAttr attr_b = {};
-  if (int e = ensure_dyn_smem(lstm_tc::lstm_bwd_walk_tcw_kernel<CH>, (int)smem, attr_b)) return e;
-  // walk: the gate recompute and dh_{t-1} (2 x 8 H (H + 1) per cell and step, as the hidden-32 count splits it) ...
-  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (D::H + 1) * rc * T, st);
-  lstm_tc::lstm_bwd_walk_tcw_kernel<CH><<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(
-      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x, static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2, cells, r.tile0,
-      r.n, T, NN, nullptr, nullptr);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  // ... and the weight gradient (8 H (H + 1) / 2 more: 12 H (H + 1) in all)
-  return lstm_dw_pass<CH, false>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, f, scale2, cells, r, T, NN, nullptr,
-                                 4.0 * D::H * (D::H + 1) * rc * T, st);
-}
-
-// the single-layer forward over the tiles r (saved: their training state, or null)
-static int lstm_forward_range(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                              void* saved, long long cells, TileRange r, int T, long long NN, int C, cudaStream_t st) {
-  using D = Dims<1>;
-  if (C == 96) return lstm_forward_tcw<3>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, r, T, NN, st);
-  if (C == 128) return lstm_forward_tcw<4>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, r, T, NN, st);
-  MPGCN_CHECK(C == D::H, "lstm forward: no tensor-core kernel for hidden=%d", C);
-  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, C).n;
-  auto kern = range ? (saved ? lstm_tc::lstm_fwd_tc_kernel<true, true> : lstm_tc::lstm_fwd_tc_kernel<false, true>)
-                    : (saved ? lstm_tc::lstm_fwd_tc_kernel<true> : lstm_tc::lstm_fwd_tc_kernel<false>);
-  prof_begin(PROF_LSTM_FWD, 8.0 * C * (C + 1) * (double)range_cells(cells, r, C) * T, st);
-  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
-                                                                  r.tile0, r.n, T, NN);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
-int lstm_last_forward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                         void* saved, int B, int T, long long NN, int C, cudaStream_t st) {
-  const long long cells = (long long)B * NN;
-  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm forward: saved buffer must be 16-byte aligned");
-  return lstm_forward_range(x_seq, w_ih, w_hh, b_ih, b_hh, hT, saved, cells, all_tiles(cells, C), T, NN, C, st);
-}
-
-int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
-                          const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
-                          int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
-  const long long cells = (long long)B * NN;
-  const LstmTcBwdLayout L = lstm_tc_bwd_layout(B, T, NN, C, saved == nullptr);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= L.total, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, L.total);
-  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm backward: saved buffer must be 16-byte aligned");
-  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
-  MPGCN_CHECK(C == 32 || C == 96 || C == 128, "lstm backward: no tensor-core kernel for hidden=%d", C);
-  uint8_t* wb = static_cast<uint8_t*>(ws);
-  float* scale2 = reinterpret_cast<float*>(wb + L.scale);
-  void* da_rec = wb + L.da;
-  float* slots = det_mode() ? reinterpret_cast<float*>(wb + L.slots) : nullptr;     // fixed-order flush instead of atomics
-  if (saved == nullptr) {          // the caller kept no forward state: rebuild it (same kernel, same bits as the training forward)
-    void* tmp = wb + L.saved;
-    if (int e = lstm_last_forward_tc(x_seq, w_ih, w_hh, b_ih, b_hh, nullptr, tmp, B, T, NN, C, st)) return e;
-    saved = tmp;
-  }
-  const int G4 = 4 * C;
-  if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
-  MPGCN_CUDA(cudaMemsetAsync(d_w_ih, 0, sizeof(float) * G4, st));
-  MPGCN_CUDA(cudaMemsetAsync(d_w_hh, 0, sizeof(float) * G4 * C, st));
-  MPGCN_CUDA(cudaMemsetAsync(d_b_ih, 0, sizeof(float) * G4, st));
-  if (C == 32 && d_x) MPGCN_CUDA(cudaMemsetAsync(d_x, 0, sizeof(float) * (size_t)cells * T, st));
-  const TileRange r = all_tiles(cells, C);
-  auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
-  if (int e = backward(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, da_rec, DetFlush{slots, false, r.n}, scale2,
-                       cells, r, T, NN, st))
-    return e;
-  return lstm_copy_bias_grad(d_b_ih, d_b_hh, G4, st);
-}
-
-// ---------------------------------------------------------------------------------------
-// stacked LSTM (L >= 2 layers): every layer on the wide kernels, hidden 32 as CH = 1
-// ---------------------------------------------------------------------------------------
-// Hidden 32 and 96 only: an upper layer's gate weights, 4H x (2H + 24) halves, take 22 KB and 162 KB of shared memory; at 128
-// they would take 280 KB, more than a CTA has.
-bool lstm_tc_stack_supported(int T, int C, int L) { return L >= 2 && (C == 32 || C == 96) && T >= 1 && T <= 256; }
-
 // training state of the stack: one lstm_tc_saved_bytes block per layer (multiples of 256 bytes)
 size_t lstm_tc_stack_saved_bytes(int B, int T, long long NN, int C, int L) { return (size_t)L * lstm_tc_saved_bytes(B, T, NN, C); }
 
-// inference forward: the h-only sequences (C halves per cell and step) that an inference layer hands to the layer above, of two
-// consecutive layers (layer l writes h[l & 1]; one sequence for L = 2)
+// stack inference forward: the h-only sequences (C halves per cell and step) that an inference layer hands to the layer above,
+// of two consecutive layers (layer l writes h[l & 1]; one sequence for L = 2)
 struct StackFwdLayout { size_t h[2], total; };
 static StackFwdLayout stack_fwd_layout(int B, int T, long long NN, int C, int L) {
   StackFwdLayout Y;
@@ -1289,7 +1154,7 @@ static StackFwdLayout stack_fwd_layout(int B, int T, long long NN, int C, int L)
 }
 size_t lstm_tc_stack_fwd_workspace_bytes(int B, int T, long long NN, int C, int L) { return stack_fwd_layout(B, T, NN, C, L).total; }
 
-// backward: the grad scale (1 KB), the fp32 gradient sequence d(h^{l-1}_t) between consecutive walks (lstm_tc::dseq_off),
+// stack backward: the grad scale (1 KB), the fp32 gradient sequence d(h^{l-1}_t) between consecutive walks (lstm_tc::dseq_off),
 // deterministic mode's slots of the dW passes (lstm_tc_slot_bytes of an upper layer, the largest; empty with the mode off) and
 // the da records of one layer (the layers run one after another).  A workspace of `every_layer` bytes keeps every layer's
 // records (layer l at da + l * da_stride) instead of reusing one region, so that they can be read back after the call.
@@ -1308,162 +1173,10 @@ static StackBwdLayout stack_bwd_layout(int B, int T, long long NN, int C, int L)
 }
 size_t lstm_tc_stack_bwd_workspace_bytes(int B, int T, long long NN, int C, int L) { return stack_bwd_layout(B, T, NN, C, L).total; }
 
-template <int CH, bool SAVE, bool UP, bool HSEQ>
-static int stack_fwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
-                           void* saved, const void* h_in, void* h_seq, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  using D = Dims<CH>;
-  auto kern = lstm_tc::lstm_fwd_tcw_kernel<CH, SAVE, UP, HSEQ>;
-  constexpr size_t smem = lstm_tc::kFwdWideSmem<CH, UP>;
-  static DynSmemAttr attr = {};
-  if (int e = ensure_dyn_smem(kern, (int)smem, attr)) return e;
-  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * ((UP ? 2 : 1) * D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
-  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
-                                                                     r.tile0, r.n, T, NN, static_cast<const __half*>(h_in),
-                                                                     static_cast<__half*>(h_seq));
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// the stack over the tiles r; training (saved != null): layer l's state at saved + l * layer_bytes
-template <int CH>
-static int stack_forward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                         const float* const* b_hh, float* hT, void* saved, size_t layer_bytes, void* ws, const StackFwdLayout& Y,
-                         long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  auto lsaved = [&](int l) { return static_cast<uint8_t*>(saved) + (size_t)l * layer_bytes; };
-  auto hbuf = [&](int l) { return static_cast<uint8_t*>(ws) + Y.h[l & 1]; };   // inference: h of layer l
-  for (int l = 0; l < L; ++l) {
-    const bool top = l == L - 1;
-    float* out = top ? hT : nullptr;
-    int e;
-    if (saved) {       // training: every layer keeps c_t | h_t; the layer above reads the h half
-      if (l == 0) e = stack_fwd_layer<CH, true, false, false>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], out, lsaved(0), nullptr, nullptr,
-                                                           cells, r, T, NN, st);
-      else e = stack_fwd_layer<CH, true, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], out, lsaved(l), lsaved(l - 1) + 1024, nullptr, cells, r, T, NN, st);
-    } else if (l == 0) {
-      e = stack_fwd_layer<CH, false, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, nullptr, nullptr, hbuf(0), cells, r, T,
-                                                  NN, st);
-    } else if (!top) {
-      e = stack_fwd_layer<CH, false, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, nullptr, hbuf(l - 1), hbuf(l),
-                                                 cells, r, T, NN, st);
-    } else {
-      e = stack_fwd_layer<CH, false, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], hT, nullptr, hbuf(l - 1), nullptr, cells,
-                                                  r, T, NN, st);
-    }
-    if (e) return e;
-  }
-  return 0;
-}
-
-template <int CH, bool UP, bool DHIN>
-static int stack_bwd_layer(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* d_hT,
-                           float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, const void* h_in, void* da_rec,
-                           float* d_seq, DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  using D = Dims<CH>;
-  const double rc = (double)range_cells(cells, r, D::H);
-  constexpr int KH = UP ? 2 * D::H : D::H;     // the input and recurrent columns of the gate GEMM
-  auto walk = lstm_tc::lstm_bwd_walk_tcw_kernel<CH, UP, DHIN>;
-  constexpr size_t smem = lstm_tc::kWalkSmem<CH, UP>;
-  static DynSmemAttr attr_w = {};
-  if (int e = ensure_dyn_smem(walk, (int)smem, attr_w)) return e;
-  // the walk and the weight gradient, counted as the single layer's are, with the gate GEMM KH + 1 deep: 8 H (KH + 1) ...
-  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (KH + 1) * rc * T, st);
-  walk<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x,
-                                                                     static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2,
-                                                                     cells, r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), d_seq);
-  prof_end(st);
-  MPGCN_CUDA(cudaGetLastError());
-  // ... and the weight gradient, 4 H (KH + 1)
-  return lstm_dw_pass<CH, UP>(x_seq, saved, da_rec, d_w_ih, d_w_hh, d_b, f, scale2, cells, r, T, NN, h_in, 4.0 * D::H * (KH + 1) * rc * T, st);
-}
-
-template <int CH>
-static int stack_backward(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                          const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b,
-                          float* d_x, const void* saved, size_t layer_bytes, uint8_t* da_rec, size_t da_stride, float* d_seq, DetFlush f,
-                          size_t slot_stride, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
-  auto lsaved = [&](int l) { return static_cast<const uint8_t*>(saved) + (size_t)l * layer_bytes; };
-  for (int l = L - 1; l >= 0; --l) {    // top-down: the walk of layer l leaves d(h^{l-1}_t) in d_seq for layer l - 1
-    const bool top = l == L - 1;
-    uint8_t* rec = da_rec + (size_t)l * da_stride;
-    // slot_stride floats apart, each layer's slots (0: the layers share one region, each reducing its own before the next)
-    const DetFlush fl = {f.slots ? f.slots + (size_t)l * slot_stride : nullptr, f.acc, f.reduce_tiles};
-    int e;
-    if (l == 0)
-      e = stack_bwd_layer<CH, false, true>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, d_w_ih[0], d_w_hh[0], d_b[0], d_x, lsaved(0),
-                                           nullptr, rec, d_seq, fl, scale2, cells, r, T, NN, st);
-    else if (top)
-      e = stack_bwd_layer<CH, true, false>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], d_hT, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                           lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, fl, scale2, cells, r, T, NN, st);
-    else
-      e = stack_bwd_layer<CH, true, true>(nullptr, w_ih[l], w_hh[l], b_ih[l], b_hh[l], nullptr, d_w_ih[l], d_w_hh[l], d_b[l], nullptr,
-                                          lsaved(l), lsaved(l - 1) + 1024, rec, d_seq, fl, scale2, cells, r, T, NN, st);
-    if (e) return e;
-  }
-  return 0;
-}
-
-int lstm_stack_forward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                          const float* const* b_hh, float* hT, void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN, int C,
-                          cudaStream_t st) {
-  MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
-  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack forward: saved buffer must be 256-byte aligned");
-  const StackFwdLayout Y = stack_fwd_layout(B, T, NN, C, L);
-  if (saved == nullptr) {      // inference: the h sequences live in the workspace
-    MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack forward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
-    MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack forward: workspace must be 256-byte aligned");
-  }
-  const long long cells = (long long)B * NN;
-  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
-  return C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, layer_bytes, ws, Y, cells, all_tiles(cells, C), T, NN, st)
-                 : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, saved, layer_bytes, ws, Y, cells, all_tiles(cells, C), T, NN, st);
-}
-
-int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
-                           float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,
-                           int C, const float* d_hT_absmax, cudaStream_t st) {
-  MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
-  const StackBwdLayout Y = stack_bwd_layout(B, T, NN, C, L);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack backward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
-  MPGCN_CHECK((reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack backward: saved buffer must be 256-byte aligned");
-  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack backward: workspace must be 256-byte aligned");
-  const long long cells = (long long)B * NN;
-  uint8_t* wb = static_cast<uint8_t*>(ws);
-  float* scale2 = reinterpret_cast<float*>(wb + Y.scale);
-  float* d_seq = reinterpret_cast<float*>(wb + Y.d_seq);
-  float* slots = det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr;     // fixed-order flush instead of atomics
-  uint8_t* da_rec = wb + Y.da;
-  const size_t da_stride = ws_bytes >= Y.every_layer ? Y.da_stride : 0;     // every layer's records, or one region
-  // one gradient scale S for the whole stack, from max|d_hT|: every walk keeps dh, dc and d_seq in units of S
-  if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
-  const int G4 = 4 * C;
-  for (int l = 0; l < L; ++l) {
-    MPGCN_CUDA(cudaMemsetAsync(d_w_ih[l], 0, sizeof(float) * G4 * (l == 0 ? 1 : C), st));
-    MPGCN_CUDA(cudaMemsetAsync(d_w_hh[l], 0, sizeof(float) * G4 * C, st));
-    MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
-  }
-  const TileRange r = all_tiles(cells, C);
-  const DetFlush f = {slots, false, r.n};
-  const size_t layer_bytes = lstm_tc_saved_bytes(B, T, NN, C);
-  const int e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, layer_bytes, da_rec,
-                                            da_stride, d_seq, f, 0, scale2, cells, r, T, NN, st)
-                        : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, layer_bytes, da_rec,
-                                            da_stride, d_seq, f, 0, scale2, cells, r, T, NN, st);
-  if (e) return e;
-  for (int l = 0; l < L; ++l)
-    if (int e2 = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e2;
-  return 0;
-}
-
-// ---------------------------------------------------------------------------------------
-// recomputing backward: the forward kept no state; it is rebuilt and walked back one chunk of tiles at a time
-// ---------------------------------------------------------------------------------------
-// Per chunk: the SAVE forward of every layer over the chunk into the chunk's state region (layer l reads layer l - 1's, as in
-// the training forward), the walks top-down, the dW passes over the chunk's records.  The kernels are those of the stored-state
-// path, so every cell sees the same state bits and the same S (one grad scale over all cells): h_T, dx and the per-cell gate
-// gradients are bitwise those of mpgcn_lstm_last_backward_saved / mpgcn_lstm_stack_backward; the weight gradients differ only
-// in fp32 summation order.  Memory: O(chunk) instead of O(B NN T C); cost: one more forward.
+// Recomputing backward: the forward kept no state; it is rebuilt and walked back one chunk of tiles at a time.  The kernels are
+// those of the stored-state path, so every cell sees the same state bits and the same S (one grad scale over all cells): h_T, dx
+// and the per-cell gate gradients are bitwise those of mpgcn_lstm_last_backward_saved / mpgcn_lstm_stack_backward; the weight
+// gradients differ only in fp32 summation order.  Memory: O(chunk) instead of O(B NN T C); cost: one more forward.
 
 // tiles of a chunk: chunk_cells rounded up to whole tiles, raised to one wave of the backward grid (one CTA per SM at every
 // width) so that no chunk leaves SMs idle, and capped at every tile
@@ -1499,23 +1212,218 @@ size_t lstm_tc_recompute_bwd_workspace_bytes(int B, int T, long long NN, int C, 
   return recompute_layout(B, T, NN, C, L, chunk_cells).total;
 }
 
-int lstm_recompute_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
-                               const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh,
-                               float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* ws, size_t ws_bytes,
-                               int B, int T, long long NN, int C, const float* d_hT_absmax, cudaStream_t st) {
-  MPGCN_CHECK(L == 1 ? lstm_tc_supported(T, C) : lstm_tc_stack_supported(T, C, L), "lstm recompute: no tensor-core kernels for L=%d, hidden=%d, T=%d",
-              L, C, T);
-  MPGCN_CHECK(chunk_cells >= 1, "lstm recompute: chunk_cells=%lld (at least 1)", chunk_cells);
-  const RecomputeLayout Y = recompute_layout(B, T, NN, C, L, chunk_cells);
-  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm recompute: workspace too small (%zu < %zu)", ws_bytes, Y.total);
-  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm recompute: workspace must be 256-byte aligned");
-  const long long cells = (long long)B * NN, all = all_tiles(cells, C).n;
-  uint8_t* wb = static_cast<uint8_t*>(ws);
-  float* scale2 = reinterpret_cast<float*>(wb + Y.scale);
-  float* d_seq = reinterpret_cast<float*>(wb + Y.d_seq);
-  float* slots = det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr;
-  void* saved = wb + Y.saved;
-  uint8_t* da_rec = wb + Y.da;
+// ---------------------------------------------------------------------------------------
+// per-layer launchers over the tiles r
+// ---------------------------------------------------------------------------------------
+// The hidden-32 single layer (saved: its training state, or null); a range of every tile runs the whole-call instance
+template <bool SAVE>
+static int lstm_forward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
+                            void* saved, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
+  using D = Dims<1>;
+  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, D::H).n;
+  auto kern = range ? lstm_tc::lstm_fwd_tc_kernel<SAVE, true> : lstm_tc::lstm_fwd_tc_kernel<SAVE>;
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, 0, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
+                                                                  r.tile0, r.n, T, NN);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Every other layer, on the wide kernels (hidden 32 in a stack as CH = 1); UP and HSEQ as in lstm_tc::lstm_fwd_tcw_kernel
+template <int CH, bool SAVE, bool UP, bool HSEQ>
+static int lstm_forward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* hT,
+                            void* saved, const void* h_in, void* h_seq, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
+  using D = Dims<CH>;
+  auto kern = lstm_tc::lstm_fwd_tcw_kernel<CH, SAVE, UP, HSEQ>;
+  constexpr size_t smem = lstm_tc::kFwdWideSmem<CH, UP>;
+  static DynSmemAttr attr = {};
+  if (int e = ensure_dyn_smem(kern, (int)smem, attr)) return e;
+  prof_begin(PROF_LSTM_FWD, 8.0 * D::H * ((UP ? 2 : 1) * D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::FWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, hT, static_cast<__half*>(saved), cells,
+                                                                     r.tile0, r.n, T, NN, static_cast<const __half*>(h_in),
+                                                                     static_cast<__half*>(h_seq));
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The backward launchers run once the grad scale and the zeroed weight gradients are in place.  f.slots: deterministic mode's
+// flush slots (lstm_tc_slot_bytes), null for the atomic flush.  The hidden-32 single layer keeps its gate gradients on chip.
+static int lstm_backward_h32(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, DetFlush f,
+                             const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
+  using D = Dims<1>;
+  float* slots = f.slots;
+  using K = decltype(&lstm_tc::lstm_bwd_saved_tc_kernel<false>);
+  static const K kerns[2][2][2] = {     // [RANGE][DET][DX]
+      {{lstm_tc::lstm_bwd_saved_tc_kernel<false>, lstm_tc::lstm_bwd_saved_tc_kernel<true>},
+       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true>}},
+      {{lstm_tc::lstm_bwd_saved_tc_kernel<false, false, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, false, true>},
+       {lstm_tc::lstm_bwd_saved_tc_kernel<false, true, true>, lstm_tc::lstm_bwd_saved_tc_kernel<true, true, true>}}};
+  static DynSmemAttr attrs[2][2][2] = {};
+  const bool range = r.tile0 != 0 || r.n != all_tiles(cells, D::H).n;
+  const K kern = kerns[range][slots != nullptr][d_x != nullptr];
+  if (int e = ensure_dyn_smem(kern, (int)lstm_tc::kBwdSavedSmem, attrs[range][slots != nullptr][d_x != nullptr])) return e;
+  prof_begin(PROF_LSTM_BWD, 12.0 * D::H * (D::H + 1) * (double)range_cells(cells, r, D::H) * T, st);
+  kern<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, lstm_tc::kBwdSavedSmem, st>>>(
+      x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, slots ? slots : d_w_hh, d_b, d_x, static_cast<const __half*>(saved), scale2, cells,
+      r.tile0, r.n, T, NN, f.acc);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  if (slots && f.reduce_tiles)
+    return reduce_slots(slots, lstm_grid(f.reduce_tiles, D::BWD_CTAS_PER_SM), (long long)D::G4 * D::H + 2 * D::G4, 1, 0,
+                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, D::G4, d_b, D::G4), st);
+  return 0;
+}
+
+// Every other layer: the walk, which writes its da records to da_rec, then the dW pass over them and, in deterministic mode, the
+// reduction of its slots.  UP and DHIN as in lstm_tc::lstm_bwd_walk_tcw_kernel; KI = H for UP, else 1.
+template <int CH, bool UP, bool DHIN>
+static int lstm_backward_tcw(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                             const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b, float* d_x, const void* saved, const void* h_in,
+                             void* da_rec, float* d_seq, DetFlush f, const float* scale2, long long cells, TileRange r, int T, long long NN,
+                             cudaStream_t st) {
+  using D = Dims<CH>;
+  const double rc = (double)range_cells(cells, r, D::H);
+  constexpr int KH = UP ? 2 * D::H : D::H;     // the input and recurrent columns of the gate GEMM
+  constexpr int KI = UP ? D::H : 1;
+  auto walk = lstm_tc::lstm_bwd_walk_tcw_kernel<CH, UP, DHIN>;
+  constexpr size_t smem = lstm_tc::kWalkSmem<CH, UP>;
+  static DynSmemAttr attr_w = {};
+  if (int e = ensure_dyn_smem(walk, (int)smem, attr_w)) return e;
+  // the walk: the gate recompute and dh_{t-1}, 2 x 8 H (KH + 1) per cell and step as the hidden-32 count splits it, of which ...
+  prof_begin(PROF_LSTM_BWD, 8.0 * D::H * (KH + 1) * rc * T, st);
+  walk<<<lstm_grid(r.n, D::BWD_CTAS_PER_SM), D::THREADS, smem, st>>>(x_seq, w_ih, w_hh, b_ih, b_hh, d_hT, d_x,
+                                                                     static_cast<const __half*>(saved), static_cast<__half*>(da_rec), scale2,
+                                                                     cells, r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), d_seq);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  // ... and the weight gradient, 4 H (KH + 1) more: 12 H (KH + 1) in all
+  float* slots = f.slots;
+  auto dw = slots ? lstm_tc::lstm_dw_tcw_kernel<CH, UP, true> : lstm_tc::lstm_dw_tcw_kernel<CH, UP>;
+  constexpr size_t dw_smem = lstm_tc::kDwSmem<CH, UP> <= 48 * 1024 ? 0 : lstm_tc::kDwSmem<CH, UP>;
+  static DynSmemAttr attr_d = {}, attr_dd = {};
+  if (dw_smem)
+    if (int e = ensure_dyn_smem(dw, (int)dw_smem, slots ? attr_dd : attr_d)) return e;
+  prof_begin(PROF_LSTM_BWD, 4.0 * D::H * (KH + 1) * rc * T, st);
+  dw<<<dim3(CH, (unsigned)lstm_dw_splits<CH>(r.n, T)), lstm_tc::DW_THREADS, dw_smem, st>>>(
+      x_seq, static_cast<const __half*>(saved), static_cast<const __half*>(da_rec), d_w_ih, slots ? slots : d_w_hh, d_b, scale2, cells,
+      r.tile0, r.n, T, NN, static_cast<const __half*>(h_in), f.acc);
+  prof_end(st);
+  MPGCN_CUDA(cudaGetLastError());
+  if (slots && f.reduce_tiles)
+    return reduce_slots(slots, lstm_dw_splits<CH>(f.reduce_tiles, T), (long long)D::G4 * (D::H + KI + 1), 1, 0,
+                        slot_image(d_w_hh, (long long)D::G4 * D::H, d_w_ih, (long long)D::G4 * KI, d_b, D::G4), st);
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
+// the layers of a call over the tiles r (DESIGN.md section 6.4)
+// ---------------------------------------------------------------------------------------
+// The hidden-32 single layer runs the hidden-32 kernels; every other layer l of L runs the wide kernels with UP = l > 0 and, in
+// the forward, HSEQ = !SAVE && l < L - 1, in the backward DHIN = l < L - 1.  There are no stacks at hidden 128 (CH = 4): the
+// entries refuse them (lstm_tc_stack_supported), and no UP, HSEQ or DHIN instance exists there.
+//
+// Forward, layers bottom-up; only the top layer writes h_T.  Training (SAVE): layer l keeps its state at saved + l * stride, and
+// the layer above reads its h half (+ 1024, see lstm_tc::h_off).  Inference: a layer below the top hands its h sequence to the
+// layer above in hseq[l & 1].
+template <int CH, bool SAVE>
+static int forward_layers(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                          const float* const* b_hh, float* hT, uint8_t* saved, size_t stride, uint8_t* const* hseq, long long cells,
+                          TileRange r, int T, long long NN, cudaStream_t st) {
+  for (int l = 0; l < L; ++l) {
+    uint8_t* own = SAVE ? saved + (size_t)l * stride : nullptr;
+    const uint8_t* h_in = l == 0 ? nullptr : SAVE ? own - stride + 1024 : hseq[(l - 1) & 1];
+    auto layer = [&](auto up, auto hseq_out) {
+      return lstm_forward_tcw<CH, SAVE, decltype(up)::value, decltype(hseq_out)::value>(
+          up ? nullptr : x_seq, w_ih[l], w_hh[l], b_ih[l], b_hh[l], l == L - 1 ? hT : nullptr, own, h_in, hseq_out ? hseq[l & 1] : nullptr,
+          cells, r, T, NN, st);
+    };
+    int e = 0;
+    if (L == 1) {
+      if constexpr (CH == 1) e = lstm_forward_h32<SAVE>(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], hT, saved, cells, r, T, NN, st);
+      else e = layer(std::false_type{}, std::false_type{});
+    } else if constexpr (CH != 4) {
+      if (l == 0) e = layer(std::false_type{}, std::bool_constant<!SAVE>{});
+      else if (l < L - 1) e = layer(std::true_type{}, std::bool_constant<!SAVE>{});
+      else e = layer(std::true_type{}, std::false_type{});
+    }
+    if (e) return e;
+  }
+  return 0;
+}
+
+// Backward, layers top-down: the walk of layer l leaves d(h^{l-1}_t) in d_seq for layer l - 1.  Layer l's state is at saved + l *
+// stride, its da records at da + l * da_stride and its deterministic slots at f.slots + l * slot_stride floats (a stride of 0:
+// the layers share one region, each reducing its slots before the next).
+template <int CH>
+static int backward_layers(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b,
+                           float* d_x, const uint8_t* saved, size_t stride, uint8_t* da, size_t da_stride, float* d_seq, DetFlush f,
+                           size_t slot_stride, const float* scale2, long long cells, TileRange r, int T, long long NN, cudaStream_t st) {
+  for (int l = L - 1; l >= 0; --l) {
+    const uint8_t* own = saved + (size_t)l * stride;
+    const DetFlush fl = {f.slots ? f.slots + (size_t)l * slot_stride : nullptr, f.acc, f.reduce_tiles};
+    auto layer = [&](auto up, auto dhin) {
+      return lstm_backward_tcw<CH, decltype(up)::value, decltype(dhin)::value>(
+          up ? nullptr : x_seq, w_ih[l], w_hh[l], b_ih[l], b_hh[l], dhin ? nullptr : d_hT, d_w_ih[l], d_w_hh[l], d_b[l], up ? nullptr : d_x,
+          own, up ? own - stride + 1024 : nullptr, da + (size_t)l * da_stride, d_seq, fl, scale2, cells, r, T, NN, st);
+    };
+    int e = 0;
+    if (L == 1) {
+      if constexpr (CH == 1)
+        e = lstm_backward_h32(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], d_hT, d_w_ih[0], d_w_hh[0], d_b[0], d_x, saved, fl, scale2, cells,
+                              r, T, NN, st);
+      else e = layer(std::false_type{}, std::false_type{});
+    } else if constexpr (CH != 4) {
+      if (l == 0) e = layer(std::false_type{}, std::true_type{});
+      else if (l < L - 1) e = layer(std::true_type{}, std::true_type{});
+      else e = layer(std::true_type{}, std::false_type{});
+    }
+    if (e) return e;
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
+// drivers and entries
+// ---------------------------------------------------------------------------------------
+int lstm_forward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                    const float* const* b_hh, float* hT, void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN, int C,
+                    cudaStream_t st) {
+  MPGCN_CHECK(lstm_tc_layers_supported(T, C, L), "lstm: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
+  const int align = L == 1 ? 16 : 256;     // a stack's layers start at multiples of lstm_tc_saved_bytes
+  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & (align - 1)) == 0, "lstm forward: saved buffer must be %d-byte aligned",
+              align);
+  uint8_t* hseq[2] = {nullptr, nullptr};
+  if (saved == nullptr && L >= 2) {      // stack inference: the h sequences live in the workspace
+    const StackFwdLayout Y = stack_fwd_layout(B, T, NN, C, L);
+    MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm forward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
+    MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm forward: workspace must be 256-byte aligned");
+    hseq[0] = static_cast<uint8_t*>(ws) + Y.h[0];
+    hseq[1] = static_cast<uint8_t*>(ws) + Y.h[1];
+  }
+  const long long cells = (long long)B * NN;
+  const size_t stride = lstm_tc_saved_bytes(B, T, NN, C);
+  uint8_t* s = static_cast<uint8_t*>(saved);
+  return with_width(C, [&](auto ch) {
+    constexpr int CH = decltype(ch)::value;
+    const TileRange r = all_tiles(cells, C);
+    return s ? forward_layers<CH, true>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, s, stride, hseq, cells, r, T, NN, st)
+             : forward_layers<CH, false>(x_seq, L, w_ih, w_hh, b_ih, b_hh, hT, s, stride, hseq, cells, r, T, NN, st);
+  });
+}
+
+// The backward of L layers: one grad scale S from max|d_hT| (every walk keeps dh, dc and d_seq in units of S), the zeroed weight
+// gradients, then per range of chunk_tiles tiles the layers top-down, and the bias gradients.  The state is either `saved` (the
+// training forward's, layer l at saved + l * stride; chunk_tiles is every tile) or, with saved == null, rebuilt per chunk into
+// `rebuild` by the training forward (same kernels, same bits).  Workspace regions as in backward_layers.
+static int lstm_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                            const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
+                            float* const* d_b_hh, float* d_x, const void* saved, void* rebuild, size_t stride, long long chunk_tiles,
+                            float* scale2, float* d_seq, float* slots, size_t slot_stride, uint8_t* da, size_t da_stride, long long cells,
+                            int T, long long NN, int C, const float* d_hT_absmax, cudaStream_t st) {
   if (int e = grad_scale_prepare(d_hT, (size_t)cells * C, scale2, d_hT_absmax, st)) return e;
   const int G4 = 4 * C;
   for (int l = 0; l < L; ++l) {
@@ -1523,34 +1431,76 @@ int lstm_recompute_backward_tc(const float* x_seq, int L, const float* const* w_
     MPGCN_CUDA(cudaMemsetAsync(d_w_hh[l], 0, sizeof(float) * G4 * C, st));
     MPGCN_CUDA(cudaMemsetAsync(d_b_ih[l], 0, sizeof(float) * G4, st));
   }
-  // every launch below writes d_x of its chunk's cells in full, so d_x needs no clearing
-  for (long long t0 = 0; t0 < all; t0 += Y.chunk_tiles) {
-    const TileRange r = {t0, Y.chunk_tiles < all - t0 ? Y.chunk_tiles : all - t0};
-    const DetFlush f = {slots, t0 > 0, t0 + r.n == all ? Y.chunk_tiles : 0};
-    int e;
-    if (L == 1) {
-      e = lstm_forward_range(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], nullptr, saved, cells, r, T, NN, C, st);
-      if (e == 0) {
-        auto backward = C == 32 ? lstm_backward_h32 : C == 96 ? lstm_backward_tcw<3> : lstm_backward_tcw<4>;
-        e = backward(x_seq, w_ih[0], w_hh[0], b_ih[0], b_hh[0], d_hT, d_w_ih[0], d_w_hh[0], d_b_ih[0], d_x, saved, da_rec, f, scale2, cells,
-                     r, T, NN, st);
-      }
-    } else {
-      const StackFwdLayout none = {};      // (a training forward keeps no h sequence in a workspace)
-      const size_t slot_floats = Y.slot_stride / sizeof(float);
-      e = C == 32 ? stack_forward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, nullptr, saved, Y.saved_stride, nullptr, none, cells, r, T, NN, st)
-                  : stack_forward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, nullptr, saved, Y.saved_stride, nullptr, none, cells, r, T, NN, st);
-      if (e == 0)
-        e = C == 32 ? stack_backward<1>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, Y.saved_stride, da_rec, 0,
-                                        d_seq, f, slot_floats, scale2, cells, r, T, NN, st)
-                    : stack_backward<3>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x, saved, Y.saved_stride, da_rec, 0,
-                                        d_seq, f, slot_floats, scale2, cells, r, T, NN, st);
-    }
+  // every walk writes d_x of its range's cells in full, so d_x needs no clearing
+  const long long all = all_tiles(cells, C).n;
+  for (long long t0 = 0; t0 < all; t0 += chunk_tiles) {
+    const TileRange r = {t0, chunk_tiles < all - t0 ? chunk_tiles : all - t0};
+    const DetFlush f = {slots, t0 > 0, t0 + r.n == all ? chunk_tiles : 0};
+    const int e = with_width(C, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      uint8_t* state = static_cast<uint8_t*>(rebuild);
+      if (rebuild)
+        if (int e = forward_layers<CH, true>(x_seq, L, w_ih, w_hh, b_ih, b_hh, nullptr, state, stride, nullptr, cells, r, T, NN, st)) return e;
+      return backward_layers<CH>(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_x,
+                                 rebuild ? state : static_cast<const uint8_t*>(saved), stride, da, da_stride, d_seq, f, slot_stride, scale2,
+                                 cells, r, T, NN, st);
+    });
     if (e) return e;
   }
   for (int l = 0; l < L; ++l)
     if (int e = lstm_copy_bias_grad(d_b_ih[l], d_b_hh[l], G4, st)) return e;
   return 0;
+}
+
+int lstm_last_backward_tc(const float* x_seq, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                          const float* d_hT, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh, float* d_x, const void* saved,
+                          int B, int T, long long NN, int C, void* ws, size_t ws_bytes, const float* d_hT_absmax, cudaStream_t st) {
+  const LstmTcBwdLayout Y = lstm_tc_bwd_layout(B, T, NN, C, saved == nullptr);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm backward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
+  MPGCN_CHECK(saved == nullptr || (reinterpret_cast<uintptr_t>(saved) & 15) == 0, "lstm backward: saved buffer must be 16-byte aligned");
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm backward: workspace must be 256-byte aligned");
+  MPGCN_CHECK(lstm_tc_supported(T, C), "lstm backward: no tensor-core kernel for hidden=%d, T=%d", C, T);
+  const long long cells = (long long)B * NN;
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  // without a saved buffer the caller kept no forward state: it is rebuilt as one chunk of every tile
+  return lstm_backward_tc(x_seq, 1, &w_ih, &w_hh, &b_ih, &b_hh, d_hT, &d_w_ih, &d_w_hh, &d_b_ih, &d_b_hh, d_x, saved,
+                          saved ? nullptr : wb + Y.saved, 0, all_tiles(cells, C).n, reinterpret_cast<float*>(wb + Y.scale), nullptr,
+                          det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr, 0, wb + Y.da, 0, cells, T, NN, C, d_hT_absmax, st);
+}
+
+int lstm_stack_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                           const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh, float* const* d_b_ih,
+                           float* const* d_b_hh, float* d_x, const void* saved, void* ws, size_t ws_bytes, int B, int T, long long NN,
+                           int C, const float* d_hT_absmax, cudaStream_t st) {
+  MPGCN_CHECK(lstm_tc_stack_supported(T, C, L), "lstm stack: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
+  const StackBwdLayout Y = stack_bwd_layout(B, T, NN, C, L);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm stack backward: workspace too small (%zu < %zu)", ws_bytes, Y.total);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(saved) & 255) == 0, "lstm stack backward: saved buffer must be 256-byte aligned");
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm stack backward: workspace must be 256-byte aligned");
+  const long long cells = (long long)B * NN;
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  const size_t da_stride = ws_bytes >= Y.every_layer ? Y.da_stride : 0;     // every layer's records, or one region
+  return lstm_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, saved, nullptr,
+                          lstm_tc_saved_bytes(B, T, NN, C), all_tiles(cells, C).n, reinterpret_cast<float*>(wb + Y.scale),
+                          reinterpret_cast<float*>(wb + Y.d_seq), det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr, 0,
+                          wb + Y.da, da_stride, cells, T, NN, C, d_hT_absmax, st);
+}
+
+int lstm_recompute_backward_tc(const float* x_seq, int L, const float* const* w_ih, const float* const* w_hh, const float* const* b_ih,
+                               const float* const* b_hh, const float* d_hT, float* const* d_w_ih, float* const* d_w_hh,
+                               float* const* d_b_ih, float* const* d_b_hh, float* d_x, long long chunk_cells, void* ws, size_t ws_bytes,
+                               int B, int T, long long NN, int C, const float* d_hT_absmax, cudaStream_t st) {
+  MPGCN_CHECK(lstm_tc_layers_supported(T, C, L), "lstm recompute: no tensor-core kernels for L=%d, hidden=%d, T=%d", L, C, T);
+  MPGCN_CHECK(chunk_cells >= 1, "lstm recompute: chunk_cells=%lld (at least 1)", chunk_cells);
+  const RecomputeLayout Y = recompute_layout(B, T, NN, C, L, chunk_cells);
+  MPGCN_CHECK(ws != nullptr && ws_bytes >= Y.total, "lstm recompute: workspace too small (%zu < %zu)", ws_bytes, Y.total);
+  MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "lstm recompute: workspace must be 256-byte aligned");
+  uint8_t* wb = static_cast<uint8_t*>(ws);
+  return lstm_backward_tc(x_seq, L, w_ih, w_hh, b_ih, b_hh, d_hT, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_x, nullptr, wb + Y.saved,
+                          Y.saved_stride, Y.chunk_tiles, reinterpret_cast<float*>(wb + Y.scale),
+                          L >= 2 ? reinterpret_cast<float*>(wb + Y.d_seq) : nullptr,
+                          det_mode() ? reinterpret_cast<float*>(wb + Y.slots) : nullptr, Y.slot_stride / sizeof(float), wb + Y.da, 0,
+                          (long long)B * NN, T, NN, C, d_hT_absmax, st);
 }
 
 }  // namespace mpgcn
