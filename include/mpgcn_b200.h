@@ -16,7 +16,11 @@
  *     (thread-local).  Nothing ever aborts the process;
  *   - `precision`: 0 = exact fp32 CUDA-core kernels; 1 = fp16-operand / fp32-accumulate
  *     wgmma tensor-core engine (requires C and H to be multiples of 32, H <= 1024, C != H allowed;
- *     any number of supports K);
+ *     any number of supports K); 2 = "bf16x3", the same engine at fp32-class accuracy: each operand a
+ *     pair hi = bf16(a), lo = bf16(a - hi), each product hi*hi + hi*lo + lo*hi accumulated in fp32
+ *     (the shapes of precision 1; whole layers of the BDGCN forward / backward only: the layer parts,
+ *     mpgcn_bdgcn_backward_supports and non-NULL x_f16 / out_f16 / d_pre_f16 extras refuse it
+ *     before any CUDA call, and their size queries return 0; the LSTM and head calls do not take it);
  *   - tensors must be 16-byte aligned; the outputs of the precision-1 layer (`out`, `dX`, `out_f16`) 32-byte aligned
  *     (256-bit stores).  Allocator-returned buffers always are;
  *   - `workspace` is caller-owned scratch of at least the size the matching *_workspace_bytes
@@ -35,7 +39,9 @@ extern "C" {
 #define MPGCN_B200_ABI_VERSION 4   /* 2: extras struct, prepared supports, LSTM training pair, dg_absmax, dyn graphs;
                                       3: layer parts (origin-row / support shards), bias_act, relu_backward, region tags;
                                       4: peer push removed: mpgcn_bdgcn_part loses peer_g / peer_rank / peer_out,
-                                         mpgcn_rows_reduce_bias_act loses part_rows */
+                                         mpgcn_rows_reduce_bias_act loses part_rows.
+                                      Precision 2 (bf16x3) and mpgcn_bdgcn_prepare_supports_ex / _supports_prepared_bytes_ex are
+                                      additions to version 4: every version-4 call keeps its meaning */
 
 #if defined(__GNUC__)
 #define MPGCN_API __attribute__((visibility("default")))
@@ -86,7 +92,8 @@ MPGCN_API int mpgcn_bdgcn_backward(const float* d_out, const float* out, const f
                          const void* saved, float* dX, float* dW, float* db, void* workspace, size_t workspace_bytes, int B, int N,
                          int K, int C, int H, int precision, void* stream);
 
-/* Optional side inputs / outputs of the tensor-core layer (precision 1; ignored by precision 0).  They carry what a caller that
+/* Optional side inputs / outputs of the tensor-core layer (precision 1; ignored by precision 0; precision 2 takes the prepared
+ * supports of mpgcn_bdgcn_prepare_supports_ex and the gradient-magnitude hand-over, and refuses the fp16 copies).  They carry what a caller that
  * chains layers already has, so that the library does not redo it; every field is nullable and results do not depend on them:
  *   go_prepared, gd_prepared   supports converted once by mpgcn_bdgcn_prepare_supports (the same G_o / G_d serve every layer of a
  *                              branch, forward and backward -- "each support staged once and reused");
@@ -110,6 +117,11 @@ typedef struct mpgcn_bdgcn_extras {
 /* planes = (dynamic ? B : 1) * K support matrices [N,N] -> fp16 padded copy + diagonal remainders (256-byte aligned buffer) */
 MPGCN_API size_t mpgcn_bdgcn_supports_prepared_bytes(long long planes, int N);
 MPGCN_API int mpgcn_bdgcn_prepare_supports(const float* G, void* prepared, size_t prepared_bytes, long long planes, int N, void* stream);
+/* the same for a given layer precision: 1 as above, 2 the bf16x3 pair of the supports (what go_prepared / gd_prepared hold in a
+ * precision-2 call); the size query returns 0 for any other precision */
+MPGCN_API size_t mpgcn_bdgcn_supports_prepared_bytes_ex(long long planes, int N, int precision);
+MPGCN_API int mpgcn_bdgcn_prepare_supports_ex(const float* G, void* prepared, size_t prepared_bytes, long long planes, int N, int precision,
+                                              void* stream);
 /* mpgcn_bdgcn_forward / mpgcn_bdgcn_backward with the optional extras (extras == NULL: identical to the plain calls) */
 MPGCN_API int mpgcn_bdgcn_forward_x(const float* X, const float* G_o, const float* G_d, int dynamic, const float* W, const float* bias, int act,
                           float* out, void* saved, void* workspace, size_t workspace_bytes, int B, int N, int K, int C, int H,

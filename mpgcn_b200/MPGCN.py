@@ -40,7 +40,7 @@ class BDGCN(nn.Module):
         self.hidden_dim = hidden_dim
         self.use_bias = use_bias
         self.activation = activation() if activation is not None else None     # a class, as in the reference (MPGCN.py:13)
-        self.precision = None          # None -> ops.default_precision(); or "auto" / "fp16" / "fp32"
+        self.precision = None          # None -> ops.default_precision(); or "auto" / "fp16" / "bf16x3" / "fp32"
         self.support_grad = False      # True: a G that requires grad gets dL/dG (opt-in: it doubles the layer's N^3 backward work)
         self.init_params()
 
@@ -102,7 +102,7 @@ class MPGCN(nn.Module):
         self.lstm_hidden_dim = lstm_hidden_dim
         self.lstm_num_layers = lstm_num_layers
         self.gcn_num_layers = gcn_num_layers
-        self.lstm_precision = None      # None -> ops.default_precision(); or "auto" / "fp16" / "fp32"
+        self.lstm_precision = None      # None -> ops.default_precision(); or "auto" / "fp16" / "fp32" ("bf16x3" reads as "auto")
         # True (or a number of cells per chunk): the tensor-core LSTM keeps no training state in the forward and its backward
         # rebuilds it a chunk at a time (ops.lstm_last), for models whose state does not fit; None -> off
         self.lstm_recompute = None

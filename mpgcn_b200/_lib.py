@@ -17,6 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 
 PREC_FP32 = 0      # exact fp32 CUDA-core kernels
 PREC_FP16_TC = 1   # fp16 operands / fp32 accumulate on tensor cores (wgmma / mma.sync)
+PREC_BF16X3 = 2    # BDGCN layers only: bf16 hi / lo operand pairs, three products per contraction, fp32 accumulate (wgmma)
 
 _lib = None
 
@@ -45,6 +46,9 @@ _SIGS = {
     "mpgcn_debug_tc_workspace_offset": (ctypes.c_longlong, [ctypes.c_int] * 5),
     "mpgcn_bdgcn_supports_prepared_bytes": (ctypes.c_size_t, [ctypes.c_longlong, ctypes.c_int]),
     "mpgcn_bdgcn_prepare_supports": (ctypes.c_int, [_c_f, _c_f, ctypes.c_size_t, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
+    "mpgcn_bdgcn_supports_prepared_bytes_ex": (ctypes.c_size_t, [ctypes.c_longlong, ctypes.c_int, ctypes.c_int]),
+    "mpgcn_bdgcn_prepare_supports_ex": (ctypes.c_int, [_c_f, _c_f, ctypes.c_size_t, ctypes.c_longlong, ctypes.c_int, ctypes.c_int,
+                                                       ctypes.c_void_p]),
     "mpgcn_bdgcn_forward_x": (ctypes.c_int, [_c_f, _c_f, _c_f, ctypes.c_int, _c_f, _c_f, ctypes.c_int, _c_f, _c_f, _c_f, ctypes.c_size_t] +
                               [ctypes.c_int] * 6 + [ctypes.c_void_p, ctypes.c_void_p]),
     "mpgcn_bdgcn_backward_x": (ctypes.c_int, [_c_f, _c_f, _c_f, _c_f, ctypes.c_int, _c_f, ctypes.c_int, _c_f, _c_f, _c_f, _c_f, _c_f,

@@ -4,10 +4,23 @@
 #include "kernels.h"
 
 namespace mpgcn {
-size_t bdgcn_saved_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_saved_bytes(s) : simt_saved_bytes(s); }
-size_t bdgcn_fwd_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_fwd_ws_bytes(s) : simt_fwd_ws_bytes(s); }
-size_t bdgcn_bwd_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_bwd_ws_bytes(s) : simt_bwd_ws_bytes(s); }
-size_t bdgcn_sgrad_workspace_bytes(const BdgcnShape& s, int precision) { return precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s); }
+// precision 2 (bf16x3) serves whole layers only: its queries are those of bdgcn_forward_tc / bdgcn_backward_tc with bf = true
+size_t bdgcn_saved_bytes(const BdgcnShape& s, int precision) {
+  if (precision == PREC_BF16X3_TC) return s.whole() ? tc_saved_bytes(s, true) : 0;
+  return precision == PREC_FP16_TC ? tc_saved_bytes(s) : simt_saved_bytes(s);
+}
+size_t bdgcn_fwd_workspace_bytes(const BdgcnShape& s, int precision) {
+  if (precision == PREC_BF16X3_TC) return s.whole() ? tc_fwd_ws_bytes(s, true) : 0;
+  return precision == PREC_FP16_TC ? tc_fwd_ws_bytes(s) : simt_fwd_ws_bytes(s);
+}
+size_t bdgcn_bwd_workspace_bytes(const BdgcnShape& s, int precision) {
+  if (precision == PREC_BF16X3_TC) return s.whole() ? tc_bwd_ws_bytes(s, true) : 0;
+  return precision == PREC_FP16_TC ? tc_bwd_ws_bytes(s) : simt_bwd_ws_bytes(s);
+}
+size_t bdgcn_sgrad_workspace_bytes(const BdgcnShape& s, int precision) {
+  if (precision == PREC_BF16X3_TC) return 0;
+  return precision == PREC_FP16_TC ? tc_sgrad_ws_bytes(s) : simt_sgrad_ws_bytes(s);
+}
 }  // namespace mpgcn
 
 using namespace mpgcn;
@@ -30,6 +43,7 @@ static int check_part(const BdgcnShape& s, int precision) {
   MPGCN_CHECK(s.B >= 1 && s.N >= 1 && s.C >= 1 && s.H >= 1, "bad BDGCN shape B=%d N=%d C=%d H=%d", s.B, s.N, s.C, s.H);
   MPGCN_CHECK(s.Ko >= 1 && s.Kd >= 1 && s.R >= 1 && s.row0 >= 0 && s.row0 + s.R <= s.N,
               "bad layer part: rows [%d, %d) of N=%d, Ko=%d, Kd=%d", s.row0, s.row0 + s.R, s.N, s.Ko, s.Kd);
+  MPGCN_CHECK(precision != PREC_BF16X3_TC, "layer parts: precision 2 (bf16x3) runs whole layers only");
   MPGCN_CHECK(precision == PREC_FP32_SIMT || precision == PREC_FP16_TC, "unknown precision %d", precision);
   if (precision == PREC_FP16_TC)
     MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024 (got C=%d H=%d Ko=%d Kd=%d)", s.C, s.H, s.Ko, s.Kd);
@@ -44,10 +58,17 @@ static double layer_flops(const BdgcnShape& s, bool backward) {
 
 static int check_shape(const BdgcnShape& s, int precision) {
   MPGCN_CHECK(s.B >= 1 && s.N >= 1 && s.K >= 1 && s.C >= 1 && s.H >= 1, "bad BDGCN shape B=%d N=%d K=%d C=%d H=%d", s.B, s.N, s.K, s.C, s.H);
-  MPGCN_CHECK(precision == PREC_FP32_SIMT || precision == PREC_FP16_TC, "unknown precision %d", precision);
+  MPGCN_CHECK(precision == PREC_FP32_SIMT || precision == PREC_FP16_TC || precision == PREC_BF16X3_TC, "unknown precision %d", precision);
   MPGCN_CHECK(s.act == 0 || s.act == 1, "unknown activation code %d", s.act);
-  if (precision == PREC_FP16_TC)
-    MPGCN_CHECK(tc_supported(s), "precision 1 (tensor cores) needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024 (got C=%d H=%d K=%d)", s.C, s.H, s.K);
+  if (precision != PREC_FP32_SIMT)
+    MPGCN_CHECK(tc_supported(s), "precision %d (tensor cores) needs C and H to be multiples of 32, from C == H == 32 up, H <= 1024 (got C=%d H=%d K=%d)", precision, s.C, s.H, s.K);
+  return 0;
+}
+
+// precision 2 takes no fp16 copies of the activations
+static int check_bf16x3_extras(const char* what, int precision, const mpgcn_bdgcn_extras* x) {
+  if (precision == PREC_BF16X3_TC && x)
+    MPGCN_CHECK(!x->x_f16 && !x->out_f16 && !x->d_pre_f16, "%s: precision 2 (bf16x3) takes no fp16 activation copies (x_f16 / out_f16 / d_pre_f16)", what);
   return 0;
 }
 
@@ -62,7 +83,7 @@ int mpgcn_get_deterministic(void) { return det_mode(); }
 int mpgcn_bdgcn_precision_supported(int B, int N, int K, int C, int H, int precision) {
   const BdgcnShape s = mk(B, N, K, C, H, 0, 0);
   if (precision == PREC_FP32_SIMT) return B >= 1 && N >= 1 && K >= 1 && C >= 1 && H >= 1;
-  if (precision == PREC_FP16_TC) return tc_supported(s) ? 1 : 0;
+  if (precision == PREC_FP16_TC || precision == PREC_BF16X3_TC) return tc_supported(s) ? 1 : 0;
   return 0;
 }
 
@@ -85,6 +106,10 @@ static BdgcnExtras to_extras(const mpgcn_bdgcn_extras* x) {
 }
 
 size_t mpgcn_bdgcn_supports_prepared_bytes(long long planes, int N) { return (planes >= 1 && N >= 1) ? bdgcn_supports_prepared_bytes(planes, N) : 0; }
+size_t mpgcn_bdgcn_supports_prepared_bytes_ex(long long planes, int N, int precision) {
+  if (precision != PREC_FP16_TC && precision != PREC_BF16X3_TC) return 0;
+  return (planes >= 1 && N >= 1) ? bdgcn_supports_prepared_bytes(planes, N, precision == PREC_BF16X3_TC) : 0;
+}
 
 int mpgcn_bdgcn_prepare_supports(const float* G, void* prepared, size_t prepared_bytes, long long planes, int N, void* stream) {
   MPGCN_CHECK(G && prepared && planes >= 1 && N >= 1, "mpgcn_bdgcn_prepare_supports: bad argument");
@@ -93,15 +118,28 @@ int mpgcn_bdgcn_prepare_supports(const float* G, void* prepared, size_t prepared
   return bdgcn_prepare_supports(G, prepared, planes, N, static_cast<cudaStream_t>(stream));
 }
 
+int mpgcn_bdgcn_prepare_supports_ex(const float* G, void* prepared, size_t prepared_bytes, long long planes, int N, int precision, void* stream) {
+  MPGCN_CHECK(precision == PREC_FP16_TC || precision == PREC_BF16X3_TC, "mpgcn_bdgcn_prepare_supports_ex: precision %d has no prepared supports",
+              precision);
+  MPGCN_CHECK(G && prepared && planes >= 1 && N >= 1, "mpgcn_bdgcn_prepare_supports_ex: bad argument");
+  const bool bf = precision == PREC_BF16X3_TC;
+  MPGCN_CHECK(prepared_bytes >= bdgcn_supports_prepared_bytes(planes, N, bf), "mpgcn_bdgcn_prepare_supports_ex: buffer too small (%zu < %zu)",
+              prepared_bytes, bdgcn_supports_prepared_bytes(planes, N, bf));
+  return bdgcn_prepare_supports(G, prepared, planes, N, static_cast<cudaStream_t>(stream), bf);
+}
+
 int mpgcn_bdgcn_forward_x(const float* X, const float* G_o, const float* G_d, int dynamic, const float* W, const float* bias, int act,
                           float* out, void* saved, void* workspace, size_t workspace_bytes, int B, int N, int K, int C, int H,
                           int precision, const mpgcn_bdgcn_extras* extras, void* stream) {
   const BdgcnShape s = mk(B, N, K, C, H, dynamic ? 1 : 0, act);
   if (int e = check_shape(s, precision)) return e;
+  if (int e = check_bf16x3_extras("mpgcn_bdgcn_forward", precision, extras)) return e;
   MPGCN_CHECK(X && G_o && G_d && W && out && workspace, "mpgcn_bdgcn_forward: null pointer argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ProfRegion region(PROF_LAYER_FWD, layer_flops(s, false), st);
   if (precision == PREC_FP16_TC) return bdgcn_forward_tc(s, X, G_o, G_d, W, bias, out, saved, workspace, workspace_bytes, to_extras(extras), st);
+  if (precision == PREC_BF16X3_TC)
+    return bdgcn_forward_tc(s, X, G_o, G_d, W, bias, out, saved, workspace, workspace_bytes, to_extras(extras), st, true);
   return bdgcn_forward_simt(s, X, G_o, G_d, W, bias, out, saved, workspace, workspace_bytes, st);      // exact path: extras unused
 }
 
@@ -117,12 +155,14 @@ int mpgcn_bdgcn_backward_x(const float* d_out, const float* out, const float* G_
                            int K, int C, int H, int precision, const mpgcn_bdgcn_extras* extras, void* stream) {
   const BdgcnShape s = mk(B, N, K, C, H, dynamic ? 1 : 0, act);
   if (int e = check_shape(s, precision)) return e;
+  if (int e = check_bf16x3_extras("mpgcn_bdgcn_backward", precision, extras)) return e;
   const bool have_out16 = extras && extras->out_f16 && precision == PREC_FP16_TC;
   MPGCN_CHECK(d_out && (out || have_out16) && G_o && G_d && W && saved && dW && workspace, "mpgcn_bdgcn_backward: null pointer argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ProfRegion region(PROF_LAYER_BWD, layer_flops(s, true), st);
-  if (precision == PREC_FP16_TC)
-    return bdgcn_backward_tc(s, d_out, out, G_o, G_d, W, saved, dX, dW, db, workspace, workspace_bytes, to_extras(extras), st);
+  if (precision == PREC_FP16_TC || precision == PREC_BF16X3_TC)
+    return bdgcn_backward_tc(s, d_out, out, G_o, G_d, W, saved, dX, dW, db, workspace, workspace_bytes, to_extras(extras), st,
+                             precision == PREC_BF16X3_TC);
   if (extras && extras->dX_absmax) MPGCN_CUDA(cudaMemsetAsync(extras->dX_absmax, 0, sizeof(float), st));      // "unknown"
   return bdgcn_backward_simt(s, d_out, out, G_o, G_d, W, saved, dX, dW, db, workspace, workspace_bytes, st);
 }
@@ -130,7 +170,7 @@ int mpgcn_bdgcn_backward_x(const float* d_out, const float* out, const float* G_
 size_t mpgcn_bdgcn_support_grad_workspace_bytes(int B, int N, int K, int C, int H, int dynamic, int precision) {
   const BdgcnShape s = mk(B, N, K, C, H, dynamic, 0);
   if (check_shape(s, precision)) return 0;
-  return bdgcn_sgrad_workspace_bytes(s, precision);
+  return bdgcn_sgrad_workspace_bytes(s, precision);      // 0 for precision 2: no support gradient
 }
 
 int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const float* G_o, const float* G_d, int dynamic, const float* W, int act,
@@ -139,6 +179,7 @@ int mpgcn_bdgcn_backward_supports(const float* d_out, const float* out, const fl
                                   float* dG_d, void* stream) {
   const BdgcnShape s = mk(B, N, K, C, H, dynamic ? 1 : 0, act);
   if (int e = check_shape(s, precision)) return e;
+  MPGCN_CHECK(precision != PREC_BF16X3_TC, "mpgcn_bdgcn_backward_supports: precision 2 (bf16x3) has no support gradient");
   const bool have_out16 = extras && extras->out_f16 && precision == PREC_FP16_TC;
   MPGCN_CHECK(d_out && (out || have_out16) && X && G_o && G_d && W && saved && dW && workspace,
               "mpgcn_bdgcn_backward_supports: null pointer argument");

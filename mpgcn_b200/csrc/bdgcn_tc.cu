@@ -1,4 +1,5 @@
-// BDGCN layer on the wgmma contraction engine (precision 1: fp16 operands, fp32 accumulate).
+// BDGCN layer on the wgmma contraction engine (precision 1: fp16 operands, fp32 accumulate; precision 2, bf16x3: every operand a
+// pair of bf16 planes hi = bf16(a), lo = bf16(a - hi), each product hi*hi + hi*lo + lo*hi, fp32 accumulate).
 //
 // Same factored algebra as bdgcn_simt.cu (reference: BDGCN.forward of MPGCN.py; factoring:
 // SURVEY.md section 7.1); each contraction is one launch of tc::contract_kernel with operands
@@ -25,6 +26,11 @@
 // The N^3 contractions act on each channel on its own, so a chunk is a 32-channel layer to them; the chunk planes are laid out
 // so that the per-chunk launch addresses them through a base offset and strides (plane index (b*K + d)*cC + lc of Z16 / Y16
 // and (b*Ko + o)*cH + hc of V16 are affine in the launch's z = b*K + d; U16 keeps FWD_B's flat (o, n) contraction per chunk).
+// bf16x3 (DESIGN.md section 3): each 16-bit tensor above (X16, G16, Z16, U16, dP16, V16, Y16, W16 / Wq16) holds bf16 instead and is
+// followed by its lo plane, a copy of its layout right behind it, so the lo plane of TMA plane z is plane z + (the tensor's plane
+// count): the engine runs each contraction as three passes over k (two for the mixes, whose resident W pair already is the
+// b_res_reps = 2 halves) and the epilogues write the 16-bit results as pairs.  No diagonal-remainder correction (a pair carries
+// 16 significant bits), no support gradients, no layer parts.
 #include "kernels.h"
 #include "tc_engine.cuh"
 
@@ -52,6 +58,18 @@ void init_params(GemmParams& p) {
   p.bm = omap(1, 1, 0, 0, 0);
   p.kb_per_slice = 1;
   p.ep.alpha = 1.f;
+}
+
+// one contraction in the precision of the call: fp16, or bf16x3 in `passes` passes of p.kb_total k-blocks over plane pairs whose lo
+// planes lie a_plane_z / b_plane_z TMA z coordinates after the hi ones (tc_engine.cuh, GemmParams::kb_pass)
+int launch(bool bf, int ak, int bk, GemmParams& p, int passes, int a_plane_z, int b_plane_z, cudaStream_t st) {
+  if (!bf) return tc::launch_contract(ak, bk, p, st);
+  p.kb_pass = p.kb_total;
+  p.kb_total *= passes;
+  p.a_plane_z = a_plane_z;
+  p.b_plane_z = b_plane_z;
+  p.ep.corr_src = nullptr;
+  return tc::launch_contract_bf16x3(ak, bk, p, st);
 }
 
 // support stack G16 [zg*K][N rows][Np]: as A_MN128 (dims m, k-rows, z) or A_K128 (dims k, m-rows, z)
@@ -112,26 +130,28 @@ static size_t rn(const BdgcnShape& s) { return (size_t)s.R * s.N; }
 static size_t g16_elems(const BdgcnShape& s, int K) { return (size_t)(s.dynamic ? s.B : 1) * K * s.N * pad8(s.N); }
 static size_t g_planes(const BdgcnShape& s, int K) { return (size_t)(s.dynamic ? s.B : 1) * K; }
 
-size_t tc_saved_bytes(const BdgcnShape& s) { return (size_t)s.B * s.Kd * rn(s) * s.C * sizeof(__half); }
+// a bf16x3 pair is two planes of 16-bit elements
+size_t tc_saved_bytes(const BdgcnShape& s, bool bf) { return (size_t)(bf ? 2 : 1) * s.B * s.Kd * rn(s) * s.C * sizeof(__half); }
 
 // workspace layouts (byte offsets); also served to tests by mpgcn_debug_tc_workspace_offset()
 struct FwdLayout { size_t x16, gd16, go16, w16, u16, z16, dd, dgo, dgo_masked, total; };
-static FwdLayout fwd_layout(const BdgcnShape& s) {
+static FwdLayout fwd_layout(const BdgcnShape& s, bool bf) {
   FwdLayout L;
   size_t off = 0;
-  L.x16 = take(off, (size_t)s.B * rn(s) * s.C * 2, 1024);
-  L.gd16 = take(off, g16_elems(s, s.Kd) * 2, 1024);
-  L.go16 = take(off, g16_elems(s, s.Ko) * 2, 1024);
+  const size_t pl = bf ? 2 : 1;                          // bf16x3: hi and lo planes
+  L.x16 = take(off, pl * s.B * rn(s) * s.C * 2, 1024);
+  L.gd16 = take(off, pl * g16_elems(s, s.Kd) * 2, 1024);
+  L.go16 = take(off, pl * g16_elems(s, s.Ko) * 2, 1024);
   L.w16 = take(off, (size_t)2 * s.Ko * s.Kd * s.C * s.H * 2, 1024);    // [hi | lo]
-  L.u16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2, 1024);
+  L.u16 = take(off, pl * s.B * s.Ko * rn(s) * s.H * 2, 1024);
   L.dd = take(off, g_planes(s, s.Kd) * s.N * 4, 1024);   // support-diagonal fp16 remainders (destination / origin)
   L.dgo = take(off, g_planes(s, s.Ko) * s.N * 4, 1024);
   L.dgo_masked = take(off, g_planes(s, s.Ko) * s.N * 4, 1024);   // origin remainders restricted to the row slab
-  L.z16 = take(off, tc_saved_bytes(s), 1024);            // used only when the caller passes no `saved` buffer
+  L.z16 = take(off, tc_saved_bytes(s, bf), 1024);        // used only when the caller passes no `saved` buffer
   L.total = align_up(off, 1024);
   return L;
 }
-size_t tc_fwd_ws_bytes(const BdgcnShape& s) { return fwd_layout(s).total; }
+size_t tc_fwd_ws_bytes(const BdgcnShape& s, bool bf) { return fwd_layout(s, bf).total; }
 // BWD_DW: rows are the Kd*cC chunks of Z16, 4 per m-tile; columns are the Ko*cH chunks of V16, all in one tile up to 8,
 // else ceil(n / 8) column tiles of dw_chunks(n) chunks each (the last one partly past n: TMA zero-fills those chunks and the
 // epilogue skips them)
@@ -139,9 +159,9 @@ static int dw_row_chunks(const BdgcnShape& s) { return s.Kd * (s.C / 32); }
 static int dw_col_chunks(const BdgcnShape& s) { return s.Ko * (s.H / 32); }
 static int dw_col_tiles(int n) { return ceil_div(n, 8); }
 static int dw_chunks(int n) { return ceil_div(n, dw_col_tiles(n)); }
-static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total) {
+static int dw_slices(const BdgcnShape& s, int* kb_per_slice, int* kb_total, int passes = 1) {
   const int kbps = ceil_div((long long)rn(s), 64);
-  const int total = s.B * kbps;
+  const int total = s.B * kbps * passes;
   const int tiles = ceil_div(dw_row_chunks(s), 4) * dw_col_tiles(dw_col_chunks(s));     // tiles per slice
   int want = device_sm_count() / tiles;
   if (want < 1) want = 1;
@@ -163,17 +183,18 @@ static int dg_max_slices(const BdgcnShape& s) {
 // deterministic mode's bias-gradient slots (relu_bwd_prep), empty with the mode off; dW and dG already reduce their split-K
 // partials in a fixed order.
 struct BwdLayout { size_t dp16, gd16, go16, v16, y16, wq16, partials, scale, x16, u16, w16, dg_partials, db_slots, total; };
-static BwdLayout bwd_layout(const BdgcnShape& s, bool sgrad) {
+static BwdLayout bwd_layout(const BdgcnShape& s, bool sgrad, bool bf = false) {
   BwdLayout L{};
   size_t off = 0;
-  L.dp16 = take(off, (size_t)s.B * s.N * s.N * s.H * 2, 1024);       // dPre: every origin row m, always
-  L.gd16 = take(off, g16_elems(s, s.Kd) * 2, 1024);
-  L.go16 = take(off, g16_elems(s, s.Ko) * 2, 1024);
-  L.v16 = take(off, (size_t)s.B * s.Ko * rn(s) * s.H * 2, 1024);
-  L.y16 = take(off, (size_t)s.B * s.Kd * rn(s) * s.C * 2, 1024);
-  L.wq16 = take(off, (size_t)s.Ko * s.Kd * s.C * s.H * 2, 1024);
+  const size_t pl = bf ? 2 : 1;                                      // bf16x3: hi and lo planes (Wq: both halves)
+  L.dp16 = take(off, pl * s.B * s.N * s.N * s.H * 2, 1024);          // dPre: every origin row m, always
+  L.gd16 = take(off, pl * g16_elems(s, s.Kd) * 2, 1024);
+  L.go16 = take(off, pl * g16_elems(s, s.Ko) * 2, 1024);
+  L.v16 = take(off, pl * s.B * s.Ko * rn(s) * s.H * 2, 1024);
+  L.y16 = take(off, pl * s.B * s.Kd * rn(s) * s.C * 2, 1024);
+  L.wq16 = take(off, pl * s.Ko * s.Kd * s.C * s.H * 2, 1024);
   int per = 1, total = 1;
-  const int slices = dw_slices(s, &per, &total);
+  const int slices = dw_slices(s, &per, &total, bf ? 3 : 1);
   L.partials = take(off, (size_t)slices * ceil_div(dw_row_chunks(s), 4) * 128 * s.Ko * s.H * 4, 1024);
   L.scale = take(off, 64, 1024);
   if (sgrad) {
@@ -186,13 +207,13 @@ static BwdLayout bwd_layout(const BdgcnShape& s, bool sgrad) {
   L.total = off;     // the slots end the workspace unpadded
   return L;
 }
-size_t tc_bwd_ws_bytes(const BdgcnShape& s) { return bwd_layout(s, false).total; }
+size_t tc_bwd_ws_bytes(const BdgcnShape& s, bool bf) { return bwd_layout(s, false, bf).total; }
 size_t tc_sgrad_ws_bytes(const BdgcnShape& s) { return bwd_layout(s, true).total; }
 
 // which: 0 x16, 1 gd16, 2 go16, 3 w16, 4 u16 (forward); 10 dp16, 11 gd16, 12 go16, 13 v16, 14 y16, 15 wq16, 16 partials,
 // 17 number of dW slices (not an offset)
 long long tc_debug_offset(const BdgcnShape& s, int which) {
-  const FwdLayout F = fwd_layout(s);
+  const FwdLayout F = fwd_layout(s, false);
   const BwdLayout Bw = bwd_layout(s, false);
   int per = 1, total = 1;
   switch (which) {
@@ -221,15 +242,17 @@ long long tc_debug_offset(const BdgcnShape& s, int which) {
 // planes per sample, G_o has Ko.
 // ---------------------------------------------------------------------------------------
 // FWD_A:  Z16[b][d][lc][n][e][l] = sum_c G_d[c][e] X16[b][n][c][32 lc + l]      one launch per input chunk lc
-static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16, __half* z16, const float* delta_d, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32;
+// bf: bf16x3 pairs (every pointer then addresses the hi plane of a pair, see the head of this file)
+static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16, __half* z16, const float* delta_d, cudaStream_t st,
+                     bool bf = false) {
+  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32, pl = bf ? 2 : 1;
   const long long NN = (long long)rn(s);
   for (int lc = 0; lc < cC; ++lc) {
     const __half* xc = x16 + lc * 32;
     GemmParams p;
     init_params(p);
-    if (int e = map_support_mn(&p.a_map, gd16, N, Np, N, (long long)g_planes(s, K))) return e;
-    if (int e = map_chunks(&p.b_map, xc, N, C, R, (long long)N * C, s.B, (long long)R * N * C, 64, 8)) return e;
+    if (int e = map_support_mn(&p.a_map, gd16, N, Np, N, (long long)g_planes(s, K) * pl)) return e;
+    if (int e = map_chunks(&p.b_map, xc, N, C, R, (long long)N * C, (long long)s.B * pl, (long long)R * N * C, 64, 8)) return e;
     p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + d -> support index
     p.bm = omap(K, kBig, 1, 0, 0);                        // -> b
     p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B * K; p.R = 8;
@@ -241,8 +264,9 @@ static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16,
     // Z[b,d,n,e,:] += (G_d[e,e] - fp16(G_d[e,e])) * X16[b,n,e,:]
     p.ep.corr_src = xc; p.ep.corr_delta = delta_d; p.ep.corr_nseg = 1;
     p.ep.cZ = (long long)R * N * C; p.ep.cI = C; p.ep.cR = (long long)N * C; p.ep.cSeg = 0;
+    if (bf) p.ep.out16 = z16 + lc * NN * 32 + (size_t)s.B * K * cC * NN * 32;     // the lo plane of Z
     prof_set_next(PROF_FWD_A, 2.0 * s.B * K * (double)R * N * N * 32);
-    if (int e = tc::launch_contract(tc::A_MN128, 64, p, st)) return e;
+    if (int e = launch(bf, tc::A_MN128, 64, p, 3, (int)g_planes(s, K), s.B, st)) return e;
   }
   return 0;
 }
@@ -251,12 +275,16 @@ static int run_fwd_a(const BdgcnShape& s, const __half* gd16, const __half* x16,
 // One tile emits all the output planes of its rows as Kout chunks of 32 columns, so one launch covers Kout <= 8 (the widest
 // wgmma, N = 256).  More output planes go in ceil(Kout / 8) groups of balanced size, one launch each: group [r0, r0 + Rg) sees
 // W from its first output plane on and writes from output plane r0 on, with the same plane stride.  Each group re-reads A.
+// bf16x3 (bf, w_halves = 2: W's hi / lo pair): the A pair runs in two passes with W resident, hi meeting both halves and lo W hi
+// only, or in three passes with W streaming (one half per pass); the output is written as a pair
 static int run_mix_group(const BdgcnShape& s, const __half* a16, const __half* w16, int w_halves, __half* d16, int tag, int Kin,
-                         int Kout, int r0, int Rg, cudaStream_t st) {
+                         int Kout, int r0, int Rg, cudaStream_t st, bool bf) {
   const long long NN = (long long)rn(s);
+  const int pl = bf ? 2 : 1;
   GemmParams p;
   init_params(p);
   w16 += (size_t)r0 * Kin * 32 * 32;                                  // W rows of output plane r0, every half
+  if (bf) p.ep.out16 = d16 + (size_t)s.B * Kout * NN * 32 + (size_t)r0 * NN * 32;   // the lo plane of the output
   d16 += (size_t)r0 * NN * 32;
   const size_t w_bytes = (size_t)Rg * w_halves * Kin * 32 * 64;        // Kin * w_halves tiles of Rg chunks x [32 k][64 B]
   int bk = 32;
@@ -264,33 +292,34 @@ static int run_mix_group(const BdgcnShape& s, const __half* a16, const __half* w
     // One k-block per tile: a single TMA box brings the Kin planes of a 128-cell tile (the single-thread producer / MMA loops
     // cost ~0.3 us per k-block, which bounded the per-plane version at a third of the HBM rate), W resident in shared memory
     bk = 32 * Kin;
-    if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin, Kin)) return e;
+    if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin * pl, Kin)) return e;
     if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Rg, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, bk, Rg)) return e;
     p.am = omap(1, kBig, Kin, 0, 0);               // z = b -> first plane b*Kin
     p.bm = omap(1, 1, 0, 1, 0);                    // resident tile index = weight half
     p.kb_total = 1; p.kb_per_seg = 1; p.b_res_reps = w_halves;
   } else {
-    if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin)) return e;
+    if (int e = map_planes(&p.a_map, a16, NN, (long long)s.B * Kin * pl)) return e;
     if (int e = map_chunks(&p.b_map, w16, (long long)Kin * 32, 32, Rg, (long long)Kin * 32 * 32, w_halves, (long long)Kout * Kin * 32 * 32, 32, Rg)) return e;
     // segment s: plane = b*Kin + (s % Kin); weight rows (s % Kin)*32 of half s / Kin  (half 0 = fp16(W), half 1 = fp16(W - half 0))
     p.am = omap(1, kBig, Kin, 1, 0, Kin, 0);
     p.bm = omap(1, 1, 0, 0, 32, Kin, 1);
-    if (w_bytes > 160 * 1024) { p.kb_total = Kin * w_halves; p.kb_per_seg = 1; }          // large K: W streams with A
+    if (w_bytes > 160 * 1024) { p.kb_total = bf ? Kin : Kin * w_halves; p.kb_per_seg = 1; }   // large K: W streams with A
     else { p.kb_total = Kin; p.kb_per_seg = 1; p.b_res_reps = w_halves; }              // W resident, A plane by plane
   }
+  const int passes = p.b_res_reps ? 2 : 3;
   p.MT = ceil_div(NN, 128); p.NT = 1; p.Z = s.B; p.R = Rg;
   p.ep.out = d16; p.ep.out_f16 = 1;
   p.ep.sZ = (long long)Kout * NN * 32; p.ep.sI = 32; p.ep.sR = NN * 32;
   p.ep.m_valid = (int)NN; p.ep.r_valid = Rg;
   prof_set_next(tag, 2.0 * s.B * (double)Kin * Rg * NN * 32 * 32);   // algorithmic flops (the fp16 hi/lo weight split doubles the executed MMAs)
-  return tc::launch_contract(tc::A_K64, bk, p, st);
+  return launch(bf, tc::A_K64, bk, p, passes, (int)(s.B * Kin), 1, st);   // lo planes: B*Kin A planes, one W half on
 }
 static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, int w_halves, __half* d16, int tag, int Kin, int Kout,
-                   cudaStream_t st) {
+                   cudaStream_t st, bool bf = false) {
   const int groups = ceil_div(Kout, 8);
   for (int g = 0, r0 = 0; g < groups; ++g) {
     const int Rg = Kout / groups + (g < Kout % groups ? 1 : 0);     // 9 -> 5 + 4, 17 -> 6 + 6 + 5
-    if (int e = run_mix_group(s, a16, w16, w_halves, d16, tag, Kin, Kout, r0, Rg, st)) return e;
+    if (int e = run_mix_group(s, a16, w16, w_halves, d16, tag, Kin, Kout, r0, Rg, st, bf)) return e;
     r0 += Rg;
   }
   return 0;
@@ -299,38 +328,41 @@ static int run_mix(const BdgcnShape& s, const __half* a16, const __half* w16, in
 // FWD_B: out[b][m][e][32 hc + h] = act( sum_{(o,n)} G_o[row0 + n][m] U16[b][hc][o][n][e][h] + bias[32 hc + h] )
 //        n < R, every m < N; one launch per output chunk hc
 static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16_all, const float* bias, float* out, __half* out16,
-                     const float* delta_o, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32;
+                     const float* delta_o, cudaStream_t st, bool bf = false) {
+  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32, pl = bf ? 2 : 1;
   const bool slab = !(R == N && s.row0 == 0);
+  const int gplanes = s.dynamic ? s.B : 1;
+  int a_lo = 0, b_lo = 0;                 // bf16x3: TMA z distance of the lo planes
   for (int hc = 0; hc < cH; ++hc) {
     const __half* u16 = u16_all + (size_t)hc * K * rn(s) * 32;
     GemmParams p;
     init_params(p);
     if (!slab) {
       // whole layer: the contraction index (o, n) is a plain row index of the flat [K*N][N] support stack and of U16
-      if (int e = map_support_mn(&p.a_map, go16, N, Np, (long long)K * N, s.dynamic ? s.B : 1)) return e;
+      if (int e = map_support_mn(&p.a_map, go16, N, Np, (long long)K * N, gplanes * pl)) return e;
       // U16 [b][hc][(o,n)][e][h] read as (h, k = (o,n) rows, r = e, b): dims listed with non-monotonic strides (the r stride,
       // 64 B, is smaller than the k stride) so that ONE box (32 ch, 64 k, 4|8 r) lands in the canonical [r][k][64 B] layout
-      if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, s.B, (long long)cH * K * N * N * 32, 64, 8)) return e;
+      if (int e = map_chunks(&p.b_map, u16, (long long)K * N, (long long)N * 32, N, 32, (long long)s.B * pl, (long long)cH * K * N * N * 32, 64, 8)) return e;
       p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, 0);
       p.bm = omap(1, kBig, 1, 0, 0);
       p.kb_total = p.kb_per_seg = ceil_div((long long)K * N, 64);
+      a_lo = gplanes; b_lo = s.B;
     } else {
       // origin-row slab: one k-segment per support o.  A = rows [row0, row0 + R) of G_o (k coordinate o*N + kk inside the flat
       // stack, base pointer moved to row0); B = U16 [b][hc][o][n < R]: TMA zero-fills rows >= R, which also cancels the rows of
       // the NEXT slab that the last k-block of a segment reads from G.
-      const long long gplanes = s.dynamic ? s.B : 1;
       {
-        const uint64_t dims[4] = {(uint64_t)N, (uint64_t)((long long)K * N - s.row0), (uint64_t)gplanes, 1};
+        const uint64_t dims[4] = {(uint64_t)N, (uint64_t)((long long)K * N - s.row0), (uint64_t)(gplanes * pl), 1};
         const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)K * N * Np * 2, (uint64_t)K * N * Np * 2 * (uint64_t)gplanes};
         const uint32_t box[4] = {64, 64, 1, 1};
         if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
       }
-      if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * cH * K - (long long)hc * K, (long long)R * N * 32, 64, 8)) return e;
+      if (int e = map_chunks(&p.b_map, u16, R, (long long)N * 32, N, 32, (long long)s.B * cH * K * pl - (long long)hc * K, (long long)R * N * 32, 64, 8)) return e;
       p.am = omap(1, s.dynamic ? kBig : 1, 1, 0, N);          // k coordinate += o * N
       p.bm = omap(1, kBig, cH * K, 1, 0);                     // plane = (b*cH + hc)*K + o, from this chunk's base
       p.kb_per_seg = ceil_div(R, 64);
       p.kb_total = K * p.kb_per_seg;
+      a_lo = gplanes; b_lo = s.B * cH * K;
     }
     p.MT = ceil_div(N, 128); p.NT = ceil_div(N, 8); p.Z = s.B; p.R = 8;
     p.ep.out = out + hc * 32; p.ep.out_f16 = 0; p.ep.out16 = out16 ? out16 + hc * 32 : nullptr;
@@ -344,27 +376,27 @@ static int run_fwd_b(const BdgcnShape& s, const __half* go16, const __half* u16_
     p.ep.cZ = slab ? (long long)R * N * 32 : (long long)cH * K * R * N * 32;
     p.ep.cSeg = (long long)R * N * 32; p.ep.cI = (long long)N * 32; p.ep.cR = 32;
     prof_set_next(PROF_FWD_B, 2.0 * s.B * K * (double)R * N * N * 32);
-    if (int e = tc::launch_contract(tc::A_MN128, 64, p, st)) return e;
+    if (int e = launch(bf, tc::A_MN128, 64, p, 3, a_lo, b_lo, st)) return e;
   }
   return 0;
 }
 
 // BWD_V: V16[b][o][hc][n][e][h] = sum_m G_o[row0 + n][m] dP16[b][m][e][32 hc + h]       n < R; one launch per output chunk hc
-static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16, __half* v16, cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32;
+static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16, __half* v16, cudaStream_t st, bool bf = false) {
+  const int N = s.N, R = s.R, K = s.Ko, Np = pad8(N), H = s.H, cH = s.H / 32, pl = bf ? 2 : 1;
   const long long NN = (long long)rn(s);
   for (int hc = 0; hc < cH; ++hc) {
     GemmParams p;
     init_params(p);
     {   // rows [row0, row0 + R) of every support plane, K-major
       const long long nz = (long long)g_planes(s, K);
-      const uint64_t dims[4] = {(uint64_t)N, (uint64_t)R, (uint64_t)nz, 1};
+      const uint64_t dims[4] = {(uint64_t)N, (uint64_t)R, (uint64_t)(nz * pl), 1};
       const uint64_t str[3] = {(uint64_t)Np * 2, (uint64_t)N * Np * 2, (uint64_t)N * Np * 2 * (uint64_t)nz};
       const uint32_t box[4] = {64, 128, 1, 1};
       if (int e = make_tmap_f16(&p.a_map, go16 + (size_t)s.row0 * Np, 4, dims, str, box, TMAP_SW128)) return e;
     }
     // dP16 [b][m][e][H] chunk hc read as (h, k = m, r = e, b), see run_fwd_b
-    if (int e = map_chunks(&p.b_map, dp16 + hc * 32, N, (long long)N * H, N, H, s.B, (long long)N * N * H, 64, 8)) return e;
+    if (int e = map_chunks(&p.b_map, dp16 + hc * 32, N, (long long)N * H, N, H, (long long)s.B * pl, (long long)N * N * H, 64, 8)) return e;
     p.am = omap(1, s.dynamic ? kBig : K, 1, 0, 0);        // z = b*K + o
     p.bm = omap(K, kBig, 1, 0, 0);
     p.MT = ceil_div(R, 128); p.NT = ceil_div(N, 8); p.Z = s.B * K; p.R = 8;
@@ -373,8 +405,9 @@ static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16
     p.ep.out = v16 + hc * NN * 32; p.ep.out_f16 = 1;      // plane (b*K + o)*cH + hc
     p.ep.sZ = cH * NN * 32; p.ep.sI = (long long)N * 32; p.ep.sR = 32;
     p.ep.m_valid = R; p.ep.r_valid = N;
+    if (bf) p.ep.out16 = v16 + hc * NN * 32 + (size_t)s.B * K * cH * NN * 32;     // the lo plane of V
     prof_set_next(PROF_BWD_V, 2.0 * s.B * K * (double)R * N * N * 32);
-    if (int e = tc::launch_contract(tc::A_K128, 64, p, st)) return e;
+    if (int e = launch(bf, tc::A_K128, 64, p, 3, (int)g_planes(s, K), s.B, st)) return e;
   }
   return 0;
 }
@@ -382,19 +415,19 @@ static int run_bwd_v(const BdgcnShape& s, const __half* go16, const __half* dp16
 // BWD_DW: P[slice][a*32 + l][(o*cH + hc)*32 + h] = sum over the slice's (b,row) range of Z16 chunk a = d*cC + lc [b][row][l] times
 // V16 chunk (o, hc) [b][row][h]; that is P[slice][d*C + c][o*H + h'] in W's channel numbering
 static int run_bwd_dw(const BdgcnShape& s, const __half* z16, const __half* v16, float* partials, int* slices_out, int* mt_out,
-                      cudaStream_t st) {
-  const int rows = dw_row_chunks(s), cols = dw_col_chunks(s);
+                      cudaStream_t st, bool bf = false) {
+  const int rows = dw_row_chunks(s), cols = dw_col_chunks(s), pl = bf ? 2 : 1, passes = bf ? 3 : 1;
   const long long NN = (long long)rn(s);
   GemmParams p;
   init_params(p);
-  if (int e = map_chunks(&p.a_map, z16, NN, 32, rows, NN * 32, s.B, (long long)rows * NN * 32, 64, 4)) return e;
-  if (int e = map_chunks(&p.b_map, v16, NN, 32, cols, NN * 32, s.B, (long long)cols * NN * 32, 64, dw_chunks(cols))) return e;
+  if (int e = map_chunks(&p.a_map, z16, NN, 32, rows, NN * 32, (long long)s.B * pl, (long long)rows * NN * 32, 64, 4)) return e;
+  if (int e = map_chunks(&p.b_map, v16, NN, 32, cols, NN * 32, (long long)s.B * pl, (long long)cols * NN * 32, 64, dw_chunks(cols))) return e;
   p.am = omap(1, 1, 0, 1, 0);           // z (slice) ignored; batch element = segment
   p.bm = omap(1, 1, 0, 1, 0);
   int per = 1, total = 1;
-  const int slices = dw_slices(s, &per, &total);
+  const int slices = dw_slices(s, &per, &total, passes);      // split-K over every pass
   p.MT = ceil_div(rows, 4); p.NT = dw_col_tiles(cols); p.Z = slices; p.R = dw_chunks(cols);   // output chunk r = nt * R + j
-  p.kb_total = total; p.kb_per_seg = ceil_div(NN, 64);
+  p.kb_total = total / passes; p.kb_per_seg = ceil_div(NN, 64);
   p.split_k = 1; p.kb_per_slice = per;
   p.ep.out = partials; p.ep.out_f16 = 0;
   p.ep.sZ = (long long)p.MT * 128 * cols * 32; p.ep.sI = (long long)cols * 32; p.ep.sR = 32;
@@ -402,19 +435,19 @@ static int run_bwd_dw(const BdgcnShape& s, const __half* z16, const __half* v16,
   *slices_out = slices;
   *mt_out = p.MT;
   prof_set_next(PROF_BWD_DW, 2.0 * s.B * (double)s.Ko * s.Kd * NN * s.C * s.H);
-  return tc::launch_contract(tc::A_MN64, 64, p, st);
+  return launch(bf, tc::A_MN64, 64, p, passes, s.B, s.B, st);
 }
 
 // BWD_DX: dX[b][n][c][32 lc + l] = sum_{d,e} G_d[c][e] Y16[b][d][lc][n][e][l]       n < R; one launch per input chunk lc
 static int run_bwd_dx(const BdgcnShape& s, const __half* gd16, const __half* y16, float* dX, const float* inv_scale, float* dx_absmax,
-                      cudaStream_t st) {
-  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32;
+                      cudaStream_t st, bool bf = false) {
+  const int N = s.N, R = s.R, K = s.Kd, Np = pad8(N), C = s.C, cC = s.C / 32, pl = bf ? 2 : 1;
   const long long NN = (long long)rn(s);
   for (int lc = 0; lc < cC; ++lc) {
     GemmParams p;
     init_params(p);
-    if (int e = map_support_k(&p.a_map, gd16, N, Np, (long long)g_planes(s, K))) return e;
-    if (int e = map_chunks(&p.b_map, y16 + lc * NN * 32, N, 32, R, (long long)N * 32, (long long)s.B * K * cC - lc, NN * 32, 64, 8)) return e;
+    if (int e = map_support_k(&p.a_map, gd16, N, Np, (long long)g_planes(s, K) * pl)) return e;
+    if (int e = map_chunks(&p.b_map, y16 + lc * NN * 32, N, 32, R, (long long)N * 32, (long long)s.B * K * cC * pl - lc, NN * 32, 64, 8)) return e;
     p.am = omap(1, s.dynamic ? kBig : 1, s.dynamic ? K : 0, 1, 0);   // support index = (b*K) + d
     p.bm = omap(1, kBig, K * cC, cC, 0);                              // plane = (b*K + d)*cC, from this chunk's base
     p.MT = ceil_div(N, 128); p.NT = ceil_div(R, 8); p.Z = s.B; p.R = 8;
@@ -423,17 +456,22 @@ static int run_bwd_dx(const BdgcnShape& s, const __half* gd16, const __half* y16
     p.ep.sZ = (long long)R * N * C; p.ep.sI = C; p.ep.sR = (long long)N * C;
     p.ep.m_valid = N; p.ep.r_valid = R;
     prof_set_next(PROF_BWD_DX, 2.0 * s.B * K * (double)R * N * N * 32);
-    if (int e = tc::launch_contract(tc::A_K128, 64, p, st)) return e;
+    if (int e = launch(bf, tc::A_K128, 64, p, 3, (int)g_planes(s, K), s.B * K * cC, st)) return e;
   }
   return 0;
 }
 
 // Prepared supports: [planes][N][Np] fp16 (padding zeroed) followed, 256-byte aligned, by the [planes][N] diagonal remainders.
 // A caller that uses the same supports for several layers / for forward and backward converts them once.
+// bf16x3: the [hi | lo] pair of [planes][N][Np] bf16 planes, no remainders.
 static size_t prep_g16_bytes(long long planes, int N) { return align_up((size_t)planes * N * pad8(N) * sizeof(__half), 256); }
-size_t bdgcn_supports_prepared_bytes(long long planes, int N) { return prep_g16_bytes(planes, N) + align_up((size_t)planes * N * sizeof(float), 256); }
-int bdgcn_prepare_supports(const float* G, void* prepared, long long planes, int N, cudaStream_t st) {
+size_t bdgcn_supports_prepared_bytes(long long planes, int N, bool bf) {
+  if (bf) return align_up((size_t)2 * planes * N * pad8(N) * sizeof(__half), 256);
+  return prep_g16_bytes(planes, N) + align_up((size_t)planes * N * sizeof(float), 256);
+}
+int bdgcn_prepare_supports(const float* G, void* prepared, long long planes, int N, cudaStream_t st, bool bf) {
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(prepared) & 255) == 0, "prepared-supports buffer must be 256-byte aligned");
+  if (bf) return cvt_f32_to_bf16x3_padded(G, static_cast<__nv_bfloat16*>(prepared), (size_t)planes * N, N, pad8(N), st);
   __half* g16 = static_cast<__half*>(prepared);
   float* delta = reinterpret_cast<float*>(static_cast<uint8_t*>(prepared) + prep_g16_bytes(planes, N));
   if (int e = cvt_f32_to_f16_padded(G, g16, (size_t)planes * N, N, pad8(N), st)) return e;
@@ -444,8 +482,15 @@ int bdgcn_prepare_supports(const float* G, void* prepared, long long planes, int
 // with the other side (static graph: Go == Gd), or converted here into the workspace
 struct SideG { const __half* g16; const float* delta; };
 static int resolve_side(const BdgcnShape& s, int K, const float* G, const void* prepared, __half* ws16, float* ws_delta, bool want_delta,
-                        SideG* out, cudaStream_t st) {
+                        SideG* out, cudaStream_t st, bool bf = false) {
   const long long planes = (long long)g_planes(s, K);
+  if (bf) {         // a bf16x3 pair, no remainders
+    MPGCN_CHECK((reinterpret_cast<uintptr_t>(prepared) & 255) == 0, "prepared-supports buffer must be 256-byte aligned");
+    out->delta = nullptr;
+    out->g16 = prepared ? static_cast<const __half*>(prepared) : ws16;
+    if (prepared) return 0;
+    return cvt_f32_to_bf16x3_padded(G, reinterpret_cast<__nv_bfloat16*>(ws16), (size_t)planes * s.N, s.N, pad8(s.N), st);
+  }
   if (prepared) {
     MPGCN_CHECK((reinterpret_cast<uintptr_t>(prepared) & 255) == 0, "prepared-supports buffer must be 256-byte aligned");
     out->g16 = static_cast<const __half*>(prepared);
@@ -463,12 +508,13 @@ static int resolve_side(const BdgcnShape& s, int K, const float* G, const void* 
 // layer forward / backward
 // ---------------------------------------------------------------------------------------
 int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
-                     float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st) {
+                     float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st, bool bf) {
   MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
               s.C, s.H, s.Ko, s.Kd);
+  MPGCN_CHECK(!bf || (s.whole() && ex.x_f16 == nullptr && ex.out_f16 == nullptr), "bf16x3: whole layers only, without fp16 side buffers");
   if (int e = check_index_range(s)) return e;
   const size_t NN = rn(s);
-  const FwdLayout L = fwd_layout(s);
+  const FwdLayout L = fwd_layout(s, bf);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_forward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "workspace must be 256-byte aligned");
   uint8_t* wb = static_cast<uint8_t*>(ws);
@@ -481,6 +527,17 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
               "bdgcn_forward: `out` and the fp16 side buffers must be 32-byte aligned (256-bit stores)");
   MPGCN_CHECK((reinterpret_cast<uintptr_t>(X) & 15) == 0, "bdgcn_forward: X must be 16-byte aligned");
 
+  if (bf) {
+    SideG gd{}, go{};
+    if (int e = cvt_f32_to_bf16x3_padded(X, reinterpret_cast<__nv_bfloat16*>(x16_ws), (size_t)s.B * NN, s.C, s.C, st)) return e;
+    if (int e = resolve_side(s, s.Kd, Gd, ex.gd_prepared, reinterpret_cast<__half*>(wb + L.gd16), nullptr, false, &gd, st, true)) return e;
+    if (Go == Gd && ex.go_prepared == nullptr) go = gd;
+    else if (int e = resolve_side(s, s.Ko, Go, ex.go_prepared, reinterpret_cast<__half*>(wb + L.go16), nullptr, false, &go, st, true)) return e;
+    if (int e = permute_w_mix_bf16x3(W, reinterpret_cast<__nv_bfloat16*>(w16), 1, s.Ko, s.Kd, s.C, s.H, st)) return e;
+    if (int e = run_fwd_a(s, gd.g16, x16_ws, z16, nullptr, st, true)) return e;
+    if (int e = run_mix(s, z16, w16, 2, u16, PROF_FWD_MIX, s.Kd * (s.C / 32), s.Ko * (s.H / 32), st, true)) return e;
+    return run_fwd_b(s, go.g16, u16, bias, out, nullptr, nullptr, st, true);
+  }
   const __half* x16 = static_cast<const __half*>(ex.x_f16);
   if (x16 == nullptr) {
     if (int e = cvt_f32_to_f16(X, x16_ws, (size_t)s.B * NN * s.C, st)) return e;
@@ -506,7 +563,7 @@ int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const
 // L: the layout, checked against the workspace; form_y: run BWD_MIX (Y16) even without dX (the support gradient reads it)
 static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                             const void* saved, float* dX, float* dW, float* db, void* ws, const BwdLayout& L, const BdgcnExtras& ex,
-                            bool form_y, cudaStream_t st) {
+                            bool form_y, cudaStream_t st, bool bf = false) {
   MPGCN_CHECK(tc_supported(s), "tensor-core path needs C and H to be multiples of 32 (H <= 1024) and Ko, Kd >= 1 (got C=%d H=%d Ko=%d Kd=%d)",
               s.C, s.H, s.Ko, s.Kd);
   if (int e = check_index_range(s)) return e;
@@ -527,6 +584,34 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
   float* partials = reinterpret_cast<float*>(wb + L.partials);
   const float* scale2 = reinterpret_cast<float*>(wb + L.scale);   // [S, 1/S]: power-of-two gradient scale (fp16 range)
 
+  if (bf) {
+    // bf16x3 keeps the power-of-two scale S of the fp16 path: exact in both directions, and harmless in bf16's range
+    MPGCN_CHECK(s.whole() && ex.d_pre_f16 == nullptr && ex.out_f16 == nullptr, "bf16x3: whole layers only, without fp16 side buffers");
+    MPGCN_CHECK(out != nullptr || !act, "bdgcn_backward: the ReLU mask needs `out`");
+    float* scale2_ws = reinterpret_cast<float*>(wb + L.scale);
+    if (int e = grad_scale_prepare(d_out, (size_t)s.B * NNfull * s.H, scale2_ws, ex.d_out_absmax, st)) return e;
+    if (int e = relu_bwd_prep_bf16x3(d_out, out, act, reinterpret_cast<__nv_bfloat16*>(wb + L.dp16), db, (size_t)s.B * NNfull * s.H, s.H,
+                                     scale2_ws, st, db_slots))
+      return e;
+    SideG gd{}, go{};
+    const bool shared = Go == Gd && s.Ko == s.Kd;
+    if (dX || shared) {
+      if (int e = resolve_side(s, s.Kd, Gd, ex.gd_prepared, reinterpret_cast<__half*>(wb + L.gd16), nullptr, false, &gd, st, true)) return e;
+    }
+    if (shared && ex.go_prepared == nullptr) go = gd;
+    else if (int e = resolve_side(s, s.Ko, Go, ex.go_prepared, reinterpret_cast<__half*>(wb + L.go16), nullptr, false, &go, st, true)) return e;
+    if (int e = run_bwd_v(s, go.g16, dp16, v16, st, true)) return e;
+    int slices = 0, mt = 0;
+    if (int e = run_bwd_dw(s, z16, v16, partials, &slices, &mt, st, true)) return e;
+    if (int e = reduce_dw_partials(partials, dW, slices, mt, s.Ko, s.Kd, s.C, s.H, scale2 + 1, st)) return e;
+    if (dX) {
+      if (ex.dx_absmax) MPGCN_CUDA(cudaMemsetAsync(ex.dx_absmax, 0, sizeof(float), st));
+      if (int e = permute_w_mix_bf16x3(W, reinterpret_cast<__nv_bfloat16*>(wq16), 0, s.Ko, s.Kd, s.C, s.H, st)) return e;
+      if (int e = run_mix(s, v16, wq16, 2, y16, PROF_BWD_MIX, s.Ko * (s.H / 32), s.Kd * (s.C / 32), st, true)) return e;
+      if (int e = run_bwd_dx(s, gd.g16, y16, dX, scale2 + 1, ex.dx_absmax, st, true)) return e;
+    }
+    return 0;
+  }
   if (ex.d_pre_f16 != nullptr) {
     // dPre arrives masked, scaled and cast (mpgcn_relu_backward_scatter_f16 wrote it into every rank's buffer): no pass over it here
     MPGCN_CHECK(s.partial && ex.d_pre_scale2 != nullptr, "bdgcn_backward: a prepared fp16 dPre needs a part call and its scale pair");
@@ -567,10 +652,10 @@ static int backward_tc_impl(const BdgcnShape& s, const float* d_out, const float
 
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
-                      cudaStream_t st) {
-  const BwdLayout L = bwd_layout(s, false);
+                      cudaStream_t st, bool bf) {
+  const BwdLayout L = bwd_layout(s, false, bf);
   MPGCN_CHECK(ws_bytes >= L.total, "bdgcn_backward: workspace too small (%zu < %zu bytes)", ws_bytes, L.total);
-  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, ex, false, st);
+  return backward_tc_impl(s, d_out, out, Go, Gd, W, saved, dX, dW, db, ws, L, ex, false, st, bf);
 }
 
 // One support-gradient contraction into the partials [slice][N][ldp] (ldp = 32 ceil(N/32): a 32-column chunk never runs into

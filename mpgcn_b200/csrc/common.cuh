@@ -6,6 +6,7 @@
 #pragma once
 
 #include <cuda.h>            // CUtensorMap (types only; libcuda is resolved at run time)
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -204,6 +205,13 @@ __device__ __forceinline__ uint32_t f2h2_sat_bits(float a, float b) {
   uint32_t r;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
   return r;
+}
+// fp32 pair (a, b) -> bf16 pairs hi = bf16_rn(x), lo = bf16_rn(x - hi) (bf16x3 operands), packed low half = a as above.  bf16
+// has fp32's exponent range: no saturation, and hi + lo carries 16 significant bits.
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
+  const float ha = __uint_as_float(hi << 16), hb = __uint_as_float(hi & 0xffff0000u);
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - hb), "f"(a - ha));
 }
 #endif  // __CUDACC__
 

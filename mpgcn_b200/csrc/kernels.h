@@ -56,6 +56,9 @@ int cvt_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t s);
 int support_diag_delta(const float* G, float* delta, size_t planes, int N, cudaStream_t s);
 // [rows][cols] fp32 -> [rows][ld] fp16 (ld >= cols, padding zeroed)
 int cvt_f32_to_f16_padded(const float* src, __half* dst, size_t rows, int cols, int ld, cudaStream_t s);
+// bf16x3 (precision 2) operand pairs: [rows][cols] fp32 -> hi = bf16_rn(x) as [rows][ld] (padding zeroed), then lo = bf16_rn(x - hi)
+// the same way right behind it (rows * ld elements on); ld = cols converts a plain array
+int cvt_f32_to_bf16x3_padded(const float* src, __nv_bfloat16* dst, size_t rows, int cols, int ld, cudaStream_t s);
 // d_pre = d_out * (out > 0) (relu) or d_out, 1 <= H <= 1024; exactly one output: fp32, or fp16(scale[0] * d_pre) (scale: device
 // scalar); db[h] = sum d_pre (nullable); db_slots (bias_grad_slot_bytes, nullable): db from per-block partials in a fixed order
 int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d_pre16, float* d_pre32, float* db, size_t n, int H,
@@ -63,6 +66,9 @@ int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d_pre1
 // the same with the ReLU mask taken from an fp16 copy of the forward output (tensor-core path: fp16 d_pre only)
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d_pre16, float* db, size_t n, int H,
                           const float* scale, cudaStream_t s, float* db_slots = nullptr);
+// the same as a bf16x3 pair of scale[0] * d_pre: hi d_pair[0, n), lo d_pair[n, 2n) (fp32 mask)
+int relu_bwd_prep_bf16x3(const float* d_out, const float* out, int relu, __nv_bfloat16* d_pair, float* db, size_t n, int H, const float* scale,
+                         cudaStream_t s, float* db_slots = nullptr);
 // scale2[0] = S = 2^k with S*max|d_out| in [16,32), scale2[1] = 1/S (S = 1 for an all-zero or non-finite input).
 // fp16 has 5 exponent bits: realistic gradients (MSE mean over B*N*N cells ~ 1e-7) must be rescaled before the cast.
 // absmax_hint: optional device scalar already holding max|d_out| (produced by the epilogue that wrote d_out): skips the pass
@@ -72,6 +78,8 @@ int permute_w_bwd(const float* W, float* wq32, int Ko, int Kd, int C, int H, cud
 // W[o][d][c][h] fp32 -> the fp16 W operand of a tensor-core channel mix (bdgcn_tc.cu), C and H multiples of 32, c = 32 lc + l,
 // h = 32 hc + h':  lo != null: forward, hi / lo = fp16 split as [(hc,o)][(d,lc)][l][h'];  lo == null: backward, [(d,lc)][(o,hc)][h'][l]
 int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s);
+// the same as a bf16x3 pair (fwd: the forward layout; else the backward one), hi pair[0, n), lo pair[n, 2n) for n = Ko*Kd*C*H
+int permute_w_mix_bf16x3(const float* W, __nv_bfloat16* pair, int fwd, int Ko, int Kd, int C, int H, cudaStream_t s);
 // dW[o][d][c][h] = sum_slices P[slice][d*C + c][o*H + h]   (P: [slice][MT*128 rows][Ko*H]; o < Ko, d < Kd)
 int reduce_dw_partials(const float* P, float* dW, int slices, int MT, int Ko, int Kd, int C, int H, const float* inv_scale, cudaStream_t s);
 // dG[n][m] (+)= inv_scale * sum_slices P[slice][n][m]   (P: [slice][N][ldp]; n, m < N; accumulate: add to dG)
@@ -170,7 +178,8 @@ struct BdgcnShape {
                     // backward receives dPre (already masked) instead of dOut
   bool whole() const { return R == N && row0 == 0 && Ko == K && Kd == K && !partial; }
 };
-enum Precision { PREC_FP32_SIMT = 0, PREC_FP16_TC = 1 };
+// PREC_BF16X3_TC: the tensor-core layer on bf16 pairs, three products per contraction (bdgcn_tc.cu; DESIGN.md section 3)
+enum Precision { PREC_FP32_SIMT = 0, PREC_FP16_TC = 1, PREC_BF16X3_TC = 2 };
 
 bool tc_supported(const BdgcnShape& s);
 // buffer sizes of a layer call in either precision (api.cu), from those of each kernel family
@@ -182,9 +191,10 @@ size_t simt_saved_bytes(const BdgcnShape& s);
 size_t simt_fwd_ws_bytes(const BdgcnShape& s);
 size_t simt_bwd_ws_bytes(const BdgcnShape& s);
 size_t simt_sgrad_ws_bytes(const BdgcnShape& s);
-size_t tc_saved_bytes(const BdgcnShape& s);
-size_t tc_fwd_ws_bytes(const BdgcnShape& s);
-size_t tc_bwd_ws_bytes(const BdgcnShape& s);
+// bf: the bf16x3 layer (every 16-bit stash / workspace tensor a hi / lo pair)
+size_t tc_saved_bytes(const BdgcnShape& s, bool bf = false);
+size_t tc_fwd_ws_bytes(const BdgcnShape& s, bool bf = false);
+size_t tc_bwd_ws_bytes(const BdgcnShape& s, bool bf = false);
 size_t tc_sgrad_ws_bytes(const BdgcnShape& s);
 long long tc_debug_offset(const BdgcnShape& s, int which);
 
@@ -228,13 +238,14 @@ struct BdgcnExtras {
   const void* d_pre_f16 = nullptr;      // backward of a PART: dPre [B,N,N,H] already masked, scaled by scale2[0] and cast to fp16
   const float* d_pre_scale2 = nullptr;  //   ... with its device [S, 1/S] pair (mpgcn_relu_backward_scatter_f16 produces both)
 };
-size_t bdgcn_supports_prepared_bytes(long long planes, int N);
-int bdgcn_prepare_supports(const float* G, void* prepared, long long planes, int N, cudaStream_t st);
+// bf: the bf16x3 layer -- supports prepared as a bf16 pair, and whole layers without the fp16 side buffers (x_f16, out_f16, d_pre_f16)
+size_t bdgcn_supports_prepared_bytes(long long planes, int N, bool bf = false);
+int bdgcn_prepare_supports(const float* G, void* prepared, long long planes, int N, cudaStream_t st, bool bf = false);
 int bdgcn_forward_tc(const BdgcnShape& s, const float* X, const float* Go, const float* Gd, const float* W, const float* bias,
-                     float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st);
+                     float* out, void* saved, void* ws, size_t ws_bytes, const BdgcnExtras& ex, cudaStream_t st, bool bf = false);
 int bdgcn_backward_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* Go, const float* Gd, const float* W,
                       const void* saved, float* dX, float* dW, float* db, void* ws, size_t ws_bytes, const BdgcnExtras& ex,
-                      cudaStream_t st);
+                      cudaStream_t st, bool bf = false);
 // the backward plus the support gradients (whole layer): static supports get dGo [K][N][N] = dG_o + dG_d summed over the batch
 // (dGd unused), dynamic ones dGo [B][K][N][N] and dGd [B][K][N][N] (either nullable).  dX / dW / db are those of the backward.
 int bdgcn_backward_supports_tc(const BdgcnShape& s, const float* d_out, const float* out, const float* X, const float* Go, const float* Gd,

@@ -218,12 +218,46 @@ int cvt_f32_to_f16_padded(const float* src, __half* dst, size_t rows, int cols, 
   return 0;
 }
 
+// ---- bf16x3 operand pairs: hi = bf16_rn(x) at dst[i], lo = bf16_rn(x - hi) at dst[total + i] ----
+__device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __float2bfloat16_rn(x);
+  lo = __float2bfloat16_rn(x - __bfloat162float(hi));
+}
+
+// [rows][cols] fp32 -> [rows][ld] pair planes (ld >= cols, padding zeroed); ld = cols is a plain conversion
+__global__ void cvt_bf16x3_padded_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, size_t rows, int cols, int ld) {
+  const size_t total = rows * (size_t)ld;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    __nv_bfloat16 hi = __float2bfloat16_rn(0.f), lo = hi;
+    if (ld == cols) {               // unpadded: no index arithmetic
+      split_bf16(src[i], hi, lo);
+    } else {
+      const size_t r = i / ld;
+      const int c = (int)(i - r * ld);
+      if (c < cols) split_bf16(src[r * cols + c], hi, lo);
+    }
+    dst[i] = hi;
+    dst[total + i] = lo;
+  }
+}
+
+int cvt_f32_to_bf16x3_padded(const float* src, __nv_bfloat16* dst, size_t rows, int cols, int ld, cudaStream_t s) {
+  if (rows == 0) return 0;
+  prof_count(PROF_ELEMENTWISE);
+  cvt_bf16x3_padded_kernel<<<grid_for(rows * ld, 256), 256, 0, s>>>(src, dst, rows, cols, ld);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // ---- ReLU backward: d_pre = d_out * [out > 0] (or d_out), stored as fp32 or as fp16(S * d_pre) into g <= 8 destinations, and the
 // per-channel bias gradient db[h] = sum d_pre.  The local pass of a layer backward is one sample and one destination; the row
 // shard's all-gather (relu_backward_scatter[_f16]) writes rows [row0, row0 + rows) of every rank's [B][N][N][H] buffer.
 enum class Mask { None, F32, F16 };   // ReLU mask source: none (linear layer), the fp32 forward output, or its fp16 copy
 template <class T>
 struct PeerPtrs { T* p[8]; };
+template <>
+struct PeerPtrs<__nv_bfloat16> { __nv_bfloat16* p[8]; size_t lo_off; };   // bf16x3 pairs: the lo plane lo_off elements behind
 
 // V consecutive values at p <-> V floats in registers; V = 4 is one 16-byte (fp32) or 8-byte (fp16) access
 __device__ __forceinline__ void ld_v(const float* p, float (&v)[1]) { v[0] = *p; }
@@ -252,6 +286,15 @@ __device__ __forceinline__ void st_v(__half* p, const float (&v)[4], float S) {
   const __half2 a = __halves2half2(f2h_sat(v[0] * S), f2h_sat(v[1] * S)), b = __halves2half2(f2h_sat(v[2] * S), f2h_sat(v[3] * S));
   __stwb(reinterpret_cast<uint2*>(p), make_uint2(*reinterpret_cast<const unsigned int*>(&a), *reinterpret_cast<const unsigned int*>(&b)));
 }
+// a bf16x3 pair of S * value: hi at p, lo at p + lo_off
+__device__ __forceinline__ void st_pair(__nv_bfloat16* p, size_t lo_off, const float (&v)[1], float S) { split_bf16(v[0] * S, p[0], p[lo_off]); }
+__device__ __forceinline__ void st_pair(__nv_bfloat16* p, size_t lo_off, const float (&v)[4], float S) {
+  uint32_t h0, l0, h1, l1;
+  split_bf16x2(v[0] * S, v[1] * S, h0, l0);
+  split_bf16x2(v[2] * S, v[3] * S, h1, l1);
+  __stwb(reinterpret_cast<uint2*>(p), make_uint2(h0, h1));
+  __stwb(reinterpret_cast<uint2*>(p + lo_off), make_uint2(l0, l1));
+}
 
 // db[c] += the block's partial sums of channel c.  The block is a multiple of H / V threads with at least H of them, so thread t
 // owns channels V * (t % (H / V)) .. + V - 1 for its whole grid-stride loop; thread c < H adds the partials of channel c in thread order.
@@ -278,7 +321,7 @@ template <int V, Mask M, class T>
 __global__ void __launch_bounds__(1024, 2) relu_bwd_kernel(const float* __restrict__ d_out, const void* __restrict__ mask, PeerPtrs<T> dst, int g, float* __restrict__ db,
                                 float* __restrict__ db_slots, const float* __restrict__ scale, size_t n, size_t full, size_t off, int H) {
   using MaskT = std::conditional_t<M == Mask::F16, __half, float>;
-  const float S = std::is_same<T, __half>::value ? __ldg(scale) : 1.f;
+  const float S = std::is_same<T, float>::value ? 1.f : __ldg(scale);
   const size_t b = blockIdx.y;
   float local[V] = {};
   for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; i < n; i += (size_t)gridDim.x * blockDim.x * V) {
@@ -291,8 +334,13 @@ __global__ void __launch_bounds__(1024, 2) relu_bwd_kernel(const float* __restri
       for (int e = 0; e < V; ++e) v[e] = o[e] > 0.f ? v[e] : 0.f;
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (j < g) st_v(dst.p[j] + b * full + off + i, v, S);
+    for (int j = 0; j < 8; ++j) {
+      if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        if (j < g) st_pair(dst.p[j] + b * full + off + i, dst.lo_off, v, S);
+      } else {
+        if (j < g) st_v(dst.p[j] + b * full + off + i, v, S);
+      }
+    }
 #pragma unroll
     for (int e = 0; e < V; ++e) local[e] += v[e];
   }
@@ -312,13 +360,17 @@ static int channel_block(int H, int V) {
 // for the vector access, else V = 1.  The exchange steps (PROF_EXCHANGE) are timed, the local pass is counted.
 template <Mask M, class T>
 static int relu_bwd_launch(const float* d_out, const void* mask, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
-                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr) {
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr, size_t lo_off = 0) {
   MPGCN_CHECK(H >= 1 && H <= 1024, "relu backward: H=%d unsupported (1..1024)", H);
   MPGCN_CHECK(g >= 1 && g <= 8, "relu backward: %d ranks unsupported (1..8)", g);
-  constexpr bool f16 = std::is_same<T, __half>::value;
+  constexpr bool f16 = !std::is_same<T, float>::value;
   MPGCN_CHECK(!f16 || scale != nullptr, "relu backward: an fp16 destination needs its scale");
   bool vec = H % 4 == 0 && (n | full | off) % 4 == 0 && aligned(d_out, 16) && (M == Mask::None || aligned(mask, M == Mask::F16 ? 8 : 16));
   PeerPtrs<T> pp{};
+  if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+    pp.lo_off = lo_off;
+    vec = vec && lo_off % 4 == 0;
+  }
   for (int j = 0; j < g; ++j) {
     MPGCN_CHECK(dsts[j] != nullptr, "relu backward: destination %d is null", j);
     pp.p[j] = dsts[j];
@@ -342,9 +394,9 @@ static int relu_bwd_launch(const float* d_out, const void* mask, T* const* dsts,
 // the same with the ReLU mask taken from the fp32 forward output (act 1) or no mask (act 0)
 template <class T>
 static int relu_bwd_launch(const float* d_out, const float* out, int act, T* const* dsts, int g, float* db, const float* scale, int B, size_t n,
-                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr) {
-  return act ? relu_bwd_launch<Mask::F32>(d_out, out, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots)
-             : relu_bwd_launch<Mask::None>(d_out, nullptr, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots);
+                           size_t full, size_t off, int H, ProfTag tag, cudaStream_t s, float* db_slots = nullptr, size_t lo_off = 0) {
+  return act ? relu_bwd_launch<Mask::F32>(d_out, out, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots, lo_off)
+             : relu_bwd_launch<Mask::None>(d_out, nullptr, dsts, g, db, scale, B, n, full, off, H, tag, s, db_slots, lo_off);
 }
 
 int relu_bwd_prep_f16mask(const float* d_out, const __half* out16, int relu, __half* d16, float* db, size_t n, int H, const float* scale,
@@ -360,6 +412,12 @@ int relu_bwd_prep(const float* d_out, const float* out, int relu, __half* d16, f
   MPGCN_CHECK((d16 == nullptr) != (d32 == nullptr), "relu_bwd_prep: exactly one of the fp16 and fp32 outputs");
   if (d16) return relu_bwd_launch(d_out, out, relu, &d16, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
   return relu_bwd_launch(d_out, out, relu, &d32, 1, db, nullptr, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots);
+}
+
+int relu_bwd_prep_bf16x3(const float* d_out, const float* out, int relu, __nv_bfloat16* d_pair, float* db, size_t n, int H, const float* scale,
+                         cudaStream_t s, float* db_slots) {
+  if (n == 0) return 0;
+  return relu_bwd_launch(d_out, out, relu, &d_pair, 1, db, scale, 1, n, n, 0, H, PROF_ELEMENTWISE, s, db_slots, n);
 }
 
 size_t bias_grad_slot_bytes(int H) { return align_up((size_t)device_sm_count() * 16 * H * sizeof(float), 256); }
@@ -417,28 +475,47 @@ int permute_w_bwd(const float* W, float* wq32, int Ko, int Kd, int C, int H, cud
   return 0;
 }
 
-// W[o][d][32 lc + l][32 hc + h] -> one [32][32] block per (output plane, input plane) of a channel mix, see kernels.h
+// W[o][d][32 lc + l][32 hc + h] -> one [32][32] block per (output plane, input plane) of a channel mix, see kernels.h: the W
+// element that lands at index i of the forward (fwd) or backward operand
+__device__ __forceinline__ float w_mix_src(const float* __restrict__ W, int i, bool fwd, int Ko, int Kd, int C, int H) {
+  const int cC = C / 32, cH = H / 32;
+  const int e0 = i % 32, e1 = (i / 32) % 32, blk = i / 1024;
+  int o, d, lc, hc, l, h;
+  if (fwd) {     // forward: i = ((hc*Ko + o)*Kd*cC + d*cC + lc)*1024 + l*32 + h
+    h = e0; l = e1;
+    const int sp = blk % (Kd * cC), r = blk / (Kd * cC);
+    d = sp / cC; lc = sp % cC; o = r % Ko; hc = r / Ko;
+  } else {       // backward: i = ((d*cC + lc)*Ko*cH + o*cH + hc)*1024 + h*32 + l
+    l = e0; h = e1;
+    const int sp = blk % (Ko * cH), r = blk / (Ko * cH);
+    o = sp / cH; hc = sp % cH; d = r / cC; lc = r % cC;
+  }
+  return W[((size_t)(o * Kd + d) * C + lc * 32 + l) * H + hc * 32 + h];
+}
 __global__ void permute_w_mix_kernel(const float* __restrict__ W, __half* __restrict__ hi, __half* __restrict__ lo, int Ko, int Kd, int C,
                                      int H) {
-  const int cC = C / 32, cH = H / 32;
   const int total = Ko * Kd * C * H;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int e0 = i % 32, e1 = (i / 32) % 32, blk = i / 1024;
-    int o, d, lc, hc, l, h;
-    if (lo) {      // forward: i = ((hc*Ko + o)*Kd*cC + d*cC + lc)*1024 + l*32 + h
-      h = e0; l = e1;
-      const int sp = blk % (Kd * cC), r = blk / (Kd * cC);
-      d = sp / cC; lc = sp % cC; o = r % Ko; hc = r / Ko;
-    } else {       // backward: i = ((d*cC + lc)*Ko*cH + o*cH + hc)*1024 + h*32 + l
-      l = e0; h = e1;
-      const int sp = blk % (Ko * cH), r = blk / (Ko * cH);
-      o = sp / cH; hc = sp % cH; d = r / cC; lc = r % cC;
-    }
-    const float v = W[((size_t)(o * Kd + d) * C + lc * 32 + l) * H + hc * 32 + h];
+    const float v = w_mix_src(W, i, lo != nullptr, Ko, Kd, C, H);
     const __half x = f2h_sat(v);
     hi[i] = x;
     if (lo) lo[i] = f2h_sat(v - __half2float(x));
   }
+}
+
+// bf16x3: the pair of W, hi at pair[i], lo at pair[total + i]
+__global__ void permute_w_mix_bf16x3_kernel(const float* __restrict__ W, __nv_bfloat16* __restrict__ pair, int fwd, int Ko, int Kd, int C, int H) {
+  const int total = Ko * Kd * C * H;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+    split_bf16(w_mix_src(W, i, fwd != 0, Ko, Kd, C, H), pair[i], pair[total + i]);
+}
+
+int permute_w_mix_bf16x3(const float* W, __nv_bfloat16* pair, int fwd, int Ko, int Kd, int C, int H, cudaStream_t s) {
+  MPGCN_CHECK(C % 32 == 0 && H % 32 == 0, "permute_w_mix: C=%d H=%d are not multiples of 32", C, H);
+  prof_count(PROF_ELEMENTWISE);
+  permute_w_mix_bf16x3_kernel<<<grid_for((size_t)Ko * Kd * C * H, 256), 256, 0, s>>>(W, pair, fwd, Ko, Kd, C, H);
+  MPGCN_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int permute_w_mix(const float* W, __half* hi, __half* lo, int Ko, int Kd, int C, int H, cudaStream_t s) {

@@ -232,21 +232,27 @@ static int make_out_map(CUtensorMap* m, const void* base, bool f16, const Epilog
   return 0;
 }
 
-template <int AK, int BK, bool BKM = false>
+template <int AK, int BK, bool BKM = false, class T = __half>
 static int launch_impl(GemmParams& p, cudaStream_t stream) {
   using C = Cfg<AK, BK>;
+  constexpr bool BF = std::is_same<T, __nv_bfloat16>::value;
   static DynSmemAttr attr = {};
-  if (int e = ensure_dyn_smem(contract_kernel<AK, BK, BKM>, kMaxSmem, attr)) return e;
+  if (int e = ensure_dyn_smem(contract_kernel<AK, BK, BKM, T>, kMaxSmem, attr)) return e;
   MPGCN_CHECK(p.R >= 1 && p.R <= 8, "R=%d out of range", p.R);
   const size_t b_stage = (size_t)p.R * BK * 64;
-  const int nres = p.b_res_reps * p.kb_total;
+  if (BF)
+    MPGCN_CHECK(p.kb_pass > 0 && p.kb_total % p.kb_pass == 0 && p.kb_pass % p.kb_per_seg == 0 && p.ep.corr_src == nullptr &&
+                    (p.ep.out_f16 ? p.ep.out16 != nullptr : p.ep.out16 == nullptr),
+                "bf16x3 contraction: kb_total=%d is not whole passes of %d k-blocks, or an fp16-only epilogue option is set", p.kb_total,
+                p.kb_pass);
+  const int nres = p.b_res_reps * (BF ? p.kb_pass : p.kb_total);
   MPGCN_CHECK(!BKM || nres == 0, "a K-major B operand streams through the ring");
   MPGCN_CHECK(p.ep.out != nullptr && p.ep.m_valid > 0 && p.ep.r_valid > 0, "contraction without an output");
   if (int e = make_out_map(&p.out_map, p.ep.out, p.ep.out_f16 != 0, p.ep, p.Z)) return e;
   const bool shadow = !p.ep.out_f16 && p.ep.out16 != nullptr;
-  if (shadow)
+  if (shadow || (BF && p.ep.out_f16))         // the fp16 shadow, or the lo plane of a bf16 pair
     if (int e = make_out_map(&p.out16_map, p.ep.out16, true, p.ep, p.Z)) return e;
-  p.st_bytes = p.ep.out_f16 ? 64 * 64 : shadow ? 64 * 128 + 64 * 64 : 64 * 128;
+  p.st_bytes = p.ep.out_f16 ? (BF ? 2 * 64 * 64 : 64 * 64) : shadow ? 64 * 128 + 64 * 64 : 64 * 128;
   const size_t fixed = smem_bytes(0, p.R, BK, 0, 0, p.st_bytes);      // everything but the ring
   int stages;
   if (nres) {
@@ -272,7 +278,7 @@ static int launch_impl(GemmParams& p, cudaStream_t stream) {
   double fl = 0;
   prof_take_next(&tag, &fl);
   prof_begin(tag, fl, stream);
-  contract_kernel<AK, BK, BKM><<<grid, kThreads1, smem, stream>>>(p);
+  contract_kernel<AK, BK, BKM, T><<<grid, kThreads1, smem, stream>>>(p);
   prof_end(stream);
   MPGCN_CUDA(cudaGetLastError());
   return 0;
@@ -290,6 +296,18 @@ int launch_contract(int ak, int bk, GemmParams& p, cudaStream_t stream) {
 }
 
 int launch_contract_bkm(GemmParams& p, cudaStream_t stream) { return launch_impl<A_K64, 32, true>(p, stream); }
+
+int launch_contract_bf16x3(int ak, int bk, GemmParams& p, cudaStream_t stream) {
+  using BF = __nv_bfloat16;
+  if (ak == A_MN128 && bk == 64) return launch_impl<A_MN128, 64, false, BF>(p, stream);
+  if (ak == A_K128 && bk == 64) return launch_impl<A_K128, 64, false, BF>(p, stream);
+  if (ak == A_K64 && bk == 32) return launch_impl<A_K64, 32, false, BF>(p, stream);
+  if (ak == A_K64 && bk == 64) return launch_impl<A_K64, 64, false, BF>(p, stream);
+  if (ak == A_K64 && bk == 96) return launch_impl<A_K64, 96, false, BF>(p, stream);
+  if (ak == A_MN64 && bk == 64) return launch_impl<A_MN64, 64, false, BF>(p, stream);
+  set_error("no bf16x3 contraction kernel for A kind %d, BK %d", ak, bk);
+  return 1;
+}
 
 }  // namespace tc
 }  // namespace mpgcn

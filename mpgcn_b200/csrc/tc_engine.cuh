@@ -3,7 +3,7 @@
 //
 //   D[z][i][(r,ch)] = alpha * sum_k A_z[k or i major] * B_z[k][(r,ch)]   (+ bias[ch], ReLU)
 //
-// * fp16 operands, fp32 accumulation in registers, M = 128 rows per tile (two consumer warpgroups of
+// * fp16 operands (or bf16 pairs in three passes: bf16x3, precision 2), fp32 accumulation in registers, M = 128 rows per tile (two consumer warpgroups of
 //   64 rows each), N = 32*R columns per tile (R <= 8 "channel chunks" of 32 = one 64-byte swizzle row).
 // * operands are staged by TMA into a multi-stage shared-memory ring in exactly the
 //   canonical wgmma layouts, so no thread ever touches operand bytes:
@@ -83,6 +83,12 @@ struct alignas(64) GemmParams {
                              // contractions that share one B block (the K supports applied to one X16 / dP16 row block) run back to
                              // back, so that block is fetched from HBM once and then served from L2
   Epilogue ep;
+  // bf16x3 (contract_kernel with T = __nv_bfloat16): every operand is a pair of bf16 planes, the lo plane a_plane_z / b_plane_z
+  // TMA z coordinates after the hi one, and the k-blocks run in passes of kb_pass (kb_total = passes * kb_pass), pass p reading
+  // A plane {hi, hi, lo}[p] and B plane {hi, lo, hi}[p].  With a resident B (the hi / lo halves of W as b_res_reps = 2) there
+  // are two passes over A: hi meets both halves, lo meets W hi only.  Unused by the fp16 instances.
+  int kb_pass;
+  int a_plane_z, b_plane_z;
 };
 
 constexpr int kConsumerWGs = 2;                        // 64 tile rows each
@@ -139,9 +145,13 @@ __device__ __forceinline__ void decode_tile(const GemmParams& p, int t, int& mt,
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) { return f2h2_sat_bits(a, b); }   // an fp16 operand never holds inf
 
-template <int AK, int BK, bool BKM = false>
+// T: the operand element type, __half (precision 1) or __nv_bfloat16 (precision 2, bf16x3: see GemmParams::kb_pass; a 16-bit
+// output is written as a bf16 hi plane to out_map and a lo plane to out16_map)
+template <int AK, int BK, bool BKM = false, class T = __half>
 __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_constant__ GemmParams p) {
   using C = Cfg<AK, BK>;
+  constexpr bool BF = std::is_same<T, __nv_bfloat16>::value;
+  static_assert(!BF || !BKM, "bf16x3 has no K-major B contraction");
   static_assert(!BKM || (AK == A_K64 && BK == 32), "a K-major B tile is one 32-wide k block, paired with a K-major SW64 A");
   constexpr int A_STAGE = C::A_STAGE;
   const int R = p.R;
@@ -150,7 +160,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int NRES = p.b_res_reps * p.kb_total;       // resident B tiles (0: B goes through the ring)
+  const int kb_res = BF ? p.kb_pass : p.kb_total;   // k-blocks per resident B rep
+  const int NRES = p.b_res_reps * kb_res;           // resident B tiles (0: B goes through the ring)
   uint8_t* sA = smem;
   uint8_t* sB = sA + (size_t)S * A_STAGE;
   uint8_t* sStore = sB + (size_t)(NRES ? NRES : S) * B_STAGE;     // 2 store buffers per consumer warpgroup
@@ -184,6 +195,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
   int p_t = blockIdx.x, p_kb = 0, p_kb1 = 0, p_kk = 0, p_sa_lo = 0, p_sa_hi = 0, p_sb_lo = 0, p_sb_hi = 0, p_zA0 = 0, p_zB0 = 0, p_mt = 0, p_nt = 0;
   int p_stage = 0;
   uint32_t p_phase = 0;
+  int p_pass = 0, p_pass_end = 0;   // bf16x3: pass of k-block p_kb, and the k-block that starts the next one
   auto p_start_tile = [&]() {
     int z;
     decode_tile(p, p_t, p_mt, p_nt, z);
@@ -191,8 +203,14 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
     p_kb1 = p.split_k ? min(p_kb + p.kb_per_slice, p.kb_total) : p.kb_total;
     p_zA0 = ((z / p.am.z_div) % p.am.z_mod) * p.am.z_mul;
     p_zB0 = ((z / p.bm.z_div) % p.bm.z_mod) * p.bm.z_mul;
-    const int seg = p_kb / p.kb_per_seg;
-    p_kk = p_kb - seg * p.kb_per_seg;
+    int kin = p_kb;                 // k-block within the pass
+    if constexpr (BF) {
+      p_pass = p_kb / p.kb_pass;
+      p_pass_end = (p_pass + 1) * p.kb_pass;
+      kin = p_kb - p_pass * p.kb_pass;
+    }
+    const int seg = kin / p.kb_per_seg;
+    p_kk = kin - seg * p.kb_per_seg;
     p_sa_lo = seg % p.am.seg_mod; p_sa_hi = seg / p.am.seg_mod;
     p_sb_lo = seg % p.bm.seg_mod; p_sb_hi = seg / p.bm.seg_mod;
   };
@@ -201,8 +219,12 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
     if (p_t >= num_tiles) return;
     mbar_wait_inline(&empty[p_stage], p_phase ^ 1u);
     mbar_arrive_expect_tx(&full[p_stage], (uint32_t)(A_STAGE + (NRES ? 0 : B_STAGE)));
-    const int zA = p_zA0 + p_sa_lo * p.am.seg_mul + p_sa_hi * p.am.seg_hi_mul;
-    const int zB = p_zB0 + p_sb_lo * p.bm.seg_mul + p_sb_hi * p.bm.seg_hi_mul;
+    int zA = p_zA0 + p_sa_lo * p.am.seg_mul + p_sa_hi * p.am.seg_hi_mul;
+    int zB = p_zB0 + p_sb_lo * p.bm.seg_mul + p_sb_hi * p.bm.seg_hi_mul;
+    if constexpr (BF) {             // the pass's planes: A {hi, hi, lo}, B {hi, lo, hi} (resident B: A {hi, lo})
+      zA += (NRES ? p_pass : p_pass >> 1) * p.a_plane_z;
+      zB += (p_pass & 1) * p.b_plane_z;
+    }
     const int kA = p_kk * BK + p_sa_lo * p.am.k_seg;
     const int kB = p_kk * BK + p_sb_lo * p.bm.k_seg;
     uint8_t* a_dst = sA + (size_t)p_stage * A_STAGE;
@@ -224,6 +246,13 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
       p_kk = 0;
       if (++p_sa_lo == p.am.seg_mod) { p_sa_lo = 0; ++p_sa_hi; }
       if (++p_sb_lo == p.bm.seg_mod) { p_sb_lo = 0; ++p_sb_hi; }
+    }
+    if constexpr (BF) {
+      if (p_kb + 1 == p_pass_end) {    // the next pass starts again at segment 0
+        ++p_pass;
+        p_pass_end += p.kb_pass;
+        p_kk = p_sa_lo = p_sa_hi = p_sb_lo = p_sb_hi = 0;
+      }
     }
     if (++p_kb == p_kb1) {
       p_t += gridDim.x;
@@ -265,13 +294,24 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
       // one k-block of MMAs stays in flight: a stage is released (and refilled by thread 0) once the MMAs of the NEXT k-block
       // are issued and wgmma.wait_group 1 has retired the ones that read it
       int prev = -1;
+      int c_pass = 0, c_pass_end = 0;       // bf16x3: the pass of kb (a resident B is indexed by the k-block within it)
+      if constexpr (BF) {
+        c_pass = kb0 / p.kb_pass;
+        c_pass_end = (c_pass + 1) * p.kb_pass;
+      }
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait_inline(&full[stage], phase);
         const uint32_t a_addr = smem_u32(sA + (size_t)stage * A_STAGE) + C::A_WG * (uint32_t)wg;
-        const int reps = NRES ? p.b_res_reps : 1;
+        int reps = NRES ? p.b_res_reps : 1;
+        int kin = kb;
+        if constexpr (BF) {
+          if (kb == c_pass_end) { ++c_pass; c_pass_end += p.kb_pass; }
+          kin = kb - c_pass * p.kb_pass;
+          if (c_pass > 0) reps = 1;         // the lo plane of A meets W hi only
+        }
         wgmma_fence();
         for (int rep = 0; rep < reps; ++rep) {
-          const uint32_t b_addr = smem_u32(sB + (size_t)(NRES ? rep * p.kb_total + kb : stage) * B_STAGE);
+          const uint32_t b_addr = smem_u32(sB + (size_t)(NRES ? rep * kb_res + kin : stage) * B_STAGE);
           const int first = (kb == kb0 && rep == 0) ? 1 : 0;
           // one dispatch on the tile width per k-block: the BK / 16 MMAs of a case then chain on the same registers
           auto kblock = [&](auto width) {
@@ -281,7 +321,7 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
               const uint64_t ad = gmma_desc(a_hi, a_addr + C::a_koff(k), C::A_LBO);
               // K-major B: the k-th 16 halves of each 64-byte row (8-row core matrices 512 B apart, as the K-major A_K64 tile)
               const uint64_t bd = BKM ? gmma_desc(b_hi, b_addr + k * 32, 16) : gmma_desc(b_hi, b_addr + k * C::B_KSTEP, C::B_LBO);
-              wgmma_n<RW, C::A_MN ? 1 : 0, BKM ? 0 : 1>(acc, ad, bd, (first && k == 0) ? 0 : 1);
+              wgmma_n<RW, C::A_MN ? 1 : 0, BKM ? 0 : 1, T>(acc, ad, bd, (first && k == 0) ? 0 : 1);
             }
           };
           switch (R) {
@@ -397,6 +437,18 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj) {
               const uint32_t o16 = (rho * 64 + 16 * jj + 4 * q) ^ (((rho >> 1) & 3) << 4);
+              if constexpr (BF) {         // a 16-bit output is a bf16 pair: hi plane, and 4 KB behind it the lo plane
+                if (p.ep.out_f16) {
+                  uint32_t hi2, lo2;
+                  split_bf16x2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1], hi2, lo2);
+                  *reinterpret_cast<uint32_t*>(buf + o16) = hi2;
+                  *reinterpret_cast<uint32_t*>(buf + 4096 + o16) = lo2;
+                } else {
+                  const uint32_t o32 = (rho * 128 + 32 * jj + 8 * q) ^ ((rho & 7) << 4);
+                  *reinterpret_cast<float2*>(buf + o32) = make_float2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
+                }
+                continue;
+              }
               const uint32_t h2 = pack_h2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
               if (p.ep.out_f16) {
                 *reinterpret_cast<uint32_t*>(buf + o16) = h2;
@@ -412,7 +464,11 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
           named_bar_sync(1 + wg, 128);
           if (tw == 0) {
             tma_store_4d(&p.out_map, buf, 0, row0, r, z);
-            if (!p.ep.out_f16 && p.ep.out16) tma_store_4d(&p.out16_map, buf + 8192, 0, row0, r, z);
+            if constexpr (BF) {
+              if (p.ep.out_f16) tma_store_4d(&p.out16_map, buf + 4096, 0, row0, r, z);
+            } else if (!p.ep.out_f16 && p.ep.out16) {
+              tma_store_4d(&p.out16_map, buf + 8192, 0, row0, r, z);
+            }
             bulk_commit();
           }
           ++st_seq;
@@ -432,6 +488,8 @@ __global__ void __launch_bounds__(kThreads1, 1) contract_kernel(const __grid_con
 int launch_contract(int ak, int bk, GemmParams& p, cudaStream_t stream);
 // the same with a K-major B operand (A_K64, BK = 32; no resident B)
 int launch_contract_bkm(GemmParams& p, cudaStream_t stream);
+// bf16x3 (precision 2): bf16 pair operands in passes, see GemmParams::kb_pass; the A kinds / BKs of launch_contract
+int launch_contract_bf16x3(int ak, int bk, GemmParams& p, cudaStream_t stream);
 
 }  // namespace tc
 }  // namespace mpgcn

@@ -19,7 +19,8 @@ import torch
 
 from . import _lib
 
-_PREC_NAMES = {"fp32": _lib.PREC_FP32, "fp16": _lib.PREC_FP16_TC, "auto": -1}
+# "bf16x3" (BDGCN layers only, never chosen by "auto"): the tensor-core layer on bf16 hi / lo operand pairs at fp32-class accuracy
+_PREC_NAMES = {"fp32": _lib.PREC_FP32, "fp16": _lib.PREC_FP16_TC, "bf16x3": _lib.PREC_BF16X3, "auto": -1}
 
 # bytes of training state (Z stash, LSTM c_t/h_t, head pre-activations) allocated by forward calls since the last .clear():
 # stays at zero under torch.no_grad() (tests/test_gpu_at_size.py::test_no_grad_allocates_no_training_state)
@@ -27,7 +28,7 @@ STASH_BYTES = collections.Counter()
 
 
 def default_precision() -> str:
-    """'auto' (tensor cores whenever the shape allows), 'fp16' or 'fp32'.  Env: MPGCN_B200_PRECISION."""
+    """'auto' (tensor cores whenever the shape allows), 'fp16', 'bf16x3' or 'fp32'.  Env: MPGCN_B200_PRECISION."""
     return os.environ.get("MPGCN_B200_PRECISION", "auto")
 
 
@@ -112,9 +113,9 @@ _SPARSE_CACHE = {}
 _SUPPORT_CACHE_MAX = 8
 
 
-def _cached(cache, G, ptr: int, make):
+def _cached(cache, G, ptr: int, make, tag=None):
     import weakref
-    key = id(G)
+    key = id(G) if tag is None else (id(G), tag)
     stream = _stream()
     e = cache.get(key)
     if e is not None:
@@ -134,14 +135,15 @@ def _cached(cache, G, ptr: int, make):
     return val
 
 
-def _prepared_supports(lib, G, Gc, planes: int, N: int):
+def _prepared_supports(lib, G, Gc, planes: int, N: int, prec=_lib.PREC_FP16_TC):
+    """The staged supports of the tensor-core layer at `prec`: fp16 + diagonal remainders (1), or the bf16x3 pair (2)."""
     def make(stream):
-        nbytes = lib.mpgcn_bdgcn_supports_prepared_bytes(planes, N)
+        nbytes = lib.mpgcn_bdgcn_supports_prepared_bytes_ex(planes, N, prec)
         blob = torch.empty(nbytes, dtype=torch.uint8, device=Gc.device)
         with torch.cuda.device(Gc.device):
-            _lib.check(lib.mpgcn_bdgcn_prepare_supports(_ptr(Gc), _ptr(blob), nbytes, planes, N, stream), "bdgcn_prepare_supports")
+            _lib.check(lib.mpgcn_bdgcn_prepare_supports_ex(_ptr(Gc), _ptr(blob), nbytes, planes, N, prec, stream), "bdgcn_prepare_supports")
         return blob
-    return _cached(_SUPPORT_CACHE, G, Gc.data_ptr(), make)
+    return _cached(_SUPPORT_CACHE, G, Gc.data_ptr(), make, None if prec == _lib.PREC_FP16_TC else prec)
 
 
 def _sparse_supports(lib, G, K: int, N: int):
@@ -175,7 +177,7 @@ class _BDGCNFn(torch.autograd.Function):
         H = W.shape[1]
         sparse = G_o.layout == torch.sparse_coo          # bdgcn() checked it: static, fp32 family, no gradient
         prec = _lib.PREC_FP32 if sparse else resolve_precision(precision, B, N, K, C, H)
-        tc = prec == _lib.PREC_FP16_TC
+        tc = prec != _lib.PREC_FP32
         Xc, Wc = _f32c(X), _f32c(W)
         Goc = torch.empty(0, device=X.device) if sparse else _f32c(G_o)
         Gdc = Goc if G_d is G_o else _f32c(G_d)
@@ -196,8 +198,8 @@ class _BDGCNFn(torch.autograd.Function):
             # epilogue then writes that copy instead of a separate cast pass reading the fp32 activation.)
             planes = (B if dynamic else 1) * K
             with torch.cuda.device(X.device):
-                go_p = _prepared_supports(lib, G_o, Goc, planes, N)
-                gd_p = go_p if G_d is G_o else _prepared_supports(lib, G_d, Gdc, planes, N)
+                go_p = _prepared_supports(lib, G_o, Goc, planes, N, prec)
+                gd_p = go_p if G_d is G_o else _prepared_supports(lib, G_d, Gdc, planes, N, prec)
             preps = (go_p, gd_p)
             ex.go_prepared, ex.gd_prepared = _ptr(go_p), _ptr(gd_p)
         ctx.sparse_nnz = None
@@ -232,7 +234,7 @@ class _BDGCNFn(torch.autograd.Function):
         dynamic, act, prec, has_bias = ctx.meta
         if saved.numel() == 0:
             raise RuntimeError("mpgcn_b200.bdgcn: backward called but forward ran without requires_grad inputs")
-        tc = prec == _lib.PREC_FP16_TC
+        tc = prec != _lib.PREC_FP32
         hint = _take_hint(ctx, d_out) if (tc and d_out.dtype == torch.float32 and d_out.is_contiguous()) else None
         d_out = _f32c(d_out)
         dev = d_out.device
@@ -291,8 +293,8 @@ def _check_sparse_supports(G, precision, grad_mode: bool) -> None:
     name = default_precision() if precision is None else precision
     if name not in _PREC_NAMES:
         raise ValueError(f"unknown precision {name!r}; expected one of {sorted(_PREC_NAMES)}")
-    if name == "fp16":
-        raise RuntimeError("mpgcn_b200.bdgcn: there are no fp16 sparse kernels; sparse supports run in fp32 (precision 'auto' or 'fp32')")
+    if name in ("fp16", "bf16x3"):
+        raise RuntimeError(f"mpgcn_b200.bdgcn: there are no {name} sparse kernels; sparse supports run in fp32 (precision 'auto' or 'fp32')")
 
 
 def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None, support_grad: bool = False) -> torch.Tensor:
@@ -305,6 +307,9 @@ def bdgcn(X: torch.Tensor, G, W: torch.Tensor, b, relu: bool, precision=None, su
     A static G given as a sparse COO tensor [K,N,N] runs the fp32 layer with its four N^3 contractions replaced by gathers over
     the stored entries (precision "auto" or "fp32"; its CSR / CSC structure is built once per tensor and cached).  Only stored
     entries are multiplied, so a non-finite X does not leak through a zero of G as it does in the dense layer."""
+    if support_grad and (default_precision() if precision is None else precision) == "bf16x3":
+        raise NotImplementedError("mpgcn_b200.bdgcn: precision 'bf16x3' has no support gradient (support_grad=True runs with 'auto', "
+                                  "'fp16' or 'fp32')")
     if isinstance(G, torch.Tensor):
         G_o = G_d = G
         dynamic = False
@@ -355,8 +360,15 @@ def lstm_recompute_chunk_cells(recompute, T, C, L) -> int:
     return max(1, LSTM_RECOMPUTE_BUDGET_BYTES * probe // per)
 
 
-def resolve_lstm_precision(name, T, C) -> int:
+def lstm_precision_name(name) -> str:
+    """The LSTM's reading of a precision name (None: ops.default_precision()): "bf16x3" is a BDGCN-layer precision, and a model
+    that runs its layers in it runs its LSTM as under "auto"."""
     name = default_precision() if name is None else name
+    return "auto" if name == "bf16x3" else name
+
+
+def resolve_lstm_precision(name, T, C) -> int:
+    name = lstm_precision_name(name)
     if name not in _PREC_NAMES:
         raise ValueError(f"unknown precision {name!r}; expected one of {sorted(_PREC_NAMES)}")
     lib = _lib.load()
@@ -455,7 +467,7 @@ def lstm_last(x_seq: torch.Tensor, w_ih, w_hh, b_ih, b_hh, precision=None, recom
 def lstm_stack_supports(name, T, C, L) -> bool:
     """Whether `lstm_stack` runs L >= 2 layers of hidden size C over T steps at precision `name`: the tensor-core kernels at
     hidden 32 and 96 ("auto" or "fp16"); there are no fp32 stacked kernels."""
-    name = default_precision() if name is None else name
+    name = lstm_precision_name(name)
     if name not in _PREC_NAMES:
         raise ValueError(f"unknown precision {name!r}; expected one of {sorted(_PREC_NAMES)}")
     code = _lib.PREC_FP16_TC if name == "auto" else _PREC_NAMES[name]
@@ -473,7 +485,7 @@ def lstm_runs_on_engine(lstm: torch.nn.LSTM, T: int, precision) -> bool:
         return False
     C, L = lstm.hidden_size, lstm.num_layers
     if L == 1:
-        explicit = precision not in (None, "auto") and C <= 64
+        explicit = precision is not None and lstm_precision_name(precision) != "auto" and C <= 64
         return explicit or lstm_engine_supports(precision, T, C)
     if lstm.dropout > 0 and lstm.training:
         return False

@@ -349,6 +349,9 @@ def _begin_forward(ctx, X, G_o, G_d, W, b, dynamic, act, precision, plan, grad_m
     N, C = X.shape[2], X.shape[3]
     K, H = G_o.shape[-3], W.shape[1]
     prec = _ENGINE.resolve_precision(precision, samples, N, K, C, H)
+    if prec == _lib.PREC_BF16X3:
+        raise NotImplementedError("mpgcn_b200.shard: precision 'bf16x3' runs whole layers only (the sharded model's layer parts have "
+                                  "fp16 and fp32 kernels); use 'auto', 'fp16' or 'fp32'")
     Xc, Goc, Wc = ops._f32c(X), ops._f32c(G_o), ops._f32c(W)
     Gdc = Goc if G_d is G_o else ops._f32c(G_d)
     keep = grad_mode and any(ctx.needs_input_grad)
